@@ -9,6 +9,8 @@ Each recipe restates one of the reference's sample scenes or one of the syntheti
 * :func:`joint_contact_stress` — config 4: stacked bridges + a grid of boxes dropped on them.
 * :func:`tumbler`         — config 3: motorised hollow container with a grid of small boxes.
 * :func:`mixed_shapes`    — circles/capsules/polygons/segments on a ground, exercising all nine manifold functions.
+* :func:`collision_zoo`   — every manifold kind, flipped pairs, dynamic segments, compound bodies, mixed frictions and
+                            shape filters, thrown sideways.
 
 All scenes are deterministic lattices (no RNG). A recipe returns a :class:`Scene` holding the world id and the
 body ids in creation order.
@@ -309,6 +311,113 @@ def mixed_shapes(lib, solver="TGS_Soft", rows=6, cols=8) -> Scene:
     return sc
 
 
+def collision_zoo(lib, solver="TGS_Soft", rows=5, cols=7) -> Scene:
+    """Every manifold kind, both pair orders, every friction mix and every filter rule in one small scene that keeps
+    changing: a static ground (box, two inward-leaning segment walls the bodies reach, a circle bump) under a lattice of
+    dynamic circles with offset centres, boxes, 5-8-gons, rounded boxes, capsules, compound bodies (2-3 shapes of
+    different kinds, local centre off the origin) and bodies carrying a segment next to a box, thrown sideways and spinning
+    so that pairs form and break and manifolds change point count.
+
+    * shape frictions cycle through {0, 0.2, 0.6, 1.0};
+    * categories 0x2 and 0x4 exclude each other by mask; column 2 shares a negative group (never collides within it),
+      column 4 a positive group of stacked capsules and circles whose masks exclude each other (collides within it all
+      the same);
+    * each row starts at a different kind, so circles are created before some of the polygons they land on: the pair's
+      primary shape (reference src/contact.c:139-154) then has the higher shape index (flipped pairs);
+    * the outer columns start just inside the walls and are thrown at them."""
+    world = lib.create_world(solver)
+    sc = Scene(lib, world, name=f"zoo{rows}x{cols}")
+    bd = default_body_def()
+    bd.position = Vec2(0.0, -1.0)
+    gid = lib.s2CreateBody(world, C.byref(bd))
+    sc.bodies.append(gid)
+    sd = default_shape_def()
+    ground = lib.s2MakeBox(12.0, 1.0)
+    lib.s2CreatePolygonShape(gid, C.byref(sd), C.byref(ground))
+    for x in (-9.0, 9.0):
+        wall = Segment(Vec2(x, 1.0), Vec2(0.7 * x, 8.0))
+        lib.s2CreateSegmentShape(gid, C.byref(sd), C.byref(wall))
+    bump = Circle(Vec2(0.5, 1.2), 0.6)
+    lib.s2CreateCircleShape(gid, C.byref(sd), C.byref(bump))
+
+    frictions = (0.0, 0.2, 0.6, 1.0)
+    nshape = 0
+
+    def shape_def(col, k):
+        nonlocal nshape
+        d = default_shape_def()
+        d.friction = frictions[nshape % 4]
+        nshape += 1
+        if k % 9 == 2:
+            d.filter = capi.Filter(0x0002, 0xFFFFFFFF & ~0x0004, 0)
+        elif k % 9 == 3:
+            d.filter = capi.Filter(0x0004, 0xFFFFFFFF, 0)
+        if col == 2:
+            d.filter = capi.Filter(0x0001, 0xFFFFFFFF, -1)
+        elif col == 4:
+            d.filter = capi.Filter(0x0008, 0xFFFFFFFF & ~0x0008, 1)
+        return d
+
+    for i in range(rows):
+        for j in range(cols):
+            k = i * cols + j
+            bd = default_body_def()
+            bd.type = capi.DYNAMIC_BODY
+            # the filtered columns start closer together than any shapes could rest: only the filter keeps them apart
+            y = 1.0 + (0.95 if j in (2, 4) else 1.4) * i
+            if j in (0, cols - 1):  # outer columns just inside the walls, thrown at them
+                side = -1.0 if j == 0 else 1.0
+                bd.position = Vec2(side * (8.1 - 2.7 * y / 7.0), y)
+                bd.linearVelocity = Vec2(3.0 * side, 0.0)
+            else:
+                bd.position = Vec2(2.0 * (j - 0.5 * (cols - 1)) + 0.3 * (i % 2), y)
+                bd.linearVelocity = Vec2(2.5 if i % 2 == 0 else -2.5, 0.5 * (j % 3) - 0.5)
+            bd.angle = 0.37 * ((k * 3) % 5) - 0.7
+            if j == 4:  # the positive group: level capsules and circles stacked 0.02 m apart, touching from the start
+                bd.position = Vec2(bd.position.x, (1.0, 1.6, 2.48, 3.15, 4.03)[i % 5] + 4.0 * (i // 5))
+                bd.angle = 0.0
+            bd.angularVelocity = 1.5 if k % 2 == 0 else -2.0
+            bid = lib.s2CreateBody(world, C.byref(bd))
+            sc.bodies.append(bid)
+            kind = (j + 3 * i) % 7  # every kind in every row but the positive group's: capsules and circles stacked
+            if j == 4:
+                kind = (4, 4, 0, 4, 0)[i % 5]
+            if kind == 0:
+                circle = Circle(Vec2(0.12, -0.05), 0.45)
+                lib.s2CreateCircleShape(bid, C.byref(shape_def(j, k)), C.byref(circle))
+            elif kind == 1:
+                box = lib.s2MakeBox(0.55, 0.35)
+                lib.s2CreatePolygonShape(bid, C.byref(shape_def(j, k)), C.byref(box))
+            elif kind == 2:
+                n = 5 + k % 4
+                pts = (Vec2 * n)(*[Vec2(0.55 * math.cos(2.0 * math.pi * (m + 0.1 * (m % 2)) / n),
+                                        0.5 * math.sin(2.0 * math.pi * (m + 0.1 * (m % 2)) / n)) for m in range(n)])
+                hull = lib.s2ComputeHull(pts, n)
+                poly = lib.s2MakePolygon(C.byref(hull))
+                lib.s2CreatePolygonShape(bid, C.byref(shape_def(j, k)), C.byref(poly))
+            elif kind == 3:
+                rounded = lib.s2MakeBox(0.4, 0.25)  # the reference has no s2MakeRoundedBox: a box with the radius set
+                rounded.radius = 0.12
+                lib.s2CreatePolygonShape(bid, C.byref(shape_def(j, k)), C.byref(rounded))
+            elif kind == 4:
+                cap = Capsule(Vec2(-0.45, 0.0), Vec2(0.45, 0.08), 0.25)
+                lib.s2CreateCapsuleShape(bid, C.byref(shape_def(j, k)), C.byref(cap))
+            elif kind == 5:
+                box = lib.s2MakeOffsetBox(0.3, 0.25, Vec2(0.35, 0.05), 0.2)
+                lib.s2CreatePolygonShape(bid, C.byref(shape_def(j, k)), C.byref(box))
+                circle = Circle(Vec2(-0.35, 0.1), 0.28)
+                lib.s2CreateCircleShape(bid, C.byref(shape_def(j, k)), C.byref(circle))
+                if k % 2 == 0:
+                    cap = Capsule(Vec2(-0.2, 0.45), Vec2(0.3, 0.5), 0.12)
+                    lib.s2CreateCapsuleShape(bid, C.byref(shape_def(j, k)), C.byref(cap))
+            else:
+                box = lib.s2MakeOffsetBox(0.4, 0.2, Vec2(0.0, 0.15), 0.0)
+                lib.s2CreatePolygonShape(bid, C.byref(shape_def(j, k)), C.byref(box))
+                seg = Segment(Vec2(-0.6, -0.2), Vec2(0.6, -0.25))
+                lib.s2CreateSegmentShape(bid, C.byref(shape_def(j, k)), C.byref(seg))
+    return sc
+
+
 RECIPES = {
     "pyramid": pyramid,
     "vertical_stack": vertical_stack,
@@ -316,6 +425,7 @@ RECIPES = {
     "joint_contact_stress": joint_contact_stress,
     "tumbler": tumbler,
     "mixed_shapes": mixed_shapes,
+    "collision_zoo": collision_zoo,
 }
 
 

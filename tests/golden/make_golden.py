@@ -1,6 +1,7 @@
 """Regenerate the golden fixtures from the UNMODIFIED reference (needs the reference built into oracle/_ref).
 
-    python tests/golden/make_golden.py
+    python tests/golden/make_golden.py          # everything
+    python tests/golden/make_golden.py host     # host_reference_sha1.json only
 
 pyramid10_tgs_soft.npz — config 1 (SURVEY §8d): Pyramid baseCount=10, s2_solverTGS_Soft, dt=1/60, 4 sub-steps, 2 relax
 iterations, warm starting; per-body origin / rotation / velocity after steps {1, 10, 60, 600}, and for every step the
@@ -70,6 +71,8 @@ def host_digests(R):
 def main():
     R = ref.load()
     host_digests(R)
+    if sys.argv[1:] == ["host"]:
+        return
     for solver in VARIANTS:
         variant_fixture(R, solver)
     sc = scenes.pyramid(R, "TGS_Soft", base_count=10)

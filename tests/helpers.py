@@ -85,6 +85,27 @@ def contact_rows_from_ref(cf: np.ndarray, ci: np.ndarray):
     return rows, slots
 
 
+STICKY_FIELDS = ("frictionAnchorA", "frictionAnchorB", "frictionNormalA", "frictionNormalB")
+
+
+def carry_sticky_friction(rows, keys, solved):
+    """The friction anchors and normals a TGS_Sticky solve writes into the manifolds (reference
+    src/solve_tgs_sticky.c:147-163) are carried into the next step's manifolds by s2UpdateContact: a new point takes those
+    of the FIRST old point with its id, an unmatched point starts at zero (reference src/contact.c:317-358). The reference
+    world is advanced with the oracle's impulses only, so this restates that carry-over on its post-collide rows, from the
+    oracle's rows of the previous step. Which points matched is checked against the reference's own persisted flags."""
+    for k, key in enumerate(keys.tolist()):
+        old = solved.get(key)
+        for i in range(2):
+            j = -1
+            if old is not None and i < rows["pointCount"][k]:
+                j = next((j for j in range(old["pointCount"]) if old["points"]["id"][j] == rows["points"]["id"][k, i]), -1)
+            if i < rows["pointCount"][k]:
+                assert (j >= 0) == bool(rows["points"]["persisted"][k, i]), "id matching differs from the reference's"
+            for name in STICKY_FIELDS:
+                rows["points"][name][k, i] = old["points"][name][j] if j >= 0 else 0.0
+
+
 def joint_rows_from_ref(jf: np.ndarray, ji: np.ndarray) -> np.ndarray:
     I, F = refmod.JOINT_I, refmod.JOINT_F
     n = jf.shape[0]

@@ -194,7 +194,31 @@ def test_manifold_functions_match_reference_bitwise(reference_if_built, product)
     assert hits > 1500  # the sweep actually produced contacts
 
 
-SWEEPS = {"polygon": polygon_sweep, "hull": hull_sweep, "manifold": manifold_sweep}
+def edge_manifold_sweep(L, is_reference):
+    """The cases of tests/narrowphase_cases.py (also run through the device kernel by test_narrowphase_gpu.py): each pair
+    from an empty cache at pose 1, then at pose 2 with the cache carried over."""
+    import narrowphase_cases as N
+    trials = []
+    for case in N.make_cases():
+        gA, gB = N.geometry(L, case["A"]), N.geometry(L, case["B"])
+        xfA = N.pose_transform(case["poseA"])
+        cache = capi.DistanceCache()
+        out = []
+        for pose in ("poseB1", "poseB2"):
+            out += _manifold(N.collide(L, case["kind"], gA, xfA, gB, N.pose_transform(case[pose]), cache))
+            out.append(struct.pack("<fi", cache.metric, cache.count) + bytes(cache.indexA) + bytes(cache.indexB))
+        trials.append(out)
+    return trials
+
+
+def test_edge_manifold_cases_match_reference_bitwise(reference_if_built, product):
+    """Separations around the speculative distance, touching, shallow and deep overlap, coincident centres, exact
+    relative angles with and without a 1e-6 rad offset, vertex against vertex, 3-8-gons with and without radius, offset
+    circles, short capsules, sizes 0.05-50 m, near the origin and 1e4 m away."""
+    _check("edge_manifold", edge_manifold_sweep(product, False), reference_if_built)
+
+
+SWEEPS = {"polygon": polygon_sweep, "hull": hull_sweep, "manifold": manifold_sweep, "edge_manifold": edge_manifold_sweep}
 
 
 def _atan2_inputs(n, seed):

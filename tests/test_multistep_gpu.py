@@ -18,7 +18,8 @@ and manifold ids evolve exactly as if the reference had solved in the device's o
 import numpy as np
 import pytest
 
-from helpers import bit_equal, body_rows_from_ref, contact_rows_from_ref, joint_rows_from_ref
+from helpers import (STICKY_FIELDS, bit_equal, body_rows_from_ref, carry_sticky_friction, contact_rows_from_ref,
+                     joint_rows_from_ref)
 from oracle import port
 from oracle import ref as refmod
 from solver2d_b200 import capi, device, scenes
@@ -48,7 +49,16 @@ def _load_bodies_into_ref(R, wid, rows):
     R.load_body_state(wid, bf)
 
 
-def _run(R, P, dev, recipe, solver, steps, vel, pos, kw, min_replays=0, setup=None):
+CONTACT_FIELDS = ("normal", "friction", "cacheCount", "cacheIndexA", "cacheIndexB", "cacheMetric")
+POINT_FIELDS = ("localAnchorA", "localAnchorB", "separation", "id", "persisted")
+
+
+def _same(g, w):
+    g, w = np.asarray(g), np.asarray(w)
+    return bit_equal(g, w) if g.dtype == np.float32 else bool(np.array_equal(g, w))
+
+
+def _run(R, P, dev, recipe, solver, steps, vel, pos, kw, min_replays=0, setup=None, observe=None):
     O = port.load()
     sr = recipe(R, solver, **kw)
     sp = recipe(P, solver, **kw)
@@ -61,6 +71,8 @@ def _run(R, P, dev, recipe, solver, steps, vel, pos, kw, min_replays=0, setup=No
         setup(dw)
     ctx = device.make_context(solver, DT, vel, pos, True)
     worst = {}
+    sticky = solver == "TGS_Sticky"
+    solved = {}  # TGS_Sticky: the oracle's rows of the previous step, by pair key
     for step in range(steps):
         cap = R.capacities(sr.world)["bodyCap"]
         pre = dw.download_all_bodies(cap)
@@ -76,6 +88,10 @@ def _run(R, P, dev, recipe, solver, steps, vel, pos, kw, min_replays=0, setup=No
             np.maximum(rows_slot["shapeA"], rows_slot["shapeB"]).astype(np.uint64)
         perm = np.argsort(keys, kind="stable")
         rows_key = rows_slot[perm]
+        if sticky:
+            carry_sticky_friction(rows_key, keys[perm], solved)
+        if observe is not None:
+            observe(R, sr.world, rows_key)
         joints = joint_rows_from_ref(*R.joints(sr.world))
 
         got_contacts = dw.download_contacts(len(rows_key) + 64)
@@ -103,6 +119,8 @@ def _run(R, P, dev, recipe, solver, steps, vel, pos, kw, min_replays=0, setup=No
         imp[slots[perm], 2] = oc["points"]["normalImpulse"][:, 1]
         imp[slots[perm], 3] = oc["points"]["tangentImpulse"][:, 1]
         R.load_contact_impulses(sr.world, imp)
+        if sticky:
+            solved = dict(zip(keys[perm].tolist(), oc.copy()))
         if len(oj):
             jimp = np.zeros((len(oj), 5), dtype=np.float32)
             jimp[:, 0:2] = oj["impulse"]
@@ -124,6 +142,30 @@ def _run(R, P, dev, recipe, solver, steps, vel, pos, kw, min_replays=0, setup=No
                 worst[name] = max(worst.get(name, 0.0), float(np.abs(g - o).max()))
         if not bit_equal(post["angularVelocity"][v], rf[v, F["w"]]):
             worst["w"] = max(worst.get("w", 0.0), float(np.abs(post["angularVelocity"][v] - rf[v, F["w"]]).max()))
+        # the contact table as the narrow phase left it (the reference's post-collide rows), and what the solver wrote back
+        for name in CONTACT_FIELDS:
+            if not _same(got_contacts[name], rows_key[name]):
+                worst["contact " + name] = 1.0
+        for name in POINT_FIELDS:
+            if not _same(got_contacts["points"][name], rows_key["points"][name]):
+                worst["contact point " + name] = 1.0
+        persisted_want = oc["frictionPersisted"] if sticky else rows_key["frictionPersisted"]
+        if not _same(got_contacts["frictionPersisted"], persisted_want):
+            worst["contact frictionPersisted"] = 1.0
+        if sticky:
+            for name in STICKY_FIELDS:
+                if not _same(got_contacts["points"][name], oc["points"][name]):
+                    worst["contact point " + name] = 1.0
+        # shape AABBs and fat AABBs written by the finalize stage (s2bFinalizeShapes)
+        sf, si = R.shapes(sr.world)
+        aabb, fat, _ = dw.download_shape_boxes(sf.shape[0])
+        sv = si[:, refmod.SHAPE_I["valid"]] == 1
+        n = min(len(aabb), len(sv))
+        assert not sv[n:].any(), f"step {step}: the device holds fewer shape slots than the reference"
+        if not _same(aabb[:n][sv[:n]], sf[:n, 0:4][sv[:n]]):
+            worst["shape aabb"] = 1.0
+        if not _same(fat[:n][sv[:n]], sf[:n, 4:8][sv[:n]]):
+            worst["shape fatAABB"] = 1.0
         live = rows_key["pointCount"] > 0
         for name in ("normalImpulse", "tangentImpulse"):
             if not bit_equal(got_contacts["points"][name][live], oc["points"][name][live]):
@@ -162,10 +204,63 @@ def test_joints_and_contacts_every_step_bit_exact(reference, product, dev):
     assert c.jointCount == 75
 
 
-@pytest.mark.parametrize("solver", ["PGS", "PGS_NGS", "PGS_NGS_Block", "PGS_Soft", "SoftStep", "TGS_NGS", "XPBD"])
+def _steps(solver, steps):
+    """Jacobi blows scenes apart in the reference as well: a few steps show it, more only measure the explosion."""
+    return 12 if solver == "Jacobi" else steps
+
+
+@pytest.mark.parametrize("solver", ["Jacobi", "PGS", "PGS_NGS", "PGS_NGS_Block", "PGS_Soft", "SoftStep", "TGS_Sticky",
+                                    "TGS_NGS", "XPBD"])
 def test_variants_every_step_bit_exact(reference, product, dev, solver):
-    c = _run(reference, product, dev, scenes.pyramid, solver, 40, 4, 2, dict(base_count=20))
-    assert c.constraintCount > 300
+    """TGS_Sticky also carries the friction anchors and normals its solve writes into the manifolds from step to step
+    (helpers.carry_sticky_friction); the device's are compared with the oracle's every step."""
+    c = _run(reference, product, dev, scenes.pyramid, solver, _steps(solver, 40), 4, 2, dict(base_count=20))
+    assert c.constraintCount > (0 if solver == "Jacobi" else 300)  # Jacobi's pyramid is mostly apart after 12 steps
+
+
+def _zoo_observer(seen):
+    """Records, from the reference's post-collide state, which manifold kinds had points, whether a pair was stored in
+    flipped order (primary shape with the higher index) and whether fat AABBs overlapped without a contact where only the
+    shape filter can have refused it (different bodies, not both static, not segment against segment)."""
+    names = {0: "capsule", 1: "circle", 2: "polygon", 3: "segment"}
+
+    def observe(R, wid, rows):
+        sf, si = R.shapes(wid)
+        bf, bi = R.bodies(wid)
+        I = refmod.SHAPE_I
+        types = si[:, I["type"]]
+        live = rows["pointCount"] > 0
+        for a, b in zip(rows["shapeA"][live], rows["shapeB"][live]):
+            seen.setdefault("kinds", set()).add((names[types[a]], names[types[b]]))
+        seen["flipped"] = seen.get("flipped", 0) + int((rows["shapeA"] > rows["shapeB"]).sum())
+        valid = np.nonzero(si[:, I["valid"]] == 1)[0]
+        fat = sf[valid, 4:8]
+        over = (fat[:, None, 0] <= fat[None, :, 2]) & (fat[None, :, 0] <= fat[:, None, 2]) & \
+               (fat[:, None, 1] <= fat[None, :, 3]) & (fat[None, :, 1] <= fat[:, None, 3])
+        body = si[valid, I["body"]]
+        static = bi[body, refmod.BODY_I["type"]] == capi.STATIC_BODY
+        seg = types[valid] == 3
+        cand = over & (body[:, None] != body[None, :]) & ~(static[:, None] & static[None, :]) & ~(seg[:, None] & seg[None, :])
+        cand = np.triu(cand, 1)
+        pairs = set(zip(np.minimum(rows["shapeA"], rows["shapeB"]).tolist(), np.maximum(rows["shapeA"], rows["shapeB"]).tolist()))
+        ia, ib = np.nonzero(cand)
+        seen["filtered"] = seen.get("filtered", 0) + sum((int(valid[x]), int(valid[y])) not in pairs for x, y in zip(ia, ib))
+    return observe
+
+
+@pytest.mark.parametrize("solver", capi.SOLVER_TYPES)
+def test_collision_zoo_every_step_bit_exact(reference, product, dev, solver):
+    """scenes.collision_zoo: all nine manifold kinds, flipped pairs, dynamic segments, rounded polygons and 5-8-gons,
+    compound bodies, mixed frictions and every filter rule, under every solver variant."""
+    seen = {}
+    _run(reference, product, dev, scenes.collision_zoo, solver, _steps(solver, 60), 4, 2, {}, observe=_zoo_observer(seen))
+    assert seen["flipped"] > 0, "no pair was stored in flipped order"
+    assert seen["filtered"] > 0, "no fat-AABB overlap was refused by the filter"
+    if solver != "Jacobi":
+        kinds = {("circle", "circle"), ("capsule", "circle"), ("capsule", "capsule"), ("polygon", "circle"),
+                 ("polygon", "capsule"), ("polygon", "polygon"), ("segment", "circle"), ("segment", "capsule"),
+                 ("segment", "polygon")}
+        assert kinds <= seen["kinds"], f"manifold kinds never touching: {sorted(kinds - seen['kinds'])}"
 
 
 def test_falling_boxes_every_step_bit_exact(reference, product, dev):

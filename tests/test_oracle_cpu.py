@@ -4,7 +4,8 @@ in the reference's own constraint order. The reference ships no tests or golden 
 import numpy as np
 import pytest
 
-from helpers import bit_equal, body_rows_from_ref, contact_rows_from_ref, joint_rows_from_ref
+from helpers import (STICKY_FIELDS, bit_equal, body_rows_from_ref, carry_sticky_friction, contact_rows_from_ref,
+                     joint_rows_from_ref)
 from oracle import port
 from oracle import ref as refmod
 from solver2d_b200 import capi, device, scenes
@@ -126,3 +127,37 @@ def test_variant_limits_motors_mouse_pinned(reference, solver):
 def test_variant_mixed_shapes_pinned(reference, solver):
     nc, _ = _pin(reference, scenes.mixed_shapes, solver, 100, 4, 2)
     assert nc > 20
+
+
+@pytest.mark.parametrize("recipe,kw", [(scenes.collision_zoo, {}), (scenes.pyramid, dict(base_count=20))],
+                         ids=["collision_zoo", "pyramid20"])
+def test_sticky_friction_carry_over_restatement_matches_reference(reference, recipe, kw):
+    """helpers.carry_sticky_friction (what the every-step GPU harness uses for TGS_Sticky) against the reference's own
+    s2UpdateContact: 60 reference steps, friction anchors and normals rebuilt from the previous step's solved manifolds."""
+    R = reference
+    sc = recipe(R, "TGS_Sticky", **kw)
+
+    def keyed():
+        rows, _ = contact_rows_from_ref(*R.contacts(sc.world))
+        keys = (np.minimum(rows["shapeA"], rows["shapeB"]).astype(np.uint64) << np.uint64(32)) | \
+            np.maximum(rows["shapeA"], rows["shapeB"]).astype(np.uint64)
+        p = np.argsort(keys, kind="stable")
+        return rows[p], keys[p]
+
+    solved, carried = {}, 0
+    for step in range(60):
+        R.step_collide(sc.world)
+        rows, keys = keyed()
+        mine = rows.copy()
+        for name in STICKY_FIELDS:
+            mine["points"][name] = 0.0
+        carry_sticky_friction(mine, keys, solved)
+        for name in STICKY_FIELDS:
+            assert bit_equal(mine["points"][name], rows["points"][name]), f"step {step}: {name}"
+        carried += int((rows["points"]["frictionNormalA"] != 0).any(axis=-1).sum())
+        R.step_solve(sc.world, DT, 4, 2, True)
+        R.step_finalize(sc.world)
+        rows, keys = keyed()
+        solved = dict(zip(keys.tolist(), rows.copy()))
+    sc.destroy()
+    assert carried > 500
