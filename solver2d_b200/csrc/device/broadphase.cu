@@ -5,8 +5,9 @@
 // hash set (src/table.c) and the fat-AABB overlap test + s2DestroyContact of world.c:149-166.
 //
 // GPU-first design instead of a port of the pointer-chasing tree:
-//   * a linear BVH (Morton order + Karras radix tree) over ALL proxies is rebuilt from scratch, fully in parallel,
-//     only on steps where some proxy left its fat AABB (or the host created/destroyed something);
+//   * a linear BVH (Morton order + Karras radix tree, collapsed into a tree of up to 8 children per node) over ALL proxies
+//     is rebuilt from scratch, fully in parallel, every 17th pass or when the host created/destroyed something, and
+//     refitted in the passes in between;
 //   * one thread per *moved* proxy walks the BVH and applies the reference's pair rules (both-moved de-duplication by
 //     proxy key, body-type rules of the three-tree query, existing pair, same body, filter, joint override, shape-type
 //     table) — so the set of created contacts equals the reference's;
@@ -28,12 +29,15 @@ struct BroadScratch
 	DevArray<int> leafIn, leafOut; // sorted leaf -> index into leafShape
 	DevArray<int> counters;		   // [0] leaf count [1] new pair count [2] kept count [3] bounds ready ...
 	DevArray<int> boundsBits;	   // 4 ordered-int encoded floats: min.x min.y max.x max.y
-	DevArray<int2> children;	   // internal nodes
-	DevArray<int> parent;		   // all nodes (internal [0,n-1), leaves [n-1, 2n-1))
-	DevArray<float4> nodeBox;	   // all nodes
-	DevArray<float4> pairBox;	   // per internal node: the boxes of its two children, adjacent
-	DevArray<int> visit;		   // refit arrival counters (internal nodes)
-	DevArray<int> nodeHeight;
+	DevArray<int2> children;	   // binary internal nodes
+	DevArray<int> parent;		   // all binary nodes (internal [0,n-1), leaves [n-1, 2n-1))
+	// the wide hierarchy (s2bBuildWide): a wide node is kept at the index of the binary node it was collapsed from
+	DevArray<float4> wideBox;	   // S2B_WIDE per wide node: the boxes of its children, adjacent
+	DevArray<int> wideChild;	   // S2B_WIDE per wide node: wide node index, ~shape for a leaf, S2B_WIDE_EMPTY
+	DevArray<int> wideCount;	   // children per wide node
+	DevArray<int> wideSlot;		   // per binary node: slot (wide parent * S2B_WIDE + i) it occupies, -1 for the root
+	DevArray<int> visit;		   // refit arrival counters (wide nodes); the last arriver resets its counter
+	DevArray<float4> rootBox;	   // box of the whole scene
 	DevArray<int> movedLeaves;	   // sorted-leaf indices of moved proxies
 	DevArray<int> movedFlag;
 	DevArray<int> largeShapes;	   // shapes of moved proxies with scene-sized boxes
@@ -92,9 +96,12 @@ void s2bFreeBroadScratch(s2bWorld* w)
 	b->boundsBits.release();
 	b->children.release();
 	b->parent.release();
-	b->nodeBox.release();
+	b->wideBox.release();
+	b->wideChild.release();
+	b->wideCount.release();
+	b->wideSlot.release();
 	b->visit.release();
-	b->nodeHeight.release();
+	b->rootBox.release();
 	b->movedLeaves.release();
 	b->movedFlag.release();
 	b->newKey.release();
@@ -106,7 +113,6 @@ void s2bFreeBroadScratch(s2bWorld* w)
 	b->mergeSrcIn.release();
 	b->mergeSrcOut.release();
 	b->cubTemp.release();
-	b->pairBox.release();
 	b->largeShapes.release();
 	b->pairHash.release();
 	for (int i = 0; i < 2; ++i)
@@ -126,14 +132,32 @@ void s2bFreeBroadScratch(s2bWorld* w)
 
 enum
 {
+	// set when the hierarchy is built, kept while it is reused
 	BC_LEAVES = 0,
-	BC_NEW_PAIRS = 1,
-	BC_KEPT = 2,
-	BC_MOVED = 3,
-	BC_HEIGHT = 4,
+	BC_HEIGHT = 1, // height of the binary hierarchy
+	// cleared by every pass
+	BC_NEW_PAIRS = 2,
+	BC_KEPT = 3,
+	BC_MOVED = 4,
 	BC_LARGE = 5, // moved proxies handled by the leaf-side query
 	BC_SIZE = 8
 };
+
+// The hierarchy the refit and the queries walk is WIDE: the binary radix tree collapsed so that a wide node stands for
+// S2B_WIDE_LEVELS binary levels (up to S2B_WIDE children). A query visiting a wide node reads the boxes of all its
+// children with one contiguous 8 x 16 B = 128 B access (one L2 line), and both walks climb a third of the levels.
+#define S2B_WIDE_LEVELS 3
+#define S2B_WIDE (1 << S2B_WIDE_LEVELS)
+#define S2B_WIDE_EMPTY (-0x7FFFFFFF - 1) // unused child slot
+// Depth bound of the radix tree: every internal node's keys share a longer common prefix than its parent's, and the
+// prefix of the (31-bit Morton code, 32-bit position) keys is 1..63 bits, so internal nodes lie at binary depth 0..62.
+// Wide nodes sit at binary depths 0, 3, ..., 60: at most 21 wide levels.
+#define S2B_MAX_INTERNAL_DEPTH 62
+#define S2B_MAX_WIDE_DEPTH (S2B_MAX_INTERNAL_DEPTH / S2B_WIDE_LEVELS)
+// A query descends into one overlapping wide child and stacks the others: it stacks at most S2B_WIDE - 1 nodes of each
+// depth 1..S2B_MAX_WIDE_DEPTH, and a stacked node is popped before anything of a smaller depth. The stack never holds more
+// than that, so no node is ever dropped.
+#define S2B_QUERY_STACK ((S2B_WIDE - 1) * S2B_MAX_WIDE_DEPTH)
 
 // ---------------------------------------------------------------------------------------------------------------
 // helpers
@@ -428,8 +452,74 @@ __global__ void s2bBuildRadixTree(const unsigned* codes, const int* counters, in
 	}
 }
 
-__global__ void s2bRefit(ShapeView s, const int* leafShape, const int* sortedLeaf, const int* counters, const int2* children,
-						 const int* parent, float4* nodeBox, float4* pairBox, int* visit, int* nodeHeight, int* countersOut)
+// one child of wide node `wide`: the binary descendant `node`, `levels` binary levels further down at most. Binary nodes
+// in between are expanded (left to right), so the children keep Morton order.
+template <int levels>
+__device__ __forceinline__ void s2bWideChildren(int wide, int node, int n, const int2* children, const int* leafShape, const int* sortedLeaf,
+												int* wideChild, int* wideSlot, int& count)
+{
+	bool leaf = node >= n - 1;
+	if constexpr (levels > 0)
+	{
+		if (leaf == false)
+		{
+			int2 ch = children[node];
+			s2bWideChildren<levels - 1>(wide, ch.x, n, children, leafShape, sortedLeaf, wideChild, wideSlot, count);
+			s2bWideChildren<levels - 1>(wide, ch.y, n, children, leafShape, sortedLeaf, wideChild, wideSlot, count);
+			return;
+		}
+	}
+	int slot = wide * S2B_WIDE + count;
+	wideChild[slot] = leaf ? ~leafShape[sortedLeaf[node - (n - 1)]] : node;
+	wideSlot[node] = slot;
+	count += 1;
+}
+
+// Collapse the binary radix tree into the wide hierarchy, one thread per binary internal node. The binary nodes at a depth
+// divisible by S2B_WIDE_LEVELS become wide nodes (kept at their binary index); their children are their descendants
+// S2B_WIDE_LEVELS levels down, or the leaves met before. The binary height (deepest leaf) is taken here once per build:
+// the refit no longer visits the binary tree.
+__global__ void s2bBuildWide(const int* leafShape, const int* sortedLeaf, int* counters, const int2* children, const int* parent,
+							 int* wideChild, int* wideCount, int* wideSlot)
+{
+	int n = counters[BC_LEAVES];
+	int u = blockIdx.x * blockDim.x + threadIdx.x;
+	if (u >= n - 1)
+	{
+		return;
+	}
+	int depth = 0;
+	for (int p = parent[u]; p >= 0; p = parent[p])
+	{
+		depth += 1;
+	}
+	int2 ch = children[u];
+	if (ch.x >= n - 1 || ch.y >= n - 1)
+	{
+		atomicMax(counters + BC_HEIGHT, depth + 1);
+	}
+	if (depth % S2B_WIDE_LEVELS != 0)
+	{
+		return;
+	}
+	int count = 0;
+	s2bWideChildren<S2B_WIDE_LEVELS - 1>(u, ch.x, n, children, leafShape, sortedLeaf, wideChild, wideSlot, count);
+	s2bWideChildren<S2B_WIDE_LEVELS - 1>(u, ch.y, n, children, leafShape, sortedLeaf, wideChild, wideSlot, count);
+	wideCount[u] = count;
+	for (int i = count; i < S2B_WIDE; ++i)
+	{
+		wideChild[u * S2B_WIDE + i] = S2B_WIDE_EMPTY;
+	}
+	if (u == 0)
+	{
+		wideSlot[0] = -1;
+	}
+}
+
+// Boxes bottom-up: a leaf thread writes its fat box into its slot in the parent wide node and counts its arrival; the last
+// child to arrive resets the counter for the next pass, unions the node's child boxes and carries that box one level up.
+__global__ void s2bRefit(ShapeView s, const int* leafShape, const int* sortedLeaf, const int* counters, const int* wideCount,
+						 const int* wideSlot, float4* wideBox, int* visit, float4* rootBox)
 {
 	int n = counters[BC_LEAVES];
 	int k = blockIdx.x * blockDim.x + threadIdx.x;
@@ -437,39 +527,42 @@ __global__ void s2bRefit(ShapeView s, const int* leafShape, const int* sortedLea
 	{
 		return;
 	}
-	int node = (n - 1) + k;
 	float4 box = s.fat[leafShape[sortedLeaf[k]]];
-	nodeBox[node] = box;
-	nodeHeight[node] = 0;
 	if (n == 1)
 	{
-		countersOut[BC_HEIGHT] = 0;
+		rootBox[0] = box;
 		return;
 	}
-	int p = parent[node];
-	while (p >= 0)
+	int slot = wideSlot[(n - 1) + k];
+	for (;;)
 	{
+		int p = slot / S2B_WIDE;
+		int count = wideCount[p];
+		wideBox[slot] = box;
 		__threadfence();
-		int arrived = atomicAdd(visit + p, 1);
-		if (arrived == 0)
+		if (atomicAdd(visit + p, 1) != count - 1)
 		{
-			return; // the sibling subtree finishes this node
+			return; // a sibling arrives later and finishes this node
 		}
-		int2 ch = children[p];
-		// L2 reads: the sibling published its box before its atomicAdd (threadfence above), L1 may not have it
-		float4 a = __ldcg(nodeBox + ch.x), b = __ldcg(nodeBox + ch.y);
-		box = make_float4(fminf(a.x, b.x), fminf(a.y, b.y), fmaxf(a.z, b.z), fmaxf(a.w, b.w));
-		nodeBox[p] = box;
-		// the two child boxes side by side with their parent: a query reads both with one 32-byte access
-		pairBox[2 * p] = a;
-		pairBox[2 * p + 1] = b;
-		int h = 1 + max(__ldcg(nodeHeight + ch.x), __ldcg(nodeHeight + ch.y));
-		nodeHeight[p] = h;
-		if (p == 0)
+		visit[p] = 0;
+		// L2 reads: the siblings published their boxes before their atomicAdd (threadfence above), L1 may not have them
+		const float4* b = wideBox + p * S2B_WIDE;
+		box = __ldcg(b);
+#pragma unroll
+		for (int i = 1; i < S2B_WIDE; ++i)
 		{
-			countersOut[BC_HEIGHT] = h;
+			if (i < count)
+			{
+				float4 c = __ldcg(b + i);
+				box = make_float4(fminf(box.x, c.x), fminf(box.y, c.y), fmaxf(box.z, c.z), fmaxf(box.w, c.w));
+			}
 		}
-		p = parent[p];
+		slot = wideSlot[p];
+		if (slot < 0)
+		{
+			rootBox[0] = box;
+			return;
+		}
 	}
 }
 
@@ -516,7 +609,7 @@ __device__ __forceinline__ void s2bBlockAppend(bool take, int value, int* list, 
 // list (s2bFindPairsLarge). One kernel, one atomic per block (round 1: flag array + split + cub select).
 #define S2B_MAX_LARGE_MOVERS 64
 
-__global__ void s2bCollectMovers(ShapeView s, const int* leafShape, const int* sortedLeaf, int* counters, const float4* nodeBox, int* movedLeaves,
+__global__ void s2bCollectMovers(ShapeView s, const int* leafShape, const int* sortedLeaf, int* counters, const float4* rootBox, int* movedLeaves,
 								 int* largeShapes)
 {
 	int n = counters[BC_LEAVES];
@@ -528,7 +621,7 @@ __global__ void s2bCollectMovers(ShapeView s, const int* leafShape, const int* s
 		moved = (s.head[shape].x & S2B_SHAPE_MOVED) != 0;
 		if (moved && n >= 256)
 		{
-			float4 root = nodeBox[0];
+			float4 root = rootBox[0];
 			float4 box = s.fat[shape];
 			float area = (box.z - box.x) * (box.w - box.y);
 			float sceneArea = (root.z - root.x) * (root.w - root.y);
@@ -652,13 +745,18 @@ __device__ __forceinline__ bool s2bMakeQuery(PairQuery& q, int shapeQ, const Sha
 }
 
 #define S2B_QUERY_BATCH 16
+#define S2B_QUERY_BLOCK 128
 
-// moved proxies with ordinary boxes: one thread walks the hierarchy
-__global__ void __launch_bounds__(128) s2bFindPairs(ShapeView s, BodyView b, const int* leafShape, const int* sortedLeaf, int* counters,
-								 const int* movedLeaves, const int2* children, const float4* pairBox,
+// moved proxies with ordinary boxes: one thread walks the wide hierarchy
+__global__ void __launch_bounds__(S2B_QUERY_BLOCK) s2bFindPairs(ShapeView s, BodyView b, const int* leafShape, const int* sortedLeaf, int* counters,
+								 const int* movedLeaves, const float4* wideBox, const int* wideChild,
 								 const unsigned long long* pairHash, unsigned long long hashMask, const unsigned long long* jointKeys,
 								 int jointKeyCount, unsigned long long* newKey, int2* newShapes, int newCap)
 {
+	// overlapping LEAVES are only collected during the walk and examined in batches afterwards: the walk (box tests) and the
+	// pair rules (shape header, hash probe, filters) are two different instruction streams, and a warp whose lanes hit
+	// leaves at different moments would otherwise execute both serially for every lane
+	__shared__ int found[S2B_QUERY_BATCH][S2B_QUERY_BLOCK];
 	int n = counters[BC_LEAVES];
 	int movedCount = counters[BC_MOVED];
 	int qi = blockIdx.x * blockDim.x + threadIdx.x;
@@ -674,64 +772,62 @@ __global__ void __launch_bounds__(128) s2bFindPairs(ShapeView s, BodyView b, con
 	}
 	float4 boxQ = s.fat[q.shapeQ];
 
-	// descend into one overlapping child directly and stack the other: half the stack traffic of push-both / pop.
-	// Overlapping LEAVES are only collected during the walk and examined in batches afterwards: the walk (box tests) and the
-	// pair rules (shape header, hash probe, filters) are two different instruction streams, and a warp whose lanes hit
-	// leaves at different moments would otherwise execute both serially for every lane.
-	int stack[64];
-	int found[S2B_QUERY_BATCH];
-	int nFound = 0;
+	// depth-first: test a wide node's children's boxes (one contiguous read), descend into the first overlapping wide child
+	// directly and stack the others, collect the overlapping leaves. The stack is sized from the depth bound of the build
+	// (S2B_QUERY_STACK).
+	int stack[S2B_QUERY_STACK];
 	int sp = 0;
 	int node = 0;
-	bool walking = true;
-	while (walking || nFound > 0)
+	int nFound = 0;
+	while (node >= 0 || nFound > 0)
 	{
-		while (walking && nFound < S2B_QUERY_BATCH)
+		while (node >= 0 && nFound <= S2B_QUERY_BATCH - S2B_WIDE)
 		{
-			if (node >= n - 1)
+			// all loads of the node first (boxes of unused slots included): one round trip per visited node
+			const float4* boxes = wideBox + node * S2B_WIDE;
+			const int4* refs = reinterpret_cast<const int4*>(wideChild + node * S2B_WIDE);
+			int child[S2B_WIDE];
+			float4 box[S2B_WIDE];
+#pragma unroll
+			for (int i = 0; i < S2B_WIDE / 4; ++i)
 			{
-				found[nFound++] = node - (n - 1);
-				if (sp == 0)
+				int4 r = refs[i];
+				child[4 * i] = r.x;
+				child[4 * i + 1] = r.y;
+				child[4 * i + 2] = r.z;
+				child[4 * i + 3] = r.w;
+			}
+#pragma unroll
+			for (int i = 0; i < S2B_WIDE; ++i)
+			{
+				box[i] = boxes[i];
+			}
+			int next = -1;
+#pragma unroll
+			for (int i = 0; i < S2B_WIDE; ++i)
+			{
+				int c = child[i];
+				if (c != S2B_WIDE_EMPTY && s2bBoxesOverlap(boxQ, box[i]))
 				{
-					walking = false;
-					break;
+					if (c < 0)
+					{
+						found[nFound++][threadIdx.x] = ~c;
+					}
+					else if (next < 0)
+					{
+						next = c;
+					}
+					else
+					{
+						stack[sp++] = c;
+					}
 				}
-				node = stack[--sp];
-				continue;
 			}
-			int2 ch = children[node];
-			bool o0 = s2bBoxesOverlap(boxQ, pairBox[2 * node]);
-			bool o1 = s2bBoxesOverlap(boxQ, pairBox[2 * node + 1]);
-			if (o0 && o1)
-			{
-				if (sp < 64)
-				{
-					stack[sp++] = ch.y;
-				}
-				node = ch.x;
-			}
-			else if (o0)
-			{
-				node = ch.x;
-			}
-			else if (o1)
-			{
-				node = ch.y;
-			}
-			else
-			{
-				if (sp == 0)
-				{
-					walking = false;
-					break;
-				}
-				node = stack[--sp];
-			}
+			node = next >= 0 ? next : (sp > 0 ? stack[--sp] : -1);
 		}
 		for (int k = 0; k < nFound; ++k)
 		{
-			s2bConsiderPair(q, leafShape[sortedLeaf[found[k]]], s, b, counters, pairHash, hashMask, jointKeys, jointKeyCount, newKey, newShapes,
-							newCap);
+			s2bConsiderPair(q, found[k][threadIdx.x], s, b, counters, pairHash, hashMask, jointKeys, jointKeyCount, newKey, newShapes, newCap);
 		}
 		nFound = 0;
 	}
@@ -914,10 +1010,12 @@ static size_t bpReserve(s2bWorld* w, BroadScratch* B)
 	B->boundsBits.reserve(4, st, false);
 	B->children.reserve(nS, st, false);
 	B->parent.reserve(2 * nS, st, false);
-	B->nodeBox.reserve(2 * nS, st, false);
-	B->pairBox.reserve(2 * nS, st, false);
-	B->visit.reserve(nS, st, false);
-	B->nodeHeight.reserve(2 * nS, st, false);
+	B->wideBox.reserve(S2B_WIDE * nS, st, false, false);
+	B->wideChild.reserve(S2B_WIDE * nS, st, false, false);
+	B->wideCount.reserve(nS, st, false, false);
+	B->wideSlot.reserve(2 * nS, st, false, false);
+	B->visit.reserve(nS, st, false); // zeroed once here: from then on every refit leaves its counters at zero
+	B->rootBox.reserve(1, st, false);
 	B->movedLeaves.reserve(nS, st, false);
 	B->movedFlag.reserve(nS, st, false);
 	B->largeShapes.reserve(S2B_MAX_LARGE_MOVERS, st, false);
@@ -951,13 +1049,12 @@ static void bpSearch(s2bWorld* w, BroadScratch* B)
 	ShapeView sv = shapeView(w);
 	BodyView bv = bodyView(w);
 	ContactColumns& cur = w->contacts[w->cur];
-	size_t nS = (size_t)shapeCap;
 	int newCap = B->newPairCap;
 
 	bool reuseTree = B->treeValid && w->pairsDirty == false && B->treeShapeCap == shapeCap && B->treeReuses < S2B_TREE_REUSE_LIMIT;
 	if (reuseTree)
 	{
-		// keep BC_LEAVES (and the stale height); clear the per-pass counters
+		// keep BC_LEAVES and BC_HEIGHT of the build; clear the per-pass counters
 		S2B_CHECK(cudaMemsetAsync(B->counters.p + BC_NEW_PAIRS, 0, sizeof(int) * (BC_SIZE - BC_NEW_PAIRS), st));
 		B->treeReuses += 1;
 	}
@@ -985,15 +1082,16 @@ static void bpSearch(s2bWorld* w, BroadScratch* B)
 
 		// ---- hierarchy ----
 		S2B_LAUNCH(w, s2bBuildRadixTree, gridFor(shapeCap, 256), 256, 0, B->mortonOut.p, B->counters.p, B->children.p, B->parent.p);
+		S2B_LAUNCH(w, s2bBuildWide, gridFor(shapeCap, 256), 256, 0, B->leafShape.p, B->leafOut.p, B->counters.p, B->children.p,
+				   B->parent.p, B->wideChild.p, B->wideCount.p, B->wideSlot.p);
 		B->treeValid = true;
 		B->treeShapeCap = shapeCap;
 		B->treeReuses = 0;
 	}
 
 	// ---- refit ----
-	S2B_CHECK(cudaMemsetAsync(B->visit.p, 0, sizeof(int) * nS, st));
-	S2B_LAUNCH(w, s2bRefit, gridFor(shapeCap, 256), 256, 0, sv, B->leafShape.p, B->leafOut.p, B->counters.p, B->children.p,
-			   B->parent.p, B->nodeBox.p, B->pairBox.p, B->visit.p, B->nodeHeight.p, B->counters.p);
+	S2B_LAUNCH(w, s2bRefit, gridFor(shapeCap, 256), 256, 0, sv, B->leafShape.p, B->leafOut.p, B->counters.p, B->wideCount.p,
+			   B->wideSlot.p, B->wideBox.p, B->visit.p, B->rootBox.p);
 
 	// ---- pair-key hash set of the current contact table (rebuilt only when the table changed) ----
 	if (B->hashVersion != w->contactTableVersion || B->pairHash.p == nullptr)
@@ -1014,11 +1112,11 @@ static void bpSearch(s2bWorld* w, BroadScratch* B)
 	}
 
 	// ---- queries from moved proxies ----
-	S2B_LAUNCH(w, s2bCollectMovers, gridFor(shapeCap, 256), 256, 0, sv, B->leafShape.p, B->leafOut.p, B->counters.p, B->nodeBox.p,
+	S2B_LAUNCH(w, s2bCollectMovers, gridFor(shapeCap, 256), 256, 0, sv, B->leafShape.p, B->leafOut.p, B->counters.p, B->rootBox.p,
 			   B->movedLeaves.p, B->largeShapes.p);
-	S2B_LAUNCH(w, s2bFindPairs, gridFor(shapeCap, 128), 128, 0, sv, bv, B->leafShape.p, B->leafOut.p, B->counters.p,
-			   B->movedLeaves.p, B->children.p, B->pairBox.p, B->pairHash.p, B->hashMask, w->jointPairKeys.p, w->jointPairCount,
-			   B->newKey.p, B->newShapes.p, newCap);
+	S2B_LAUNCH(w, s2bFindPairs, gridFor(shapeCap, S2B_QUERY_BLOCK), S2B_QUERY_BLOCK, 0, sv, bv, B->leafShape.p, B->leafOut.p,
+			   B->counters.p, B->movedLeaves.p, B->wideBox.p, B->wideChild.p, B->pairHash.p, B->hashMask, w->jointPairKeys.p,
+			   w->jointPairCount, B->newKey.p, B->newShapes.p, newCap);
 	S2B_LAUNCH(w, s2bFindPairsLarge, gridFor(shapeCap, 256), 256, 0, sv, bv, B->leafShape.p, B->counters.p, B->largeShapes.p,
 			   B->pairHash.p, B->hashMask, w->jointPairKeys.p, w->jointPairCount, B->newKey.p, B->newShapes.p, newCap);
 
