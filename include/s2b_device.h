@@ -80,6 +80,7 @@ typedef struct s2bShapeRow
 	int32_t count;
 	float vertices[16];
 	float normals[16];
+	float restitution; // s2ShapeDef.restitution (used when the world has restitution enabled: s2b_set_restitution)
 } s2bShapeRow;
 
 #define S2B_SHAPE_MOVED 0x10
@@ -138,6 +139,7 @@ typedef struct s2bContactRow
 	int32_t cacheCount;
 	uint8_t cacheIndexA[4], cacheIndexB[4];
 	float cacheMetric;
+	float restitution; // max of the two shapes' restitution, mixed when the pair is created (reference src/contact.c:49-52)
 } s2bContactRow;
 
 // ---- step context ---------------------------------------------------------------------------------------------
@@ -213,6 +215,11 @@ S2B_API void s2b_set_regions(s2bWorld* world, int mode);
 // tickets (1: a constraint waits only for the previous constraint on each of its bodies; no barrier inside a sweep).
 // Same bits either way; the ticketed form measured SLOWER (75 k pollers saturate L2), kept as an experiment.
 S2B_API void s2b_set_dataflow(s2bWorld* world, int enable);
+// Restitution (an extension: the reference stores it and never applies it). enable = 0 (default): contacts do not bounce.
+// enable = 1: the solver stage ends with one Gauss-Seidel pass over the contact constraints, in the stage's own solve order,
+// that drives the normal velocity of every manifold point towards -e * (its approach speed at the start of the stage), for
+// points whose approach was faster than `threshold` (m/s) and which carry a normal impulse (DESIGN.md §3.7).
+S2B_API void s2b_set_restitution(s2bWorld* world, int enable, float threshold);
 
 // ---- host -> device -------------------------------------------------------------------------------------------
 

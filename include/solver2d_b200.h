@@ -15,6 +15,14 @@ extern "C"
 // counters, NCCL packing). The handle is owned by the world.
 S2B_API s2bWorld* s2World_GetDevice(s2WorldId worldId);
 
+// Bounce contacts by their shapes' restitution (default off: restitution is ignored, as in the reference). A contact's
+// restitution is the larger of its two shapes' s2ShapeDef.restitution. Takes effect at the next s2World_Step.
+S2B_API void s2World_EnableRestitution(s2WorldId worldId, bool enable);
+// Approach speed (m/s) below which a contact does not bounce. Default 1 m/s, the reference's world->restitutionThreshold.
+// A threshold that is not finite or is negative is rejected (the world keeps its threshold). Takes effect at the next
+// s2World_Step.
+S2B_API void s2World_SetRestitutionThreshold(s2WorldId worldId, float threshold);
+
 // Push every pending host-side edit to the device now (s2World_Step does this itself).
 S2B_API void s2World_Flush(s2WorldId worldId);
 

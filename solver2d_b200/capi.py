@@ -246,6 +246,9 @@ _API = {
     "s2MakeCapsule": (Polygon, [Vec2, Vec2, C.c_float]),
     "s2MakePolygon": (Polygon, [C.POINTER(Hull)]),
     "s2ComputeHull": (Hull, [C.POINTER(Vec2), C.c_int32]),
+    # extensions (include/solver2d_b200.h): restitution is off unless a world enables it
+    "s2World_EnableRestitution": (None, [WorldId, C.c_bool]),
+    "s2World_SetRestitutionThreshold": (None, [WorldId, C.c_float]),
 }
 
 class Transform(C.Structure):

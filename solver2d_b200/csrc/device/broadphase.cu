@@ -914,7 +914,7 @@ __global__ void s2bMergeKeys(const int* counters, const int* keepSlots, const un
 	}
 }
 
-// s2CreateContact for new pairs (reference src/contact.c:156-229: empty manifold, empty cache, mixed friction), plain
+// s2CreateContact for new pairs (reference src/contact.c:156-229: empty manifold, empty cache, mixed friction and restitution), plain
 // copy for survivors
 __global__ void s2bGatherContactsSorted(const int* counters, const unsigned long long* sortedKey, const int* sortedSrc, ContactView src,
 										ContactView dst, const int2* newShapes, ShapeView s, int sticky, int shapeBits)
@@ -954,7 +954,9 @@ __global__ void s2bGatherContactsSorted(const int* counters, const unsigned long
 		dst.info[t] = make_int4(0, 0, 0, 0);
 		// s2MixFriction (reference src/contact.c:42-45)
 		float friction = sqrtf(s.fr[sh.x].x * s.fr[sh.y].x);
-		dst.nf[t] = make_float4(0.0f, 0.0f, friction, 0.0f);
+		// s2MixRestitution (reference src/contact.c:49-52)
+		float restitution = S2_MAX(s.restitution[sh.x], s.restitution[sh.y]);
+		dst.nf[t] = make_float4(0.0f, 0.0f, friction, restitution);
 		dst.color[t] = -1;
 		for (int p = 0; p < 2; ++p)
 		{

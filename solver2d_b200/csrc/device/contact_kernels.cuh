@@ -272,6 +272,73 @@ __device__ __forceinline__ void s2bStoreVelocities(const SolveArgs& a, const Bod
 }
 
 // ---------------------------------------------------------------------------------------------------------------
+// restitution
+// ---------------------------------------------------------------------------------------------------------------
+// The restitution pass (an extension, DESIGN.md §3.7; the reference stores restitution and never applies it). Runs after
+// the variant's whole program, once per contact constraint in the stage's solve order. A point bounces when its approach
+// speed at the start of the stage, vr (SolveArgs::restVr), was faster than the threshold and it carries a normal impulse:
+// the impulse that takes its current normal velocity to -e * vr is added, clamped so that the accumulated impulse stays
+// >= 0, at the anchors captured with vr. Works on the manifold and the body columns directly (body slots from the contact
+// table): by now every body is back in global memory and the constraint rows may address a region's shared copy.
+__device__ __forceinline__ void s2bApplyRestitution(const SolveArgs& a, int t)
+{
+	int slot = a.cc.src[t];
+	float4 mnf = a.contacts.nf[slot];
+	float e = mnf.w;
+	if (e == 0.0f)
+	{
+		return;
+	}
+	int2 bodies = a.contacts.bodies[slot];
+	int pointCount = S2B_CI_COUNT(a.contacts.info[slot].x);
+	float4 velA = a.bodies.vel[bodies.x], velB = a.bodies.vel[bodies.y];
+	float mA = velA.w, mB = velB.w;
+	float iA = a.bodies.prm[bodies.x].w, iB = a.bodies.prm[bodies.y].w;
+	s2Vec2 vA = V2(velA.x, velA.y), vB = V2(velB.x, velB.y);
+	float wA = velA.z, wB = velB.z;
+	s2Vec2 normal = V2(mnf.x, mnf.y);
+	float4 captured = a.restVr[slot];
+	float vr[2] = {captured.x, captured.y};
+	float normalMass[2] = {captured.z, captured.w};
+	bool applied = false;
+
+#pragma unroll
+	for (int j = 0; j < 2; ++j)
+	{
+		if (j < pointCount)
+		{
+			float4 mi = a.contacts.impulse[j][slot];
+			if (vr[j] > -a.restitutionThreshold || mi.y == 0.0f)
+			{
+				continue;
+			}
+			float4 r = a.restR[j][slot];
+			s2Vec2 rA = V2(r.x, r.y), rB = V2(r.z, r.w);
+			s2Vec2 vrB = s2Add(vB, s2CrossSV(wB, rB));
+			s2Vec2 vrA = s2Add(vA, s2CrossSV(wA, rA));
+			float vn = s2Dot(s2Sub(vrB, vrA), normal);
+			float impulse = -normalMass[j] * (vn + e * vr[j]);
+			float newImpulse = S2_MAX(mi.y + impulse, 0.0f);
+			impulse = newImpulse - mi.y;
+			mi.y = newImpulse;
+			a.contacts.impulse[j][slot] = mi;
+			s2Vec2 P = s2MulSV(impulse, normal);
+			vA = s2MulSub(vA, mA, P);
+			wA -= iA * s2Cross(rA, P);
+			vB = s2MulAdd(vB, mB, P);
+			wB += iB * s2Cross(rB, P);
+			applied = true;
+		}
+	}
+
+	if (applied)
+	{
+		BodyPair bp = {bodies.x, bodies.y, velA, velB, (mA != 0.0f) || (iA != 0.0f), (mB != 0.0f) || (iB != 0.0f)};
+		s2bStoreVelocities(a, bp, vA, wA, vB, wB);
+	}
+}
+
+// ---------------------------------------------------------------------------------------------------------------
 // s2WarmStartContacts (reference src/solve_common.c:276-326): impulses applied at the current anchors.
 // ---------------------------------------------------------------------------------------------------------------
 __device__ __forceinline__ void s2bWarmStartContact(const SolveArgs& a, int t)

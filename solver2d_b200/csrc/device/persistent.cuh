@@ -921,3 +921,5 @@ template <int SOLVER> __global__ void __launch_bounds__(S2B_BLOCK) s2bPersistent
 
 // host-side handle of an instantiation (defined in persistent_*.cu)
 void* s2bPersistentKernel(int solverType);
+// the instantiation that runs the restitution pass (S2B_RESTITUTION_PROGRAM, persistent_r.cu)
+void* s2bRestitutionKernel();

@@ -68,6 +68,7 @@ enum ContactOp
 	COP_STORE,
 	COP_STORE_SCALED, // XPBD stores impulse * inv_h
 	COP_TGS_SOFT_RELAX_STORE, // the LAST relax sweep of TGS_Soft: also writes the impulses to the manifolds (no separate store pass)
+	COP_RESTITUTION,		  // the restitution pass (s2bApplyRestitution): only in the program of S2B_RESTITUTION_PROGRAM
 };
 
 enum JointOp
@@ -88,6 +89,10 @@ enum JointOp
 	JOP_XPBD,
 	JOP_STORE,
 };
+
+// The instantiation of the persistent kernel that runs the restitution pass after a variant's program (solver.cu): its
+// program is one Gauss-Seidel pass of COP_RESTITUTION and it carries no other operation.
+#define S2B_RESTITUTION_PROGRAM 10
 
 struct PassDesc
 {
@@ -119,6 +124,10 @@ __host__ __device__ constexpr bool s2bUsesBodyOp(int solver, int op)
 	{
 		return true;
 	}
+	if (solver == S2B_RESTITUTION_PROGRAM)
+	{
+		return false;
+	}
 	switch (op)
 	{
 		case BOP_INTEGRATE_VELOCITIES:
@@ -146,6 +155,10 @@ __host__ __device__ constexpr bool s2bUsesContactOp(int solver, int op)
 	if (solver < 0)
 	{
 		return true;
+	}
+	if (solver == S2B_RESTITUTION_PROGRAM)
+	{
+		return op == COP_RESTITUTION;
 	}
 	switch (op)
 	{
@@ -204,6 +217,10 @@ __host__ __device__ constexpr bool s2bUsesJointOp(int solver, int op)
 	if (solver < 0)
 	{
 		return true;
+	}
+	if (solver == S2B_RESTITUTION_PROGRAM)
+	{
+		return false;
 	}
 	switch (op)
 	{
@@ -472,6 +489,12 @@ template <int SOLVER> __device__ __forceinline__ void s2bRunContactOpT(int op, c
 			if constexpr (s2bUsesContactOp(SOLVER, COP_STORE_SCALED))
 			{
 				s2bStoreContactImpulses(a, t, a.xpbdInvH);
+			}
+			break;
+		case COP_RESTITUTION:
+			if constexpr (s2bUsesContactOp(SOLVER, COP_RESTITUTION))
+			{
+				s2bApplyRestitution(a, t);
 			}
 			break;
 		default:

@@ -117,7 +117,7 @@ struct ContactColumns
 	DevArray<int2> shapes;			  // (A, B) in manifold order
 	DevArray<int2> bodies;			  // (A, B)
 	DevArray<int4> info;			  // x: count/flags, y: id0 | id1 << 16, z: GJK cache (count | iA<<2.. ), w: cache metric bits
-	DevArray<float4> nf;			  // normal.x normal.y friction 0
+	DevArray<float4> nf;			  // normal.x normal.y friction restitution
 	DevArray<int> color;			  // colour the constraint was last solved with (-1: none)
 	DevArray<float4> anchor[2];		  // localAnchorA.xy localAnchorB.xy   (body-origin relative, body frame)
 	DevArray<float4> impulse[2];	  // separation normalImpulse tangentImpulse 0
@@ -257,6 +257,7 @@ struct ShapeView
 	float2* verts;	 // [shape * 8 + i]
 	float2* normals; // [shape * 8 + i]
 	int capacity;
+	float* restitution; // per shape
 };
 
 // per-joint columns (slot order)
@@ -312,6 +313,8 @@ struct s2bWorld
 	int regionCutLimit = 3; // S2B_REGION_CUT_LIMIT
 	int dataflow = 0;	// ticketed Gauss-Seidel passes in the persistent kernel (experimental, measured slower: DESIGN.md §3.1);
 						// s2b_set_dataflow / S2B_DATAFLOW=1 enable it
+	int restitution = 0;			   // s2b_set_restitution: end the solver stage with the restitution pass
+	float restitutionThreshold = 1.0f; // approach speed (m/s) below which a contact does not bounce
 	int gatherWarm = 1; // per-body warm-start gather (warm_gather.cuh); s2b_set_warm_gather / S2B_WARM_GATHER=0 disable it
 	int smCount = 132;
 	int coopSupported = 0;
@@ -332,6 +335,7 @@ struct s2bWorld
 	DevArray<int4> sHead, sFilter;
 	DevArray<float4> sAabb, sFat;
 	DevArray<float2> sFr, sVerts, sNormals;
+	DevArray<float> sRestitution;
 
 	// joints
 	int jointCap = 0;
@@ -434,6 +438,7 @@ inline ShapeView shapeView(s2bWorld* w)
 	v.verts = w->sVerts.p;
 	v.normals = w->sNormals.p;
 	v.capacity = w->shapeCap;
+	v.restitution = w->sRestitution.p;
 	return v;
 }
 

@@ -116,6 +116,9 @@ void s2bFreeSolverScratch(s2bWorld* w)
 	s->src.release();
 	s->warmP.release();
 	s->warmAnchor.release();
+	s->restVr.release();
+	s->restR[0].release();
+	s->restR[1].release();
 	s->jhead.release();
 	s->janchor.release();
 	s->jmass.release();
@@ -2101,6 +2104,55 @@ __global__ void s2bMeterWork(const int* counts, int passes, unsigned long long* 
 	work[1] += 1ull;
 }
 
+// Restitution capture (DESIGN.md §3.7), before anything of the stage has run: per contact slot with points and e > 0, the
+// approach speed vr and the normal mass of each point at the stage-start velocities, at the anchors the variants' prepare
+// forms (rA = qA (localAnchorA - localCenterA)). The same definition for all ten variants, whatever their prepare sees.
+__global__ void s2bCaptureRestitution(ContactView c, BodyView b, int contactCount, float4* vrOut, float4* r0Out, float4* r1Out)
+{
+	int slot = blockIdx.x * blockDim.x + threadIdx.x;
+	if (slot >= contactCount)
+	{
+		return;
+	}
+	float4 mnf = c.nf[slot];
+	int pointCount = S2B_CI_COUNT(c.info[slot].x);
+	if (pointCount == 0 || mnf.w == 0.0f)
+	{
+		return; // the pass skips the contact without reading its row
+	}
+	int2 bodies = c.bodies[slot];
+	float4 velA = b.vel[bodies.x], velB = b.vel[bodies.y];
+	float4 poseA = b.pose[bodies.x], poseB = b.pose[bodies.y];
+	float4 orgA = b.org[bodies.x], orgB = b.org[bodies.y];
+	float mA = velA.w, mB = velB.w;
+	float iA = b.prm[bodies.x].w, iB = b.prm[bodies.y].w;
+	s2Rot qA = R2(poseA.z, poseA.w), qB = R2(poseB.z, poseB.w);
+	s2Vec2 vA = V2(velA.x, velA.y), vB = V2(velB.x, velB.y);
+	float wA = velA.z, wB = velB.z;
+	s2Vec2 normal = V2(mnf.x, mnf.y);
+	float vr[2] = {0.0f, 0.0f}, normalMass[2] = {0.0f, 0.0f};
+	float4 r[2] = {make_float4(0.0f, 0.0f, 0.0f, 0.0f), make_float4(0.0f, 0.0f, 0.0f, 0.0f)};
+#pragma unroll
+	for (int j = 0; j < 2; ++j)
+	{
+		if (j < pointCount)
+		{
+			float4 la = c.anchor[j][slot];
+			s2Vec2 rA = s2RotateVector(qA, s2Sub(V2(la.x, la.y), V2(orgA.z, orgA.w)));
+			s2Vec2 rB = s2RotateVector(qB, s2Sub(V2(la.z, la.w), V2(orgB.z, orgB.w)));
+			vr[j] = s2Dot(normal, s2Sub(s2Add(vB, s2CrossSV(wB, rB)), s2Add(vA, s2CrossSV(wA, rA))));
+			float rnA = s2Cross(rA, normal);
+			float rnB = s2Cross(rB, normal);
+			float k = mA + mB + iA * rnA * rnA + iB * rnB * rnB;
+			normalMass[j] = k > 0.0f ? 1.0f / k : 0.0f;
+			r[j] = make_float4(rA.x, rA.y, rB.x, rB.y);
+		}
+	}
+	vrOut[slot] = make_float4(vr[0], vr[1], normalMass[0], normalMass[1]);
+	r0Out[slot] = r[0];
+	r1Out[slot] = r[1];
+}
+
 // ---------------------------------------------------------------------------------------------------------------
 // host driver
 // ---------------------------------------------------------------------------------------------------------------
@@ -2604,6 +2656,7 @@ struct SolvePlan
 	int contactCount = 0, jointCap = 0, bodyCap = 0, maxItems = 0;
 	size_t nC = 1, nJ = 1, nI = 1;
 	VariantColumns cols;
+	bool restitution = false; // capture + restitution pass around the variant's program
 	int threads = S2B_BLOCK;
 	int grid = 1;	 // blocks of the persistent kernel
 	int regions = 0; // region-local schedule: == grid, or 0
@@ -2771,6 +2824,21 @@ static void planSolve(s2bWorld* w, SolverScratch* s, SolvePlan& pl)
 	{
 		s->warmP.reserve(nC, st, false);
 		s->warmAnchor.reserve(2 * nC, st, false);
+	}
+	// (s2Solve_XPBD's early return, with dt == 0 or no sub-steps, has skipped the stage before this; the other variants run
+	// their program with dt == 0, without the pass)
+	pl.restitution = w->restitution != 0 && ctx.dt != 0.0f;
+	if (pl.restitution)
+	{
+		s->restVr.reserve(nC, st, false);
+		s->restR[0].reserve(nC, st, false);
+		s->restR[1].reserve(nC, st, false);
+	}
+	else if (w->restitution == 0 && s->restVr.p != nullptr)
+	{
+		s->restVr.release();
+		s->restR[0].release();
+		s->restR[1].release();
 	}
 	for (int p = 0; p < 2; ++p)
 	{
@@ -3103,6 +3171,39 @@ static void enqueueSchedule(s2bWorld* w, SolverScratch* s, SolvePlan& pl)
 	}
 }
 
+// The restitution pass (DESIGN.md §3.7) after the variant's program: one Gauss-Seidel pass of COP_RESTITUTION over the same
+// group / region / overflow tables, so in the solve order s2b_download_solve_order reports. Persistent: its own instantiation
+// on the same grid (regions map one-to-one onto blocks), continuing the grid barrier's arrival count where the variant's kernel
+// left it. Launch by launch: the same kernels as every other group pass.
+static void enqueueRestitutionPass(s2bWorld* w, SolverScratch* s, const SolvePlan& pl, const SolveArgs& base, PassPtrs pp)
+{
+	SolveArgs a = base;
+	a.restVr = s->restVr.p;
+	a.restR[0] = s->restR[0].p;
+	a.restR[1] = s->restR[1].p;
+	a.restitutionThreshold = w->restitutionThreshold;
+	// the serial overflow group walks global memory (the kernel is launched without dynamic shared memory), and the pass is
+	// synchronised by grid barriers even where the variant's passes used tickets
+	a.ovBodies = nullptr;
+	a.ovBodySlot = nullptr;
+	a.bodyLocal = nullptr;
+	a.bodyTicket = nullptr;
+	a.trace = nullptr;
+	ProgramBuilder b;
+	b.segment(1);
+	b.add(groupPass(JOP_NONE, COP_RESTITUTION));
+	if (pl.usePersistent)
+	{
+		void* args[] = {&a, &pp, &b.prog};
+		S2B_CHECK(cudaLaunchCooperativeKernel(s2bRestitutionKernel(), dim3(pl.grid), dim3(pl.threads), args, 0, w->stream));
+		w->kernelLaunches += 1;
+	}
+	else
+	{
+		runProgramLaunchByLaunch(w, a, pp, b.prog, pl.host, pl.hostNJ, pl.hostNC);
+	}
+}
+
 // the argument block + the iteration itself (persistent kernel or launch by launch) + the work meter
 static void enqueueIterate(s2bWorld* w, SolverScratch* s, SolvePlan& pl, bool capturing)
 {
@@ -3203,6 +3304,11 @@ static void enqueueIterate(s2bWorld* w, SolverScratch* s, SolvePlan& pl, bool ca
 	s->lastJointSlots = pp.jointSlots;
 	s->lastJPerm = pp.jPerm;
 	s->lastArgsValid = true;
+	if (pl.restitution && pl.contactCount > 0)
+	{
+		S2B_LAUNCH(w, s2bCaptureRestitution, gridFor(pl.contactCount, S2B_BLOCK), S2B_BLOCK, 0, a.contacts, a.bodies, pl.contactCount, s->restVr.p,
+				   s->restR[0].p, s->restR[1].p);
+	}
 	if (pl.usePersistent)
 	{
 		// wavefront tables hold CNT_GROUPS levels and no overflow group; the overflow counts are zero so the kernel
@@ -3236,6 +3342,10 @@ static void enqueueIterate(s2bWorld* w, SolverScratch* s, SolvePlan& pl, bool ca
 	{
 		runProgramLaunchByLaunch(w, a, pp, pl.program, pl.host, pl.hostNJ, pl.hostNC);
 		w->solveKernelTimed = false;
+	}
+	if (pl.restitution && pl.contactCount > 0)
+	{
+		enqueueRestitutionPass(w, s, pl, a, pp);
 	}
 
 	// work meter: constraint-iterations of this step = (contact constraints + joints) x solve passes (SURVEY §8d)
@@ -3283,6 +3393,8 @@ void s2bSolve(s2bWorld* w, int solverType, const s2bStepContext* ctxIn)
 		put(&w->contactTableVersion, sizeof(w->contactTableVersion));
 		put(&w->scheduleEpoch, sizeof(w->scheduleEpoch));
 		put(&w->gravity, sizeof(w->gravity));
+		put(&w->restitution, sizeof(w->restitution));
+		put(&w->restitutionThreshold, sizeof(w->restitutionThreshold));
 		if (s->graphExec != nullptr && sig == s->graphSig)
 		{
 			if (s->scheduleSig != sig)
@@ -3303,7 +3415,7 @@ void s2bSolve(s2bWorld* w, int solverType, const s2bStepContext* ctxIn)
 	}
 	if (graphable && s->graphExec != nullptr && getenv("S2B_GRAPH_DEBUG") != nullptr)
 	{
-		// which part of the signature moved? layout: ctx | 10 ints | epoch | table version | schedule epoch | gravity
+		// which part of the signature moved? layout: ctx | 10 ints | epoch | table version | schedule epoch | gravity | restitution
 		size_t n = std::min(sig.size(), s->graphSig.size());
 		for (size_t k = 0; k < n; ++k)
 		{

@@ -66,9 +66,23 @@ struct SolveArgs
 	const int* ovBodies;	 // [0] count, then body slots (null: walk in global memory)
 	const int* ovBodySlot;	 // per body: position in that list, or -1
 	// ticketed ("dataflow") Gauss-Seidel passes: null when the passes synchronise with grid barriers instead
-	int* bodyTicket;			   // per body: incident-item executions completed in this launch
-	const int2 *cFlowA, *cFlowB;   // per contact constraint and side: {ordinal in the body's incidence list, its degree} or -1
-	const int2 *jFlowA, *jFlowB;   // same per joint constraint
+	int* bodyTicket; // per body: incident-item executions completed in this launch
+	union
+	{
+		struct
+		{
+			const int2 *cFlowA, *cFlowB; // per contact constraint and side: {ordinal in the body's incidence list, its degree} or -1
+			const int2 *jFlowA, *jFlowB; // same per joint constraint
+		};
+		// The restitution pass (DESIGN.md §3.7) runs without tickets, so its inputs share these slots: SolveArgs, and with it
+		// the parameter layout and stack frame of every variant's kernel, stays the size it is without restitution.
+		struct
+		{
+			const float4* restVr;	// per contact slot, captured at the start of the stage: vr0 vr1 normalMass0 normalMass1
+			const float4* restR[2]; // per contact slot: rA.xy rB.xy of point 0 / 1
+			float restitutionThreshold;
+		};
+	};
 	unsigned long long* trace; // diagnostic: block 0 stamps %globaltimer after every grid barrier (null = off)
 	int traceCap;
 	int flowSleepNs;			   // back-off between polls (0 = none)
@@ -142,6 +156,8 @@ struct SolverScratch
 	DevArray<float> sep[2];
 	DevArray<int> src;
 	DevArray<float4> warmP, warmAnchor; // ConstraintView::warmP (1 per constraint), ::warmAnchor (2 per constraint)
+	// restitution capture, per contact slot (SolveArgs::restVr / restR); allocated while restitution is enabled
+	DevArray<float4> restVr, restR[2];
 
 	// joint constraint columns
 	DevArray<int4> jhead;

@@ -59,6 +59,7 @@ __global__ void s2bScatterShapes(const s2bShapeRow* __restrict__ rows, int count
 	s.aabb[i] = make_float4(r->aabb[0], r->aabb[1], r->aabb[2], r->aabb[3]);
 	s.fat[i] = make_float4(r->fatAABB[0], r->fatAABB[1], r->fatAABB[2], r->fatAABB[3]);
 	s.fr[i] = make_float2(r->friction, r->radius);
+	s.restitution[i] = r->restitution;
 	for (int k = 0; k < 8; ++k)
 	{
 		s.verts[i * 8 + k] = make_float2(r->vertices[2 * k], r->vertices[2 * k + 1]);
@@ -124,7 +125,7 @@ __global__ void s2bScatterContacts(const s2bContactRow* __restrict__ rows, int c
 				(r->points[0].persisted ? S2B_CI_PERSISTED0 : 0) | (r->points[1].persisted ? S2B_CI_PERSISTED1 : 0);
 	int ids = (r->points[0].id & 0xFFFF) | ((r->points[1].id & 0xFFFF) << 16);
 	c.info[t] = make_int4(flags, ids, s2bPackCache(r), __float_as_int(r->cacheMetric));
-	c.nf[t] = make_float4(r->normal[0], r->normal[1], r->friction, 0.0f);
+	c.nf[t] = make_float4(r->normal[0], r->normal[1], r->friction, r->restitution);
 	c.color[t] = -1;
 	for (int p = 0; p < 2; ++p)
 	{
@@ -235,6 +236,7 @@ __global__ void s2bGatherContacts(s2bContactRow* rows, int count, ContactView c,
 	r.pointCount = S2B_CI_COUNT(info.x);
 	r.frictionPersisted = (info.x & S2B_CI_FRICTION_PERSISTED) ? 1 : 0;
 	r.friction = nf.z;
+	r.restitution = nf.w;
 	r.normal[0] = nf.x;
 	r.normal[1] = nf.y;
 	for (int p = 0; p < 2; ++p)
@@ -444,6 +446,7 @@ extern "C" void s2b_world_destroy(s2bWorld* w)
 	w->sAabb.release();
 	w->sFat.release();
 	w->sFr.release();
+	w->sRestitution.release();
 	w->sVerts.release();
 	w->sNormals.release();
 	w->jHead.release();
@@ -560,6 +563,16 @@ extern "C" void s2b_set_regions(s2bWorld* w, int enable)
 	w->scheduleEpoch += 1;
 }
 
+extern "C" void s2b_set_restitution(s2bWorld* w, int enable, float threshold)
+{
+	// a threshold that is not a finite, non-negative speed is ignored (the previous one stays)
+	if (isfinite(threshold) && threshold >= 0.0f)
+	{
+		w->restitutionThreshold = threshold;
+	}
+	w->restitution = enable != 0 ? 1 : 0;
+}
+
 static void reserveBodies(s2bWorld* w, int cap)
 {
 	if (cap <= w->bodyCap)
@@ -591,6 +604,7 @@ static void reserveShapes(s2bWorld* w, int cap)
 	w->sAabb.reserve(cap, s);
 	w->sFat.reserve(cap, s);
 	w->sFr.reserve(cap, s);
+	w->sRestitution.reserve(cap, s);
 	w->shapeCap = (int)w->sHead.cap;
 	w->sVerts.reserve((size_t)w->shapeCap * 8, s);
 	w->sNormals.reserve((size_t)w->shapeCap * 8, s);

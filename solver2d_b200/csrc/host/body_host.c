@@ -226,6 +226,7 @@ static s2ShapeId s2CreateShape(s2BodyId bodyId, const s2ShapeDef* def, const voi
 	shape->type = shapeType;
 	shape->density = def->density;
 	shape->friction = def->friction;
+	S2_ASSERT(s2IsValid(def->restitution) && def->restitution >= 0.0f);
 	shape->restitution = def->restitution;
 	shape->userData = def->userData;
 	shape->filter = def->filter;

@@ -203,6 +203,10 @@ typedef struct s2World
 	s2bWorld* device;
 	s2IndexList dirtyBodies, dirtyForces, dirtyShapes, dirtyJoints;
 	bool jointPairsDirty;
+	// restitution (include/solver2d_b200.h): pushed to the device by the next flush when restitutionDirty
+	bool enableRestitution;
+	float restitutionThreshold;
+	bool restitutionDirty;
 	bool stateFresh;	 // host body / joint state mirrors the device
 	bool boxesFresh;	 // host shape AABBs mirror the device
 	uint64_t stepId;

@@ -189,6 +189,7 @@ static void s2FillShapeRow(s2bShapeRow* r, const s2Shape* s)
 	r->maskBits = s->filter.maskBits;
 	r->groupIndex = s->filter.groupIndex;
 	r->friction = s->friction;
+	r->restitution = s->restitution;
 	r->aabb[0] = s->aabb.lowerBound.x;
 	r->aabb[1] = s->aabb.lowerBound.y;
 	r->aabb[2] = s->aabb.upperBound.x;
@@ -357,6 +358,12 @@ void s2FlushToDevice(s2World* world)
 		world->dirtyJoints.count = 0;
 	}
 
+	if (world->restitutionDirty)
+	{
+		s2b_set_restitution(dev, world->enableRestitution ? 1 : 0, world->restitutionThreshold);
+		world->restitutionDirty = false;
+	}
+
 	if (world->jointPairsDirty)
 	{
 		// Two key lists (body pair = lo << 32 | hi):
@@ -498,6 +505,7 @@ s2WorldId s2CreateWorld(const s2WorldDef* def)
 	world->jointPool = s2CreatePool(sizeof(s2Joint), 4);
 	world->joints = (s2Joint*)world->jointPool.memory;
 	world->gravity = s2MakeVec2(0.0f, -10.0f);
+	world->restitutionThreshold = 1.0f; // reference src/world.c:98
 	world->stepId = 0;
 	world->revision = (uint16_t)(revision + 1);
 	world->stateFresh = true;
@@ -746,6 +754,25 @@ void s2World_QueryAABB(s2WorldId worldId, s2Box aabb, s2QueryCallbackFcn* fcn, v
 s2bWorld* s2World_GetDevice(s2WorldId worldId)
 {
 	return s2GetWorldFromId(worldId)->device;
+}
+
+void s2World_EnableRestitution(s2WorldId worldId, bool enable)
+{
+	s2World* world = s2GetWorldFromId(worldId);
+	world->enableRestitution = enable;
+	world->restitutionDirty = true;
+}
+
+void s2World_SetRestitutionThreshold(s2WorldId worldId, float threshold)
+{
+	s2World* world = s2GetWorldFromId(worldId);
+	S2_ASSERT(s2IsValid(threshold) && threshold >= 0.0f);
+	if (s2IsValid(threshold) == false || threshold < 0.0f)
+	{
+		return; // rejected: the world keeps its threshold
+	}
+	world->restitutionThreshold = threshold;
+	world->restitutionDirty = true;
 }
 
 void s2World_Flush(s2WorldId worldId)

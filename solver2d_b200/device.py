@@ -24,7 +24,7 @@ BODY_ROW = np.dtype([
 SHAPE_ROW = np.dtype([
     ("index", "<i4"), ("flags", "<i4"), ("body", "<i4"), ("proxyKey", "<i4"), ("categoryBits", "<u4"),
     ("maskBits", "<u4"), ("groupIndex", "<i4"), ("friction", "<f4"), ("aabb", "<f4", 4), ("fatAABB", "<f4", 4),
-    ("radius", "<f4"), ("count", "<i4"), ("vertices", "<f4", 16), ("normals", "<f4", 16),
+    ("radius", "<f4"), ("count", "<i4"), ("vertices", "<f4", 16), ("normals", "<f4", 16), ("restitution", "<f4"),
 ], align=True)
 
 JOINT_ROW = np.dtype([
@@ -44,6 +44,7 @@ CONTACT_ROW = np.dtype([
     ("shapeA", "<i4"), ("shapeB", "<i4"), ("bodyA", "<i4"), ("bodyB", "<i4"), ("pointCount", "<i4"),
     ("frictionPersisted", "<i4"), ("friction", "<f4"), ("normal", "<f4", 2), ("points", CONTACT_POINT, 2),
     ("cacheCount", "<i4"), ("cacheIndexA", "u1", 4), ("cacheIndexB", "u1", 4), ("cacheMetric", "<f4"),
+    ("restitution", "<f4"),
 ], align=True)
 
 
@@ -76,6 +77,7 @@ ABI_SYMBOLS = [
     "s2b_download_solve_order", "s2b_download_islands", "s2b_prefetch_pairs", "s2b_get_counters", "s2b_pack_body_state", "s2b_timed_steps", "s2b_last_stage_ms",
     "s2b_flush_l2", "s2b_time_color_kernel", "s2b_version", "s2b_abi_sizes", "s2b_upload_forces", "s2b_host_alloc",
     "s2b_host_free", "s2b_sync_body_state", "s2b_set_warm_gather", "s2b_eval_atan2", "s2b_set_dataflow", "s2b_set_regions", "s2b_set_graph", "s2b_get_stream", "s2b_add_forces", "s2b_download_transforms",
+    "s2b_set_restitution",
 ]
 
 
@@ -113,6 +115,7 @@ class Device:
         L.s2b_world_create.argtypes = [C.c_int, C.c_int]
         L.s2b_world_destroy.argtypes = [vp]
         L.s2b_set_gravity.argtypes = [vp, C.c_float, C.c_float]
+        L.s2b_set_restitution.argtypes = [vp, C.c_int, C.c_float]
         for name in ("s2b_set_schedule", "s2b_set_max_colors", "s2b_set_persistent", "s2b_set_warm_gather", "s2b_set_dataflow", "s2b_set_regions", "s2b_set_graph"):
             getattr(L, name).argtypes = [vp, C.c_int]
         for name in ("s2b_upload_bodies", "s2b_upload_shapes", "s2b_upload_joints"):
@@ -223,6 +226,11 @@ class DeviceWorld:
         """Region-local schedule of the persistent kernel: 0 / False never, 1 when the cut set needs few colours (default),
         2 / True always. See DESIGN.md §3.1."""
         self.L.s2b_set_regions(self.h, 2 if mode is True else (0 if mode is False else int(mode)))
+
+    def set_restitution(self, enable: bool, threshold: float = 1.0):
+        """Restitution pass at the end of the solver stage (off by default; DESIGN.md §3.7). `threshold`: approach speed
+        (m/s) below which a contact does not bounce; a negative or non-finite value is ignored."""
+        self.L.s2b_set_restitution(self.h, 1 if enable else 0, threshold)
 
     def set_warm_gather(self, enable: bool):
         self.L.s2b_set_warm_gather(self.h, 1 if enable else 0)

@@ -11,6 +11,7 @@ Each recipe restates one of the reference's sample scenes or one of the syntheti
 * :func:`mixed_shapes`    — circles/capsules/polygons/segments on a ground, exercising all nine manifold functions.
 * :func:`collision_zoo`   — every manifold kind, flipped pairs, dynamic segments, compound bodies, mixed frictions and
                             shape filters, thrown sideways.
+* :func:`bouncers`        — shapes with restitution dropped from several heights (the restitution extension).
 
 All scenes are deterministic lattices (no RNG). A recipe returns a :class:`Scene` holding the world id and the
 body ids in creation order.
@@ -42,31 +43,34 @@ class Scene:
         self.lib.s2DestroyWorld(self.world)
 
 
-def _ground(lib, world, half_width, half_height=1.0, y=-1.0):
+def _ground(lib, world, half_width, half_height=1.0, y=-1.0, restitution=0.0):
     bd = default_body_def()
     bd.position = Vec2(0.0, y)
     gid = lib.s2CreateBody(world, C.byref(bd))
     box = lib.s2MakeBox(half_width, half_height)
     sd = default_shape_def()
+    sd.restitution = restitution
     lib.s2CreatePolygonShape(gid, C.byref(sd), C.byref(box))
     return gid
 
 
-def pyramid(lib: capi.Solver2D, solver="TGS_Soft", base_count=10) -> Scene:
+def pyramid(lib: capi.Solver2D, solver="TGS_Soft", base_count=10, restitution=0.0) -> Scene:
     """Pyramid recipe, reference samples/collection/sample_contact.cpp:511-552.
 
     The reference ground is ``s2MakeBox(100, 1)``; for base_count > 200 the ground half-width is widened to
-    ``0.5*N + 50`` so the base row still rests on it (SURVEY §8d config 2).
+    ``0.5*N + 50`` so the base row still rests on it (SURVEY §8d config 2). ``restitution`` is given to every shape (the
+    sample's 0 by default).
     """
     world = lib.create_world(solver)
     sc = Scene(lib, world, name=f"pyramid{base_count}")
     half_width = 100.0 if base_count <= 200 else 0.5 * base_count + 50.0
-    sc.bodies.append(_ground(lib, world, half_width))
+    sc.bodies.append(_ground(lib, world, half_width, restitution=restitution))
 
     bd = default_body_def()
     bd.type = capi.DYNAMIC_BODY
     sd = default_shape_def()
     sd.density = 1.0
+    sd.restitution = restitution
     h = 0.5
     box = lib.s2MakeSquare(h)
     shift = 1.0 * h
@@ -427,6 +431,98 @@ RECIPES = {
     "mixed_shapes": mixed_shapes,
     "collision_zoo": collision_zoo,
 }
+
+
+BOUNCER_RESTITUTION = (0.0, 0.25, 0.6, 1.0)
+# drop heights above the ground (m): impact speeds sqrt(2 g h) of about 0.45, 1.4, 3.2 and 6.3 m/s, on both sides of the
+# default 1 m/s restitution threshold
+BOUNCER_DROPS = (0.01, 0.1, 0.5, 2.0)
+
+
+def bouncers(lib: capi.Solver2D, solver="TGS_Soft", columns=16, rows=4, joints=True, platform=True) -> Scene:
+    """Restitution coverage. A ground of boxes (restitution 0 and 0.5 alternating) and segments, bordered by two walls; above
+    it `rows` x `columns` circles, boxes, capsules and rounded polygons with restitution 0, 0.25, 0.6 and 1, each column
+    dropped from one of BOUNCER_DROPS. With `joints`: the three revolute-jointed boxes of restitution 1 of the reference's
+    "Ragdoll Stress" sample (samples/collection/sample_joints.cpp:261 sets shapeDef.restitution = 1). With `platform`: a
+    kinematic platform moving up and down under the last columns. Shape count ~ columns x rows + columns / 2 + 8."""
+    world = lib.create_world(solver)
+    sc = Scene(lib, world, name=f"bouncers{rows}x{columns}")
+    pitch = 1.6
+    half = 0.5 * pitch * columns + 4.0
+    bd = default_body_def()
+    bd.position = Vec2(0.0, -1.0)
+    gid = lib.s2CreateBody(world, C.byref(bd))
+    sc.bodies.append(gid)
+    sd = default_shape_def()
+    tiles = max(2, columns // 2)
+    tile = 2.0 * half / tiles
+    for t in range(tiles):
+        sd.restitution = 0.5 if t % 2 == 1 else 0.0
+        box = lib.s2MakeOffsetBox(0.5 * tile, 1.0, Vec2(-half + (t + 0.5) * tile, 0.0), 0.0)
+        lib.s2CreatePolygonShape(gid, C.byref(sd), C.byref(box))
+    sd.restitution = 0.0
+    for x in (-half, half):
+        lib.s2CreateSegmentShape(gid, C.byref(sd), C.byref(Segment(Vec2(x, 1.0), Vec2(x, 30.0))))
+    # a segment strip lying on the ground under the first columns (segment-vs-shape manifolds)
+    sd.restitution = 0.5
+    lib.s2CreateSegmentShape(gid, C.byref(sd), C.byref(Segment(Vec2(-half + 1.0, 1.0), Vec2(-half + 6.0, 1.0))))
+
+    bd = default_body_def()
+    bd.type = capi.DYNAMIC_BODY
+    for j in range(columns):
+        drop = BOUNCER_DROPS[j % len(BOUNCER_DROPS)]
+        for i in range(rows):
+            k = i * columns + j
+            # each row falls as a layer: lower rows land first, the layers do not start in contact
+            bd.position = Vec2(-0.5 * pitch * (columns - 1) + pitch * j, 1.0 + 0.6 + drop + 1.6 * i)
+            bd.angle = 0.0
+            bid = lib.s2CreateBody(world, C.byref(bd))
+            sd.restitution = BOUNCER_RESTITUTION[(j + i) % len(BOUNCER_RESTITUTION)]
+            kind = (i + j // 4) % 4
+            if kind == 0:
+                lib.s2CreateCircleShape(bid, C.byref(sd), C.byref(Circle(Vec2(0.0, 0.0), 0.5)))
+            elif kind == 1:
+                box = lib.s2MakeBox(0.5, 0.4)
+                lib.s2CreatePolygonShape(bid, C.byref(sd), C.byref(box))
+            elif kind == 2:
+                lib.s2CreateCapsuleShape(bid, C.byref(sd), C.byref(Capsule(Vec2(-0.3, 0.0), Vec2(0.3, 0.0), 0.3)))
+            else:
+                rounded = lib.s2MakeBox(0.4, 0.3)  # a box with the radius set: rounded polygon
+                rounded.radius = 0.1
+                lib.s2CreatePolygonShape(bid, C.byref(sd), C.byref(rounded))
+            sc.bodies.append(bid)
+    if joints:
+        # Ragdoll Stress: boxes joined by revolute joints, every shape with restitution 1
+        sd.restitution = 1.0
+        prev = None
+        box = lib.s2MakeBox(0.5, 0.25)
+        x0, y0 = -3.0, 1.0 + 0.6 + 1.6 * rows + 3.0
+        for n in range(3):
+            bd.position = Vec2(x0 + 1.0 * n, y0)
+            bid = lib.s2CreateBody(world, C.byref(bd))
+            lib.s2CreatePolygonShape(bid, C.byref(sd), C.byref(box))
+            sc.bodies.append(bid)
+            if prev is not None:
+                jd = default_revolute_def()
+                pivot = Vec2(x0 + 1.0 * n - 0.5, y0)
+                jd.bodyIdA = prev
+                jd.bodyIdB = bid
+                jd.localAnchorA = lib.s2Body_GetLocalPoint(prev, pivot)
+                jd.localAnchorB = lib.s2Body_GetLocalPoint(bid, pivot)
+                sc.joints.append(lib.s2CreateRevoluteJoint(world, C.byref(jd)))
+            prev = bid
+    if platform:
+        kd = default_body_def()
+        kd.type = capi.KINEMATIC_BODY
+        kd.position = Vec2(0.5 * pitch * (columns - 1) - 1.0, 1.0 + 0.6 + 1.6 * rows + 6.0)
+        kd.linearVelocity = Vec2(0.0, -1.5)
+        pid = lib.s2CreateBody(world, C.byref(kd))
+        sd.restitution = 0.6
+        box = lib.s2MakeBox(1.5, 0.2)
+        lib.s2CreatePolygonShape(pid, C.byref(sd), C.byref(box))
+        sc.bodies.append(pid)
+        sc.piles["platform"] = pid
+    return sc
 
 
 def pyramid_rows(base_count: int):
