@@ -91,6 +91,7 @@ enum
 {
 	S2B_JOINT_REVOLUTE = 0,
 	S2B_JOINT_MOUSE = 1,
+	S2B_JOINT_WELD = 2, // never carries S2B_JOINT_ENABLE_LIMIT or S2B_JOINT_ENABLE_MOTOR
 };
 
 #define S2B_JOINT_ENABLE_LIMIT 0x10
@@ -110,7 +111,7 @@ typedef struct s2bJointRow
 	// mouse
 	float hertz, dampingRatio;
 	float target[2];
-	// accumulated impulses (simulation state)
+	// accumulated impulses (simulation state); a weld keeps its angular impulse in motorImpulse
 	float impulse[2];
 	float motorImpulse, lowerImpulse, upperImpulse;
 } s2bJointRow;

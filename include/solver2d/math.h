@@ -10,6 +10,7 @@
 #pragma once
 
 #include "solver2d/atan2_f32.h"
+#include "solver2d/constants.h"
 #include "solver2d/types.h"
 
 #include <math.h>
@@ -279,6 +280,21 @@ S2_INLINE float s2RelativeAngle(s2Rot b, s2Rot a)
 	float s = b.s * a.c - b.c * a.s;
 	float c = b.c * a.c + b.s * a.s;
 	return S2_ATAN2F(s, c);
+}
+
+// Brings an angle difference into [-pi, pi] with one add or subtract of 2 pi: enough for the difference of two angles
+// in [-pi, pi], such as the weld joint's relative angle minus its reference angle.
+S2_INLINE float s2UnwindAngle(float angle)
+{
+	if (angle < -s2_pi)
+	{
+		return angle + 2.0f * s2_pi;
+	}
+	if (angle > s2_pi)
+	{
+		return angle - 2.0f * s2_pi;
+	}
+	return angle;
 }
 
 S2_INLINE s2Vec2 s2RotateVector(s2Rot q, s2Vec2 v)

@@ -23,6 +23,31 @@ S2B_API void s2World_EnableRestitution(s2WorldId worldId, bool enable);
 // s2World_Step.
 S2B_API void s2World_SetRestitutionThreshold(s2WorldId worldId, float threshold);
 
+// Weld joint: holds body B rigidly to body A, the anchor points together and angle(B) - angle(A) at referenceAngle.
+// It is as rigid as the solver variant makes a revolute joint's point constraint (DESIGN.md §3.8). Anchors are relative
+// to each body's origin. Destroy it with s2DestroyJoint.
+typedef struct s2WeldJointDef
+{
+	s2BodyId bodyIdA;
+	s2BodyId bodyIdB;
+	s2Vec2 localAnchorA;
+	s2Vec2 localAnchorB;
+	float referenceAngle; // angle(B) - angle(A) at rest
+	float drawSize;
+	bool collideConnected; // keep the contacts the two bodies already have
+} s2WeldJointDef;
+
+S2_INLINE struct s2WeldJointDef s2DefaultWeldJointDef(void)
+{
+	s2WeldJointDef def = S2_ZERO_INIT;
+	def.bodyIdA = s2_nullBodyId;
+	def.bodyIdB = s2_nullBodyId;
+	def.drawSize = 1.0f;
+	return def;
+}
+
+S2B_API s2JointId s2CreateWeldJoint(s2WorldId worldId, const s2WeldJointDef* def);
+
 // Push every pending host-side edit to the device now (s2World_Step does this itself).
 S2B_API void s2World_Flush(s2WorldId worldId);
 

@@ -139,6 +139,19 @@ class RevoluteJointDef(C.Structure):
     ]
 
 
+class WeldJointDef(C.Structure):
+    """s2WeldJointDef (include/solver2d_b200.h): an extension, absent from the reference."""
+    _fields_ = [
+        ("bodyIdA", BodyId),
+        ("bodyIdB", BodyId),
+        ("localAnchorA", Vec2),
+        ("localAnchorB", Vec2),
+        ("referenceAngle", C.c_float),
+        ("drawSize", C.c_float),
+        ("collideConnected", C.c_bool),
+    ]
+
+
 class Statistics(C.Structure):
     _fields_ = [
         ("bodyCount", C.c_int32),
@@ -199,6 +212,15 @@ def default_revolute_def() -> RevoluteJointDef:
     return d
 
 
+def default_weld_def() -> WeldJointDef:
+    """s2DefaultWeldJointDef (include/solver2d_b200.h)."""
+    d = WeldJointDef()
+    d.bodyIdA = BodyId(-1, -1, 0)
+    d.bodyIdB = BodyId(-1, -1, 0)
+    d.drawSize = 1.0
+    return d
+
+
 def default_mouse_def() -> MouseJointDef:
     """s2DefaultMouseJointDef (reference include/solver2d/joint_types.h:28-37)."""
     d = MouseJointDef()
@@ -249,6 +271,7 @@ _API = {
     # extensions (include/solver2d_b200.h): restitution is off unless a world enables it
     "s2World_EnableRestitution": (None, [WorldId, C.c_bool]),
     "s2World_SetRestitutionThreshold": (None, [WorldId, C.c_float]),
+    "s2CreateWeldJoint": (JointId, [WorldId, C.POINTER(WeldJointDef)]),
 }
 
 class Transform(C.Structure):

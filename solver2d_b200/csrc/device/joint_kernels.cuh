@@ -141,12 +141,14 @@ template <int KIND> __device__ __forceinline__ void s2bPrepareJoint(const SolveA
 
 	bool enableLimit = (flags & S2B_JOINT_ENABLE_LIMIT) != 0;
 	bool enableMotor = (flags & S2B_JOINT_ENABLE_MOTOR) != 0;
+	bool weld = S2B_JOINT_TYPE(flags) == S2B_JOINT_WELD;
 	if (enableLimit == false || fixedRotation || warmStart == false)
 	{
 		limp.x = 0.0f;
 		limp.y = 0.0f;
 	}
-	if (enableMotor == false || fixedRotation || warmStart == false)
+	// a weld's angular impulse (imp.z) is kept or dropped together with its point impulse
+	if (weld ? warmStart == false : (enableMotor == false || fixedRotation || warmStart == false))
 	{
 		imp.z = 0.0f;
 	}
@@ -312,21 +314,63 @@ template <int KIND> __device__ __forceinline__ void s2bSolveRevoluteVelocity(con
 	bool enableLimit = (head.x & S2B_JOINT_ENABLE_LIMIT) != 0;
 	bool enableMotor = (head.x & S2B_JOINT_ENABLE_MOTOR) != 0;
 
-	if (enableMotor && fixedRotation == false)
+	// A weld has no motor: its one bilateral angular row (DESIGN.md §3.8) takes the motor row's place and column (imp.z).
+	// The rotations do not change in a velocity pass. The soft flavour evaluates the angle once for the weld and the
+	// limits; the Baumgarte flavour evaluates it where each row needs it. Both give the same bits; each choice is the
+	// one that keeps its kernels' stack frame and spills at what they are without the weld (DESIGN.md §3.8).
+	bool weld = S2B_JOINT_TYPE(head.x) == S2B_JOINT_WELD;
+	float jointAngle = 0.0f;
+	if (KIND == JSOLVE_SOFT && (enableLimit || weld) && fixedRotation == false)
 	{
-		float Cdot = wB - wA - motor.y;
-		float impulse = -axialMass * Cdot;
-		float oldImpulse = imp.z;
-		float maxImpulse = h * motor.x;
-		imp.z = S2_CLAMP(imp.z + impulse, -maxImpulse, maxImpulse);
-		impulse = imp.z - oldImpulse;
+		jointAngle = s2RelativeAngle(qB, qA) - lim.x;
+	}
+	if ((enableMotor || weld) && fixedRotation == false)
+	{
+		float impulse;
+		if (weld)
+		{
+			float C = s2UnwindAngle(KIND == JSOLVE_SOFT ? jointAngle : s2RelativeAngle(qB, qA) - lim.x);
+			float bias = 0.0f;
+			float massScale = 1.0f;
+			float impulseScale = 0.0f;
+			if (KIND == JSOLVE_SOFT)
+			{
+				if (useBias)
+				{
+					bias = coef.x * C;
+					massScale = coef.y;
+					impulseScale = coef.z;
+				}
+			}
+			else
+			{
+				// as this flavour's point row, the Baumgarte bias is applied in every pass
+				bias = s2_baumgarte * inv_h * C;
+			}
+			float Cdot = wB - wA;
+			impulse = KIND == JSOLVE_SOFT ? -axialMass * massScale * (Cdot + bias) - impulseScale * imp.z
+										  : -axialMass * (Cdot + bias);
+			imp.z += impulse;
+		}
+		else
+		{
+			float Cdot = wB - wA - motor.y;
+			impulse = -axialMass * Cdot;
+			float oldImpulse = imp.z;
+			float maxImpulse = h * motor.x;
+			imp.z = S2_CLAMP(imp.z + impulse, -maxImpulse, maxImpulse);
+			impulse = imp.z - oldImpulse;
+		}
 		wA -= iA * impulse;
 		wB += iB * impulse;
 	}
 
 	if (enableLimit && fixedRotation == false)
 	{
-		float jointAngle = s2RelativeAngle(qB, qA) - lim.x;
+		if (KIND != JSOLVE_SOFT)
+		{
+			jointAngle = s2RelativeAngle(qB, qA) - lim.x;
+		}
 
 		// lower limit
 		{
@@ -521,6 +565,14 @@ __device__ __forceinline__ void s2bSolveRevoluteRigid(const SolveArgs& a, int t,
 		wA -= iA * impulse;
 		wB += iB * impulse;
 	}
+	else if (S2B_JOINT_TYPE(head.x) == S2B_JOINT_WELD && fixedRotation == false)
+	{
+		// weld angular row, rigid (DESIGN.md §3.8): the position error is left to the NGS position pass
+		float impulse = -axialMass * (wB - wA);
+		imp.z += impulse;
+		wA -= iA * impulse;
+		wB += iB * impulse;
+	}
 
 	if ((head.x & S2B_JOINT_ENABLE_LIMIT) && fixedRotation == false)
 	{
@@ -623,6 +675,14 @@ __device__ __forceinline__ void s2bSolveJointPosition(const SolveArgs& a, int t)
 		qA = s2IntegrateRot(qA, -iA * limitImpulse);
 		qB = s2IntegrateRot(qB, iB * limitImpulse);
 	}
+	else if (S2B_JOINT_TYPE(head.x) == S2B_JOINT_WELD && fixedRotation == false)
+	{
+		// weld angular row (DESIGN.md §3.8); the point row below then runs on the corrected rotations
+		float C = s2UnwindAngle(s2RelativeAngle(qB, qA) - lim.x);
+		float p = -axialMass * S2_CLAMP(C, -s2_maxAngularCorrection, s2_maxAngularCorrection);
+		qA = s2IntegrateRot(qA, -iA * p);
+		qB = s2IntegrateRot(qB, iB * p);
+	}
 
 	{
 		s2Vec2 rA = s2RotateVector(qA, V2(anchor.x, anchor.y));
@@ -671,6 +731,15 @@ __device__ __forceinline__ void s2bSolveJointXpbd(const SolveArgs& a, int t)
 	float4 poseA = a.bodies.pose[ia], poseB = a.bodies.pose[ib];
 	s2Vec2 dcA = V2(poseA.x, poseA.y), dcB = V2(poseB.x, poseB.y);
 	s2Rot qA = R2(poseA.z, poseA.w), qB = R2(poseB.z, poseB.w);
+	float mA = mass.x, iA = mass.y, mB = mass.z, iB = mass.w;
+	if (S2B_JOINT_TYPE(head.x) == S2B_JOINT_WELD && iA + iB != 0.0f)
+	{
+		// weld angular row, zero compliance (DESIGN.md §3.8); the point row below then runs on the corrected rotations
+		float C = s2UnwindAngle(s2RelativeAngle(qB, qA) - jc.lim[t].x);
+		float p = -C / (iA + iB);
+		qA = s2IntegrateRot(qA, -iA * p);
+		qB = s2IntegrateRot(qB, iB * p);
+	}
 	s2Vec2 rA = s2RotateVector(qA, V2(anchor.x, anchor.y));
 	s2Vec2 rB = s2RotateVector(qB, V2(anchor.z, anchor.w));
 	s2Vec2 separation = s2Add(s2Add(s2Sub(dcB, dcA), s2Sub(rB, rA)), V2(d0.x, d0.y));
@@ -682,7 +751,6 @@ __device__ __forceinline__ void s2bSolveJointXpbd(const SolveArgs& a, int t)
 		float invLength = 1.0f / c;
 		n = V2(invLength * separation.x, invLength * separation.y);
 	}
-	float mA = mass.x, iA = mass.y, mB = mass.z, iB = mass.w;
 	if (mA == 0.0f && mB == 0.0f)
 	{
 		return;

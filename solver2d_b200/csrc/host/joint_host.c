@@ -1,6 +1,7 @@
 // solver2d-b200 — joints behind the public API (behaviour of reference src/joint.c:154-292, src/revolute_joint.c:825-888,
 // src/mouse_joint.c:18-29). Host bookkeeping only: the joint solvers run on the device.
 #include "s2_host.h"
+#include "solver2d_b200.h"
 
 #include <string.h>
 
@@ -68,6 +69,26 @@ s2JointId s2CreateRevoluteJoint(s2WorldId worldId, const s2RevoluteJointDef* def
 	joint->enableMotor = def->enableMotor;
 	// collideConnected == false removes the contacts that already exist between the two bodies (the pair pass does it on
 	// the device); new contacts between jointed bodies are never created either way
+	joint->collideConnected = def->collideConnected;
+
+	s2JointId jointId = {joint->object.index, world->index, joint->object.revision};
+	return jointId;
+}
+
+// The weld has no counterpart in the reference. Its row carries no limit or motor flags; like a revolute joint created
+// with collideConnected == false it removes the contacts that already exist between its bodies.
+s2JointId s2CreateWeldJoint(s2WorldId worldId, const s2WeldJointDef* def)
+{
+	s2World* world = s2GetWorldFromId(worldId);
+	s2Body* bodyA = world->bodies + def->bodyIdA.index;
+	s2Body* bodyB = world->bodies + def->bodyIdB.index;
+
+	s2Joint* joint = s2AllocJoint(world, bodyA, bodyB);
+	joint->type = s2_weldJoint;
+	joint->drawSize = def->drawSize;
+	joint->localOriginAnchorA = def->localAnchorA;
+	joint->localOriginAnchorB = def->localAnchorB;
+	joint->referenceAngle = def->referenceAngle;
 	joint->collideConnected = def->collideConnected;
 
 	s2JointId jointId = {joint->object.index, world->index, joint->object.revision};

@@ -85,6 +85,7 @@ typedef enum s2JointType
 {
 	s2_revoluteJoint,
 	s2_mouseJoint,
+	s2_weldJoint,
 } s2JointType;
 
 typedef struct s2Body

@@ -238,7 +238,21 @@ static void s2FillJointRow(s2bJointRow* r, const s2Joint* j)
 	{
 		return;
 	}
-	r->flags = S2B_ROW_VALID | ((j->type == s2_mouseJoint ? S2B_JOINT_MOUSE : S2B_JOINT_REVOLUTE) << 1);
+	int type = S2B_JOINT_REVOLUTE;
+	switch (j->type)
+	{
+		case s2_revoluteJoint:
+			type = S2B_JOINT_REVOLUTE;
+			break;
+		case s2_mouseJoint:
+			type = S2B_JOINT_MOUSE;
+			break;
+		case s2_weldJoint:
+			type = S2B_JOINT_WELD;
+			break;
+	}
+	r->flags = S2B_ROW_VALID | (type << 1);
+	// a weld is created with enableLimit == enableMotor == false, so its row never carries either flag
 	r->flags |= j->enableLimit ? S2B_JOINT_ENABLE_LIMIT : 0;
 	r->flags |= j->enableMotor ? S2B_JOINT_ENABLE_MOTOR : 0;
 	r->flags |= j->collideConnected ? S2B_JOINT_COLLIDE_CONNECTED : 0;
@@ -369,8 +383,8 @@ void s2FlushToDevice(s2World* world)
 		// Two key lists (body pair = lo << 32 | hi):
 		//   block   — every live joint: s2ShouldBodiesCollide (reference src/body.c:386-417) vetoes a new contact between
 		//             jointed bodies and does not look at collideConnected;
-		//   destroy — revolute joints created with collideConnected == false: contacts that already exist between the two
-		//             bodies are removed (reference src/joint.c:214-217).
+		//   destroy — revolute and weld joints created with collideConnected == false: contacts that already exist between
+		//             the two bodies are removed (reference src/joint.c:214-217).
 		int cap = world->jointPool.capacity;
 		uint64_t* block = (uint64_t*)malloc(sizeof(uint64_t) * (size_t)(cap > 0 ? cap : 1));
 		uint64_t* destroy = (uint64_t*)malloc(sizeof(uint64_t) * (size_t)(cap > 0 ? cap : 1));
@@ -385,7 +399,7 @@ void s2FlushToDevice(s2World* world)
 			uint64_t lo = (uint64_t)(j->bodyIndexA < j->bodyIndexB ? j->bodyIndexA : j->bodyIndexB);
 			uint64_t hi = (uint64_t)(j->bodyIndexA < j->bodyIndexB ? j->bodyIndexB : j->bodyIndexA);
 			block[nBlock++] = (lo << 32) | hi;
-			if (j->type == s2_revoluteJoint && j->collideConnected == false)
+			if ((j->type == s2_revoluteJoint || j->type == s2_weldJoint) && j->collideConnected == false)
 			{
 				destroy[nDestroy++] = (lo << 32) | hi;
 			}

@@ -66,6 +66,8 @@ SCHEDULE_COLOR, SCHEDULE_WAVEFRONT = 0, 1
 ROW_VALID = 0x1
 SHAPE_MOVED = 0x10
 JOINT_ENABLE_LIMIT, JOINT_ENABLE_MOTOR, JOINT_COLLIDE_CONNECTED = 0x10, 0x20, 0x40
+# joint types, stored in flags bits 1-3 (a weld keeps its angular impulse in the motorImpulse column)
+JOINT_REVOLUTE, JOINT_MOUSE, JOINT_WELD = 0, 1, 2
 
 # symbols declared in include/s2b_device.h (checked by the CPU test-suite against the built library)
 ABI_SYMBOLS = [

@@ -12,6 +12,7 @@ Each recipe restates one of the reference's sample scenes or one of the syntheti
 * :func:`collision_zoo`   — every manifold kind, flipped pairs, dynamic segments, compound bodies, mixed frictions and
                             shape filters, thrown sideways.
 * :func:`bouncers`        — shapes with restitution dropped from several heights (the restitution extension).
+* :func:`welded_structures` — cantilevers, welded assemblies, a welded platform rider and a chain (the weld joint).
 
 All scenes are deterministic lattices (no RNG). A recipe returns a :class:`Scene` holding the world id and the
 body ids in creation order.
@@ -522,6 +523,120 @@ def bouncers(lib: capi.Solver2D, solver="TGS_Soft", columns=16, rows=4, joints=T
         lib.s2CreatePolygonShape(pid, C.byref(sd), C.byref(box))
         sc.bodies.append(pid)
         sc.piles["platform"] = pid
+    return sc
+
+
+WELDED_PITCH = 30.0  # width of one copy of welded_structures (m)
+
+
+def welded_structures(lib: capi.Solver2D, solver="TGS_Soft", copies=1, platform=True) -> Scene:
+    """Weld joint coverage, `copies` side by side (about 30 bodies each). Per copy:
+
+    * two cantilever beams of five boxes welded end to end to a static wall; in the second, the boxes alternate between
+      angle 0 and 3 rad, so its welds have reference angles of +3 and -3 rad (near +-pi: the unwind is exercised);
+    * an L and a T of welded boxes dropped onto a small pile, the L pulled by a mouse joint (first copy only);
+    * with `platform`: a dynamic box welded onto a kinematic platform that moves sideways;
+    * a hanging chain of three revolute links (limits on the first, a motor on the second) ending in a welded pair, whose
+      weld keeps collideConnected.
+
+    On a library without s2CreateWeldJoint (the reference) every weld is created as a revolute joint with limits and
+    motor off, with the same bodies, anchors, reference angle and collideConnected: the broad phase treats every joint
+    alike, so both libraries see the same pairs. ``sc.piles["welds"]`` lists the indices into ``sc.joints`` of the welds."""
+    world = lib.create_world(solver)
+    sc = Scene(lib, world, name=f"welded{copies}")
+    sc.piles["welds"] = []
+    has_weld = "s2CreateWeldJoint" not in lib.missing
+    gid = _ground(lib, world, 0.5 * WELDED_PITCH * copies + 5.0)
+    sc.bodies.append(gid)
+    sd = default_shape_def()
+
+    def body(kind, x, y, angle=0.0, hx=0.5, hy=0.125, vx=0.0):
+        bd = default_body_def()
+        bd.type = kind
+        bd.position = Vec2(x, y)
+        bd.angle = angle
+        bd.linearVelocity = Vec2(vx, 0.0)
+        bid = lib.s2CreateBody(world, C.byref(bd))
+        box = lib.s2MakeBox(hx, hy)
+        lib.s2CreatePolygonShape(bid, C.byref(sd), C.byref(box))
+        sc.bodies.append(bid)
+        return bid
+
+    def weld(a, b, pivot, reference_angle, collide=False):
+        if has_weld:
+            jd = capi.default_weld_def()
+        else:
+            jd = default_revolute_def()
+        jd.bodyIdA = a
+        jd.bodyIdB = b
+        jd.localAnchorA = lib.s2Body_GetLocalPoint(a, pivot)
+        jd.localAnchorB = lib.s2Body_GetLocalPoint(b, pivot)
+        jd.referenceAngle = reference_angle
+        jd.collideConnected = collide
+        create = lib.s2CreateWeldJoint if has_weld else lib.s2CreateRevoluteJoint
+        sc.piles["welds"].append(len(sc.joints))
+        sc.joints.append(create(world, C.byref(jd)))
+
+    D, S, K = capi.DYNAMIC_BODY, capi.STATIC_BODY, capi.KINEMATIC_BODY
+    for k in range(copies):
+        x0 = -0.5 * WELDED_PITCH * (copies - 1) + WELDED_PITCH * k - 12.0
+        # cantilevers
+        for beam, y in enumerate((6.0, 9.0)):
+            wall = body(S, x0, y, hx=0.25, hy=1.0)
+            prev, prev_angle = wall, 0.0
+            for i in range(5):
+                angle = 3.0 if beam == 1 and i % 2 == 0 else 0.0
+                bid = body(D, x0 + 0.75 + 1.0 * i, y, angle=angle)
+                weld(prev, bid, Vec2(x0 + 0.25 + 1.0 * i, y), angle - prev_angle)
+                prev, prev_angle = bid, angle
+        # a small pile, an L and a T dropped onto it
+        for i in range(3):
+            for j in range(2):
+                body(D, x0 + 7.0 + 1.05 * i, 0.25 + 0.5 * j, hx=0.5, hy=0.25)
+        a = body(D, x0 + 7.5, 3.0)
+        b = body(D, x0 + 8.0 - 0.125, 3.0 + 0.375, angle=0.5 * math.pi, hx=0.5, hy=0.125)
+        weld(a, b, Vec2(x0 + 8.0 - 0.125, 3.0), 0.5 * math.pi)
+        ell = a
+        a = body(D, x0 + 8.0, 5.0)
+        b = body(D, x0 + 8.0, 5.0 - 0.625, angle=0.5 * math.pi)
+        weld(a, b, Vec2(x0 + 8.0, 5.0 - 0.125), 0.5 * math.pi)
+        c = body(D, x0 + 8.0, 5.0 + 0.375, hx=0.25, hy=0.25)
+        weld(a, c, Vec2(x0 + 8.0, 5.0 + 0.125), 0.0)
+        if k == 0:
+            md = default_mouse_def()
+            md.bodyIdA = gid
+            md.bodyIdB = ell
+            md.target = Vec2(x0 + 6.0, 4.0)
+            md.hertz = 3.0
+            md.dampingRatio = 0.7
+            sc.joints.append(lib.s2CreateMouseJoint(world, C.byref(md)))
+        if platform:
+            p = body(K, x0 + 12.0, 2.0, hx=1.0, hy=0.125, vx=0.5)
+            q = body(D, x0 + 12.0, 2.0 + 0.375, hx=0.25, hy=0.25)
+            weld(p, q, Vec2(x0 + 12.0, 2.0 + 0.125), 0.0)
+        # revolute chain ending in a welded pair
+        anchor = body(S, x0 + 17.0, 10.0, hx=0.25, hy=0.25)
+        prev = anchor
+        for i in range(3):
+            bid = body(D, x0 + 17.5 + 1.0 * i, 10.0)
+            jd = default_revolute_def()
+            pivot = Vec2(x0 + 17.0 + 1.0 * i, 10.0)
+            jd.bodyIdA = prev
+            jd.bodyIdB = bid
+            jd.localAnchorA = lib.s2Body_GetLocalPoint(prev, pivot)
+            jd.localAnchorB = lib.s2Body_GetLocalPoint(bid, pivot)
+            if i == 0:
+                jd.enableLimit = True
+                jd.lowerAngle = -0.5 * math.pi
+                jd.upperAngle = 0.25 * math.pi
+            elif i == 1:
+                jd.enableMotor = True
+                jd.motorSpeed = 0.5
+                jd.maxMotorTorque = 5.0
+            sc.joints.append(lib.s2CreateRevoluteJoint(world, C.byref(jd)))
+            prev = bid
+        end = body(D, x0 + 20.75, 10.0, hx=0.25, hy=0.25)
+        weld(prev, end, Vec2(x0 + 20.5, 10.0), 0.0, collide=True)
     return sc
 
 
