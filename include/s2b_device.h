@@ -92,6 +92,7 @@ enum
 	S2B_JOINT_REVOLUTE = 0,
 	S2B_JOINT_MOUSE = 1,
 	S2B_JOINT_WELD = 2, // never carries S2B_JOINT_ENABLE_LIMIT or S2B_JOINT_ENABLE_MOTOR
+	S2B_JOINT_PRISMATIC = 3,
 };
 
 #define S2B_JOINT_ENABLE_LIMIT 0x10
@@ -114,6 +115,10 @@ typedef struct s2bJointRow
 	// accumulated impulses (simulation state); a weld keeps its angular impulse in motorImpulse
 	float impulse[2];
 	float motorImpulse, lowerImpulse, upperImpulse;
+	// prismatic: the sliding axis in body A's frame (unit length). A prismatic row also reuses the revolute columns:
+	// lowerAngle / upperAngle hold the translation limits (m), maxMotorTorque the maximum motor force (N), impulse[2] the
+	// (perpendicular, angular) block impulse and motorImpulse / lowerImpulse / upperImpulse the axial impulses.
+	float localAxisA[2];
 } s2bJointRow;
 
 // One contact (shape pair) with its persistent manifold; mirrors s2Contact + s2Manifold + s2DistanceCache

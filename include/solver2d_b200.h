@@ -48,6 +48,51 @@ S2_INLINE struct s2WeldJointDef s2DefaultWeldJointDef(void)
 
 S2B_API s2JointId s2CreateWeldJoint(s2WorldId worldId, const s2WeldJointDef* def);
 
+// Prismatic (slider) joint: body B slides along an axis fixed in body A, keeps angle(B) - angle(A) at referenceAngle and
+// may have translation limits and a linear motor (DESIGN.md §3.9). Anchors are relative to each body's origin; the
+// translation is measured along the axis from anchor A to anchor B. Under XPBD the motor is not applied. Destroy it with
+// s2DestroyJoint.
+typedef struct s2PrismaticJointDef
+{
+	s2BodyId bodyIdA;
+	s2BodyId bodyIdB;
+	s2Vec2 localAnchorA;
+	s2Vec2 localAnchorB;
+	s2Vec2 localAxisA;	  // the sliding axis in body A's frame; normalized at creation
+	float referenceAngle; // angle(B) - angle(A) at rest
+	bool enableLimit;
+	float lowerTranslation; // m
+	float upperTranslation; // m
+	bool enableMotor;
+	float motorSpeed;	 // m/s
+	float maxMotorForce; // N
+	float drawSize;
+	bool collideConnected; // keep the contacts the two bodies already have
+} s2PrismaticJointDef;
+
+S2_INLINE struct s2PrismaticJointDef s2DefaultPrismaticJointDef(void)
+{
+	s2PrismaticJointDef def = S2_ZERO_INIT;
+	def.bodyIdA = s2_nullBodyId;
+	def.bodyIdB = s2_nullBodyId;
+	def.localAxisA.x = 1.0f;
+	def.drawSize = 1.0f;
+	return def;
+}
+
+// Returns s2_nullJointId (and creates nothing) for an axis of zero length or with a non-finite component, or for
+// lowerTranslation > upperTranslation.
+S2B_API s2JointId s2CreatePrismaticJoint(s2WorldId worldId, const s2PrismaticJointDef* def);
+S2B_API void s2PrismaticJoint_EnableLimit(s2JointId jointId, bool enableLimit);
+// Ignored when lower > upper (the joint keeps its limits).
+S2B_API void s2PrismaticJoint_SetLimits(s2JointId jointId, float lower, float upper);
+S2B_API void s2PrismaticJoint_EnableMotor(s2JointId jointId, bool enableMotor);
+S2B_API void s2PrismaticJoint_SetMotorSpeed(s2JointId jointId, float motorSpeed);
+// The motor force of the last step (N): inverseTimeStep times the motor impulse.
+S2B_API float s2PrismaticJoint_GetMotorForce(s2JointId jointId, float inverseTimeStep);
+// The current translation (m) along the world axis, from anchor A to anchor B.
+S2B_API float s2PrismaticJoint_GetTranslation(s2JointId jointId);
+
 // Push every pending host-side edit to the device now (s2World_Step does this itself).
 S2B_API void s2World_Flush(s2WorldId worldId);
 

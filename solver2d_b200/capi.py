@@ -152,6 +152,26 @@ class WeldJointDef(C.Structure):
     ]
 
 
+class PrismaticJointDef(C.Structure):
+    """s2PrismaticJointDef (include/solver2d_b200.h): an extension, absent from the reference."""
+    _fields_ = [
+        ("bodyIdA", BodyId),
+        ("bodyIdB", BodyId),
+        ("localAnchorA", Vec2),
+        ("localAnchorB", Vec2),
+        ("localAxisA", Vec2),
+        ("referenceAngle", C.c_float),
+        ("enableLimit", C.c_bool),
+        ("lowerTranslation", C.c_float),
+        ("upperTranslation", C.c_float),
+        ("enableMotor", C.c_bool),
+        ("motorSpeed", C.c_float),
+        ("maxMotorForce", C.c_float),
+        ("drawSize", C.c_float),
+        ("collideConnected", C.c_bool),
+    ]
+
+
 class Statistics(C.Structure):
     _fields_ = [
         ("bodyCount", C.c_int32),
@@ -221,6 +241,16 @@ def default_weld_def() -> WeldJointDef:
     return d
 
 
+def default_prismatic_def() -> PrismaticJointDef:
+    """s2DefaultPrismaticJointDef (include/solver2d_b200.h)."""
+    d = PrismaticJointDef()
+    d.bodyIdA = BodyId(-1, -1, 0)
+    d.bodyIdB = BodyId(-1, -1, 0)
+    d.localAxisA = Vec2(1.0, 0.0)
+    d.drawSize = 1.0
+    return d
+
+
 def default_mouse_def() -> MouseJointDef:
     """s2DefaultMouseJointDef (reference include/solver2d/joint_types.h:28-37)."""
     d = MouseJointDef()
@@ -272,6 +302,13 @@ _API = {
     "s2World_EnableRestitution": (None, [WorldId, C.c_bool]),
     "s2World_SetRestitutionThreshold": (None, [WorldId, C.c_float]),
     "s2CreateWeldJoint": (JointId, [WorldId, C.POINTER(WeldJointDef)]),
+    "s2CreatePrismaticJoint": (JointId, [WorldId, C.POINTER(PrismaticJointDef)]),
+    "s2PrismaticJoint_EnableLimit": (None, [JointId, C.c_bool]),
+    "s2PrismaticJoint_SetLimits": (None, [JointId, C.c_float, C.c_float]),
+    "s2PrismaticJoint_EnableMotor": (None, [JointId, C.c_bool]),
+    "s2PrismaticJoint_SetMotorSpeed": (None, [JointId, C.c_float]),
+    "s2PrismaticJoint_GetMotorForce": (C.c_float, [JointId, C.c_float]),
+    "s2PrismaticJoint_GetTranslation": (C.c_float, [JointId]),
 }
 
 class Transform(C.Structure):

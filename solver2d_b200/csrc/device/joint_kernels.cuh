@@ -104,8 +104,35 @@ template <int KIND> __device__ __forceinline__ void s2bPrepareJoint(const SolveA
 	jc.anchor[t] = make_float4(lA.x, lA.y, lB.x, lB.y);
 	jc.mass[t] = make_float4(mA, iA, mB, iB);
 	jc.lim[t] = lim;
-	jc.motor[t] = make_float4(motor.x, motor.y, 0.0f, 0.0f);
 	jc.coef[t] = make_float4(a.softJoint.bias, a.softJoint.mass, a.softJoint.impulse, 0.0f);
+
+	if (S2B_JOINT_TYPE(flags) == S2B_JOINT_PRISMATIC)
+	{
+		// DESIGN.md §3.9: the local axis rides in the motor row's spare zw; every mass is formed fresh in each solve.
+		// Limit and motor impulses are kept only with their flag and a warm start, the block impulse with the warm start.
+		float4 axis = a.joints.target[slot];
+		jc.motor[t] = make_float4(motor.x, motor.y, axis.z, axis.w);
+		jc.d0ax[t] = make_float4(centerDiff0.x, centerDiff0.y, 0.0f, 0.0f);
+		jc.pivot[t] = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
+		if (KIND == JPREP_XPBD || warmStart == false)
+		{
+			imp = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
+			limp = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
+		}
+		if ((flags & S2B_JOINT_ENABLE_LIMIT) == 0)
+		{
+			limp.x = 0.0f;
+			limp.y = 0.0f;
+		}
+		if ((flags & S2B_JOINT_ENABLE_MOTOR) == 0)
+		{
+			imp.z = 0.0f;
+		}
+		jc.imp[t] = imp;
+		jc.limp[t] = limp;
+		return;
+	}
+	jc.motor[t] = make_float4(motor.x, motor.y, 0.0f, 0.0f);
 
 	if (KIND == JPREP_XPBD)
 	{
@@ -170,6 +197,361 @@ __device__ __forceinline__ void s2bStoreJointImpulses(const SolveArgs& a, int t)
 }
 
 // ---------------------------------------------------------------------------------------------------------------
+// prismatic joint (extension, DESIGN.md §3.9; definition: tests/prismatic_oracle.c). Body B slides along an axis fixed
+// in body A: rows motor, lower limit, upper limit (along the axis), then a 2x2 block holding the perpendicular
+// separation and the relative angle. Every mass depends on the current separation d, so each solve forms it fresh.
+// Row columns: lim = (referenceAngle, lowerTranslation, upperTranslation), motor = (maxMotorForce, motorSpeed,
+// localAxisA.xy), imp = (perpendicular, angular, motor), limp = (lower, upper).
+// ---------------------------------------------------------------------------------------------------------------
+
+// the joint frame at the given poses: centre-of-mass-relative anchors, d = (dcB - dcA) + (rB - rA) + centerDiff0 and
+// the world axis
+struct PrismaticFrame
+{
+	s2Vec2 rA, rB, d, axis;
+};
+
+__device__ __forceinline__ PrismaticFrame s2bPrismaticFrame(float4 anchor, float4 d0, float4 motor, s2Vec2 dcA, s2Rot qA, s2Vec2 dcB,
+															s2Rot qB)
+{
+	PrismaticFrame f;
+	f.rA = s2RotateVector(qA, V2(anchor.x, anchor.y));
+	f.rB = s2RotateVector(qB, V2(anchor.z, anchor.w));
+	f.d = s2Add(s2Add(s2Sub(dcB, dcA), s2Sub(f.rB, f.rA)), V2(d0.x, d0.y));
+	f.axis = s2RotateVector(qA, V2(motor.z, motor.w));
+	return f;
+}
+
+// what warm starting adds to each body: v -/+= m * P, w -/+= i * L. Shared by the constraint-by-constraint warm start and
+// the per-body gather (warm_gather.cuh), so both add the same bits.
+struct PrismaticWarm
+{
+	s2Vec2 P;
+	float LA, LB;
+};
+
+__device__ __forceinline__ PrismaticWarm s2bPrismaticWarmTerms(const SolveArgs& a, int t)
+{
+	const JointConstraintView& jc = a.jc;
+	int4 head = jc.head[t];
+	float4 imp = jc.imp[t];
+	float4 limp = jc.limp[t];
+	float4 poseA = a.bodies.pose[head.y], poseB = a.bodies.pose[head.z];
+	PrismaticFrame f = s2bPrismaticFrame(jc.anchor[t], jc.d0ax[t], jc.motor[t], V2(poseA.x, poseA.y), R2(poseA.z, poseA.w),
+										 V2(poseB.x, poseB.y), R2(poseB.z, poseB.w));
+	s2Vec2 perp = s2LeftPerp(f.axis);
+	s2Vec2 dA = s2Add(f.d, f.rA);
+	float axialImpulse = imp.z + limp.x - limp.y;
+	PrismaticWarm w;
+	w.P = s2Add(s2MulSV(axialImpulse, f.axis), s2MulSV(imp.x, perp));
+	w.LA = axialImpulse * s2Cross(dA, f.axis) + imp.x * s2Cross(dA, perp) + imp.y;
+	w.LB = axialImpulse * s2Cross(f.rB, f.axis) + imp.x * s2Cross(f.rB, perp) + imp.y;
+	return w;
+}
+
+enum PrismaticSolveKind
+{
+	PSOLVE_SOFT = 0,	  // Jacobi, PGS_Soft, SoftStep, TGS_Soft
+	PSOLVE_BAUMGARTE = 1, // PGS, TGS_Sticky
+	PSOLVE_RIGID = 2,	  // PGS_NGS, PGS_NGS_Block, TGS_NGS
+};
+
+// the bias, mass scale and impulse scale of one row with position error C (a limit row when `limit`: speculative when
+// the limit is not reached)
+template <int KIND>
+__device__ __forceinline__ float3 s2bPrismaticBias(float C, bool limit, float4 coef, float h, float inv_h, bool useBias)
+{
+	float bias = 0.0f, massScale = 1.0f, impulseScale = 0.0f;
+	if (KIND == PSOLVE_RIGID)
+	{
+		bias = limit ? S2_MAX(C, 0.0f) / h : 0.0f;
+	}
+	else if (limit && C > 0.0f)
+	{
+		bias = C * inv_h;
+	}
+	else if (KIND == PSOLVE_BAUMGARTE)
+	{
+		bias = s2_baumgarte * inv_h * C;
+	}
+	else if (useBias)
+	{
+		bias = coef.x * C;
+		massScale = coef.y;
+		impulseScale = coef.z;
+	}
+	return make_float3(bias, massScale, impulseScale);
+}
+
+template <int KIND>
+__device__ __forceinline__ void s2bSolvePrismaticVelocity(const SolveArgs& a, int t, float h, float inv_h, bool useBias)
+{
+	const JointConstraintView& jc = a.jc;
+	int4 head = jc.head[t];
+	int ia = head.y, ib = head.z;
+	float4 mass = jc.mass[t];
+	float4 lim = jc.lim[t];
+	float4 motor = jc.motor[t];
+	float4 coef = jc.coef[t];
+	float4 imp = jc.imp[t];
+	float4 limp = jc.limp[t];
+	float4 velA = a.bodies.vel[ia], velB = a.bodies.vel[ib];
+	float4 poseA = a.bodies.pose[ia], poseB = a.bodies.pose[ib];
+	s2Vec2 vA = V2(velA.x, velA.y), vB = V2(velB.x, velB.y);
+	float wA = velA.z, wB = velB.z;
+	float mA = mass.x, iA = mass.y, mB = mass.z, iB = mass.w;
+	s2Rot qA = R2(poseA.z, poseA.w), qB = R2(poseB.z, poseB.w);
+	PrismaticFrame f = s2bPrismaticFrame(jc.anchor[t], jc.d0ax[t], motor, V2(poseA.x, poseA.y), qA, V2(poseB.x, poseB.y), qB);
+	s2Vec2 axis = f.axis;
+	s2Vec2 dA = s2Add(f.d, f.rA);
+	float translation = s2Dot(axis, f.d);
+	float a1 = s2Cross(dA, axis), a2 = s2Cross(f.rB, axis);
+	float k = mA + mB + iA * a1 * a1 + iB * a2 * a2;
+	float axialMass = k > 0.0f ? 1.0f / k : 0.0f;
+
+	if (head.x & S2B_JOINT_ENABLE_MOTOR)
+	{
+		float Cdot = s2Dot(axis, s2Sub(vB, vA)) + a2 * wB - a1 * wA;
+		float impulse = axialMass * (motor.y - Cdot);
+		float oldImpulse = imp.z;
+		float maxImpulse = h * motor.x;
+		imp.z = S2_CLAMP(oldImpulse + impulse, -maxImpulse, maxImpulse);
+		impulse = imp.z - oldImpulse;
+		s2Vec2 P = s2MulSV(impulse, axis);
+		vA = s2MulSub(vA, mA, P);
+		wA -= iA * (impulse * a1);
+		vB = s2MulAdd(vB, mB, P);
+		wB += iB * (impulse * a2);
+	}
+
+	if (head.x & S2B_JOINT_ENABLE_LIMIT)
+	{
+		// lower limit
+		{
+			float3 s = s2bPrismaticBias<KIND>(translation - lim.y, true, coef, h, inv_h, useBias);
+			float Cdot = s2Dot(axis, s2Sub(vB, vA)) + a2 * wB - a1 * wA;
+			float impulse = -axialMass * s.y * (Cdot + s.x) - s.z * limp.x;
+			float oldImpulse = limp.x;
+			limp.x = S2_MAX(oldImpulse + impulse, 0.0f);
+			impulse = limp.x - oldImpulse;
+			s2Vec2 P = s2MulSV(impulse, axis);
+			vA = s2MulSub(vA, mA, P);
+			wA -= iA * (impulse * a1);
+			vB = s2MulAdd(vB, mB, P);
+			wB += iB * (impulse * a2);
+		}
+		// upper limit (signs flipped so C stays positive when satisfied); it relaxes with its own impulse
+		{
+			float3 s = s2bPrismaticBias<KIND>(lim.z - translation, true, coef, h, inv_h, useBias);
+			float Cdot = s2Dot(axis, s2Sub(vA, vB)) + a1 * wA - a2 * wB;
+			float impulse = -axialMass * s.y * (Cdot + s.x) - s.z * limp.y;
+			float oldImpulse = limp.y;
+			limp.y = S2_MAX(oldImpulse + impulse, 0.0f);
+			impulse = limp.y - oldImpulse;
+			s2Vec2 P = s2MulSV(impulse, axis);
+			vA = s2MulAdd(vA, mA, P);
+			wA += iA * (impulse * a1);
+			vB = s2MulSub(vB, mB, P);
+			wB -= iB * (impulse * a2);
+		}
+	}
+
+	// the 2x2 block: perpendicular separation and relative angle
+	{
+		s2Vec2 perp = s2LeftPerp(axis);
+		float sA = s2Cross(dA, perp), sB = s2Cross(f.rB, perp);
+		s2Vec2 Cdot = V2(s2Dot(perp, s2Sub(vB, vA)) + sB * wB - sA * wA, wB - wA);
+		s2Vec2 C = V2(s2Dot(perp, f.d), s2UnwindAngle(s2RelativeAngle(qB, qA) - lim.x));
+		float3 sx = s2bPrismaticBias<KIND>(C.x, false, coef, h, inv_h, useBias);
+		float3 sy = s2bPrismaticBias<KIND>(C.y, false, coef, h, inv_h, useBias);
+		float k11 = mA + mB + iA * sA * sA + iB * sB * sB;
+		float k12 = iA * sA + iB * sB;
+		float k22 = iA + iB;
+		if (k22 == 0.0f)
+		{
+			k22 = 1.0f; // both rotations fixed: keeps K invertible
+		}
+		s2Mat22 K;
+		K.cx = V2(k11, k12);
+		K.cy = V2(k12, k22);
+		s2Vec2 b = s2Solve22(K, V2(Cdot.x + sx.x, Cdot.y + sy.x));
+		s2Vec2 impulse = V2(-sx.y * b.x - sx.z * imp.x, -sy.y * b.y - sy.z * imp.y);
+		imp.x += impulse.x;
+		imp.y += impulse.y;
+		s2Vec2 P = s2MulSV(impulse.x, perp);
+		float LA = impulse.x * sA + impulse.y;
+		float LB = impulse.x * sB + impulse.y;
+		vA = s2MulSub(vA, mA, P);
+		wA -= iA * LA;
+		vB = s2MulAdd(vB, mB, P);
+		wB += iB * LB;
+	}
+
+	jc.imp[t] = imp;
+	jc.limp[t] = limp;
+	s2bStoreJointVelocities(a, ia, ib, velA, velB, vA, wA, vB, wB, mA, iA, mB, iB);
+}
+
+// NGS position pass: the block on the current poses (corrections clamped), then the limit row on the corrected poses
+__device__ __forceinline__ void s2bSolvePrismaticPosition(const SolveArgs& a, int t)
+{
+	const JointConstraintView& jc = a.jc;
+	int4 head = jc.head[t];
+	int ia = head.y, ib = head.z;
+	float4 anchor = jc.anchor[t];
+	float4 mass = jc.mass[t];
+	float4 d0 = jc.d0ax[t];
+	float4 lim = jc.lim[t];
+	float4 motor = jc.motor[t];
+	float4 poseA = a.bodies.pose[ia], poseB = a.bodies.pose[ib];
+	s2Vec2 dcA = V2(poseA.x, poseA.y), dcB = V2(poseB.x, poseB.y);
+	s2Rot qA = R2(poseA.z, poseA.w), qB = R2(poseB.z, poseB.w);
+	float mA = mass.x, iA = mass.y, mB = mass.z, iB = mass.w;
+
+	{
+		PrismaticFrame f = s2bPrismaticFrame(anchor, d0, motor, dcA, qA, dcB, qB);
+		s2Vec2 perp = s2LeftPerp(f.axis);
+		s2Vec2 dA = s2Add(f.d, f.rA);
+		float sA = s2Cross(dA, perp), sB = s2Cross(f.rB, perp);
+		s2Vec2 C;
+		C.x = S2_CLAMP(s2Dot(perp, f.d), -s2_maxLinearCorrection, s2_maxLinearCorrection);
+		C.y = S2_CLAMP(s2UnwindAngle(s2RelativeAngle(qB, qA) - lim.x), -s2_maxAngularCorrection, s2_maxAngularCorrection);
+		float k11 = mA + mB + iA * sA * sA + iB * sB * sB;
+		float k12 = iA * sA + iB * sB;
+		float k22 = iA + iB;
+		if (k22 == 0.0f)
+		{
+			k22 = 1.0f;
+		}
+		s2Mat22 K;
+		K.cx = V2(k11, k12);
+		K.cy = V2(k12, k22);
+		s2Vec2 impulse = s2Solve22(K, s2Neg(C));
+		s2Vec2 P = s2MulSV(impulse.x, perp);
+		float LA = impulse.x * sA + impulse.y;
+		float LB = impulse.x * sB + impulse.y;
+		dcA = s2MulSub(dcA, mA, P);
+		qA = s2IntegrateRot(qA, -iA * LA);
+		dcB = s2MulAdd(dcB, mB, P);
+		qB = s2IntegrateRot(qB, iB * LB);
+	}
+
+	if (head.x & S2B_JOINT_ENABLE_LIMIT)
+	{
+		PrismaticFrame f = s2bPrismaticFrame(anchor, d0, motor, dcA, qA, dcB, qB);
+		s2Vec2 dA = s2Add(f.d, f.rA);
+		float a1 = s2Cross(dA, f.axis), a2 = s2Cross(f.rB, f.axis);
+		float translation = s2Dot(f.axis, f.d);
+		float C = 0.0f;
+		if (S2_ABS(lim.z - lim.y) < 2.0f * s2_linearSlop)
+		{
+			C = S2_CLAMP(translation - lim.y, -s2_maxLinearCorrection, s2_maxLinearCorrection);
+		}
+		else if (translation <= lim.y)
+		{
+			C = S2_CLAMP(translation - lim.y + s2_linearSlop, -s2_maxLinearCorrection, 0.0f);
+		}
+		else if (translation >= lim.z)
+		{
+			C = S2_CLAMP(translation - lim.z - s2_linearSlop, 0.0f, s2_maxLinearCorrection);
+		}
+		float k = mA + mB + iA * a1 * a1 + iB * a2 * a2;
+		float impulse = k > 0.0f ? -C / k : 0.0f;
+		s2Vec2 P = s2MulSV(impulse, f.axis);
+		dcA = s2MulSub(dcA, mA, P);
+		qA = s2IntegrateRot(qA, -iA * (impulse * a1));
+		dcB = s2MulAdd(dcB, mB, P);
+		qB = s2IntegrateRot(qB, iB * (impulse * a2));
+	}
+
+	if ((mA != 0.0f) || (iA != 0.0f))
+	{
+		a.bodies.pose[ia] = make_float4(dcA.x, dcA.y, qA.s, qA.c);
+	}
+	if ((mB != 0.0f) || (iB != 0.0f))
+	{
+		a.bodies.pose[ib] = make_float4(dcB.x, dcB.y, qB.s, qB.c);
+	}
+}
+
+// XPBD, zero compliance: the angle row (as the weld's), the perpendicular row, then the limits as position inequalities.
+// The motor is not applied, as the revolute joint's XPBD form ignores its motor.
+__device__ __forceinline__ void s2bSolvePrismaticXpbd(const SolveArgs& a, int t)
+{
+	const JointConstraintView& jc = a.jc;
+	int4 head = jc.head[t];
+	int ia = head.y, ib = head.z;
+	float4 anchor = jc.anchor[t];
+	float4 mass = jc.mass[t];
+	float4 d0 = jc.d0ax[t];
+	float4 lim = jc.lim[t];
+	float4 motor = jc.motor[t];
+	float4 poseA = a.bodies.pose[ia], poseB = a.bodies.pose[ib];
+	s2Vec2 dcA = V2(poseA.x, poseA.y), dcB = V2(poseB.x, poseB.y);
+	s2Rot qA = R2(poseA.z, poseA.w), qB = R2(poseB.z, poseB.w);
+	float mA = mass.x, iA = mass.y, mB = mass.z, iB = mass.w;
+
+	if (iA + iB != 0.0f)
+	{
+		float C = s2UnwindAngle(s2RelativeAngle(qB, qA) - lim.x);
+		float p = -C / (iA + iB);
+		qA = s2IntegrateRot(qA, -iA * p);
+		qB = s2IntegrateRot(qB, iB * p);
+	}
+
+	{
+		PrismaticFrame f = s2bPrismaticFrame(anchor, d0, motor, dcA, qA, dcB, qB);
+		s2Vec2 perp = s2LeftPerp(f.axis);
+		float sA = s2Cross(s2Add(f.d, f.rA), perp), sB = s2Cross(f.rB, perp);
+		float k = mA + mB + iA * sA * sA + iB * sB * sB;
+		if (k > 0.0f)
+		{
+			float lambda = -s2Dot(perp, f.d) / k;
+			s2Vec2 P = s2MulSV(lambda, perp);
+			dcA = s2MulSub(dcA, mA, P);
+			qA = s2IntegrateRot(qA, -iA * (lambda * sA));
+			dcB = s2MulAdd(dcB, mB, P);
+			qB = s2IntegrateRot(qB, iB * (lambda * sB));
+		}
+	}
+
+	if (head.x & S2B_JOINT_ENABLE_LIMIT)
+	{
+		PrismaticFrame f = s2bPrismaticFrame(anchor, d0, motor, dcA, qA, dcB, qB);
+		float a1 = s2Cross(s2Add(f.d, f.rA), f.axis), a2 = s2Cross(f.rB, f.axis);
+		float translation = s2Dot(f.axis, f.d);
+		float C = 0.0f;
+		if (translation < lim.y)
+		{
+			C = translation - lim.y;
+		}
+		else if (translation > lim.z)
+		{
+			C = translation - lim.z;
+		}
+		float k = mA + mB + iA * a1 * a1 + iB * a2 * a2;
+		if (C != 0.0f && k > 0.0f)
+		{
+			float lambda = -C / k;
+			s2Vec2 P = s2MulSV(lambda, f.axis);
+			dcA = s2MulSub(dcA, mA, P);
+			qA = s2IntegrateRot(qA, -iA * (lambda * a1));
+			dcB = s2MulAdd(dcB, mB, P);
+			qB = s2IntegrateRot(qB, iB * (lambda * a2));
+		}
+	}
+
+	if ((mA != 0.0f) || (iA != 0.0f))
+	{
+		a.bodies.pose[ia] = make_float4(dcA.x, dcA.y, qA.s, qA.c);
+	}
+	if ((mB != 0.0f) || (iB != 0.0f))
+	{
+		a.bodies.pose[ib] = make_float4(dcB.x, dcB.y, qB.s, qB.c);
+	}
+}
+
+// ---------------------------------------------------------------------------------------------------------------
 // warm start: s2WarmStartRevolute (reference src/revolute_joint.c:107-150), s2WarmStartMouse (mouse_joint.c:85-107)
 // ---------------------------------------------------------------------------------------------------------------
 __device__ __forceinline__ void s2bWarmStartJoint(const SolveArgs& a, int t)
@@ -195,6 +577,19 @@ __device__ __forceinline__ void s2bWarmStartJoint(const SolveArgs& a, int t)
 		{
 			a.bodies.vel[ib] = make_float4(vB.x, vB.y, wB, velB.w);
 		}
+		return;
+	}
+
+	if (S2B_JOINT_TYPE(head.x) == S2B_JOINT_PRISMATIC)
+	{
+		float4 velA = a.bodies.vel[ia], velB = a.bodies.vel[ib];
+		float mA = mass.x, iA = mass.y, mB = mass.z, iB = mass.w;
+		PrismaticWarm pw = s2bPrismaticWarmTerms(a, t);
+		s2Vec2 vA = s2MulSub(V2(velA.x, velA.y), mA, pw.P);
+		float wA = velA.z - iA * pw.LA;
+		s2Vec2 vB = s2MulAdd(V2(velB.x, velB.y), mB, pw.P);
+		float wB = velB.z + iB * pw.LB;
+		s2bStoreJointVelocities(a, ia, ib, velA, velB, vA, wA, vB, wB, mA, iA, mB, iB);
 		return;
 	}
 
@@ -513,6 +908,11 @@ __device__ __forceinline__ void s2bSolveJointSoft(const SolveArgs& a, int t, flo
 		}
 		return;
 	}
+	if (S2B_JOINT_TYPE(flags) == S2B_JOINT_PRISMATIC)
+	{
+		s2bSolvePrismaticVelocity<PSOLVE_SOFT>(a, t, h, inv_h, useBias);
+		return;
+	}
 	s2bSolveRevoluteVelocity<JSOLVE_SOFT>(a, t, h, inv_h, useBias);
 }
 
@@ -523,6 +923,11 @@ __device__ __forceinline__ void s2bSolveJointBaumgarte(const SolveArgs& a, int t
 	if (S2B_JOINT_TYPE(flags) == S2B_JOINT_MOUSE)
 	{
 		s2bSolveMouse(a, t);
+		return;
+	}
+	if (S2B_JOINT_TYPE(flags) == S2B_JOINT_PRISMATIC)
+	{
+		s2bSolvePrismaticVelocity<PSOLVE_BAUMGARTE>(a, t, h, inv_h, useBias);
 		return;
 	}
 	s2bSolveRevoluteVelocity<JSOLVE_BAUMGARTE>(a, t, h, inv_h, useBias);
@@ -628,6 +1033,11 @@ __device__ __forceinline__ void s2bSolveJointRigid(const SolveArgs& a, int t, fl
 		s2bSolveMouse(a, t);
 		return;
 	}
+	if (S2B_JOINT_TYPE(a.jc.head[t].x) == S2B_JOINT_PRISMATIC)
+	{
+		s2bSolvePrismaticVelocity<PSOLVE_RIGID>(a, t, h, 0.0f /* inv_h: unused by the rigid rows */, false);
+		return;
+	}
 	s2bSolveRevoluteRigid(a, t, h);
 }
 
@@ -641,6 +1051,11 @@ __device__ __forceinline__ void s2bSolveJointPosition(const SolveArgs& a, int t)
 	int4 head = jc.head[t];
 	if (S2B_JOINT_TYPE(head.x) == S2B_JOINT_MOUSE)
 	{
+		return;
+	}
+	if (S2B_JOINT_TYPE(head.x) == S2B_JOINT_PRISMATIC)
+	{
+		s2bSolvePrismaticPosition(a, t);
 		return;
 	}
 	int ia = head.y, ib = head.z;
@@ -721,6 +1136,11 @@ __device__ __forceinline__ void s2bSolveJointXpbd(const SolveArgs& a, int t)
 	if (S2B_JOINT_TYPE(head.x) == S2B_JOINT_MOUSE)
 	{
 		s2bSolveMouse(a, t);
+		return;
+	}
+	if (S2B_JOINT_TYPE(head.x) == S2B_JOINT_PRISMATIC)
+	{
+		s2bSolvePrismaticXpbd(a, t);
 		return;
 	}
 	const float compliance = 0.0f;

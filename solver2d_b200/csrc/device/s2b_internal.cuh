@@ -267,7 +267,7 @@ struct JointView
 	float4* anchors; // localOriginAnchorA.xy localOriginAnchorB.xy
 	float4* lim;	// referenceAngle lowerAngle upperAngle 0
 	float4* motor;	// maxMotorTorque motorSpeed hertz dampingRatio
-	float4* target; // mouse target.xy 0 0
+	float4* target; // mouse target.xy, prismatic localAxisA.xy
 	float4* imp;	// impulse.x impulse.y motorImpulse 0
 	float4* limp;	// lowerImpulse upperImpulse 0 0
 	int* color;		// colour the joint was last solved with (-1: none)
@@ -282,7 +282,7 @@ struct JointConstraintView
 	float4* mass;	// invMassA invIA invMassB invIB
 	float4* d0ax;	// centerDiff0.xy axialMass 0
 	float4* lim;	// referenceAngle lowerAngle upperAngle 0
-	float4* motor;	// maxMotorTorque motorSpeed 0 0
+	float4* motor;	// maxMotorTorque motorSpeed 0 0 (prismatic: maxMotorForce motorSpeed localAxisA.xy)
 	float4* coef;	// biasCoefficient massCoefficient impulseCoefficient 0
 	float4* pivot;	// pivotMass cx.x cx.y cy.x cy.y (mouse, non-fresh revolute)
 	float4* imp;	// impulse.x impulse.y motorImpulse 0        (r/w)

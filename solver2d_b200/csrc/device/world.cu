@@ -91,7 +91,7 @@ __global__ void s2bScatterJoints(const s2bJointRow* __restrict__ rows, int count
 							   r->localOriginAnchorB[1]);
 	j.lim[i] = make_float4(r->referenceAngle, r->lowerAngle, r->upperAngle, 0.0f);
 	j.motor[i] = make_float4(r->maxMotorTorque, r->motorSpeed, r->hertz, r->dampingRatio);
-	j.target[i] = make_float4(r->target[0], r->target[1], 0.0f, 0.0f);
+	j.target[i] = make_float4(r->target[0], r->target[1], r->localAxisA[0], r->localAxisA[1]);
 	j.imp[i] = make_float4(r->impulse[0], r->impulse[1], r->motorImpulse, 0.0f);
 	j.limp[i] = make_float4(r->lowerImpulse, r->upperImpulse, 0.0f, 0.0f);
 }
@@ -209,6 +209,8 @@ __global__ void s2bGatherJoints(s2bJointRow* rows, int count, JointView j)
 	r.dampingRatio = motor.w;
 	r.target[0] = target.x;
 	r.target[1] = target.y;
+	r.localAxisA[0] = target.z;
+	r.localAxisA[1] = target.w;
 	r.impulse[0] = imp.x;
 	r.impulse[1] = imp.y;
 	r.motorImpulse = imp.z;

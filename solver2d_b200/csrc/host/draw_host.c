@@ -79,6 +79,25 @@ static void s2DrawJoint(s2DebugDraw* draw, s2World* world, const s2Joint* joint)
 	draw->DrawPoint(pA, 5.0f, s2Rgb(0.3f, 0.3f, 0.9f), draw->context);
 	draw->DrawPoint(pB, 5.0f, s2Rgb(0.4f, 0.4f, 0.4f), draw->context);
 
+	if (joint->type == s2_prismaticJoint)
+	{
+		// the axis through anchor A (drawSize each way), a mark across the axis at each translation limit, and the
+		// segment from anchor A to anchor B
+		const float L = joint->drawSize;
+		s2Vec2 axis = s2RotateVector(bodyA->rot, joint->localAxisA);
+		s2Vec2 perp = s2MulSV(0.5f * L, s2LeftPerp(axis));
+		draw->DrawSegment(s2MulSub(pA, L, axis), s2MulAdd(pA, L, axis), s2Rgb(0.7f, 0.7f, 0.7f), draw->context);
+		if (joint->enableLimit)
+		{
+			s2Vec2 lower = s2MulAdd(pA, joint->lowerAngle, axis);
+			s2Vec2 upper = s2MulAdd(pA, joint->upperAngle, axis);
+			draw->DrawSegment(s2Sub(lower, perp), s2Add(lower, perp), s2Rgb(0.3f, 0.9f, 0.3f), draw->context);
+			draw->DrawSegment(s2Sub(upper, perp), s2Add(upper, perp), s2Rgb(0.9f, 0.3f, 0.3f), draw->context);
+		}
+		draw->DrawSegment(pA, pB, s2Rgb(0.5f, 0.8f, 0.8f), draw->context);
+		return;
+	}
+
 	const float L = joint->drawSize;
 	s2Color grey = s2Rgb(0.7f, 0.7f, 0.7f);
 	s2Vec2 r = s2RotateVector(bodyB->rot, s2MakeVec2(L * cosf(joint->referenceAngle), L * sinf(joint->referenceAngle)));

@@ -157,3 +157,97 @@ float s2RevoluteJoint_GetMotorTorque(s2JointId jointId, float inverseTimeStep)
 	s2SyncStateToHost(world);
 	return inverseTimeStep * world->joints[jointId.index].motorImpulse;
 }
+
+// The prismatic joint has no counterpart in the reference (DESIGN.md §3.9). Degenerate input creates nothing and returns
+// s2_nullJointId: an axis that cannot be normalized, or lowerTranslation > upperTranslation.
+s2JointId s2CreatePrismaticJoint(s2WorldId worldId, const s2PrismaticJointDef* def)
+{
+	s2Vec2 axis = def->localAxisA;
+	float length = s2Length(axis);
+	if (s2IsValidVec2(axis) == false || s2IsValid(length) == false || length == 0.0f ||
+		(def->lowerTranslation <= def->upperTranslation) == false)
+	{
+		return s2_nullJointId;
+	}
+
+	s2World* world = s2GetWorldFromId(worldId);
+	s2Body* bodyA = world->bodies + def->bodyIdA.index;
+	s2Body* bodyB = world->bodies + def->bodyIdB.index;
+
+	s2Joint* joint = s2AllocJoint(world, bodyA, bodyB);
+	joint->type = s2_prismaticJoint;
+	joint->drawSize = def->drawSize;
+	joint->localOriginAnchorA = def->localAnchorA;
+	joint->localOriginAnchorB = def->localAnchorB;
+	joint->localAxisA = s2MakeVec2(axis.x / length, axis.y / length);
+	joint->referenceAngle = def->referenceAngle;
+	joint->lowerAngle = def->lowerTranslation;
+	joint->upperAngle = def->upperTranslation;
+	joint->maxMotorTorque = def->maxMotorForce;
+	joint->motorSpeed = def->motorSpeed;
+	joint->enableLimit = def->enableLimit;
+	joint->enableMotor = def->enableMotor;
+	joint->collideConnected = def->collideConnected;
+
+	s2JointId jointId = {joint->object.index, world->index, joint->object.revision};
+	return jointId;
+}
+
+void s2PrismaticJoint_EnableLimit(s2JointId jointId, bool enableLimit)
+{
+	s2World* world;
+	s2Joint* joint = s2GetJointForEdit(jointId, &world);
+	joint->enableLimit = enableLimit;
+	s2MarkJointDirty(world, joint);
+}
+
+void s2PrismaticJoint_SetLimits(s2JointId jointId, float lower, float upper)
+{
+	if ((lower <= upper) == false)
+	{
+		return; // rejected: the joint keeps its limits
+	}
+	s2World* world;
+	s2Joint* joint = s2GetJointForEdit(jointId, &world);
+	joint->lowerAngle = lower;
+	joint->upperAngle = upper;
+	s2MarkJointDirty(world, joint);
+}
+
+void s2PrismaticJoint_EnableMotor(s2JointId jointId, bool enableMotor)
+{
+	s2World* world;
+	s2Joint* joint = s2GetJointForEdit(jointId, &world);
+	joint->enableMotor = enableMotor;
+	s2MarkJointDirty(world, joint);
+}
+
+void s2PrismaticJoint_SetMotorSpeed(s2JointId jointId, float motorSpeed)
+{
+	s2World* world;
+	s2Joint* joint = s2GetJointForEdit(jointId, &world);
+	joint->motorSpeed = motorSpeed;
+	s2MarkJointDirty(world, joint);
+}
+
+float s2PrismaticJoint_GetMotorForce(s2JointId jointId, float inverseTimeStep)
+{
+	s2World* world = s2GetWorldFromIndex(jointId.world);
+	s2SyncStateToHost(world);
+	return inverseTimeStep * world->joints[jointId.index].motorImpulse;
+}
+
+float s2PrismaticJoint_GetTranslation(s2JointId jointId)
+{
+	s2World* world = s2GetWorldFromIndex(jointId.world);
+	s2SyncStateToHost(world);
+	const s2Joint* joint = world->joints + jointId.index;
+	const s2Body* bodyA = world->bodies + joint->bodyIndexA;
+	const s2Body* bodyB = world->bodies + joint->bodyIndexB;
+	s2Transform xfA = {bodyA->origin, bodyA->rot};
+	s2Transform xfB = {bodyB->origin, bodyB->rot};
+	s2Vec2 pA = s2TransformPoint(xfA, joint->localOriginAnchorA);
+	s2Vec2 pB = s2TransformPoint(xfB, joint->localOriginAnchorB);
+	s2Vec2 axis = s2RotateVector(bodyA->rot, joint->localAxisA);
+	return s2Dot(axis, s2Sub(pB, pA));
+}

@@ -86,6 +86,7 @@ typedef enum s2JointType
 	s2_revoluteJoint,
 	s2_mouseJoint,
 	s2_weldJoint,
+	s2_prismaticJoint,
 } s2JointType;
 
 typedef struct s2Body
@@ -157,10 +158,13 @@ typedef struct s2Joint
 	float drawSize;
 	bool collideConnected;
 
-	// revolute
+	// revolute; a prismatic joint keeps its translation limits in lowerAngle / upperAngle and its maximum motor force in
+	// maxMotorTorque, as its device row does
 	bool enableMotor, enableLimit;
 	float maxMotorTorque, motorSpeed;
 	float referenceAngle, lowerAngle, upperAngle;
+	// prismatic
+	s2Vec2 localAxisA;
 	// mouse
 	float hertz, dampingRatio;
 	s2Vec2 targetA;

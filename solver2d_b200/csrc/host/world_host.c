@@ -250,6 +250,9 @@ static void s2FillJointRow(s2bJointRow* r, const s2Joint* j)
 		case s2_weldJoint:
 			type = S2B_JOINT_WELD;
 			break;
+		case s2_prismaticJoint:
+			type = S2B_JOINT_PRISMATIC;
+			break;
 	}
 	r->flags = S2B_ROW_VALID | (type << 1);
 	// a weld is created with enableLimit == enableMotor == false, so its row never carries either flag
@@ -276,6 +279,8 @@ static void s2FillJointRow(s2bJointRow* r, const s2Joint* j)
 	r->motorImpulse = j->motorImpulse;
 	r->lowerImpulse = j->lowerImpulse;
 	r->upperImpulse = j->upperImpulse;
+	r->localAxisA[0] = j->localAxisA.x;
+	r->localAxisA[1] = j->localAxisA.y;
 }
 
 static int s2CompareU64(const void* a, const void* b)
@@ -383,8 +388,8 @@ void s2FlushToDevice(s2World* world)
 		// Two key lists (body pair = lo << 32 | hi):
 		//   block   — every live joint: s2ShouldBodiesCollide (reference src/body.c:386-417) vetoes a new contact between
 		//             jointed bodies and does not look at collideConnected;
-		//   destroy — revolute and weld joints created with collideConnected == false: contacts that already exist between
-		//             the two bodies are removed (reference src/joint.c:214-217).
+		//   destroy — revolute, weld and prismatic joints created with collideConnected == false: contacts that already
+		//             exist between the two bodies are removed (reference src/joint.c:214-217).
 		int cap = world->jointPool.capacity;
 		uint64_t* block = (uint64_t*)malloc(sizeof(uint64_t) * (size_t)(cap > 0 ? cap : 1));
 		uint64_t* destroy = (uint64_t*)malloc(sizeof(uint64_t) * (size_t)(cap > 0 ? cap : 1));
@@ -399,7 +404,7 @@ void s2FlushToDevice(s2World* world)
 			uint64_t lo = (uint64_t)(j->bodyIndexA < j->bodyIndexB ? j->bodyIndexA : j->bodyIndexB);
 			uint64_t hi = (uint64_t)(j->bodyIndexA < j->bodyIndexB ? j->bodyIndexB : j->bodyIndexA);
 			block[nBlock++] = (lo << 32) | hi;
-			if ((j->type == s2_revoluteJoint || j->type == s2_weldJoint) && j->collideConnected == false)
+			if ((j->type == s2_revoluteJoint || j->type == s2_weldJoint || j->type == s2_prismaticJoint) && j->collideConnected == false)
 			{
 				destroy[nDestroy++] = (lo << 32) | hi;
 			}

@@ -32,6 +32,7 @@ JOINT_ROW = np.dtype([
     ("localOriginAnchorB", "<f4", 2), ("referenceAngle", "<f4"), ("lowerAngle", "<f4"), ("upperAngle", "<f4"),
     ("maxMotorTorque", "<f4"), ("motorSpeed", "<f4"), ("hertz", "<f4"), ("dampingRatio", "<f4"), ("target", "<f4", 2),
     ("impulse", "<f4", 2), ("motorImpulse", "<f4"), ("lowerImpulse", "<f4"), ("upperImpulse", "<f4"),
+    ("localAxisA", "<f4", 2),
 ], align=True)
 
 CONTACT_POINT = np.dtype([
@@ -66,8 +67,9 @@ SCHEDULE_COLOR, SCHEDULE_WAVEFRONT = 0, 1
 ROW_VALID = 0x1
 SHAPE_MOVED = 0x10
 JOINT_ENABLE_LIMIT, JOINT_ENABLE_MOTOR, JOINT_COLLIDE_CONNECTED = 0x10, 0x20, 0x40
-# joint types, stored in flags bits 1-3 (a weld keeps its angular impulse in the motorImpulse column)
-JOINT_REVOLUTE, JOINT_MOUSE, JOINT_WELD = 0, 1, 2
+# joint types, stored in flags bits 1-3 (a weld keeps its angular impulse in the motorImpulse column; a prismatic row keeps
+# its translation limits in lowerAngle / upperAngle and its maximum motor force in maxMotorTorque)
+JOINT_REVOLUTE, JOINT_MOUSE, JOINT_WELD, JOINT_PRISMATIC = 0, 1, 2, 3
 
 # symbols declared in include/s2b_device.h (checked by the CPU test-suite against the built library)
 ABI_SYMBOLS = [

@@ -13,6 +13,8 @@ Each recipe restates one of the reference's sample scenes or one of the syntheti
                             shape filters, thrown sideways.
 * :func:`bouncers`        — shapes with restitution dropped from several heights (the restitution extension).
 * :func:`welded_structures` — cantilevers, welded assemblies, a welded platform rider and a chain (the weld joint).
+* :func:`sliders`         — pistons, an elevator, an inclined slider, a kinematic carriage, a slider-crank and a mouse
+                            joint on a slider (the prismatic joint).
 
 All scenes are deterministic lattices (no RNG). A recipe returns a :class:`Scene` holding the world id and the
 body ids in creation order.
@@ -637,6 +639,139 @@ def welded_structures(lib: capi.Solver2D, solver="TGS_Soft", copies=1, platform=
             prev = bid
         end = body(D, x0 + 20.75, 10.0, hx=0.25, hy=0.25)
         weld(prev, end, Vec2(x0 + 20.5, 10.0), 0.0, collide=True)
+    return sc
+
+
+SLIDERS_PITCH = 32.0  # width of one copy of sliders (m)
+
+
+def sliders(lib: capi.Solver2D, solver="TGS_Soft", copies=1, kinematic=True) -> Scene:
+    """Prismatic joint coverage, `copies` side by side (about 20 bodies each). Per copy:
+
+    * three pistons on static posts, motors driving boxes up against gravity: one with force to spare, one capped by an
+      upper limit, and one whose maxMotorForce (4 N) is below its 10 N load, so it sinks onto the ground;
+    * an elevator platform with both limits and a motor, carrying a small pile of boxes;
+    * a slider on an axis inclined at 0.5 rad in a body turned by 0.2 rad, with referenceAngle 0.4 - 0.2, thrown along the
+      axis into its upper limit and falling back onto its lower one;
+    * with `kinematic`: a box sliding on a kinematic body that moves sideways (limits and a weak motor);
+    * a slider-crank: a motorised revolute crank on a static hub, a connecting rod, and a piston on a prismatic joint;
+    * a horizontal slider with limits, pulled off its axis by a mouse joint (first copy only).
+
+    On a library without s2CreatePrismaticJoint (the reference) every prismatic joint is created as a revolute joint with
+    limits and motor off, with the same bodies, anchors, reference angle and collideConnected: the broad phase treats every
+    joint alike, so both libraries see the same pairs. ``sc.piles["prismatic"]`` lists the indices into ``sc.joints`` of the
+    prismatic joints, ``sc.piles["prismatic_defs"]`` their definitions (dicts of s2PrismaticJointDef fields, the axis as
+    given) and ``sc.piles["prismatic_bodies"]`` their (bodyIdA, bodyIdB), so that a test can turn the stand-in rows into
+    prismatic rows."""
+    world = lib.create_world(solver)
+    sc = Scene(lib, world, name=f"sliders{copies}")
+    sc.piles["prismatic"] = []
+    sc.piles["prismatic_defs"] = []
+    sc.piles["prismatic_bodies"] = []
+    has_prismatic = "s2CreatePrismaticJoint" not in lib.missing
+    gid = _ground(lib, world, 0.5 * SLIDERS_PITCH * copies + 5.0)
+    sc.bodies.append(gid)
+    sd = default_shape_def()
+
+    def body(kind, x, y, angle=0.0, hx=0.5, hy=0.125, vx=0.0, vy=0.0):
+        bd = default_body_def()
+        bd.type = kind
+        bd.position = Vec2(x, y)
+        bd.angle = angle
+        bd.linearVelocity = Vec2(vx, vy)
+        bid = lib.s2CreateBody(world, C.byref(bd))
+        box = lib.s2MakeBox(hx, hy)
+        lib.s2CreatePolygonShape(bid, C.byref(sd), C.byref(box))
+        sc.bodies.append(bid)
+        return bid
+
+    def prismatic(a, b, pivot, axis, reference_angle=0.0, limit=None, motor=None, collide=False):
+        d = dict(localAnchorA=tuple(lib.s2Body_GetLocalPoint(a, pivot)), localAnchorB=tuple(lib.s2Body_GetLocalPoint(b, pivot)),
+                 localAxisA=axis, referenceAngle=reference_angle, enableLimit=limit is not None,
+                 lowerTranslation=limit[0] if limit else 0.0, upperTranslation=limit[1] if limit else 0.0,
+                 enableMotor=motor is not None, motorSpeed=motor[0] if motor else 0.0,
+                 maxMotorForce=motor[1] if motor else 0.0, collideConnected=collide)
+        if has_prismatic:
+            jd = capi.default_prismatic_def()
+            for name, value in d.items():
+                setattr(jd, name, Vec2(*value) if isinstance(value, tuple) else value)
+            create = lib.s2CreatePrismaticJoint
+        else:
+            jd = default_revolute_def()
+            jd.localAnchorA = Vec2(*d["localAnchorA"])
+            jd.localAnchorB = Vec2(*d["localAnchorB"])
+            jd.referenceAngle = reference_angle
+            jd.collideConnected = collide
+            create = lib.s2CreateRevoluteJoint
+        jd.bodyIdA = a
+        jd.bodyIdB = b
+        sc.piles["prismatic"].append(len(sc.joints))
+        sc.piles["prismatic_defs"].append(d)
+        sc.piles["prismatic_bodies"].append((a, b))
+        jid = create(world, C.byref(jd))
+        sc.joints.append(jid)
+        return jid
+
+    def revolute(a, b, pivot, motor=None):
+        jd = default_revolute_def()
+        jd.bodyIdA = a
+        jd.bodyIdB = b
+        jd.localAnchorA = lib.s2Body_GetLocalPoint(a, pivot)
+        jd.localAnchorB = lib.s2Body_GetLocalPoint(b, pivot)
+        if motor is not None:
+            jd.enableMotor = True
+            jd.motorSpeed, jd.maxMotorTorque = motor
+        sc.joints.append(lib.s2CreateRevoluteJoint(world, C.byref(jd)))
+
+    D, S, K = capi.DYNAMIC_BODY, capi.STATIC_BODY, capi.KINEMATIC_BODY
+    up = (0.0, 1.0)
+    for k in range(copies):
+        x0 = -0.5 * SLIDERS_PITCH * (copies - 1) + SLIDERS_PITCH * k - 14.0
+        # pistons: 1 kg boxes (10 N) on static posts
+        for i, (limit, motor) in enumerate((((-1.0, 3.0), (0.5, 200.0)), ((-1.0, 0.5), (1.0, 200.0)), (None, (0.5, 4.0)))):
+            x = x0 + 1.5 * i
+            post = body(S, x, 0.25, hx=0.25, hy=0.25)
+            load = body(D, x, 1.5, hx=0.5, hy=0.5)
+            prismatic(post, load, Vec2(x, 1.5), up, limit=limit, motor=motor)
+        # elevator with a small pile
+        base = body(S, x0 + 7.0, 0.25, hx=0.25, hy=0.25)
+        deck = body(D, x0 + 7.0, 1.5, hx=1.5, hy=0.125)
+        prismatic(base, deck, Vec2(x0 + 7.0, 1.5), up, limit=(-1.0, 1.5), motor=(1.0, 100.0))
+        for i in range(3):
+            body(D, x0 + 6.3 + 0.7 * i, 1.875, hx=0.25, hy=0.25)
+        body(D, x0 + 6.65, 2.375, hx=0.25, hy=0.25)
+        # inclined slider, thrown into its limits
+        frame = body(S, x0 + 11.0, 3.0, angle=0.2, hx=0.25, hy=0.25)
+        c, s = math.cos(0.7), math.sin(0.7)  # world direction of the axis: 0.2 + 0.5 rad
+        slider = body(D, x0 + 11.0 + c, 3.0 + s, angle=0.4, hx=0.375, hy=0.125, vx=4.0 * c, vy=4.0 * s)
+        prismatic(frame, slider, Vec2(x0 + 11.0 + c, 3.0 + s), (2.0 * math.cos(0.5), 2.0 * math.sin(0.5)),
+                  reference_angle=0.4 - 0.2, limit=(0.0, 2.0))
+        # a box riding a kinematic carriage
+        if kinematic:
+            carriage = body(K, x0 + 15.0, 2.0, hx=1.0, hy=0.125, vx=0.5)
+            rider = body(D, x0 + 15.0, 2.375, hx=0.25, hy=0.25)
+            prismatic(carriage, rider, Vec2(x0 + 15.0, 2.375), (1.0, 0.0), limit=(-0.75, 0.75), motor=(0.3, 5.0))
+        # slider-crank
+        hub = body(S, x0 + 20.0, 3.0, hx=0.1, hy=0.1)
+        crank = body(D, x0 + 20.5, 3.0, hx=0.5, hy=0.1)
+        revolute(hub, crank, Vec2(x0 + 20.0, 3.0), motor=(2.0, 50.0))
+        rod = body(D, x0 + 22.0, 3.0, hx=1.0, hy=0.1)
+        revolute(crank, rod, Vec2(x0 + 21.0, 3.0))
+        piston = body(D, x0 + 23.0, 3.0, hx=0.25, hy=0.25)
+        revolute(rod, piston, Vec2(x0 + 23.0, 3.0))
+        prismatic(hub, piston, Vec2(x0 + 23.0, 3.0), (1.0, 0.0))
+        # horizontal slider pulled by a mouse joint
+        rail = body(S, x0 + 27.0, 1.0, hx=0.25, hy=0.25)
+        carriage = body(D, x0 + 27.0, 1.5, hx=0.5, hy=0.125)
+        prismatic(rail, carriage, Vec2(x0 + 27.0, 1.5), (1.0, 0.0), limit=(-1.0, 1.0), collide=True)
+        if k == 0:
+            md = default_mouse_def()
+            md.bodyIdA = gid
+            md.bodyIdB = carriage
+            md.target = Vec2(x0 + 29.0, 2.5)
+            md.hertz = 3.0
+            md.dampingRatio = 0.7
+            sc.joints.append(lib.s2CreateMouseJoint(world, C.byref(md)))
     return sc
 
 
