@@ -189,6 +189,7 @@ typedef struct s2bCounters
 	int32_t cutCount;		 // constraints that straddle two regions (solved in device-wide steps)
 	int32_t cutGroupCount;	 // colours of the cut set = device-wide steps per Gauss-Seidel sweep
 	int32_t recolouredCount; /* constraints moved out of a sparse top colour by Kempe chains so far (colouring, DESIGN.md 3.2) */
+	int32_t neighbourSync;	 // blocks of the persistent kernel whose colour steps wait only for neighbouring blocks; 0 = grid barriers
 } s2bCounters;
 
 // ---- lifecycle ------------------------------------------------------------------------------------------------
@@ -311,6 +312,11 @@ S2B_API int s2b_download_contacts(s2bWorld* world, s2bContactRow* rows, int maxC
 // Returns the item count. (Feeds the order-permuted oracle in the parity tests.)
 S2B_API int s2b_download_solve_order(s2bWorld* world, int32_t* items, int maxItems, int32_t* groupSizes, int maxGroups,
 							 int32_t* groupCount);
+// Neighbour tables of the last schedule (DESIGN.md 3.1, neighbour-synchronised colour steps): returns the number of blocks B
+// whose colour steps wait only for their neighbours (0: the mode is off). When maxBlocks >= B, table[b * 17] receives the
+// neighbour count of block b and table[b * 17 + 1 ...] the neighbours. Block b runs items [b * s, (b + 1) * s) of every
+// group of n items that s2b_download_solve_order reports, s = ceil(n / B) rounded up to a multiple of 32.
+S2B_API int s2b_download_neighbour_blocks(s2bWorld* world, int32_t* table, int maxBlocks);
 S2B_API void s2b_get_counters(s2bWorld* world, s2bCounters* out);
 // Islands = connected components of the constraint graph of the last s2b_solve over the movable bodies (contacts with at
 // least one point and joints connect; static and kinematic bodies do not — two piles on one ground are two islands). The

@@ -62,13 +62,15 @@ struct S2bSync
 	unsigned base;	   // arrival count at kernel start
 	unsigned arrivals; // arrivals expected since then (barriers passed x blocks)
 	int pending;	   // what ran since the last synchronisation: 0 nothing, 1 region-local work, 2 device-wide work
-	int code;		   // trace code of the last phase executed (pass kind << 8 | op; bit 7 of the kind byte: device-wide step)
+	int code;		   // trace code of the last phase executed (pass kind << 8 | op; kind byte bit 7: device-wide step, bits 7+6:
+					   // overflow group, bit 6 alone: neighbour-synchronised colour step)
 };
 
 #define S2B_PENDING_NONE 0
 #define S2B_PENDING_LOCAL 1
 #define S2B_PENDING_GLOBAL 2
 #define S2B_PENDING_FLOW 3 // a ticketed pass: orders itself against the next ticketed pass, anything else needs the barrier
+#define S2B_PENDING_NEIGHBOURS 4 // a neighbour-synchronised colour step: orders itself against the next one, anything else needs the barrier
 
 __device__ __forceinline__ unsigned s2bLdAcquireU32(const unsigned* p)
 {
@@ -100,7 +102,7 @@ __device__ __forceinline__ void s2bGridBarrier(const SolveArgs& a, S2bSync& s)
 // phase ran in between
 __device__ __forceinline__ void s2bSyncBeforeLocal(const SolveArgs& a, S2bSync& s)
 {
-	if (s.pending == S2B_PENDING_GLOBAL)
+	if (s.pending == S2B_PENDING_GLOBAL || s.pending == S2B_PENDING_NEIGHBOURS)
 	{
 		s2bGridBarrier(a, s);
 		s2bTrace(a, s.code);
@@ -120,6 +122,56 @@ __device__ __forceinline__ void s2bSyncBeforeGlobal(const SolveArgs& a, S2bSync&
 	}
 }
 
+// ---- neighbour-synchronised colour steps (DESIGN.md §3.1) -----------------------------------------------------------
+// Block b runs the b-th share of every device-wide colour (s2bGroupShare). Two blocks are neighbours when constraints they
+// run share a movable body (solver.cu, s2bBlockEdgesKernel). Between two colour steps a block therefore only has to wait for
+// its neighbours to finish the previous step, not for the whole grid: each block owns an epoch word (one 128-byte line),
+// counts its neighbour-synchronised steps in it with a release store, and before step e waits with acquire loads until every
+// neighbour has published e - 1 (the acquire also invalidates the SM's L1, as the grid barrier's does). Body passes, flat
+// passes and the overflow group still take the grid barrier (`pending` says a neighbour step ran).
+// Why the order is the serial one: any two constraints that share a movable body run on the same block or on neighbours, so
+// every read-after-write and write-after-read between colours is ordered by the epochs; inside a colour no two constraints
+// share a movable body, so they commute.
+// Why it cannot deadlock: the launch is cooperative (every block is resident), every block runs the same steps, and a block
+// only ever waits for a neighbour (a symmetric relation) to reach an epoch lower than the one it is about to publish. The block
+// whose published epoch is the smallest therefore always finds its wait satisfied and moves on.
+// Epochs are monotonic across launches (as barrier[0]): every block of a launch publishes the same sequence base + 1, base + 2,
+// ..., and block 0 leaves the final value in barrier[S2B_EPOCH_BASE_WORD] for the next launch (the restitution kernel
+// continues it). A block the previous launches did not run holds an older, smaller value, which no wait accepts.
+
+// sNbr: the block's neighbour count, its neighbours, then (S2B_NBR_EPOCH) the epoch of its last colour step, written by thread 0
+// only (kept in shared memory rather than in every thread's registers: only warp 0 reads it)
+#define S2B_NBR_EPOCH S2B_NSYNC_STRIDE
+
+__device__ __forceinline__ void s2bNeighbourWait(const SolveArgs& a, S2bSync& s, int* sNbr)
+{
+	// lanes 0 .. n-1 of warp 0 poll one neighbour each, all at once
+	__syncwarp();
+	if (threadIdx.x < sNbr[0])
+	{
+		const unsigned* flag = a.barrier + S2B_EPOCH_WORD(sNbr[1 + threadIdx.x]);
+		unsigned epoch = (unsigned)sNbr[S2B_NBR_EPOCH];
+		while ((int)(s2bLdAcquireU32(flag) - epoch) < 0)
+		{
+		}
+	}
+	__syncthreads();
+	s2bTrace(a, s.code);
+}
+
+// the colour step is done in this block: publish its epoch
+__device__ __forceinline__ void s2bPublishEpoch(const SolveArgs& a, S2bSync& s, int* sNbr)
+{
+	__syncthreads();
+	if (threadIdx.x == 0)
+	{
+		unsigned epoch = (unsigned)sNbr[S2B_NBR_EPOCH] + 1u;
+		sNbr[S2B_NBR_EPOCH] = (int)epoch;
+		asm volatile("st.release.gpu.global.u32 [%0], %1;" ::"l"(a.barrier + S2B_EPOCH_WORD(blockIdx.x)), "r"(epoch) : "memory");
+	}
+	s.pending = S2B_PENDING_NEIGHBOURS;
+}
+
 // ---- passes ------------------------------------------------------------------------------------------------------
 
 // what does not change during the launch, read once
@@ -132,6 +184,7 @@ struct S2bLaunchInfo
 	int hubs;		  // hub bodies (body passes run over them grid-wide)
 	int bodyBegin, bodyEnd; // this block's range of regBodies
 	bool regions;
+	bool neighbours;	// device-wide colour steps are neighbour-synchronised (grid-uniform)
 	bool foldPositions; // TGS_Soft: the bias sweep integrates positions (ConstraintView::lastTouch), the body pass is skipped
 	bool resident;		// TGS_Soft: the region's velocity / pose rows live in shared memory for the whole launch
 };
@@ -394,7 +447,7 @@ __device__ __forceinline__ void s2bTouchJoint(const SolveArgs& a, int t, bool bo
 // device-wide groups (cut colours / wavefront levels, a grid barrier before each), then the serial overflow group.
 template <int SOLVER>
 __device__ __forceinline__ void s2bGroupPass(int jointOp, int contactOp, const SolveArgs& a, const PassPtrs& p, const S2bLaunchInfo& li,
-											 S2bSync& sync, const int* sRegJ, const int* sRegC, const int* sGroupJ, const int* sGroupC)
+											 S2bSync& sync, const int* sRegJ, const int* sRegC, const int* sGroupJ, const int* sGroupC, int* sNbr)
 {
 	int traceCode = (PASS_GROUP << 8) | contactOp;
 	if (li.regions && li.primary > 0)
@@ -466,8 +519,6 @@ __device__ __forceinline__ void s2bGroupPass(int jointOp, int contactOp, const S
 		sync.code = traceCode;
 	}
 
-	int stride = gridDim.x * blockDim.x;
-	int tid = blockIdx.x * blockDim.x + threadIdx.x;
 	for (int g = 0; g < li.groups; ++g)
 	{
 		int jBegin, cBegin, jEnd, cEnd;
@@ -479,57 +530,93 @@ __device__ __forceinline__ void s2bGroupPass(int jointOp, int contactOp, const S
 		{
 			jBegin = a.jGroupOff[g], jEnd = a.jGroupOff[g + 1], cBegin = a.cGroupOff[g], cEnd = a.cGroupOff[g + 1];
 		}
-		int nj = jointOp != JOP_NONE ? jEnd - jBegin : 0;
-		int nc = contactOp != COP_NONE ? cEnd - cBegin : 0;
-		if (nj + nc == 0)
+		if ((jointOp != JOP_NONE ? jEnd - jBegin : 0) + (contactOp != COP_NONE ? cEnd - cBegin : 0) == 0)
 		{
 			continue; // uniform: every thread reads the same table
 		}
-		if (SOLVER == 7 && (contactOp == COP_TGS_SOFT_BIAS || contactOp == COP_TGS_SOFT_RELAX || contactOp == COP_TGS_SOFT_RELAX_STORE) && nj == 0)
+		// this block's share of the group's items u (joints, then contacts), whatever the pass's ops: the mapping the neighbour
+		// tables were built from
+		int njAll = jEnd - jBegin;
+		int n = njAll + cEnd - cBegin;
+		int share = s2bGroupShare(n, gridDim.x);
+		int uEnd = min(n, ((int)blockIdx.x + 1) * share);
+		int u = (int)blockIdx.x * share + threadIdx.x;
+		if (SOLVER == 7 && (contactOp == COP_TGS_SOFT_BIAS || contactOp == COP_TGS_SOFT_RELAX || contactOp == COP_TGS_SOFT_RELAX_STORE) &&
+			(jointOp == JOP_NONE || njAll == 0))
 		{
 			// The headline op. Nothing in a thread's constraint row is written by another thread (the impulses by this very
 			// thread, one sweep ago), so the row is fetched BEFORE the barrier: what remains after it is the dependent part
 			// proper — the two bodies, the arithmetic, the stores (one L2 round trip less per device-wide step).
-			bool mine = tid < nc;
+			bool mine = u >= njAll && u < uEnd;
 			bool store = contactOp == COP_TGS_SOFT_RELAX_STORE;
 			bool bias = contactOp == COP_TGS_SOFT_BIAS;
 			bool fold = bias && li.foldPositions;
+			int t = cBegin + u - njAll;
 			ContactStream cs;
 			if (mine)
 			{
-				cs = s2bLoadContactStream(a, cBegin + tid, store);
-				cs.last = fold ? a.cc.lastTouch[cBegin + tid] : 0;
+				cs = s2bLoadContactStream(a, t, store);
+				cs.last = fold ? a.cc.lastTouch[t] : 0;
 			}
-			s2bSyncBeforeGlobal(a, sync);
+			if (sync.pending == S2B_PENDING_NEIGHBOURS)
+			{
+				s2bNeighbourWait(a, sync, sNbr);
+			}
+			else
+			{
+				s2bSyncBeforeGlobal(a, sync);
+			}
 			bool writeWarm = bias ? a.ctx.extraIterations == 0 : true;
 			if (mine)
 			{
-				s2bSolveContactTgsSoftStream(a, cBegin + tid, cs, a.ctx.inv_h, bias, writeWarm, store);
+				s2bSolveContactTgsSoftStream(a, t, cs, a.ctx.inv_h, bias, writeWarm, store);
 			}
-			for (int t = tid + stride; t < nc; t += stride)
+			for (u += blockDim.x; u < uEnd; u += blockDim.x)
 			{
-				ContactStream more = s2bLoadContactStream(a, cBegin + t, store);
-				more.last = fold ? a.cc.lastTouch[cBegin + t] : 0;
-				s2bSolveContactTgsSoftStream(a, cBegin + t, more, a.ctx.inv_h, bias, writeWarm, store);
+				t = cBegin + u - njAll;
+				if (u >= njAll)
+				{
+					ContactStream more = s2bLoadContactStream(a, t, store);
+					more.last = fold ? a.cc.lastTouch[t] : 0;
+					s2bSolveContactTgsSoftStream(a, t, more, a.ctx.inv_h, bias, writeWarm, store);
+				}
 			}
 		}
 		else
 		{
-			s2bSyncBeforeGlobal(a, sync);
-			for (int t = tid; t < nj + nc; t += stride)
+			if (sync.pending == S2B_PENDING_NEIGHBOURS)
 			{
-				if (t < nj)
+				s2bNeighbourWait(a, sync, sNbr);
+			}
+			else
+			{
+				s2bSyncBeforeGlobal(a, sync);
+			}
+			for (; u < uEnd; u += blockDim.x)
+			{
+				if (u < njAll)
 				{
-					s2bRunJointOpT<SOLVER>(jointOp, a, jBegin + t, p);
+					if (jointOp != JOP_NONE)
+					{
+						s2bRunJointOpT<SOLVER>(jointOp, a, jBegin + u, p);
+					}
 				}
-				else
+				else if (contactOp != COP_NONE)
 				{
-					s2bRunContactOpT<SOLVER>(contactOp, a, cBegin + (t - nj));
+					s2bRunContactOpT<SOLVER>(contactOp, a, cBegin + (u - njAll));
 				}
 			}
 		}
-		sync.pending = S2B_PENDING_GLOBAL;
-		sync.code = traceCode | 0x8000;
+		if (li.neighbours)
+		{
+			s2bPublishEpoch(a, sync, sNbr);
+			sync.code = traceCode | 0x4000;
+		}
+		else
+		{
+			sync.pending = S2B_PENDING_GLOBAL;
+			sync.code = traceCode | 0x8000;
+		}
 	}
 	int ovC = contactOp != COP_NONE ? li.ovC : 0;
 	int ovJ = jointOp != JOP_NONE ? li.ovJ : 0;
@@ -770,14 +857,21 @@ __device__ __forceinline__ void s2bFlowPass(int jointOp, int contactOp, const So
 // ---- the kernel --------------------------------------------------------------------------------------------------
 
 // The whole solver stage of one step: the variant's program from prepare to store, one launch.
-template <int SOLVER> __global__ void __launch_bounds__(S2B_BLOCK) s2bPersistentSolveT(SolveArgs a, PassPtrs p, Program prog)
+// The restitution instantiation runs on the variant's grid (one block per SM), so it is told that one resident block per SM
+// is enough: left to itself ptxas keeps it at 64 registers (two blocks per SM) and spills.
+template <int SOLVER> __global__ void __launch_bounds__(S2B_BLOCK, SOLVER == S2B_RESTITUTION_PROGRAM ? 1 : 0) s2bPersistentSolveT(SolveArgs a, PassPtrs p, Program prog)
 {
 	__shared__ int sRegJ[S2B_REG_STRIDE], sRegC[S2B_REG_STRIDE];
 	__shared__ int sGroupJ[S2B_MAX_COLORS + 2], sGroupC[S2B_MAX_COLORS + 2];
+	__shared__ int sNbr[S2B_NSYNC_STRIDE + 1];
 
 	S2bSync sync;
 	sync.base = *((volatile unsigned*)(a.barrier + 32));
 	sync.arrivals = 0;
+	if (threadIdx.x == 0)
+	{
+		sNbr[S2B_NBR_EPOCH] = (int)*((volatile unsigned*)(a.barrier + S2B_EPOCH_BASE_WORD));
+	}
 	sync.pending = S2B_PENDING_NONE;
 	sync.code = 0;
 	s2bTrace(a, 0xFFFF);
@@ -791,6 +885,15 @@ template <int SOLVER> __global__ void __launch_bounds__(S2B_BLOCK) s2bPersistent
 	li.ovC = a.counts[CNT_OVERFLOW_C];
 	li.regions = a.regions > 0 && a.counts[CNT_REGIONS_ON] != 0;
 	li.hubs = (li.regions && a.heavyBodies != nullptr) ? a.heavyBodies[0] : 0;
+	li.neighbours = a.nsyncNbr != nullptr && a.counts[CNT_NSYNC] == (int)gridDim.x && li.regions == false && li.ovC + li.ovJ == 0 &&
+					a.bodyTicket == nullptr;
+	if (li.neighbours)
+	{
+		for (int k = threadIdx.x; k < S2B_NSYNC_STRIDE; k += blockDim.x)
+		{
+			sNbr[k] = a.nsyncNbr[blockIdx.x * S2B_NSYNC_STRIDE + k];
+		}
+	}
 	// s2IntegratePositions folded into the TGS_Soft bias sweep: only in the plain colour schedule of a scene without joints,
 	// hub bodies or an overflow group (every movable body with a constraint then has a CONTACT as its last toucher, and
 	// every bias step runs through the branch below that looks at the marks); all of it is grid-uniform
@@ -872,7 +975,7 @@ template <int SOLVER> __global__ void __launch_bounds__(S2B_BLOCK) s2bPersistent
 					else
 					{
 						s2bGroupPass<SOLVER>(pass.jointOp, pass.contactOp, a, p, li, sync, sRegJ, sRegC, groupsInShared ? sGroupJ : nullptr,
-											 groupsInShared ? sGroupC : nullptr);
+											 groupsInShared ? sGroupC : nullptr, sNbr);
 					}
 				}
 				else if (pass.kind == PASS_BODY && li.foldPositions && pass.bodyOp == BOP_INTEGRATE_POSITIONS)
@@ -911,11 +1014,18 @@ template <int SOLVER> __global__ void __launch_bounds__(S2B_BLOCK) s2bPersistent
 			}
 		}
 	}
-	// hand the arrival count to the next launch (every block has read the base long before block 0 gets here)
+	// hand the arrival count and the epoch to the next launch. Every block has read both bases before block 0 gets here if a
+	// grid barrier lies between; neighbour waits alone do not ensure that (blocks of another island may not have started), so a
+	// launch without a grid barrier (the restitution pass) takes one here.
+	if (li.neighbours && sync.arrivals == 0)
+	{
+		s2bGridBarrier(a, sync);
+	}
 	s2bTrace(a, sync.code);
 	if (blockIdx.x == 0 && threadIdx.x == 0 && gridDim.x > 1)
 	{
 		a.barrier[32] = sync.base + sync.arrivals;
+		a.barrier[S2B_EPOCH_BASE_WORD] = (unsigned)sNbr[S2B_NBR_EPOCH];
 	}
 }
 

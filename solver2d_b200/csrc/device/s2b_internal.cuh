@@ -376,6 +376,8 @@ struct s2bWorld
 	int residentRegions = 1; // TGS_Soft: regions with nothing device-wide to solve keep their bodies in shared memory (S2B_RESIDENT=0 disables)
 	int hubDegree = 48; // constraints of a body with more incident constraints go to the serial overflow group uncoloured (S2B_HUB_DEGREE, 0 = colour them)
 	int fusePositions = 1; // TGS_Soft: s2IntegratePositions folded into the bias sweep (S2B_FUSE_POSITIONS=0 disables)
+	int neighbourSync = 1; // device-wide colour steps wait for neighbouring blocks only, where the device finds that possible
+						   // (persistent.cuh; S2B_NEIGHBOUR_SYNC=0 keeps a grid barrier before every colour step)
 	int kempeGrid = 0;
 	DevArray<int> dMovedFlag; // [0] = number of proxies moved in last finalize (device counter)
 	int pairPassCount = 0;

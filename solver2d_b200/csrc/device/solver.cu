@@ -1512,6 +1512,137 @@ __global__ void s2bFinishGroups(int* counts, const int* cOff, const int* jOff, c
 	counts[CNT_RESIDENT] = resident ? 1 : 0;
 }
 
+// ---- neighbour tables of the device-wide colour steps (persistent.cuh, "neighbour-synchronised colour steps") ---------
+// Block b runs the b-th share of every colour (s2bGroupShare). Two blocks are NEIGHBOURS when constraints they run share a
+// movable body, in any two colours. The solve order inside a colour follows the constraints' natural order, which is
+// spatially coherent on a pile, so a block's shares of the different colours cover about the same bodies and a block has a
+// handful of neighbours. Static and kinematic bodies are never written by a sweep (s2bItemEndpoints drops them) and make no
+// edge.
+
+// per item: the block that runs it (regions off: group g = colour g; the overflow group gets -1)
+__global__ void s2bItemBlockKernel(const int* counts, const int* cPerm, const int* jPerm, const int* cGroupOff, const int* jGroupOff, int blocks,
+								   int* itemBlock)
+{
+	int nJ = counts[CNT_JOINTS], nC = counts[CNT_CONTACTS];
+	int p = blockIdx.x * blockDim.x + threadIdx.x;
+	if (p >= nJ + nC)
+	{
+		return;
+	}
+	bool isContact = p >= nJ;
+	int t = isContact ? p - nJ : p;
+	const int* off = isContact ? cGroupOff : jGroupOff;
+	// largest g in [0, S2B_MAX_COLORS] with off[g] <= t
+	int lo = 0, hi = S2B_MAX_COLORS;
+	while (lo < hi)
+	{
+		int mid = (lo + hi + 1) >> 1;
+		if (off[mid] <= t)
+		{
+			lo = mid;
+		}
+		else
+		{
+			hi = mid - 1;
+		}
+	}
+	int block = -1;
+	if (lo < S2B_MAX_COLORS)
+	{
+		int nj = jGroupOff[lo + 1] - jGroupOff[lo];
+		int n = nj + cGroupOff[lo + 1] - cGroupOff[lo];
+		int u = isContact ? nj + t - cGroupOff[lo] : t - jGroupOff[lo];
+		block = u / s2bGroupShare(n, blocks);
+	}
+	itemBlock[isContact ? nJ + cPerm[t] : jPerm[t]] = block;
+}
+
+// per movable body: every pair of distinct blocks that run one of its constraints is an edge (bits[a * words + b / 32])
+// (a hub, an overflow constraint or a body spread over too many blocks sets the "cannot be used" word bits[blocks * words])
+__global__ void s2bBlockEdgesKernel(int bodyCapacity, const int* adjStart, const int* adj, const int* itemBlock, int blocks, int words,
+									unsigned* bits)
+{
+	int i = blockIdx.x * blockDim.x + threadIdx.x;
+	if (i >= bodyCapacity)
+	{
+		return;
+	}
+	int begin = adjStart[i], end = adjStart[i + 1];
+	if (end - begin > S2B_HEAVY_DEGREE)
+	{
+		atomicOr(bits + (size_t)blocks * words, 1u);
+		return;
+	}
+	int seen[S2B_NSYNC_BODY_BLOCKS];
+	int n = 0;
+	for (int k = begin; k < end; ++k)
+	{
+		int b = itemBlock[adj[k]];
+		bool fresh = b >= 0;
+		for (int m = 0; m < n && fresh; ++m)
+		{
+			fresh = seen[m] != b;
+		}
+		if (b < 0 || (fresh && n == S2B_NSYNC_BODY_BLOCKS))
+		{
+			atomicOr(bits + (size_t)blocks * words, 1u);
+			return;
+		}
+		if (fresh)
+		{
+			seen[n++] = b;
+		}
+	}
+	for (int x = 0; x < n; ++x)
+	{
+		for (int y = 0; y < n; ++y)
+		{
+			unsigned* w = bits + (size_t)seen[x] * words + (seen[y] >> 5);
+			unsigned bit = 1u << (seen[y] & 31);
+			if (x != y && (*w & bit) == 0)
+			{
+				atomicOr(w, bit);
+			}
+		}
+	}
+}
+
+// One block of >= `blocks` threads: the neighbour list of every block, and the decision, grid-uniform for the kernel that
+// reads it: on when the colour steps are device-wide (regions off), there are at least two of them, no serial overflow
+// group follows them, and every block has at most S2B_NSYNC_K neighbours.
+__global__ void s2bNeighbourListKernel(int* counts, int blocks, int words, const unsigned* bits, int* nbr)
+{
+	int b = threadIdx.x;
+	bool fail = false;
+	if (b < blocks)
+	{
+		int n = 0;
+		for (int k = 0; k < words; ++k)
+		{
+			unsigned m = bits[(size_t)b * words + k];
+			while (m != 0)
+			{
+				int other = k * 32 + __ffs(m) - 1;
+				m &= m - 1;
+				if (n < S2B_NSYNC_K)
+				{
+					nbr[b * S2B_NSYNC_STRIDE + 1 + n] = other;
+				}
+				n += 1;
+			}
+		}
+		nbr[b * S2B_NSYNC_STRIDE] = n;
+		fail = n > S2B_NSYNC_K;
+	}
+	fail = __syncthreads_or(fail ? 1 : 0) != 0;
+	if (threadIdx.x == 0)
+	{
+		bool on = fail == false && bits[(size_t)blocks * words] == 0 && blocks > 1 && counts[CNT_REGIONS_ON] == 0 && counts[CNT_GROUPS] > 1 &&
+				  counts[CNT_OVERFLOW_C] + counts[CNT_OVERFLOW_J] == 0;
+		counts[CNT_NSYNC] = on ? blocks : 0;
+	}
+}
+
 // The distinct bodies the serial overflow group touches (movable or not), numbered in arrival order (the numbering is
 // only a cache layout: persistent.cuh stages these bodies in shared memory for the serial walk).
 __global__ void s2bOverflowBodiesKernel(const int* counts, const int* jGroupOff, const int* cGroupOff, const int* jPerm, const int* cPerm,
@@ -2660,6 +2791,7 @@ struct SolvePlan
 	int threads = S2B_BLOCK;
 	int grid = 1;	 // blocks of the persistent kernel
 	int regions = 0; // region-local schedule: == grid, or 0
+	bool neighbourSync = false; // the schedule builds neighbour tables for the colour steps (the device decides whether to use them)
 	HostPlan host;	 // launch-by-launch / wavefront modes
 	int hostNC = 0, hostNJ = 0;
 };
@@ -2814,7 +2946,15 @@ static void planSolve(s2bWorld* w, SolverScratch* s, SolvePlan& pl)
 		s->flow.reserve(2 * nC + 2 * nJ, st, false);
 		s->bodyTicket.reserve((size_t)bodyCap + 2, st, false);
 	}
-	w->solveBarrier.reserve(64, st, true, true);
+	pl.neighbourSync = w->schedule == S2B_SCHEDULE_COLOR && pl.usePersistent && w->neighbourSync != 0 && pl.dataflow == false && pl.grid > 1;
+	if (pl.neighbourSync)
+	{
+		s->itemBlock.reserve(nI, st, false);
+		s->nsyncBits.reserve((size_t)pl.grid * ((pl.grid + 31) / 32) + 1, st, false);
+		// (kept on growth: a graph replayed without a schedule rebuild reads the tables whenever CNT_NSYNC names its grid)
+		s->nsyncNbr.reserve((size_t)pl.grid * S2B_NSYNC_STRIDE, st, true);
+	}
+	w->solveBarrier.reserve(S2B_BARRIER_WORDS, st, true, true);
 	w->schedDirty.reserve(4, st, true, true);
 	// (+2 rows: the bulk-staged colour kernel may read up to two rows past the last constraint)
 	s->idx.reserve(nC + 2, st, false);
@@ -2968,6 +3108,7 @@ static void enqueueSchedule(s2bWorld* w, SolverScratch* s, SolvePlan& pl)
 
 	bool needHostCounts = (w->schedule == S2B_SCHEDULE_WAVEFRONT) || pl.usePersistent == false;
 	s->regions = 0;
+	S2B_CHECK(cudaMemsetAsync(s->counts.p + CNT_NSYNC, 0, sizeof(int), st));
 	if (maxItems > 0)
 	{
 		bool wantAdj = w->schedule == S2B_SCHEDULE_COLOR || pl.needInc;
@@ -3077,6 +3218,16 @@ static void enqueueSchedule(s2bWorld* w, SolverScratch* s, SolvePlan& pl)
 			S2B_CHECK(cudaMemsetAsync(s->ovBodies.p, 0, sizeof(int), st));
 			S2B_LAUNCH(w, s2bOverflowBodiesKernel, gridFor(maxItems, 256), 256, 0, s->counts.p, s->jGroupOff.p, s->cGroupOff.p, s->jPerm.p,
 					   s->cPerm.p, s->jointSlots.p, s->activeSlots.p, jointView(w), makeView(w->contacts[w->cur]), s->ovBodySlot.p, s->ovBodies.p);
+			if (pl.neighbourSync)
+			{
+				int words = (pl.grid + 31) / 32;
+				S2B_LAUNCH(w, s2bItemBlockKernel, gridFor(maxItems, 256), 256, 0, s->counts.p, s->cPerm.p, s->jPerm.p, s->cGroupOff.p, s->jGroupOff.p,
+						   pl.grid, s->itemBlock.p);
+				S2B_CHECK(cudaMemsetAsync(s->nsyncBits.p, 0, sizeof(unsigned) * ((size_t)pl.grid * words + 1), st));
+				S2B_LAUNCH(w, s2bBlockEdgesKernel, gridFor(bodyCap, 256), 256, 0, bodyCap, s->adjStart.p, s->adj.p, s->itemBlock.p, pl.grid, words,
+						   s->nsyncBits.p);
+				S2B_LAUNCH(w, s2bNeighbourListKernel, 1, 512, 0, s->counts.p, pl.grid, words, s->nsyncBits.p, s->nsyncNbr.p);
+			}
 		}
 
 		if (needHostCounts)
@@ -3286,6 +3437,7 @@ static void enqueueIterate(s2bWorld* w, SolverScratch* s, SolvePlan& pl, bool ca
 	a.jRegOff = s->jRegOff.p;
 	a.cRegOff = s->cRegOff.p;
 	a.barrier = w->solveBarrier.p;
+	a.nsyncNbr = pl.neighbourSync ? s->nsyncNbr.p : nullptr;
 	bool stagedOverflow = w->schedule == S2B_SCHEDULE_COLOR && pl.usePersistent && pl.maxItems > 0;
 	a.ovBodies = stagedOverflow ? s->ovBodies.p : nullptr;
 	a.ovBodySlot = stagedOverflow ? s->ovBodySlot.p : nullptr;
@@ -3589,6 +3741,23 @@ extern "C" float s2b_last_solve_kernel_ms(s2bWorld* w)
 	return ms;
 }
 
+extern "C" int s2b_download_neighbour_blocks(s2bWorld* w, int32_t* table, int maxBlocks)
+{
+	S2B_CHECK(cudaSetDevice(w->device));
+	SolverScratch* s = s2bGetSolverScratch(w);
+	S2B_CHECK(cudaStreamSynchronize(w->stream));
+	int blocks = 0;
+	if (s->counts.p != nullptr)
+	{
+		S2B_CHECK(cudaMemcpy(&blocks, s->counts.p + CNT_NSYNC, sizeof(int), cudaMemcpyDeviceToHost));
+	}
+	if (blocks > 0 && table != nullptr && maxBlocks >= blocks)
+	{
+		S2B_CHECK(cudaMemcpy(table, s->nsyncNbr.p, sizeof(int) * (size_t)blocks * S2B_NSYNC_STRIDE, cudaMemcpyDeviceToHost));
+	}
+	return blocks;
+}
+
 extern "C" int s2b_download_solve_order(s2bWorld* w, int32_t* items, int maxItems, int32_t* groupSizes, int maxGroups,
 										int32_t* groupCount)
 {
@@ -3744,6 +3913,7 @@ extern "C" void s2b_get_counters(s2bWorld* w, s2bCounters* out)
 		out->cutCount = w->scratch->regions > 0 ? counts[CNT_CUT] : 0;
 		out->regionCount = counts[CNT_REGIONS_ON] != 0 ? w->scratch->regions : 0;
 		out->overflowCount = counts[CNT_OVERFLOW_C] + counts[CNT_OVERFLOW_J];
+		out->neighbourSync = counts[CNT_NSYNC];
 		if (w->scratch->kempeState.p != nullptr)
 		{
 			int ks[4];

@@ -38,8 +38,27 @@ enum
 	CNT_RESIDENT = 22,	 // 1: every region runs out of shared memory (persistent.cuh, "resident regions"); decided by s2bFinishGroups
 	CNT_CUT_ABORT = 20,	// the cut colouring gave up: it needs more colours than regions are worth
 	CNT_BOUNDS = 16,	// 4 slots: order-preserving keys of max x, max -x, max y, max -y over the bodies' centres
+	CNT_NSYNC = 23,		// grid the neighbour tables were built for: device-wide colour steps wait for neighbouring blocks only; 0 = off
 	CNT_SIZE = 32
 };
+
+// Device-wide group steps: block b runs items [b * share, (b + 1) * share) of a group of n items (its joints, then its
+// contacts). Every block gets work and a warp's rows stay contiguous (coalesced column loads). The neighbour tables
+// (solver.cu, s2bItemBlockKernel) are built from the same mapping.
+__host__ __device__ __forceinline__ int s2bGroupShare(int n, int blocks)
+{
+	return ((n + blocks - 1) / blocks + 31) & ~31;
+}
+
+// neighbour-synchronised colour steps (persistent.cuh): per block, the number of its neighbours, then up to S2B_NSYNC_K ids
+#define S2B_NSYNC_K 16
+#define S2B_NSYNC_STRIDE (S2B_NSYNC_K + 1)
+// distinct blocks one body's constraints may be spread over before the mode gives up (a hub)
+#define S2B_NSYNC_BODY_BLOCKS 8
+// SolveArgs::barrier layout: [64 + 32 b] = epoch of block b (one 128-byte line each), [33] = epoch at the next launch's start
+#define S2B_EPOCH_BASE_WORD 33
+#define S2B_EPOCH_WORD(b) (64 + 32 * (b))
+#define S2B_BARRIER_WORDS S2B_EPOCH_WORD(512)
 
 struct SolveArgs
 {
@@ -61,7 +80,9 @@ struct SolveArgs
 	const int* jRegOff;		 // regions x (S2B_MAX_COLORS + 1): joint-constraint stream offsets of (region, colour)
 	const int* cRegOff;		 // same for contact constraints
 	const int* bodyLocal;	 // per body: its position in its region's slice of regBodies (resident regions); null: not offered
-	unsigned* barrier;		 // [0] monotonic arrival counter of the grid barrier, [32] its value at the start of the next launch
+	unsigned* barrier;		 // [0] monotonic arrival counter of the grid barrier, [32] its value at the start of the next launch;
+							 // epochs of the neighbour-synchronised colour steps: S2B_EPOCH_WORD(b), S2B_EPOCH_BASE_WORD
+	const int* nsyncNbr;	 // per block: S2B_NSYNC_STRIDE entries, neighbour count then neighbour blocks (used when CNT_NSYNC == grid)
 	// serial overflow group on a shared-memory copy of its bodies (persistent.cuh): the distinct bodies its constraints touch
 	const int* ovBodies;	 // [0] count, then body slots (null: walk in global memory)
 	const int* ovBodySlot;	 // per body: position in that list, or -1
@@ -141,6 +162,9 @@ struct SolverScratch
 	DevArray<int> heavyBodies;
 	DevArray<int> longBodies;			// [0] count, then bodies whose incidence list is sorted by a whole block
 	DevArray<int> ovBodies, ovBodySlot; // bodies of the serial overflow group (SolveArgs::ovBodies)
+	DevArray<int> itemBlock;			// per item: block that runs it in its device-wide colour step (-1: overflow group)
+	DevArray<unsigned> nsyncBits;		// grid x words block adjacency bits, + 1 word: "the mode cannot be used"
+	DevArray<int> nsyncNbr;				// SolveArgs::nsyncNbr
 	DevArray<int2> flow;	  // cFlowA | cFlowB | jFlowA | jFlowB
 	DevArray<int> bodyTicket; // + 1 int error flag at the end
 	int flowErrorOffset = 0;

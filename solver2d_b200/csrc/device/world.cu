@@ -403,6 +403,11 @@ extern "C" s2bWorld* s2b_world_create(int cudaDevice, int solverType)
 		{
 			w->dataflow = atoi(env) != 0 ? 1 : 0;
 		}
+		env = getenv("S2B_NEIGHBOUR_SYNC");
+		if (env != nullptr)
+		{
+			w->neighbourSync = atoi(env) != 0 ? 1 : 0;
+		}
 	}
 	w->solverType = solverType;
 	w->sticky = (solverType == 6); // s2_solverTGS_Sticky

@@ -60,7 +60,8 @@ class Counters(C.Structure):
                 ("groupCount", C.c_int32), ("overflowCount", C.c_int32), ("treeHeight", C.c_int32),
                 ("movedCount", C.c_int32), ("pairPassCount", C.c_int32), ("kernelLaunches", C.c_int32),
                 ("graphReplays", C.c_int32), ("graphCaptures", C.c_int32), ("scratchBytes", C.c_int64),
-                ("regionCount", C.c_int32), ("cutCount", C.c_int32), ("cutGroupCount", C.c_int32), ("recolouredCount", C.c_int32)]
+                ("regionCount", C.c_int32), ("cutCount", C.c_int32), ("cutGroupCount", C.c_int32), ("recolouredCount", C.c_int32),
+                ("neighbourSync", C.c_int32)]
 
 
 SCHEDULE_COLOR, SCHEDULE_WAVEFRONT = 0, 1
@@ -81,8 +82,9 @@ ABI_SYMBOLS = [
     "s2b_download_solve_order", "s2b_download_islands", "s2b_prefetch_pairs", "s2b_get_counters", "s2b_pack_body_state", "s2b_timed_steps", "s2b_last_stage_ms",
     "s2b_flush_l2", "s2b_time_color_kernel", "s2b_version", "s2b_abi_sizes", "s2b_upload_forces", "s2b_host_alloc",
     "s2b_host_free", "s2b_sync_body_state", "s2b_set_warm_gather", "s2b_eval_atan2", "s2b_set_dataflow", "s2b_set_regions", "s2b_set_graph", "s2b_get_stream", "s2b_add_forces", "s2b_download_transforms",
-    "s2b_set_restitution",
+    "s2b_set_restitution", "s2b_download_neighbour_blocks",
 ]
+NSYNC_STRIDE = 17  # entries per block of s2b_download_neighbour_blocks
 
 
 def make_context(solver: str, dt: float, vel_iters: int, pos_iters: int, warm_start: bool = True) -> StepContext:
@@ -140,6 +142,8 @@ class Device:
         L.s2b_download_contacts.argtypes = [vp, vp, C.c_int]
         L.s2b_download_solve_order.restype = C.c_int
         L.s2b_download_solve_order.argtypes = [vp, vp, C.c_int, vp, C.c_int, vp]
+        L.s2b_download_neighbour_blocks.restype = C.c_int
+        L.s2b_download_neighbour_blocks.argtypes = [vp, vp, C.c_int]
         L.s2b_get_counters.argtypes = [vp, C.POINTER(Counters)]
         L.s2b_pack_body_state.argtypes = [vp, C.c_int, C.c_int, vp]
         L.s2b_timed_steps.restype = C.c_float
@@ -314,6 +318,14 @@ class DeviceWorld:
         n = self.L.s2b_download_solve_order(self.h, items.ctypes.data, max_items, sizes.ctypes.data, max_groups,
                                             C.byref(groups))
         return items[:n], sizes[:groups.value]
+
+    def neighbour_blocks(self):
+        """Neighbour lists of the colour steps' blocks ([] when every colour step takes the grid barrier)."""
+        blocks = self.L.s2b_download_neighbour_blocks(self.h, None, 0)
+        table = np.zeros(max(blocks, 1) * NSYNC_STRIDE, dtype=np.int32)
+        self.L.s2b_download_neighbour_blocks(self.h, table.ctypes.data, blocks)
+        rows = table.reshape(-1, NSYNC_STRIDE)[:blocks]
+        return [row[1:1 + row[0]].tolist() for row in rows]
 
     def counters(self) -> Counters:
         c = Counters()

@@ -36,8 +36,10 @@ agg = {}
 for c, d in zip(code[1:], dt):
     kind = int(c) >> 8
     # an interval ends at a grid barrier and is labelled with the LAST phase before it (region-local phases that ran since
-    # the previous barrier are inside the same interval); bit 7: device-wide step (cut colour), bits 7+6: overflow group
-    key = (names.get(kind & 0x3F, "?") + ("/cut" if (kind & 0xC0) == 0x80 else "/ovf" if (kind & 0xC0) == 0xC0 else ""), int(c) & 0xFF)
+    # the previous barrier are inside the same interval); bit 7: device-wide step (cut colour), bits 7+6: overflow group,
+    # bit 6 alone: a neighbour-synchronised colour step (the interval ends at block 0's neighbour wait, not at a grid barrier)
+    tag = {0x80: "/cut", 0xC0: "/ovf", 0x40: "/nbr"}.get(kind & 0xC0, "")
+    key = (names.get(kind & 0x3F, "?") + tag, int(c) & 0xFF)
     agg.setdefault(key, []).append(int(d))
 print("stamps", n, "total us", (ns[-1] - ns[0]) / 1e3)
 for key, v in sorted(agg.items(), key=lambda kv: -sum(kv[1])):
@@ -45,4 +47,4 @@ for key, v in sorted(agg.items(), key=lambda kv: -sum(kv[1])):
 print("sequence (us):", [round(float(d) / 1e3, 2) for d in dt[:60]])
 c = dw.counters()
 print("constraints", c.constraintCount, "colours", c.groupCount, "overflow", c.overflowCount, "regions", c.regionCount, "cut", c.cutCount,
-      "cut colours", c.cutGroupCount, "recoloured", c.recolouredCount, "stage ms", dw.stage_ms(), "kernel ms", dev.lib.s2b_last_solve_kernel_ms(dw.h) if hasattr(dev.lib, "s2b_last_solve_kernel_ms") else None)
+      "cut colours", c.cutGroupCount, "recoloured", c.recolouredCount, "neighbour-synced blocks", c.neighbourSync, "stage ms", dw.stage_ms(), "kernel ms", dev.lib.s2b_last_solve_kernel_ms(dw.h) if hasattr(dev.lib, "s2b_last_solve_kernel_ms") else None)
