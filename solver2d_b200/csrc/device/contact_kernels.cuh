@@ -394,7 +394,7 @@ struct ContactStream
 	float4 la0, la1, pm0, pm1;
 	float2 l0, l1;
 	int slot; // contact slot of the row (only loaded by the sweep that also stores the impulses to the manifold)
-	int last; // ConstraintView::lastTouch bits (only loaded by a bias sweep that also integrates positions)
+	int last; // ConstraintView::lastTouch marks (only loaded by a bias sweep that also integrates positions)
 };
 
 __device__ __forceinline__ ContactStream s2bLoadContactStream(const SolveArgs& a, int t, bool withSlot = false)
@@ -586,13 +586,13 @@ __device__ __forceinline__ void s2bSolveContactTgsSoftStream(const SolveArgs& a,
 	// touch: the same arithmetic on the values just stored as s2bIntegratePosition applies after a device-wide barrier
 	// (cs.last is only ever non-zero in a bias sweep of the persistent kernel that folds the position pass; marked bodies
 	// are movable, hence valid and not static)
-	if (cs.last & 1)
+	if (cs.last & S2B_TOUCH_LAST_A)
 	{
 		s2Vec2 dp = s2MulAdd(dcA, a.ctx.h, vA);
 		s2Rot q = s2IntegrateRot(qA, a.ctx.h * wA);
 		poseRows[ia] = make_float4(dp.x, dp.y, q.s, q.c);
 	}
-	if (cs.last & 2)
+	if (cs.last & S2B_TOUCH_LAST_B)
 	{
 		s2Vec2 dp = s2MulAdd(dcB, a.ctx.h, vB);
 		s2Rot q = s2IntegrateRot(qB, a.ctx.h * wB);

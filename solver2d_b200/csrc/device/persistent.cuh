@@ -186,6 +186,8 @@ struct S2bLaunchInfo
 	bool regions;
 	bool neighbours;	// device-wide colour steps are neighbour-synchronised (grid-uniform)
 	bool foldPositions; // TGS_Soft: the bias sweep integrates positions (ConstraintView::lastTouch), the body pass is skipped
+	bool firstTouch;	// TGS_Soft, with foldPositions: the bias sweep also warm-starts velocities (S2B_TOUCH_FIRST_*), the
+						// warm-start body pass is skipped and finalize sub-steps the bodies without constraints
 	bool resident;		// TGS_Soft: the region's velocity / pose rows live in shared memory for the whole launch
 };
 
@@ -232,6 +234,11 @@ template <int SOLVER> __device__ __forceinline__ void s2bBodyPass(int bodyOp, co
 		int stride = gridDim.x * blockDim.x;
 		for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < a.bodies.capacity; i += stride)
 		{
+			if (SOLVER == 7 && li.firstTouch && bodyOp == BOP_FINALIZE_POSITIONS)
+			{
+				// (no warm-start pass ran: the sub-steps of a body without constraints are still owed)
+				s2bSubstepFreeBody(a, i, a.ctx.h, a.ctx.iterations);
+			}
 			s2bRunBodyOpT<SOLVER>(bodyOp, a, i);
 		}
 	}
@@ -551,12 +558,22 @@ __device__ __forceinline__ void s2bGroupPass(int jointOp, int contactOp, const S
 			bool store = contactOp == COP_TGS_SOFT_RELAX_STORE;
 			bool bias = contactOp == COP_TGS_SOFT_BIAS;
 			bool fold = bias && li.foldPositions;
+			// first-touch warm start: the marked bodies of a row are gathered right before its solve (warm_gather.cuh)
+			int firstMarks = bias && li.firstTouch ? S2B_TOUCH_FIRST_A | S2B_TOUCH_FIRST_B : 0;
 			int t = cBegin + u - njAll;
 			ContactStream cs;
 			if (mine)
 			{
 				cs = s2bLoadContactStream(a, t, store);
 				cs.last = fold ? a.cc.lastTouch[t] : 0;
+				if (cs.last & firstMarks & S2B_TOUCH_FIRST_A)
+				{
+					s2bFirstTouchPrefetch(a, cs.idx.x);
+				}
+				if (cs.last & firstMarks & S2B_TOUCH_FIRST_B)
+				{
+					s2bFirstTouchPrefetch(a, cs.idx.y & S2B_CF_INDEX_MASK);
+				}
 			}
 			if (sync.pending == S2B_PENDING_NEIGHBOURS)
 			{
@@ -569,6 +586,15 @@ __device__ __forceinline__ void s2bGroupPass(int jointOp, int contactOp, const S
 			bool writeWarm = bias ? a.ctx.extraIterations == 0 : true;
 			if (mine)
 			{
+				if (cs.last & firstMarks)
+				{
+					// (the row is fetched again after the gather instead of being held through it: holding it spilled. The
+					// solve's body loads wait for the fetched indices, one L2 round trip more on a marked row)
+					int last = cs.last;
+					s2bFirstTouchWarm(a, cs.idx, last);
+					cs = s2bLoadContactStream(a, t, store);
+					cs.last = last;
+				}
 				s2bSolveContactTgsSoftStream(a, t, cs, a.ctx.inv_h, bias, writeWarm, store);
 			}
 			for (u += blockDim.x; u < uEnd; u += blockDim.x)
@@ -576,8 +602,13 @@ __device__ __forceinline__ void s2bGroupPass(int jointOp, int contactOp, const S
 				t = cBegin + u - njAll;
 				if (u >= njAll)
 				{
+					int last = fold ? a.cc.lastTouch[t] : 0;
+					if (last & firstMarks)
+					{
+						s2bFirstTouchWarm(a, a.cc.idx[t], last);
+					}
 					ContactStream more = s2bLoadContactStream(a, t, store);
-					more.last = fold ? a.cc.lastTouch[t] : 0;
+					more.last = last;
 					s2bSolveContactTgsSoftStream(a, t, more, a.ctx.inv_h, bias, writeWarm, store);
 				}
 			}
@@ -899,6 +930,11 @@ template <int SOLVER> __global__ void __launch_bounds__(S2B_BLOCK, SOLVER == S2B
 	// every bias step runs through the branch below that looks at the marks); all of it is grid-uniform
 	li.foldPositions = SOLVER == 7 && a.cc.lastTouch != nullptr && li.regions == false && li.nJ == 0 && li.ovC + li.ovJ == 0 &&
 					   (a.heavyBodies == nullptr || a.heavyBodies[0] == 0) && a.bodyTicket == nullptr && li.nC > 0;
+	// the warm-start gather folded into the same sweep, at each body's first constraint: wherever positions are folded, unless a
+	// constraint reads a kinematic body. Such a body has no incidence list (s2bItemEndpoints) and only the warm-start pass
+	// integrates its pose every sub-step (alsoPosition), so that pass stays. (A program with the fold always warm-starts:
+	// lastTouch is only handed over with the gather on.)
+	li.firstTouch = li.foldPositions && a.counts[CNT_KINEMATIC_ITEMS] == 0;
 	li.resident = SOLVER == 7 && li.regions && a.bodyLocal != nullptr && a.counts[CNT_RESIDENT] != 0 && a.bodyTicket == nullptr;
 	li.bodyBegin = li.bodyEnd = 0;
 	if (li.regions)
@@ -980,7 +1016,12 @@ template <int SOLVER> __global__ void __launch_bounds__(S2B_BLOCK, SOLVER == S2B
 				}
 				else if (pass.kind == PASS_BODY && li.foldPositions && pass.bodyOp == BOP_INTEGRATE_POSITIONS)
 				{
-					// done by the bias sweep before it (and by the velocity pass for bodies without constraints)
+					// done by the bias sweep before it (and for bodies without constraints by the velocity pass, or by finalize)
+				}
+				else if (pass.kind == PASS_BODY && li.firstTouch && pass.bodyOp == BOP_INTEGRATE_VELOCITIES_WARM)
+				{
+					// done by the bias sweep after it (and for bodies without constraints by finalize): the previous sweep's last
+					// colour step flows into the bias sweep's first one through a neighbour wait
 				}
 				else if (pass.kind == PASS_BODY)
 				{

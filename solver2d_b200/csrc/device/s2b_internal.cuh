@@ -215,14 +215,22 @@ struct ConstraintView
 	// prepare-time world anchors for SoftStep). Null when the variant does not gather.
 	float4* warmP;
 	float4* warmAnchor;
-	// per constraint: bit 0 / bit 1 = this constraint is the LAST one of the solve order that touches its body A / B. The
-	// TGS_Soft bias sweep then integrates that body's position itself (s2IntegratePositions folded into the sweep, one
-	// device-wide step less per sub-step; persistent.cuh). Null: positions are integrated by their own body pass.
+	// per constraint, the touch marks: bit 0 / bit 1 = this constraint is the LAST one of the solve order that touches its
+	// body A / B, bit 2 / bit 3 = it is the FIRST one (S2B_TOUCH_*). The TGS_Soft bias sweep then integrates a last-touched
+	// body's position itself (s2IntegratePositions folded into the sweep) and warm-starts a first-touched body's velocity
+	// itself (the warm-start gather folded into the sweep), one device-wide body pass less each per sub-step (persistent.cuh).
+	// Null: positions are integrated and velocities gathered by their own body passes.
 	const int* lastTouch;
 	// sticky extras
 	float4* fanchor[2]; // COM-relative local friction anchors A.xy B.xy
 	float2* tsep[2];	// tangentSeparation, spare
 };
+
+// ConstraintView::lastTouch bits
+#define S2B_TOUCH_LAST_A 1
+#define S2B_TOUCH_LAST_B 2
+#define S2B_TOUCH_FIRST_A 4
+#define S2B_TOUCH_FIRST_B 8
 
 #define S2B_CF_TWO_POINTS 0x40000000
 #define S2B_CF_STATIC_SOFT 0x80000000u

@@ -197,7 +197,7 @@ __global__ void s2bFlagActive(ContactView contacts, int contactCount, JointView 
 // Conflict endpoints of every item (joints first, then contacts, both in natural order): a body index if the
 // constraint can change that body's velocity/position, else -1 (SURVEY §7 H3: static and kinematic bodies are
 // excluded from conflict detection and from write-back).
-__global__ void s2bItemEndpoints(const int* counts, const int* jointSlots, const int* activeSlots, JointView joints,
+__global__ void s2bItemEndpoints(int* counts, const int* jointSlots, const int* activeSlots, JointView joints,
 								 ContactView contacts, BodyView bodies, int2* itemBodies, int* degree)
 {
 	int nJ = counts[CNT_JOINTS], nC = counts[CNT_CONTACTS];
@@ -239,6 +239,11 @@ __global__ void s2bItemEndpoints(const int* counts, const int* jointSlots, const
 	if (a == b && a >= 0)
 	{
 		b = -1;
+	}
+	if (a == -2 || b == -2)
+	{
+		// the persistent kernel keeps the TGS_Soft warm-start body pass then: it integrates the pose this constraint reads
+		atomicAdd(counts + CNT_KINEMATIC_ITEMS, 1);
 	}
 	itemBodies[i] = make_int2(a, b);
 	if (degree != nullptr)
@@ -2079,10 +2084,11 @@ __global__ void __launch_bounds__(256) s2bSortLongIncidenceKernel(const int* lon
 	}
 }
 
-// ConstraintView::lastTouch from the sorted incidence lists: the last entry of a body's list is the last constraint of the
-// solve order that touches it. Bit 2 marks a constraint row as such for side A (bit 0) / B (bit 1); a body whose last
-// toucher is a joint gets no mark at all (the persistent kernel only folds when there are no joints).
-__global__ void s2bLastTouchKernel(int bodyCapacity, const int* incStart, const int* incList, int* lastTouch)
+// The touch marks of ConstraintView::lastTouch from the sorted incidence lists: the last entry of a body's list is the last
+// constraint of the solve order that touches it (S2B_TOUCH_LAST_A / _B on that row, by the body's side), the first entry
+// the first one (S2B_TOUCH_FIRST_A / _B). A body whose first or last toucher is a joint gets no such mark (the persistent
+// kernel only uses the marks when there are no joints).
+__global__ void s2bTouchMarksKernel(int bodyCapacity, const int* incStart, const int* incList, int* touchMarks)
 {
 	int i = blockIdx.x * blockDim.x + threadIdx.x;
 	if (i >= bodyCapacity)
@@ -2095,7 +2101,12 @@ __global__ void s2bLastTouchKernel(int bodyCapacity, const int* incStart, const 
 		int e = incList[end - 1];
 		if (e & S2B_INC_CONTACT)
 		{
-			atomicOr(lastTouch + (e >> 2), (e & S2B_INC_SIDE_B) ? 2 : 1);
+			atomicOr(touchMarks + (e >> 2), (e & S2B_INC_SIDE_B) ? S2B_TOUCH_LAST_B : S2B_TOUCH_LAST_A);
+		}
+		e = incList[begin];
+		if (e & S2B_INC_CONTACT)
+		{
+			atomicOr(touchMarks + (e >> 2), (e & S2B_INC_SIDE_B) ? S2B_TOUCH_FIRST_B : S2B_TOUCH_FIRST_A);
 		}
 	}
 }
@@ -3298,7 +3309,7 @@ static void enqueueSchedule(s2bWorld* w, SolverScratch* s, SolvePlan& pl)
 			if (contactCount > 0)
 			{
 				S2B_CHECK(cudaMemsetAsync(s->lastTouch.p, 0, sizeof(int) * (size_t)contactCount, st));
-				S2B_LAUNCH(w, s2bLastTouchKernel, gridFor(bodyCap, 256), 256, 0, bodyCap, s->adjStart.p, s->incList.p, s->lastTouch.p);
+				S2B_LAUNCH(w, s2bTouchMarksKernel, gridFor(bodyCap, 256), 256, 0, bodyCap, s->adjStart.p, s->incList.p, s->lastTouch.p);
 			}
 		}
 	}

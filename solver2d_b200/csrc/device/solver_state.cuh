@@ -39,6 +39,7 @@ enum
 	CNT_CUT_ABORT = 20,	// the cut colouring gave up: it needs more colours than regions are worth
 	CNT_BOUNDS = 16,	// 4 slots: order-preserving keys of max x, max -x, max y, max -y over the bodies' centres
 	CNT_NSYNC = 23,		// grid the neighbour tables were built for: device-wide colour steps wait for neighbouring blocks only; 0 = off
+	CNT_KINEMATIC_ITEMS = 24, // constraints with an endpoint no constraint moves but whose pose changes (kinematic, s2bItemEndpoints -2)
 	CNT_SIZE = 32
 };
 

@@ -170,7 +170,8 @@ __device__ __forceinline__ void s2bGatherFour(const SolveArgs& a, const int (&e)
 // FIXED = true : prepare-time anchors (s2WarmStartContacts_Fixed, reference src/solve_soft_step.c:16-63)
 // alsoPosition: the bias sweep integrates the positions of the bodies it touches (ConstraintView::lastTouch); a body
 // without any constraint is touched by nobody, so its position is integrated here, right after its velocity (nothing in
-// between changes either)
+// between changes either). Only where this pass still runs beside the folded position integration: when a constraint reads
+// a kinematic body (persistent.cuh, S2bLaunchInfo::firstTouch); otherwise the finalize pass sub-steps such bodies.
 // velOut: where the new velocity goes (the region's shared-memory copy in a resident launch); null = the body's row
 template <bool FIXED>
 __device__ __forceinline__ void s2bIntegrateVelocityWarmHead(const SolveArgs& a, int i, float h, const GatherHead& hd, bool alsoPosition = false,
@@ -251,6 +252,59 @@ __device__ __forceinline__ void s2bIntegrateVelocityWarmHead(const SolveArgs& a,
 template <bool FIXED> __device__ __forceinline__ void s2bIntegrateVelocityWarm(const SolveArgs& a, int i, float h)
 {
 	s2bIntegrateVelocityWarmHead<FIXED>(a, i, h, s2bLoadGatherHead(a, i));
+}
+
+// ---- first-touch warm start (TGS_Soft, persistent.cuh) -----------------------------------------------------------------
+// The warm start of a body reads its own row, its rotation and the warm rows of its constraints. Between the end of a
+// sub-step's last sweep and the body's FIRST constraint in the next bias sweep none of them changes, so the thread that
+// solves that constraint runs the gather of the body right before the solve (S2B_TOUCH_FIRST_* marks), with the same
+// operations in the same order as the body pass, instead of a device-wide body pass before the sweep.
+
+// before the colour step's wait: the read-only part of the marked bodies' heads into L2 (an L1 prefetch would be lost: the
+// acquire of the wait invalidates L1)
+__device__ __forceinline__ void s2bPrefetchL2(const void* ptr)
+{
+	asm volatile("prefetch.global.L2 [%0];" ::"l"(ptr));
+}
+
+__device__ __forceinline__ void s2bFirstTouchPrefetch(const SolveArgs& a, int i)
+{
+	s2bPrefetchL2(a.bodies.flags + i);
+	s2bPrefetchL2(a.bodies.prm + i);
+	s2bPrefetchL2(a.bodies.frc + i);
+	s2bPrefetchL2(a.incStart + i);
+}
+
+// after the wait, before the solve: s2IntegrateVelocities + the gathered warm start of the marked bodies, one after the other
+// (one inlined copy of the gather; two heads held at once spilled)
+__device__ __forceinline__ void s2bFirstTouchWarm(const SolveArgs& a, int2 idx, int marks)
+{
+#pragma unroll 1
+	for (int side = 0; side < 2; ++side)
+	{
+		if (marks & (side == 0 ? S2B_TOUCH_FIRST_A : S2B_TOUCH_FIRST_B))
+		{
+			int i = side == 0 ? idx.x : idx.y & S2B_CF_INDEX_MASK;
+			s2bIntegrateVelocityWarmHead<false>(a, i, a.ctx.h, s2bLoadGatherHead(a, i));
+		}
+	}
+}
+
+// A body no constraint touches, in a launch whose bias sweeps warm-start at the first touch: nothing in the launch reads it,
+// so the finalize pass runs all its sub-steps at once — s2IntegrateVelocities, then s2IntegratePositions, `substeps` times:
+// the operations the per-sub-step body passes applied to it, in their order.
+__device__ __forceinline__ void s2bSubstepFreeBody(const SolveArgs& a, int i, float h, int substeps)
+{
+	unsigned f = a.bodies.flags[i];
+	if ((f & S2B_BODY_VALID) == 0 || S2B_BODY_TYPE(f) == S2B_BODY_STATIC || a.incStart[i] != a.incStart[i + 1])
+	{
+		return;
+	}
+	for (int s = 0; s < substeps; ++s)
+	{
+		s2bIntegrateVelocityWarm<false>(a, i, h); // (an empty incidence list: the velocity part only)
+		s2bIntegratePosition(a, i, h);
+	}
 }
 
 // the body pass of the persistent kernel without regions: every body slot, grid-stride, the next body's head loaded ahead
