@@ -34,6 +34,10 @@ typedef struct s2bWorld s2bWorld;
 // body rows only: the slot already holds this body on the device, so the row's force / torque are ADDED to what the device
 // accumulated since the last step (bulk forces) instead of replacing it
 #define S2B_BODY_ADD_FORCE 0x8
+// body rows only: the body was moved by s2Body_SetTransform. A row with S2B_BODY_ADD_FORCE and without this flag keeps the
+// body's delta position on the device (XPBD leaves a kinematic body's growing from step to step, DESIGN.md §3.8); any
+// other row starts the body at zero
+#define S2B_BODY_TELEPORT 0x10
 
 // One rigid body; mirrors the solver-relevant fields of s2Body (reference src/body.h:16-76).
 typedef struct s2bBodyRow
@@ -296,6 +300,9 @@ S2B_API void* s2b_get_stream(s2bWorld* world);
 S2B_API void s2b_download_bodies(s2bWorld* world, s2bBodyRow* rows, int count);
 // every slot 0..capacity-1 in order
 S2B_API void s2b_download_all_bodies(s2bWorld* world, s2bBodyRow* rows, int capacity);
+// delta position of body slots [0, capacity): 2 floats (x, y) per slot. Zero between steps for every body but a kinematic one
+// under XPBD.
+S2B_API void s2b_download_delta_positions(s2bWorld* world, float* xy, int capacity);
 // The lazy read-back behind s2Body_GetPosition & co: 12 floats per body slot {origin.xy, position.xy, rot.sc, v.xy, w,
 // force.xy, torque} gathered on the device and copied into a pinned buffer owned by the world. The pointer stays valid
 // until the next call. Synchronises.

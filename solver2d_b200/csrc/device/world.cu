@@ -29,7 +29,11 @@ __global__ void s2bScatterBodies(const s2bBodyRow* __restrict__ rows, int count,
 		}
 	}
 	b.vel[i] = make_float4(r.linearVelocity[0], r.linearVelocity[1], r.angularVelocity, r.invMass);
-	b.pose[i] = make_float4(0.0f, 0.0f, r.rot[0], r.rot[1]);
+	// a body the device already holds keeps its delta position (reference src/body.c:337-350 set only the velocity; XPBD
+	// carries a kinematic body's from step to step); a new body, a reused slot or a teleported body starts at zero
+	bool keepDelta = (r.flags & (S2B_BODY_ADD_FORCE | S2B_BODY_TELEPORT)) == S2B_BODY_ADD_FORCE;
+	float4 pose = b.pose[i];
+	b.pose[i] = make_float4(keepDelta ? pose.x : 0.0f, keepDelta ? pose.y : 0.0f, r.rot[0], r.rot[1]);
 	b.pos[i] = make_float4(r.position[0], r.position[1], r.invI, r.I);
 	b.org[i] = make_float4(r.origin[0], r.origin[1], r.localCenter[0], r.localCenter[1]);
 	if (r.flags & S2B_BODY_ADD_FORCE)
@@ -992,6 +996,36 @@ extern "C" void s2b_download_all_bodies(s2bWorld* w, s2bBodyRow* rows, int capac
 	S2B_CHECK(cudaMallocAsync((void**)&d, sizeof(s2bBodyRow) * (size_t)capacity, w->stream));
 	S2B_LAUNCH(w, s2bGatherBodies, gridFor(capacity, 128), 128, 0, d, capacity, bodyView(w), 0);
 	S2B_CHECK(cudaMemcpyAsync(rows, d, sizeof(s2bBodyRow) * (size_t)capacity, cudaMemcpyDeviceToHost, w->stream));
+	S2B_CHECK(cudaFreeAsync(d, w->stream));
+	S2B_CHECK(cudaStreamSynchronize(w->stream));
+}
+
+__global__ void s2bGatherDeltaPositions(float2* out, int count, BodyView b)
+{
+	int i = blockIdx.x * blockDim.x + threadIdx.x;
+	if (i < count)
+	{
+		float4 pose = b.pose[i];
+		out[i] = make_float2(pose.x, pose.y);
+	}
+}
+
+extern "C" void s2b_download_delta_positions(s2bWorld* w, float* xy, int capacity)
+{
+	S2B_CHECK(cudaSetDevice(w->device));
+	if (capacity > w->bodyCap)
+	{
+		memset(xy + 2 * (size_t)w->bodyCap, 0, sizeof(float2) * (size_t)(capacity - w->bodyCap));
+		capacity = w->bodyCap;
+	}
+	if (capacity <= 0)
+	{
+		return;
+	}
+	float2* d = nullptr;
+	S2B_CHECK(cudaMallocAsync((void**)&d, sizeof(float2) * (size_t)capacity, w->stream));
+	S2B_LAUNCH(w, s2bGatherDeltaPositions, gridFor(capacity, 128), 128, 0, d, capacity, bodyView(w));
+	S2B_CHECK(cudaMemcpyAsync(xy, d, sizeof(float2) * (size_t)capacity, cudaMemcpyDeviceToHost, w->stream));
 	S2B_CHECK(cudaFreeAsync(d, w->stream));
 	S2B_CHECK(cudaStreamSynchronize(w->stream));
 }

@@ -42,6 +42,7 @@ s2BodyId s2CreateBody(s2WorldId worldId, const s2BodyDef* def)
 	slot->jointCount = 0;
 	// device mirror: not there yet (rowDirty / forceDirty keep their value — a reused slot may already sit in the dirty list)
 	slot->onDevice = false;
+	slot->teleported = false;
 	s2MarkBodyDirty(world, slot);
 
 	return (s2BodyId){slot->object.index, worldId.index, slot->object.revision};
@@ -327,6 +328,8 @@ void s2Body_SetTransform(s2BodyId bodyId, s2Vec2 position, float angle)
 	body->origin = position;
 	body->rot = s2MakeRot(angle);
 	body->position = s2Add(s2RotateVector(body->rot, body->localCenter), body->origin);
+	// the body is placed exactly where asked: the delta position XPBD carries for a kinematic body goes (DESIGN.md §3.8)
+	body->teleported = true;
 	s2MarkBodyDirty(world, body);
 	s2Transform xf = {body->origin, body->rot};
 	for (int32_t si = body->shapeList; si != S2_NULL_INDEX;)

@@ -119,6 +119,7 @@ typedef struct s2Body
 	// dirty bookkeeping
 	bool rowDirty;	 // whole row must be re-uploaded
 	bool forceDirty; // only force / torque changed
+	bool teleported; // moved by s2Body_SetTransform since the last upload: the device resets its delta position
 	bool onDevice;	 // the device already holds a row for this body: uploads add its pending force instead of setting it
 } s2Body;
 

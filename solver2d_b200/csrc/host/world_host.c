@@ -150,7 +150,8 @@ static void* s2Staging(s2World* world, size_t bytes)
 static void s2FillBodyRow(s2bBodyRow* r, const s2Body* b)
 {
 	r->index = b->object.index;
-	r->flags = s2IsFree(&b->object) ? 0 : (S2B_ROW_VALID | ((int32_t)b->type << 1) | (b->onDevice ? S2B_BODY_ADD_FORCE : 0));
+	r->flags = s2IsFree(&b->object) ? 0 : (S2B_ROW_VALID | ((int32_t)b->type << 1) | (b->onDevice ? S2B_BODY_ADD_FORCE : 0) |
+											 (b->teleported ? S2B_BODY_TELEPORT : 0));
 	r->origin[0] = b->origin.x;
 	r->origin[1] = b->origin.y;
 	r->position[0] = b->position.x;
@@ -304,6 +305,7 @@ void s2FlushToDevice(s2World* world)
 			b->rowDirty = false;
 			b->forceDirty = false;
 			b->onDevice = s2IsFree(&b->object) == false;
+			b->teleported = false;
 			// the pending force now lives on the device, which zeroes it at the end of the step (reference src/world.c:275-276)
 			b->force = s2Vec2_zero;
 			b->torque = 0.0f;

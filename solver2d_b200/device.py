@@ -82,7 +82,7 @@ ABI_SYMBOLS = [
     "s2b_download_solve_order", "s2b_download_islands", "s2b_prefetch_pairs", "s2b_get_counters", "s2b_pack_body_state", "s2b_timed_steps", "s2b_last_stage_ms",
     "s2b_flush_l2", "s2b_time_color_kernel", "s2b_version", "s2b_abi_sizes", "s2b_upload_forces", "s2b_host_alloc",
     "s2b_host_free", "s2b_sync_body_state", "s2b_set_warm_gather", "s2b_eval_atan2", "s2b_set_dataflow", "s2b_set_regions", "s2b_set_graph", "s2b_get_stream", "s2b_add_forces", "s2b_download_transforms",
-    "s2b_set_restitution", "s2b_download_neighbour_blocks",
+    "s2b_set_restitution", "s2b_download_neighbour_blocks", "s2b_download_delta_positions",
 ]
 NSYNC_STRIDE = 17  # entries per block of s2b_download_neighbour_blocks
 
@@ -137,6 +137,7 @@ class Device:
         L.s2b_download_bodies.argtypes = [vp, vp, C.c_int]
         L.s2b_download_all_bodies.argtypes = [vp, vp, C.c_int]
         L.s2b_download_shape_boxes.argtypes = [vp, vp, vp, vp, C.c_int]
+        L.s2b_download_delta_positions.argtypes = [vp, vp, C.c_int]
         L.s2b_download_joints.argtypes = [vp, vp, C.c_int]
         L.s2b_download_contacts.restype = C.c_int
         L.s2b_download_contacts.argtypes = [vp, vp, C.c_int]
@@ -281,6 +282,13 @@ class DeviceWorld:
         rows = np.zeros(cap, dtype=BODY_ROW)
         self.L.s2b_download_all_bodies(self.h, rows.ctypes.data, cap)
         return rows
+
+    def download_delta_positions(self, capacity: int | None = None) -> np.ndarray:
+        """(capacity, 2) delta position of every body slot (read-only; not part of the body row)."""
+        cap = self.body_cap if capacity is None else capacity
+        out = np.zeros((cap, 2), dtype=np.float32)
+        self.L.s2b_download_delta_positions(self.h, out.ctypes.data, cap)
+        return out
 
     def download_joints(self, capacity: int | None = None) -> np.ndarray:
         cap = self.joint_cap if capacity is None else capacity

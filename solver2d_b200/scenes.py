@@ -15,6 +15,8 @@ Each recipe restates one of the reference's sample scenes or one of the syntheti
 * :func:`welded_structures` — cantilevers, welded assemblies, a welded platform rider and a chain (the weld joint).
 * :func:`sliders`         — pistons, an elevator, an inclined slider, a kinematic carriage, a slider-crank and a mouse
                             joint on a slider (the prismatic joint).
+* :func:`kinematic_rigs`  — piles on sliding kinematic platforms and a turntable, joints hanging from moving kinematic
+                            carriages (kinematic bodies under every solver variant).
 
 All scenes are deterministic lattices (no RNG). A recipe returns a :class:`Scene` holding the world id and the
 body ids in creation order.
@@ -772,6 +774,114 @@ def sliders(lib: capi.Solver2D, solver="TGS_Soft", copies=1, kinematic=True) -> 
             md.hertz = 3.0
             md.dampingRatio = 0.7
             sc.joints.append(lib.s2CreateMouseJoint(world, C.byref(md)))
+    return sc
+
+
+KINEMATIC_RIGS_PITCH = 24.0  # width of one platform of kinematic_rigs (m)
+
+
+def kinematic_rigs(lib: capi.Solver2D, solver="TGS_Soft", platforms=4, base_count=12, prismatic=True, turning=True) -> Scene:
+    """Kinematic bodies carrying dynamic ones, `platforms` side by side. Per platform:
+
+    * a kinematic platform sliding sideways (alternate platforms left and right), a pyramid of `base_count` boxes on it;
+    * a kinematic carriage above it, moving sideways and turning slowly, with a pendulum on a revolute joint (limits on), a
+      slider on a prismatic joint (limits and a weak motor) and a box on a second revolute joint (motor on).
+    Beside them a kinematic turntable turning at 0.25 rad/s with a small pyramid on it, and a mouse joint pulling the
+    first pendulum.
+
+    With `turning` False the carriages and the turntable keep their angle. On a library without s2CreatePrismaticJoint,
+    or with `prismatic` False on either library, each prismatic joint is a
+    revolute joint with limits and motor off (the stand-in of :func:`sliders`). ``sc.piles`` holds "kinematic" (the ids of
+    the kinematic bodies), "prismatic" / "prismatic_defs" / "prismatic_bodies" as :func:`sliders` does."""
+    world = lib.create_world(solver)
+    sc = Scene(lib, world, name=f"kinematic_rigs{platforms}")
+    sc.piles.update(kinematic=[], prismatic=[], prismatic_defs=[], prismatic_bodies=[])
+    has_prismatic = prismatic and "s2CreatePrismaticJoint" not in lib.missing
+    gid = _ground(lib, world, 0.5 * KINEMATIC_RIGS_PITCH * (platforms + 1) + 5.0, y=-12.0)
+    sc.bodies.append(gid)
+    sd = default_shape_def()
+    sd.density = 1.0
+    D, K = capi.DYNAMIC_BODY, capi.KINEMATIC_BODY
+
+    def body(kind, x, y, hx, hy, vx=0.0, w=0.0, angle=0.0):
+        bd = default_body_def()
+        bd.type = kind
+        bd.position = Vec2(x, y)
+        bd.angle = angle
+        bd.linearVelocity = Vec2(vx, 0.0)
+        bd.angularVelocity = w
+        bid = lib.s2CreateBody(world, C.byref(bd))
+        lib.s2CreatePolygonShape(bid, C.byref(sd), C.byref(lib.s2MakeBox(hx, hy)))
+        sc.bodies.append(bid)
+        if kind == K:
+            sc.piles["kinematic"].append(bid)
+        return bid
+
+    def pile(x0, y0, base, h=0.5):
+        for i in range(base):
+            for j in range(i, base):
+                body(D, x0 + (i + 1.0) * h + 2.0 * (j - i) * h - h * base, y0 + (2.0 * i + 1.0) * h, h, h)
+
+    def revolute(a, b, pivot, limit=None, motor=None):
+        jd = default_revolute_def()
+        jd.bodyIdA, jd.bodyIdB = a, b
+        jd.localAnchorA = lib.s2Body_GetLocalPoint(a, pivot)
+        jd.localAnchorB = lib.s2Body_GetLocalPoint(b, pivot)
+        if limit is not None:
+            jd.enableLimit = True
+            jd.lowerAngle, jd.upperAngle = limit
+        if motor is not None:
+            jd.enableMotor = True
+            jd.motorSpeed, jd.maxMotorTorque = motor
+        jid = lib.s2CreateRevoluteJoint(world, C.byref(jd))
+        sc.joints.append(jid)
+        return jid
+
+    def slider(a, b, pivot, axis, limit, motor):
+        d = dict(localAnchorA=tuple(lib.s2Body_GetLocalPoint(a, pivot)), localAnchorB=tuple(lib.s2Body_GetLocalPoint(b, pivot)),
+                 localAxisA=axis, referenceAngle=0.0, enableLimit=True, lowerTranslation=limit[0],
+                 upperTranslation=limit[1], enableMotor=True, motorSpeed=motor[0], maxMotorForce=motor[1],
+                 collideConnected=False)
+        if has_prismatic:
+            jd = capi.default_prismatic_def()
+            for name, value in d.items():
+                setattr(jd, name, Vec2(*value) if isinstance(value, tuple) else value)
+            create = lib.s2CreatePrismaticJoint
+        else:
+            jd = default_revolute_def()
+            jd.localAnchorA = Vec2(*d["localAnchorA"])
+            jd.localAnchorB = Vec2(*d["localAnchorB"])
+            create = lib.s2CreateRevoluteJoint
+        jd.bodyIdA, jd.bodyIdB = a, b
+        sc.piles["prismatic"].append(len(sc.joints))
+        sc.piles["prismatic_defs"].append(d)
+        sc.piles["prismatic_bodies"].append((a, b))
+        sc.joints.append(create(world, C.byref(jd)))
+
+    first = None
+    for k in range(platforms):
+        x0 = -0.5 * KINEMATIC_RIGS_PITCH * platforms + KINEMATIC_RIGS_PITCH * k
+        body(K, x0, -1.0, 0.5 * base_count + 1.5, 0.5, vx=0.6 if k % 2 == 0 else -0.4)
+        pile(x0, -0.5, base_count)
+        carriage = body(K, x0, base_count + 4.0, 3.0, 0.2, vx=0.5 if k % 2 == 0 else -0.5,
+                        w=(0.1 if k % 2 == 0 else -0.1) if turning else 0.0)
+        pendulum = body(D, x0 - 2.0, base_count + 2.5, 0.15, 0.75)
+        revolute(carriage, pendulum, Vec2(x0 - 2.0, base_count + 3.25), limit=(-0.6, 0.6))
+        rider = body(D, x0 + 0.5, base_count + 4.45, 0.25, 0.25)
+        slider(carriage, rider, Vec2(x0 + 0.5, base_count + 4.45), (1.0, 0.0), (-1.0, 1.0), (0.4, 3.0))
+        crank = body(D, x0 + 2.0, base_count + 3.0, 0.6, 0.1, angle=0.3)
+        revolute(carriage, crank, Vec2(x0 + 2.0, base_count + 3.8), motor=(1.5, 20.0))
+        first = pendulum if first is None else first
+    x0 = 0.5 * KINEMATIC_RIGS_PITCH * platforms + 2.0
+    body(K, x0, -1.0, 4.5, 0.5, w=0.25 if turning else 0.0)
+    pile(x0, -0.5, 6)
+    md = default_mouse_def()
+    md.bodyIdA, md.bodyIdB = gid, first
+    p = lib.s2Body_GetPosition(first)
+    md.target = Vec2(p.x + 1.5, p.y + 0.5)
+    md.hertz = 3.0
+    md.dampingRatio = 0.7
+    sc.joints.append(lib.s2CreateMouseJoint(world, C.byref(md)))
     return sc
 
 

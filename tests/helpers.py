@@ -136,6 +136,45 @@ def joint_rows_from_ref(jf: np.ndarray, ji: np.ndarray) -> np.ndarray:
     return rows
 
 
+def load_bodies_into_ref(R: refmod.Reference, wid, rows: np.ndarray):
+    """Device body rows -> the reference world's bodies (state fields only; mass data and flags are construction-time).
+    Dynamic bodies start the step with deltaPosition zero, as every finalize leaves them; the other bodies keep the
+    reference's own, which XPBD's finalize leaves growing for a kinematic body (ref_delta_positions)."""
+    F = refmod.BODY_F
+    bf, bi = R.bodies(wid)
+    n = min(len(rows), bf.shape[0])
+    valid = bi[:n, 0] == 1
+    for name, col, width in (("origin", F["origin"], 2), ("position", F["position"], 2), ("rot", F["rot"], 2),
+                             ("linearVelocity", F["v"], 2)):
+        bf[:n, col:col + width][valid] = rows[name][:n][valid]
+    bf[:n, F["w"]][valid] = rows["angularVelocity"][:n][valid]
+    dynamic = valid & (bi[:n, 1] == capi.DYNAMIC_BODY)
+    bf[:n, F["dp"]:F["dp"] + 2][dynamic] = 0.0
+    bf[:n, F["force"]:F["force"] + 2][valid] = rows["force"][:n][valid]
+    bf[:n, F["torque"]][valid] = rows["torque"][:n][valid]
+    R.load_body_state(wid, bf)
+
+
+def ref_delta_positions(R: refmod.Reference, wid) -> np.ndarray:
+    """(bodyCap, 2) deltaPosition of every body slot of a reference world."""
+    bf, _ = R.bodies(wid)
+    F = refmod.BODY_F
+    return np.ascontiguousarray(bf[:, F["dp"]:F["dp"] + 2])
+
+
+def store_oracle_bodies(R: refmod.Reference, wid, ob: np.ndarray, odp: np.ndarray):
+    """Advance the reference world's bodies with an oracle stage's result: pose, velocities and deltaPosition."""
+    F = refmod.BODY_F
+    bf, bi = R.bodies(wid)
+    valid = bi[:, 0] == 1
+    bf[:, F["position"]:F["position"] + 2][valid] = ob["position"][valid]
+    bf[:, F["rot"]:F["rot"] + 2][valid] = ob["rot"][valid]
+    bf[:, F["v"]:F["v"] + 2][valid] = ob["linearVelocity"][valid]
+    bf[:, F["w"]][valid] = ob["angularVelocity"][valid]
+    bf[:, F["dp"]:F["dp"] + 2][valid] = odp[valid]
+    R.load_body_state(wid, bf)
+
+
 def load_device_world_from_ref(dev: device.Device, R: refmod.Reference, wid, solver: str) -> device.DeviceWorld:
     """Mirror the current state of a reference world (bodies, joints, contacts in pool order) into a device world."""
     dw = dev.create_world(capi.SOLVER[solver])

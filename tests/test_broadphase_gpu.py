@@ -13,8 +13,9 @@ import pytest
 from oracle import port
 from oracle import ref as refmod
 from solver2d_b200 import capi, device, scenes
-from test_multistep_gpu import _load_bodies_into_ref, _run
-from helpers import contact_rows_from_ref, body_rows_from_ref, joint_rows_from_ref, bit_equal
+from test_multistep_gpu import _run
+from helpers import (contact_rows_from_ref, body_rows_from_ref, joint_rows_from_ref, bit_equal, load_bodies_into_ref,
+                     ref_delta_positions, store_oracle_bodies)
 
 pytestmark = pytest.mark.gpu
 DT = 1.0 / 60.0
@@ -191,7 +192,7 @@ def test_pair_table_shapes_destroyed_and_recreated(reference, product, dev):
             edits[step](sp)
             dev.lib.s2World_Flush(sp.world)
         cap = R.capacities(sr.world)["bodyCap"]
-        _load_bodies_into_ref(R, sr.world, dw.download_all_bodies(cap))
+        load_bodies_into_ref(R, sr.world, dw.download_all_bodies(cap))
         R.step_collide(sr.world)
         sp.step(DT, 4, 2, True)
 
@@ -210,14 +211,9 @@ def test_pair_table_shapes_destroyed_and_recreated(reference, product, dev):
         bodies = body_rows_from_ref(*R.bodies(sr.world))
         joints = joint_rows_from_ref(*R.joints(sr.world))
         order, _ = dw.solve_order(len(rows_key) + len(joints) + 16, max_groups=200000)
-        ob, oc, _ = O.solve(capi.SOLVER[solver], bodies, rows_key, joints, ctx, order=order)
-        bf, bi = R.bodies(sr.world)
-        valid = bi[:, 0] == 1
-        for name, col in (("position", F["position"]), ("rot", F["rot"]), ("linearVelocity", F["v"])):
-            bf[:, col:col + 2][valid] = ob[name][valid]
-        bf[:, F["w"]][valid] = ob["angularVelocity"][valid]
-        bf[:, F["dp"]:F["dp"] + 2][valid] = 0.0
-        R.load_body_state(sr.world, bf)
+        ob, oc, _, odp = O.solve(capi.SOLVER[solver], bodies, rows_key, joints, ctx, order=order,
+                                 dp=ref_delta_positions(R, sr.world))
+        store_oracle_bodies(R, sr.world, ob, odp)
         imp = np.zeros((cf.shape[0], 4), dtype=np.float32)
         imp[slots[perm], 0] = oc["points"]["normalImpulse"][:, 0]
         imp[slots[perm], 1] = oc["points"]["tangentImpulse"][:, 0]

@@ -19,7 +19,7 @@ import numpy as np
 import pytest
 
 from helpers import (STICKY_FIELDS, bit_equal, body_rows_from_ref, carry_sticky_friction, contact_rows_from_ref,
-                     joint_rows_from_ref)
+                     joint_rows_from_ref, load_bodies_into_ref, ref_delta_positions, store_oracle_bodies)
 from oracle import port
 from oracle import ref as refmod
 from solver2d_b200 import capi, device, scenes
@@ -33,22 +33,6 @@ def product():
     return capi.Solver2D(device.LIB_PATH)
 
 
-def _load_bodies_into_ref(R, wid, rows):
-    """Device body rows -> the reference world's bodies (state fields only; mass data and flags are construction-time)."""
-    F = refmod.BODY_F
-    bf, bi = R.bodies(wid)
-    n = min(len(rows), bf.shape[0])
-    valid = bi[:n, 0] == 1
-    for name, col, width in (("origin", F["origin"], 2), ("position", F["position"], 2), ("rot", F["rot"], 2),
-                             ("linearVelocity", F["v"], 2)):
-        bf[:n, col:col + width][valid] = rows[name][:n][valid]
-    bf[:n, F["w"]][valid] = rows["angularVelocity"][:n][valid]
-    bf[:n, F["dp"]:F["dp"] + 2][valid] = 0.0
-    bf[:n, F["force"]:F["force"] + 2][valid] = rows["force"][:n][valid]
-    bf[:n, F["torque"]][valid] = rows["torque"][:n][valid]
-    R.load_body_state(wid, bf)
-
-
 CONTACT_FIELDS = ("normal", "friction", "cacheCount", "cacheIndexA", "cacheIndexB", "cacheMetric")
 POINT_FIELDS = ("localAnchorA", "localAnchorB", "separation", "id", "persisted")
 
@@ -58,8 +42,12 @@ def _same(g, w):
     return bit_equal(g, w) if g.dtype == np.float32 else bool(np.array_equal(g, w))
 
 
-def _run(R, P, dev, recipe, solver, steps, vel, pos, kw, min_replays=0, setup=None, observe=None):
-    O = port.load()
+def _run(R, P, dev, recipe, solver, steps, vel, pos, kw, min_replays=0, setup=None, observe=None, oracle=None,
+         as_joints=None, before_step=None, after_step=None):
+    """`oracle`: the oracle to replay (default oracle.port's); `as_joints(joints, sc)`: turns the reference's joint rows
+    into the device's (stand-ins); `before_step(step, (lib, scene) pairs)`: public-API calls made on both worlds before a
+    step; `after_step(dw)`: called after every checked step."""
+    O = port.load() if oracle is None else oracle
     sr = recipe(R, solver, **kw)
     sp = recipe(P, solver, **kw)
     # push the freshly built scene to the device now (s2World_Step would do it): the first step is checked like any other
@@ -74,9 +62,12 @@ def _run(R, P, dev, recipe, solver, steps, vel, pos, kw, min_replays=0, setup=No
     sticky = solver == "TGS_Sticky"
     solved = {}  # TGS_Sticky: the oracle's rows of the previous step, by pair key
     for step in range(steps):
+        if before_step is not None:
+            before_step(step, ((R, sr), (P, sp)))
+            dev.lib.s2World_Flush(sp.world)
         cap = R.capacities(sr.world)["bodyCap"]
         pre = dw.download_all_bodies(cap)
-        _load_bodies_into_ref(R, sr.world, pre)
+        load_bodies_into_ref(R, sr.world, pre)
         R.step_collide(sr.world)
 
         sp.step(DT, vel, pos, True)
@@ -93,6 +84,8 @@ def _run(R, P, dev, recipe, solver, steps, vel, pos, kw, min_replays=0, setup=No
         if observe is not None:
             observe(R, sr.world, rows_key)
         joints = joint_rows_from_ref(*R.joints(sr.world))
+        if as_joints is not None:
+            joints = as_joints(joints, sr)
 
         got_contacts = dw.download_contacts(len(rows_key) + 64)
         assert len(got_contacts) == len(rows_key), f"step {step}: contact tables differ in size"
@@ -101,18 +94,12 @@ def _run(R, P, dev, recipe, solver, steps, vel, pos, kw, min_replays=0, setup=No
         assert np.array_equal(got_contacts["pointCount"], rows_key["pointCount"]), f"step {step}: manifold point counts differ"
 
         order, sizes = dw.solve_order(len(rows_key) + len(joints) + 16, max_groups=200000)
-        ob, oc, oj = O.solve(capi.SOLVER[solver], bodies, rows_key, joints, ctx, order=order)
+        ob, oc, oj, odp = O.solve(capi.SOLVER[solver], bodies, rows_key, joints, ctx, order=order,
+                                  dp=ref_delta_positions(R, sr.world))
 
         # advance the reference world with the oracle's result
         F = refmod.BODY_F
-        bf, bi = R.bodies(sr.world)
-        valid = bi[:, 0] == 1
-        bf[:, F["position"]:F["position"] + 2][valid] = ob["position"][valid]
-        bf[:, F["rot"]:F["rot"] + 2][valid] = ob["rot"][valid]
-        bf[:, F["v"]:F["v"] + 2][valid] = ob["linearVelocity"][valid]
-        bf[:, F["w"]][valid] = ob["angularVelocity"][valid]
-        bf[:, F["dp"]:F["dp"] + 2][valid] = 0.0
-        R.load_body_state(sr.world, bf)
+        store_oracle_bodies(R, sr.world, ob, odp)
         imp = np.zeros((cf.shape[0], 4), dtype=np.float32)
         imp[slots[perm], 0] = oc["points"]["normalImpulse"][:, 0]
         imp[slots[perm], 1] = oc["points"]["tangentImpulse"][:, 0]
@@ -142,6 +129,10 @@ def _run(R, P, dev, recipe, solver, steps, vel, pos, kw, min_replays=0, setup=No
                 worst[name] = max(worst.get(name, 0.0), float(np.abs(g - o).max()))
         if not bit_equal(post["angularVelocity"][v], rf[v, F["w"]]):
             worst["w"] = max(worst.get("w", 0.0), float(np.abs(post["angularVelocity"][v] - rf[v, F["w"]]).max()))
+        # the delta position a stage leaves (non-zero for a kinematic body under XPBD)
+        got_dp = dw.download_delta_positions(cap)
+        if not bit_equal(got_dp[v], rf[v, F["dp"]:F["dp"] + 2]):
+            worst["deltaPosition"] = float(np.abs(got_dp[v] - rf[v, F["dp"]:F["dp"] + 2]).max())
         # the contact table as the narrow phase left it (the reference's post-collide rows), and what the solver wrote back
         for name in CONTACT_FIELDS:
             if not _same(got_contacts[name], rows_key[name]):
@@ -177,6 +168,8 @@ def _run(R, P, dev, recipe, solver, steps, vel, pos, kw, min_replays=0, setup=No
                 if not bit_equal(got_joints[name][jlive], oj[name][jlive]):
                     worst["joint " + name] = 1.0
         assert not worst, f"{solver} step {step}: device != reference pipeline replayed in the device's order: {worst}"
+        if after_step is not None:
+            after_step(dw)
     c = dw.counters()
     assert c.graphReplays >= min_replays, f"the solver stage was replayed as a graph only {c.graphReplays} times"
     sr.destroy()

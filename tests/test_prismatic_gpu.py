@@ -17,7 +17,8 @@ import numpy as np
 import pytest
 
 import prismatic_oracle
-from helpers import bit_equal, body_rows_from_ref, carry_sticky_friction, contact_rows_from_ref, joint_rows_from_ref
+from helpers import (bit_equal, body_rows_from_ref, carry_sticky_friction, contact_rows_from_ref, joint_rows_from_ref,
+                     load_bodies_into_ref, ref_delta_positions, store_oracle_bodies)
 from oracle import port
 from oracle import ref as refmod
 from solver2d_b200 import capi, device, scenes
@@ -131,21 +132,6 @@ def test_stage_matches_oracle(reference, dev, solver, mode, persistent, gather):
 
 # ---- every step through the public API -----------------------------------------------------------------------------------
 
-def _load_bodies_into_ref(R, wid, rows):
-    F = refmod.BODY_F
-    bf, bi = R.bodies(wid)
-    n = min(len(rows), bf.shape[0])
-    valid = bi[:n, 0] == 1
-    for name, col, width in (("origin", F["origin"], 2), ("position", F["position"], 2), ("rot", F["rot"], 2),
-                             ("linearVelocity", F["v"], 2)):
-        bf[:n, col:col + width][valid] = rows[name][:n][valid]
-    bf[:n, F["w"]][valid] = rows["angularVelocity"][:n][valid]
-    bf[:n, F["dp"]:F["dp"] + 2][valid] = 0.0
-    bf[:n, F["force"]:F["force"] + 2][valid] = rows["force"][:n][valid]
-    bf[:n, F["torque"]][valid] = rows["torque"][:n][valid]
-    R.load_body_state(wid, bf)
-
-
 def _flush(dev, world):
     dev.lib.s2World_Flush.restype = None
     dev.lib.s2World_Flush.argtypes = [capi.WorldId]
@@ -159,12 +145,8 @@ def test_sliders_every_step(reference, product, dev, solver):
     impulses."""
     R, P = reference, product
     O = prismatic_oracle.load()
-    # XPBD leaves out the kinematic carriage: with a joint from a kinematic body to a dynamic one, XPBD's steps drift from
-    # the reference's from the second step on, with a revolute joint as much as with any other (DESIGN.md §3.8). The
-    # carriage is still checked under XPBD, stage by stage, in test_stage_matches_oracle.
-    kw = dict(kinematic=solver != "XPBD")
-    sr = scenes.sliders(R, solver, **kw)
-    sp = scenes.sliders(P, solver, **kw)
+    sr = scenes.sliders(R, solver)
+    sp = scenes.sliders(P, solver)
     assert "s2CreatePrismaticJoint" in R.missing and "s2CreatePrismaticJoint" not in P.missing
     slots = _slots(sp)
     assert slots == _slots(sr)
@@ -180,7 +162,7 @@ def test_sliders_every_step(reference, product, dev, solver):
     limits_hit = 0
     for step in range(60):
         cap = R.capacities(sr.world)["bodyCap"]
-        _load_bodies_into_ref(R, sr.world, dw.download_all_bodies(cap))
+        load_bodies_into_ref(R, sr.world, dw.download_all_bodies(cap))
         R.step_collide(sr.world)
         sp.step(DT, 4, 2, True)
 
@@ -199,17 +181,11 @@ def test_sliders_every_step(reference, product, dev, solver):
         contacts_seen += len(rows_key)
 
         order, _ = dw.solve_order(len(rows_key) + len(joints) + 16, max_groups=200000)
-        ob, oc, oj = O.solve(capi.SOLVER[solver], bodies, rows_key, joints, ctx, order=order)
+        ob, oc, oj, odp = O.solve(capi.SOLVER[solver], bodies, rows_key, joints, ctx, order=order,
+                                  dp=ref_delta_positions(R, sr.world))
         limits_hit += int(np.count_nonzero(oj["lowerImpulse"][slots]) + np.count_nonzero(oj["upperImpulse"][slots]))
 
-        bf, bi = R.bodies(sr.world)
-        valid = bi[:, 0] == 1
-        bf[:, F["position"]:F["position"] + 2][valid] = ob["position"][valid]
-        bf[:, F["rot"]:F["rot"] + 2][valid] = ob["rot"][valid]
-        bf[:, F["v"]:F["v"] + 2][valid] = ob["linearVelocity"][valid]
-        bf[:, F["w"]][valid] = ob["angularVelocity"][valid]
-        bf[:, F["dp"]:F["dp"] + 2][valid] = 0.0
-        R.load_body_state(sr.world, bf)
+        store_oracle_bodies(R, sr.world, ob, odp)
         imp = np.zeros((cf.shape[0], 4), dtype=np.float32)
         imp[cslots[perm], 0] = oc["points"]["normalImpulse"][:, 0]
         imp[cslots[perm], 1] = oc["points"]["tangentImpulse"][:, 0]
@@ -233,6 +209,7 @@ def test_sliders_every_step(reference, product, dev, solver):
         for name, col in (("position", F["position"]), ("rot", F["rot"]), ("linearVelocity", F["v"])):
             assert bit_equal(post[name][v], rf[v, col:col + 2]), f"step {step}: {name}"
         assert bit_equal(post["angularVelocity"][v], rf[v, F["w"]]), f"step {step}: angularVelocity"
+        assert bit_equal(dw.download_delta_positions(cap)[v], rf[v, F["dp"]:F["dp"] + 2]), f"step {step}: deltaPosition"
         live = rows_key["pointCount"] > 0
         got_after = dw.download_contacts(len(rows_key) + 64)
         assert bit_equal(got_after["points"]["normalImpulse"][live], oc["points"]["normalImpulse"][live]), f"step {step}"

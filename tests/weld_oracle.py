@@ -5,7 +5,6 @@ untouched), keyed by the hash of every source it includes. `solve` has the signa
 """
 from __future__ import annotations
 
-import ctypes as C
 import glob
 import hashlib
 import os
@@ -14,7 +13,6 @@ import tempfile
 
 from helpers import ROOT
 from oracle import port
-from solver2d_b200 import device
 
 SRC = os.path.join(ROOT, "tests", "weld_oracle.c")
 
@@ -41,11 +39,8 @@ def build() -> str:
 
 
 class WeldOracle(port.Oracle):
-    def __init__(self):  # noqa: D107 - the same entry point as the oracle's, from the weld build
-        self.lib = C.CDLL(build())
-        self.lib.s2o_solve.restype = C.c_int
-        self.lib.s2o_solve.argtypes = [C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_void_p,
-                                       C.c_int, C.POINTER(device.StepContext), C.c_float, C.c_float]
+    def __init__(self):  # noqa: D107 - the same entry points as the oracle's, from the weld build
+        super().__init__(build())
 
 
 _cached = None
