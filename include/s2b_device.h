@@ -194,6 +194,7 @@ typedef struct s2bCounters
 	int32_t cutGroupCount;	 // colours of the cut set = device-wide steps per Gauss-Seidel sweep
 	int32_t recolouredCount; /* constraints moved out of a sparse top colour by Kempe chains so far (colouring, DESIGN.md 3.2) */
 	int32_t neighbourSync;	 // blocks of the persistent kernel whose colour steps wait only for neighbouring blocks; 0 = grid barriers
+	int32_t narrowphaseRowSteps; // solver stages so far whose contact rows the narrow phase wrote (their prepare pass skipped them)
 } s2bCounters;
 
 // ---- lifecycle ------------------------------------------------------------------------------------------------

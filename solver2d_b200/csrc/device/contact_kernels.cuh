@@ -115,22 +115,31 @@ enum PrepareKind
 	PREPARE_COLD = 2, // s2PrepareContacts_XPBD (reference src/solve_xpbd.c:18-86): never warm starts
 };
 
-// Builds row t of the constraint stream from contact slot src[t]. Writes are coalesced (row t), reads gather the
-// persistent manifold and the two bodies.
-template <int KIND> __device__ __forceinline__ void s2bPrepareContact(const SolveArgs& a, int t)
+// The points of a manifold in the contact table: its local anchors and separation + stored impulses, read where used.
+struct S2bTablePoints
+{
+	const ContactView& c;
+	int slot;
+	__device__ __forceinline__ float4 anchor(int j) const
+	{
+		return c.anchor[j][slot];
+	}
+	__device__ __forceinline__ float4 impulse(int j) const
+	{
+		return c.impulse[j][slot];
+	}
+};
+
+// Writes row t of the constraint stream from one manifold and its two bodies: the manifold's normal / friction (mnf), its
+// points (POINTS::anchor(j) / impulse(j) = the table's anchor[j] / impulse[j] columns, asked for j < pointCount only), and
+// per body the local centre (org.zw), the rotation (pose.zw), the inverse mass (vel.w) and the inverse inertia (prm.w).
+// Writes are coalesced (row t). Called by the solver's prepare pass, which gathers these values through src[t], and by the
+// narrow phase, which has them in registers when the solve schedule stands (narrowphase.cu): the row format lives here only.
+template <int KIND, typename POINTS>
+__device__ __forceinline__ void s2bWriteContactRow(const SolveArgs& a, int t, int2 bodies, int pointCount, float4 mnf, const POINTS& points,
+												   float4 orgA, float4 orgB, float4 poseA, float4 poseB, float mA, float mB, float iA, float iB)
 {
 	const ConstraintView& cc = a.cc;
-	int slot = cc.src[t];
-	int2 bodies = a.contacts.bodies[slot];
-	int4 info = a.contacts.info[slot];
-	float4 mnf = a.contacts.nf[slot];
-	int pointCount = S2B_CI_COUNT(info.x);
-
-	float4 velA = a.bodies.vel[bodies.x], velB = a.bodies.vel[bodies.y];
-	float4 poseA = a.bodies.pose[bodies.x], poseB = a.bodies.pose[bodies.y];
-	float4 orgA = a.bodies.org[bodies.x], orgB = a.bodies.org[bodies.y];
-	float mA = velA.w, mB = velB.w;
-	float iA = a.bodies.prm[bodies.x].w, iB = a.bodies.prm[bodies.y].w;
 	s2Rot qA = R2(poseA.z, poseA.w), qB = R2(poseB.z, poseB.w);
 	s2Vec2 normal = V2(mnf.x, mnf.y);
 	s2Vec2 tangent = s2RightPerp(normal);
@@ -163,8 +172,8 @@ template <int KIND> __device__ __forceinline__ void s2bPrepareContact(const Solv
 	{
 		if (j < pointCount)
 		{
-			float4 la = a.contacts.anchor[j][slot];
-			float4 mi = a.contacts.impulse[j][slot];
+			float4 la = points.anchor(j);
+			float4 mi = points.impulse(j);
 			float separation = mi.x;
 			// PGS prepare tests cp->separation <= 0 on the zero-filled scratch, i.e. always true (SURVEY §8a N1), so
 			// both prepare flavours take the stored impulses whenever warm starting is on.
@@ -223,6 +232,24 @@ template <int KIND> __device__ __forceinline__ void s2bPrepareContact(const Solv
 		s2bWriteWarmImpulses(a, t, normal, tangent, pointCount, warmLam[0], warmLam[1]);
 		s2bWriteWarmAnchors(a, t, warmAnchor[0], warmAnchor[1]);
 	}
+}
+
+// Builds row t of the constraint stream from contact slot src[t]: gathers the persistent manifold and the two bodies.
+// Skipped on the steps whose rows the narrow phase has already written (CNT_ROWS_READY, persistent.cuh).
+template <int KIND> __device__ __forceinline__ void s2bPrepareContact(const SolveArgs& a, int t)
+{
+	int slot = a.cc.src[t];
+	int2 bodies = a.contacts.bodies[slot];
+	int4 info = a.contacts.info[slot];
+	float4 mnf = a.contacts.nf[slot];
+	int pointCount = S2B_CI_COUNT(info.x);
+
+	float4 velA = a.bodies.vel[bodies.x], velB = a.bodies.vel[bodies.y];
+	float4 poseA = a.bodies.pose[bodies.x], poseB = a.bodies.pose[bodies.y];
+	float4 orgA = a.bodies.org[bodies.x], orgB = a.bodies.org[bodies.y];
+	float iA = a.bodies.prm[bodies.x].w, iB = a.bodies.prm[bodies.y].w;
+	S2bTablePoints points = {a.contacts, slot};
+	s2bWriteContactRow<KIND>(a, t, bodies, pointCount, mnf, points, orgA, orgB, poseA, poseB, velA.w, velB.w, iA, iB);
 }
 
 // s2StoreContactImpulses (reference src/solve_common.c:396-410): scatter accumulated impulses back to the manifolds.

@@ -8,7 +8,11 @@
 // Traffic per polygon-polygon contact: 2 shape headers + 2 x (count x 16 B) geometry + 2 x 32 B body transform read,
 // ~112 B of manifold columns read and written. Arithmetic (GJK + clip) dominates; the kernel is latency/ALU bound,
 // not bandwidth bound.
-#include "s2b_internal.cuh"
+//
+// While the solve schedule stands, each thread also writes its constraint's row of the solver's constraint stream
+// (s2bWriteContactRow): it holds the manifold and both bodies' transforms already, and the solver's prepare pass, which
+// would gather them all again, is skipped (DESIGN.md §3.4).
+#include "contact_kernels.cuh"
 
 #include "shared/s2_collide.h"
 
@@ -20,6 +24,20 @@
 #define S2B_NP_POLY_WORDS 34
 #define S2B_NP_THREAD_WORDS (2 * S2B_NP_POLY_WORDS + 1)
 static_assert(sizeof(s2Polygon) == 4 * S2B_NP_POLY_WORDS, "s2Polygon layout");
+
+// the points of a manifold just computed, for s2bWriteContactRow: what the table's anchor / impulse columns now hold
+struct S2bFreshPoints
+{
+	float4 anchor0, anchor1, impulse0, impulse1;
+	__device__ __forceinline__ float4 anchor(int j) const
+	{
+		return j == 0 ? anchor0 : anchor1;
+	}
+	__device__ __forceinline__ float4 impulse(int j) const
+	{
+		return j == 0 ? impulse0 : impulse1;
+	}
+};
 
 __device__ __forceinline__ void s2bLoadPolygon(s2Polygon* poly, const ShapeView& s, int shape, int count, float radius)
 {
@@ -52,13 +70,22 @@ __device__ __forceinline__ void s2bLoadLocalPolygon(s2Polygon* poly, const Shape
 	poly->radius = radius;
 }
 
-__global__ void __launch_bounds__(S2B_NP_BLOCK) s2bUpdateContactsKernel(ContactView c, int contactCount, ShapeView s, BodyView b, int sticky, int* schedDirty)
+// KIND < 0: the manifolds only. KIND = PREPARE_SOFT / PREPARE_COLD: also row rowOf[i] of the constraint stream of `a` for every
+// manifold with points that has a row. Thread 0 says which in *rowsReady (CNT_ROWS_READY of the solver's counts; null before
+// the first solve), for the schedule gate.
+template <int KIND>
+__global__ void __launch_bounds__(S2B_NP_BLOCK) s2bUpdateContactsKernel(ContactView c, int contactCount, ShapeView s, BodyView b, int sticky,
+																		  int* schedDirty, SolveArgs a, const int* rowOf, int* rowsReady)
 {
 	__shared__ float polyStore[S2B_NP_BLOCK * S2B_NP_THREAD_WORDS];
 	s2Polygon* polyA = reinterpret_cast<s2Polygon*>(polyStore + threadIdx.x * S2B_NP_THREAD_WORDS);
 	s2Polygon* polyB = reinterpret_cast<s2Polygon*>(polyStore + threadIdx.x * S2B_NP_THREAD_WORDS + S2B_NP_POLY_WORDS);
 
 	int i = blockIdx.x * blockDim.x + threadIdx.x;
+	if (i == 0 && rowsReady != nullptr)
+	{
+		*rowsReady = KIND >= 0 ? 1 : 0;
+	}
 	if (i >= contactCount)
 	{
 		return;
@@ -197,6 +224,32 @@ __global__ void __launch_bounds__(S2B_NP_BLOCK) s2bUpdateContactsKernel(ContactV
 	c.anchor[1][i] = make_float4(m.points[1].localAnchorA.x, m.points[1].localAnchorA.y, m.points[1].localAnchorB.x, m.points[1].localAnchorB.y);
 	c.impulse[0][i] = newImp0;
 	c.impulse[1][i] = newImp1;
+
+	if constexpr (KIND >= 0)
+	{
+		// the row prepare would build from what was just stored: a manifold without points has no row, a manifold that gained
+		// its first point has none yet (both raised schedDirty above: the rebuilt schedule's prepare writes every row)
+		int t = pointCount > 0 ? rowOf[i] : -1;
+		if (t >= 0)
+		{
+			int2 bodies = c.bodies[i];
+			if (bodies.x != bodyA || bodies.y != bodyB)
+			{
+				*schedDirty = 1; // (never seen: the table's bodies are its shapes' bodies) prepare gathers the table's bodies
+			}
+			else
+			{
+				float mA = b.vel[bodyA].w, mB = b.vel[bodyB].w;
+				float iA = b.prm[bodyA].w, iB = b.prm[bodyB].w;
+				S2bFreshPoints points = {
+					make_float4(m.points[0].localAnchorA.x, m.points[0].localAnchorA.y, m.points[0].localAnchorB.x, m.points[0].localAnchorB.y),
+					make_float4(m.points[1].localAnchorA.x, m.points[1].localAnchorA.y, m.points[1].localAnchorB.x, m.points[1].localAnchorB.y),
+					newImp0, newImp1};
+				s2bWriteContactRow<KIND>(a, t, bodies, pointCount, make_float4(m.normal.x, m.normal.y, nf.z, nf.w), points, orgA, orgB, poseA, poseB,
+										 mA, mB, iA, iB);
+			}
+		}
+	}
 }
 
 void s2bNarrowphaseUpdate(s2bWorld* w)
@@ -205,6 +258,27 @@ void s2bNarrowphaseUpdate(s2bWorld* w)
 	{
 		return;
 	}
-	S2B_LAUNCH(w, s2bUpdateContactsKernel, gridFor(w->contactCount, S2B_NP_BLOCK), S2B_NP_BLOCK, 0, makeView(w->contacts[w->cur]), w->contactCount,
-			   shapeView(w), bodyView(w), w->sticky ? 1 : 0, w->schedDirty.p);
+	SolveArgs a;
+	memset(&a, 0, sizeof(a));
+	const int* rowOf = nullptr;
+	int* rowsReady = nullptr;
+	int kind = s2bNarrowphaseRows(w, &a, &rowOf, &rowsReady);
+	ContactView c = makeView(w->contacts[w->cur]);
+	int grid = gridFor(w->contactCount, S2B_NP_BLOCK);
+	int sticky = w->sticky ? 1 : 0;
+	if (kind == PREPARE_SOFT)
+	{
+		S2B_LAUNCH(w, s2bUpdateContactsKernel<PREPARE_SOFT>, grid, S2B_NP_BLOCK, 0, c, w->contactCount, shapeView(w), bodyView(w), sticky,
+				   w->schedDirty.p, a, rowOf, rowsReady);
+	}
+	else if (kind == PREPARE_COLD)
+	{
+		S2B_LAUNCH(w, s2bUpdateContactsKernel<PREPARE_COLD>, grid, S2B_NP_BLOCK, 0, c, w->contactCount, shapeView(w), bodyView(w), sticky,
+				   w->schedDirty.p, a, rowOf, rowsReady);
+	}
+	else
+	{
+		S2B_LAUNCH(w, s2bUpdateContactsKernel<-1>, grid, S2B_NP_BLOCK, 0, c, w->contactCount, shapeView(w), bodyView(w), sticky, w->schedDirty.p, a,
+				   rowOf, rowsReady);
+	}
 }

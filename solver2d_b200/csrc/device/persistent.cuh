@@ -1041,16 +1041,30 @@ template <int SOLVER> __global__ void __launch_bounds__(S2B_BLOCK, SOLVER == S2B
 						sync.code = code;
 					}
 				}
-				else if ((pass.jointOp == JOP_NONE || li.nJ == 0) && (pass.contactOp == COP_NONE || li.nC == 0))
-				{
-					// nothing to do for anybody (the counts are grid-uniform): no barrier either
-				}
 				else
 				{
-					s2bSyncBeforeGlobal(a, sync);
-					s2bFlatPass<SOLVER>(pass.jointOp, pass.contactOp, a, p, li);
-					sync.pending = S2B_PENDING_GLOBAL;
-					sync.code = (PASS_FLAT << 8) | pass.contactOp;
+					int contactOp = pass.contactOp;
+					if constexpr (s2bUsesContactOp(SOLVER, COP_PREPARE) || s2bUsesContactOp(SOLVER, COP_PREPARE_COLD))
+					{
+						if ((contactOp == COP_PREPARE || contactOp == COP_PREPARE_COLD) && a.counts[CNT_ROWS_READY] != 0)
+						{
+							// the narrow phase has written this step's contact rows (narrowphase.cu): prepare leaves the contacts
+							// alone, and without joints the pass and its barrier go (grid-uniform: nothing writes the count while
+							// the kernel runs)
+							contactOp = COP_NONE;
+						}
+					}
+					if ((pass.jointOp == JOP_NONE || li.nJ == 0) && (contactOp == COP_NONE || li.nC == 0))
+					{
+						// nothing to do for anybody (the counts are grid-uniform): no barrier either
+					}
+					else
+					{
+						s2bSyncBeforeGlobal(a, sync);
+						s2bFlatPass<SOLVER>(pass.jointOp, contactOp, a, p, li);
+						sync.pending = S2B_PENDING_GLOBAL;
+						sync.code = (PASS_FLAT << 8) | contactOp;
+					}
 				}
 			}
 		}

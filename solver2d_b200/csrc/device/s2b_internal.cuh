@@ -386,6 +386,8 @@ struct s2bWorld
 	int fusePositions = 1; // TGS_Soft: s2IntegratePositions folded into the bias sweep (S2B_FUSE_POSITIONS=0 disables)
 	int neighbourSync = 1; // device-wide colour steps wait for neighbouring blocks only, where the device finds that possible
 						   // (persistent.cuh; S2B_NEIGHBOUR_SYNC=0 keeps a grid barrier before every colour step)
+	int narrowphasePrepare = 1; // while the solve schedule stands, the narrow phase writes the contact rows and the solver's
+								// prepare pass skips them (narrowphase.cu; S2B_NARROWPHASE_PREPARE=0 leaves it all to prepare)
 	int kempeGrid = 0;
 	DevArray<int> dMovedFlag; // [0] = number of proxies moved in last finalize (device counter)
 	int pairPassCount = 0;

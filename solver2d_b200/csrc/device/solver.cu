@@ -1686,14 +1686,16 @@ __global__ void s2bOverflowBodiesKernel(const int* counts, const int* jGroupOff,
 	}
 }
 
-// src[t] = contact slot of the constraint at solve position t
-__global__ void s2bBuildSources(const int* counts, const int* cPerm, const int* activeSlots, int* src)
+// src[t] = contact slot of the constraint at solve position t, and its inverse rowOf[slot] = t (rowOf arrives filled with -1: slots without a row keep it)
+__global__ void s2bBuildSources(const int* counts, const int* cPerm, const int* activeSlots, int* src, int* rowOf)
 {
 	int n = counts[CNT_CONTACTS];
 	int t = blockIdx.x * blockDim.x + threadIdx.x;
 	if (t < n)
 	{
-		src[t] = activeSlots[cPerm[t]];
+		int slot = activeSlots[cPerm[t]];
+		src[t] = slot;
+		rowOf[slot] = t;
 	}
 }
 
@@ -2764,7 +2766,10 @@ static void buildWavefront(s2bWorld* w, SolverScratch* s, int nJ, int nC, HostPl
 // [1] replays since the last rebuild, [2] a rebuild skipped the pass because the scene was churning, [3] the value of [1]
 // when the rebuild that is about to run was asked for. A scene that has gone quiet with a skipped pass still owed gets ONE
 // rebuild of its own, so that it does not keep the extra colours for good.
-__global__ void s2bScheduleGate(cudaGraphConditionalHandle handle, int* dirty)
+// counts[CNT_ROWS_READY]: the narrow phase has written this step's contact rows into the schedule that stands; kept (and the
+// step counted in dirty[S2B_SCHED_ROW_STEPS]) when no rebuild is taken, so the solver skips their prepare; cleared when one
+// is (the rebuild clears it too).
+__global__ void s2bScheduleGate(cudaGraphConditionalHandle handle, int* dirty, int* counts)
 {
 	int v = dirty[0];
 	dirty[0] = 0;
@@ -2783,6 +2788,14 @@ __global__ void s2bScheduleGate(cudaGraphConditionalHandle handle, int* dirty)
 			dirty[3] = quiet;
 			dirty[1] = 0;
 		}
+	}
+	if (v != 0)
+	{
+		counts[CNT_ROWS_READY] = 0;
+	}
+	else if (counts[CNT_ROWS_READY] != 0)
+	{
+		dirty[S2B_SCHED_ROW_STEPS] += 1;
 	}
 	cudaGraphSetConditional(handle, v != 0 ? 1u : 0u);
 }
@@ -2966,11 +2979,12 @@ static void planSolve(s2bWorld* w, SolverScratch* s, SolvePlan& pl)
 		s->nsyncNbr.reserve((size_t)pl.grid * S2B_NSYNC_STRIDE, st, true);
 	}
 	w->solveBarrier.reserve(S2B_BARRIER_WORDS, st, true, true);
-	w->schedDirty.reserve(4, st, true, true);
+	w->schedDirty.reserve(S2B_SCHED_WORDS, st, true, true);
 	// (+2 rows: the bulk-staged colour kernel may read up to two rows past the last constraint)
 	s->idx.reserve(nC + 2, st, false);
 	s->nf.reserve(nC + 2, st, false);
 	s->src.reserve(nC, st, false);
+	s->rowOf.reserve(nC, st, false);
 	if (pl.gatherWarm)
 	{
 		s->warmP.reserve(nC, st, false);
@@ -3093,6 +3107,8 @@ static void enqueueSchedule(s2bWorld* w, SolverScratch* s, SolvePlan& pl)
 
 	// ---- gather ----
 	S2B_CHECK(cudaMemsetAsync(w->schedDirty.p, 0, sizeof(int), st)); // what follows is the rebuild the flag asks for
+	// (this also clears CNT_ROWS_READY: rows the narrow phase wrote for the schedule being replaced are stale, prepare writes
+	// every row of the new one)
 	S2B_CHECK(cudaMemsetAsync(s->counts.p, 0, sizeof(int) * CNT_SIZE, st));
 	{
 		int n = std::max(contactCount, jointCap);
@@ -3274,7 +3290,8 @@ static void enqueueSchedule(s2bWorld* w, SolverScratch* s, SolvePlan& pl)
 
 		if (contactCount > 0)
 		{
-			S2B_LAUNCH(w, s2bBuildSources, gridFor(contactCount, 256), 256, 0, s->counts.p, s->cPerm.p, s->activeSlots.p, s->src.p);
+			S2B_CHECK(cudaMemsetAsync(s->rowOf.p, 0xFF, sizeof(int) * (size_t)contactCount, st));
+			S2B_LAUNCH(w, s2bBuildSources, gridFor(contactCount, 256), 256, 0, s->counts.p, s->cPerm.p, s->activeSlots.p, s->src.p, s->rowOf.p);
 		}
 
 		if (pl.needInc)
@@ -3516,6 +3533,62 @@ static void enqueueIterate(s2bWorld* w, SolverScratch* s, SolvePlan& pl, bool ca
 		w->dWork.reserve(4, st, true);
 		S2B_LAUNCH(w, s2bMeterWork, 1, 1, 0, s->counts.p, pl.countedPasses, w->dWork.p);
 	}
+
+	// can the next step's narrow phase write the contact rows into these columns (s2bNarrowphaseRows)? Only where the next
+	// solve can be a graph replay (an eager solve always rebuilds the schedule) and the program prepares its contacts with
+	// s2bPrepareContact
+	SolverScratch::RowTarget rt;
+	rt.args = a;
+	bool replayable = w->schedule == S2B_SCHEDULE_COLOR && pl.usePersistent && w->useGraph != 0 && s->graphDisabled == false && s->traceCap == 0;
+	if (w->narrowphasePrepare != 0 && replayable && pl.contactCount > 0)
+	{
+		for (int g = 0; g < pl.program.segmentCount; ++g)
+		{
+			for (int k = 0; k < pl.program.passCount[g]; ++k)
+			{
+				PassDesc d = pl.program.passes[g][k];
+				if (d.kind == PASS_FLAT && d.contactOp == COP_PREPARE)
+				{
+					rt.kind = PREPARE_SOFT;
+				}
+				else if (d.kind == PASS_FLAT && d.contactOp == COP_PREPARE_COLD)
+				{
+					rt.kind = PREPARE_COLD;
+				}
+			}
+		}
+	}
+	rt.cur = w->cur;
+	rt.contactCount = pl.contactCount;
+	rt.tableVersion = w->contactTableVersion;
+	rt.epoch = s2bAllocEpoch();
+	s->rows = rt;
+	if (capturing)
+	{
+		s->graphRows = rt; // what a replay of this graph leaves for the next narrow phase (s2bSolve)
+	}
+}
+
+int s2bNarrowphaseRows(s2bWorld* w, SolveArgs* args, const int** rowOf, int** rowsReady)
+{
+	SolverScratch* s = w->scratch;
+	*rowsReady = (s != nullptr && s->counts.p != nullptr) ? s->counts.p + CNT_ROWS_READY : nullptr;
+	if (w->narrowphasePrepare == 0 || s == nullptr || s->rows.kind < 0)
+	{
+		return -1;
+	}
+	// the same contact table (no pair commit or upload since) and no re-allocation: rowOf and the columns are the ones the
+	// last solve used, sized for this table. Whether the schedule still stands, and whether this step's solve replays the
+	// graph those columns belong to, is known on the device only: s2bScheduleGate / enqueueSchedule decide whether the rows
+	// are used or rebuilt.
+	const SolverScratch::RowTarget& rt = s->rows;
+	if (rt.cur != w->cur || rt.contactCount != w->contactCount || rt.tableVersion != w->contactTableVersion || rt.epoch != s2bAllocEpoch())
+	{
+		return -1;
+	}
+	*args = rt.args;
+	*rowOf = s->rowOf.p;
+	return rt.kind;
 }
 
 void s2bSolve(s2bWorld* w, int solverType, const s2bStepContext* ctxIn)
@@ -3568,6 +3641,7 @@ void s2bSolve(s2bWorld* w, int solverType, const s2bStepContext* ctxIn)
 				s->scheduleSig = sig;
 			}
 			S2B_CHECK(cudaGraphLaunch(s->graphExec, st));
+			s->rows = s->graphRows;
 			s->stepsSinceEager += 1;
 			w->kernelLaunches += s->graphLaunches;
 			w->solveKernelTimed = true;
@@ -3642,7 +3716,8 @@ void s2bSolve(s2bWorld* w, int solverType, const s2bStepContext* ctxIn)
 		{
 			cudaKernelNodeParams kp = {};
 			int* dirty = w->schedDirty.p;
-			void* args[] = {&handle, &dirty};
+			int* counts = s->counts.p;
+			void* args[] = {&handle, &dirty, &counts};
 			kp.func = (void*)s2bScheduleGate;
 			kp.gridDim = dim3(1);
 			kp.blockDim = dim3(1);
@@ -3948,6 +4023,10 @@ extern "C" void s2b_get_counters(s2bWorld* w, s2bCounters* out)
 	out->kernelLaunches = w->kernelLaunches;
 	out->graphReplays = w->scratch != nullptr ? w->scratch->graphReplays : 0;
 	out->graphCaptures = w->scratch != nullptr ? w->scratch->graphCaptures : 0;
+	if (w->schedDirty.p != nullptr)
+	{
+		S2B_CHECK(cudaMemcpy(&out->narrowphaseRowSteps, w->schedDirty.p + S2B_SCHED_ROW_STEPS, sizeof(int), cudaMemcpyDeviceToHost));
+	}
 }
 
 extern "C" void s2b_set_solve_trace(s2bWorld* w, int capacity)

@@ -40,6 +40,7 @@ enum
 	CNT_BOUNDS = 16,	// 4 slots: order-preserving keys of max x, max -x, max y, max -y over the bodies' centres
 	CNT_NSYNC = 23,		// grid the neighbour tables were built for: device-wide colour steps wait for neighbouring blocks only; 0 = off
 	CNT_KINEMATIC_ITEMS = 24, // constraints with an endpoint no constraint moves but whose pose changes (kinematic, s2bItemEndpoints -2)
+	CNT_ROWS_READY = 25, // 1: the narrow phase wrote this solve's contact rows, prepare leaves them (narrowphase.cu, s2bScheduleGate)
 	CNT_SIZE = 32
 };
 
@@ -180,6 +181,7 @@ struct SolverScratch
 	DevArray<float2> lambda[2], tsep[2];
 	DevArray<float> sep[2];
 	DevArray<int> src;
+	DevArray<int> rowOf; // per contact slot: its row in the solve order (the inverse of src), -1: none; built with the schedule
 	DevArray<float4> warmP, warmAnchor; // ConstraintView::warmP (1 per constraint), ::warmAnchor (2 per constraint)
 	// restitution capture, per contact slot (SolveArgs::restVr / restR); allocated while restitution is enabled
 	DevArray<float4> restVr, restR[2];
@@ -207,6 +209,16 @@ struct SolverScratch
 	const int* lastJointSlots = nullptr;
 	const int* lastJPerm = nullptr;
 	bool lastArgsValid = false;
+	// where the next step's narrow phase may write the contact rows (s2bNarrowphaseRows): those of the last solve that ran,
+	// eager or a graph replay (then the ones the graph was captured with)
+	struct RowTarget
+	{
+		SolveArgs args;
+		int kind = -1; // prepare kind of the solve's program; -1: the solve cannot take rows from the narrow phase
+		int cur = 0, contactCount = 0;			   // the contact table and allocations it was planned for
+		unsigned long long tableVersion = 0, epoch = 0;
+	};
+	RowTarget rows, graphRows;
 
 	// host mirrors (valid when the last solve synchronised: multi-launch and wavefront modes)
 	int hostContacts = 0, hostJoints = 0, hostGroups = 0, hostOverflowC = 0, hostOverflowJ = 0;
@@ -215,3 +227,13 @@ struct SolverScratch
 };
 
 SolverScratch* s2bGetSolverScratch(s2bWorld* w);
+
+// schedDirty words (s2b_internal.cuh): [0] rebuild wanted, [1..3] the Kempe pass's view of the recent past, [4] solves whose
+// contact rows came from the narrow phase (s2bCounters::narrowphaseRowSteps); see s2bScheduleGate
+#define S2B_SCHED_ROW_STEPS 4
+#define S2B_SCHED_WORDS 8
+
+// The prepare kind (PREPARE_SOFT / PREPARE_COLD) the narrow phase writes this step's contact rows with, into *args' columns
+// at the rows *rowOf names; -1: it writes none. *rowsReady: where it says whether it did (counts[CNT_ROWS_READY], null before
+// the first solve); s2bScheduleGate decides whether the solver then uses them.
+int s2bNarrowphaseRows(s2bWorld* w, SolveArgs* args, const int** rowOf, int** rowsReady);

@@ -412,10 +412,15 @@ extern "C" s2bWorld* s2b_world_create(int cudaDevice, int solverType)
 		{
 			w->neighbourSync = atoi(env) != 0 ? 1 : 0;
 		}
+		env = getenv("S2B_NARROWPHASE_PREPARE");
+		if (env != nullptr)
+		{
+			w->narrowphasePrepare = atoi(env) != 0 ? 1 : 0;
+		}
 	}
 	w->solverType = solverType;
 	w->sticky = (solverType == 6); // s2_solverTGS_Sticky
-	w->schedDirty.reserve(4, w->stream, true, true);
+	w->schedDirty.reserve(8, w->stream, true, true); // S2B_SCHED_WORDS
 	w->solveBarrier.reserve(64, w->stream, true, true);
 	S2B_CHECK(cudaMallocHost((void**)&w->hostMail, MAIL_COUNT * sizeof(int)));
 	memset(w->hostMail, 0, MAIL_COUNT * sizeof(int));
