@@ -65,7 +65,11 @@ struct BroadScratch
 	int searchedCount = 0;
 	size_t prefetchTempBytes = 0;
 	cudaEvent_t evSearch[2] = {nullptr, nullptr};
-	cudaEvent_t searchDone = nullptr;
+	cudaEvent_t searchDone = nullptr;  // behind the copy of the counters to the mailbox (bpSearch)
+	cudaEvent_t searchKernels = nullptr; // behind the search's kernels: the mailbox copy on mailStream waits for it
+	// the counters' copy to the mailbox runs on a stream of its own: on the world's stream the step would wait for it, and on
+	// the transforms' side stream (s2b_download_transforms) the read-back would wait for the whole search
+	cudaStream_t mailStream = nullptr;
 };
 
 #define S2B_TREE_REUSE_LIMIT 16
@@ -125,6 +129,12 @@ void s2bFreeBroadScratch(s2bWorld* w)
 	if (b->searchDone != nullptr)
 	{
 		cudaEventDestroy(b->searchDone);
+		cudaEventDestroy(b->searchKernels);
+	}
+	if (b->mailStream != nullptr)
+	{
+		cudaStreamSynchronize(b->mailStream); // (its copy writes into the pinned mailbox)
+		cudaStreamDestroy(b->mailStream);
 	}
 	delete b;
 	w->broad = nullptr;
@@ -518,11 +528,20 @@ __global__ void s2bBuildWide(const int* leafShape, const int* sortedLeaf, int* c
 
 // Boxes bottom-up: a leaf thread writes its fat box into its slot in the parent wide node and counts its arrival; the last
 // child to arrive resets the counter for the next pass, unions the node's child boxes and carries that box one level up.
-__global__ void s2bRefit(ShapeView s, const int* leafShape, const int* sortedLeaf, const int* counters, const int* wideCount,
+// The refit is the first kernel of every search, and nothing before it in the pass touches the per-pass counters, so it clears
+// them (a memset on the stream in its place cost more than the refit's leaf threads wait for it).
+__global__ void s2bRefit(ShapeView s, const int* leafShape, const int* sortedLeaf, int* counters, const int* wideCount,
 						 const int* wideSlot, float4* wideBox, int* visit, float4* rootBox)
 {
 	int n = counters[BC_LEAVES];
 	int k = blockIdx.x * blockDim.x + threadIdx.x;
+	if (k == 0)
+	{
+		for (int c = BC_NEW_PAIRS; c < BC_SIZE; ++c)
+		{
+			counters[c] = 0;
+		}
+	}
 	if (k >= n)
 	{
 		return;
@@ -1056,8 +1075,7 @@ static void bpSearch(s2bWorld* w, BroadScratch* B)
 	bool reuseTree = B->treeValid && w->pairsDirty == false && B->treeShapeCap == shapeCap && B->treeReuses < S2B_TREE_REUSE_LIMIT;
 	if (reuseTree)
 	{
-		// keep BC_LEAVES and BC_HEIGHT of the build; clear the per-pass counters
-		S2B_CHECK(cudaMemsetAsync(B->counters.p + BC_NEW_PAIRS, 0, sizeof(int) * (BC_SIZE - BC_NEW_PAIRS), st));
+		// keep BC_LEAVES and BC_HEIGHT of the build; s2bRefit clears the per-pass counters
 		B->treeReuses += 1;
 	}
 	else
@@ -1128,7 +1146,32 @@ static void bpSearch(s2bWorld* w, BroadScratch* B)
 		S2B_LAUNCH(w, s2bCollectKeptContacts, gridFor(oldCount, 256), 256, 0, makeView(cur), oldCount, sv, w->jointDestroyKeys.p,
 				   w->jointDestroyCount, B->keepSlots.p, B->counters.p);
 	}
-	S2B_CHECK(cudaMemcpyAsync(w->hostMail + MAIL_BC_BASE, B->counters.p, sizeof(int) * BC_SIZE, cudaMemcpyDeviceToHost, st));
+	// The counters go to the mailbox on mailStream, behind the search's kernels only, so that the world's stream does not
+	// wait for the copy. searchDone passes once they have arrived, and the moved-proxy counter's copy too (s2bFinalize):
+	// whoever waits for this pass's counters has that one behind it as well. The next pass clears the counters only after
+	// the host has waited for searchDone (or gave up on this search).
+	if (B->searchDone == nullptr)
+	{
+		S2B_CHECK(cudaEventCreateWithFlags(&B->searchDone, cudaEventDisableTiming));
+		S2B_CHECK(cudaEventCreateWithFlags(&B->searchKernels, cudaEventDisableTiming));
+	}
+	cudaStream_t cs = st;
+	if (w->sideCopies != 0)
+	{
+		if (B->mailStream == nullptr)
+		{
+			S2B_CHECK(cudaStreamCreateWithFlags(&B->mailStream, cudaStreamNonBlocking));
+		}
+		cs = B->mailStream;
+		S2B_CHECK(cudaEventRecord(B->searchKernels, st));
+		S2B_CHECK(cudaStreamWaitEvent(cs, B->searchKernels, 0));
+	}
+	if (w->movedEvent != nullptr)
+	{
+		S2B_CHECK(cudaStreamWaitEvent(cs, w->movedEvent, 0));
+	}
+	S2B_CHECK(cudaMemcpyAsync(w->hostMail + MAIL_BC_BASE, B->counters.p, sizeof(int) * BC_SIZE, cudaMemcpyDeviceToHost, cs));
+	S2B_CHECK(cudaEventRecord(B->searchDone, cs));
 	B->searchedCount = oldCount;
 	B->searchedVersion = w->contactTableVersion;
 }
@@ -1216,13 +1259,11 @@ void s2bPrefetchPairSearch(s2bWorld* w)
 	{
 		S2B_CHECK(cudaEventCreate(&B->evSearch[0]));
 		S2B_CHECK(cudaEventCreate(&B->evSearch[1]));
-		S2B_CHECK(cudaEventCreateWithFlags(&B->searchDone, cudaEventDisableTiming));
 	}
 	B->prefetchTempBytes = bpReserve(w, B);
 	S2B_CHECK(cudaEventRecord(B->evSearch[0], w->stream));
 	bpSearch(w, B);
 	S2B_CHECK(cudaEventRecord(B->evSearch[1], w->stream));
-	S2B_CHECK(cudaEventRecord(B->searchDone, w->stream));
 	B->prefetched = true;
 	B->prefetchEpoch = w->uploadEpoch;
 	B->searchTimed = true;
@@ -1251,6 +1292,11 @@ void s2bBroadphaseUpdatePairs(s2bWorld* w)
 	cudaStream_t st = w->stream;
 	BroadScratch* B = getBroad(w);
 	w->dMovedFlag.reserve(4, st, true);
+	// nothing of this pass (s2bClearMovedFlags) may reset the moved-proxy counter before its copy to the mailbox has read it
+	if (w->movedEvent != nullptr)
+	{
+		S2B_CHECK(cudaStreamWaitEvent(st, w->movedEvent, 0));
+	}
 
 	// ---- the search was started behind the previous step: its counters are (about to be) in the mailbox ----
 	if (B->prefetched)
@@ -1306,7 +1352,7 @@ void s2bBroadphaseUpdatePairs(s2bWorld* w)
 		bpSearch(w, B);
 		// the new table size has to be known on the host (column reservation): one small synchronising read-back, paid only
 		// when the search could not be started behind the previous step (first steps, after uploads, settled scenes)
-		S2B_CHECK(cudaStreamSynchronize(st));
+		S2B_CHECK(cudaEventSynchronize(B->searchDone));
 		const int* hc = w->hostMail + MAIL_BC_BASE;
 		int fresh = hc[BC_NEW_PAIRS], kept = hc[BC_KEPT];
 		if (fresh > B->newPairCap)

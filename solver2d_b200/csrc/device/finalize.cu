@@ -113,11 +113,27 @@ void s2bFinalize(s2bWorld* w)
 	{
 		S2B_LAUNCH(w, s2bFinalizeShapes, gridFor(w->shapeCap, 256), 256, 0, shapeView(w), bodyView(w), w->dMovedFlag.p);
 	}
-	// publish the moved-proxy counter to the pinned mailbox; the next step reads it after this step has drained
-	S2B_CHECK(cudaMemcpyAsync(w->hostMail + MAIL_MOVED, w->dMovedFlag.p, sizeof(int), cudaMemcpyDeviceToHost, st));
+	// publish the moved-proxy counter to the pinned mailbox; the next step reads it after this step has drained. The copy
+	// runs on the side stream, behind finalize only: on the world's stream the device-to-host copy (and the counter memset
+	// after it) between finalize and the pair search queued behind it left the device idle for ~20 us per step (H100). Until
+	// movedEvent has passed, the counter must not be reset (s2bBroadphaseUpdatePairs waits for it) and the mailbox slot
+	// must not be read (s2bBroadphaseUpdatePairs, s2b_get_counters).
 	if (w->movedEvent == nullptr)
 	{
 		S2B_CHECK(cudaEventCreateWithFlags(&w->movedEvent, cudaEventDisableTiming));
+		S2B_CHECK(cudaEventCreateWithFlags(&w->finalizedEvent, cudaEventDisableTiming));
 	}
-	S2B_CHECK(cudaEventRecord(w->movedEvent, st));
+	cudaStream_t cs = st;
+	if (w->sideCopies != 0)
+	{
+		if (w->copyStream == nullptr)
+		{
+			S2B_CHECK(cudaStreamCreateWithFlags(&w->copyStream, cudaStreamNonBlocking));
+		}
+		cs = w->copyStream;
+		S2B_CHECK(cudaEventRecord(w->finalizedEvent, st));
+		S2B_CHECK(cudaStreamWaitEvent(cs, w->finalizedEvent, 0));
+	}
+	S2B_CHECK(cudaMemcpyAsync(w->hostMail + MAIL_MOVED, w->dMovedFlag.p, sizeof(int), cudaMemcpyDeviceToHost, cs));
+	S2B_CHECK(cudaEventRecord(w->movedEvent, cs));
 }

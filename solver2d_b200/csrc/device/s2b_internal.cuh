@@ -412,11 +412,12 @@ struct s2bWorld
 	bool solveKernelTimed = false;
 	cudaEvent_t markEvents[2] = {nullptr, nullptr};
 	cudaEvent_t movedEvent = nullptr; // recorded behind the D2H copy of the moved-proxy counter at the end of every step
+	cudaEvent_t finalizedEvent = nullptr; // recorded behind finalize's kernels: the side stream's copies wait for it
 	// transforms are read back on a stream of their own when finalize was the last thing to write them: the read-back then
 	// runs beside whatever the world's stream has queued behind finalize (the pair search of the next step) instead of after it
 	cudaStream_t copyStream = nullptr;
 	unsigned long long xfSeq = 0, finalizeSeq = ~0ull; // bumped by everything that writes body transforms / at the last finalize
-	int sideCopies = 1;								   // S2B_SIDE_COPIES=0: read back on the world's stream
+	int sideCopies = 1;								   // S2B_SIDE_COPIES=0: all read-backs on the world's stream
 	StageTimer timer;
 	float stageMs[4] = {0, 0, 0, 0};
 

@@ -3981,6 +3981,10 @@ extern "C" void s2b_get_counters(s2bWorld* w, s2bCounters* out)
 {
 	S2B_CHECK(cudaSetDevice(w->device));
 	S2B_CHECK(cudaStreamSynchronize(w->stream));
+	if (w->movedEvent != nullptr)
+	{
+		S2B_CHECK(cudaEventSynchronize(w->movedEvent)); // the moved-proxy counter's copy (side stream, s2bFinalize)
+	}
 	memset(out, 0, sizeof(*out));
 	out->bodyCapacity = w->bodyCap;
 	out->shapeCapacity = w->shapeCap;

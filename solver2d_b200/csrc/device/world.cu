@@ -494,12 +494,14 @@ extern "C" void s2b_world_destroy(s2bWorld* w)
 	}
 	if (w->copyStream != nullptr)
 	{
+		cudaStreamSynchronize(w->copyStream); // (its copies write into the pinned mailbox freed below)
 		cudaStreamDestroy(w->copyStream);
 		w->copyStream = nullptr;
 	}
 	if (w->movedEvent != nullptr)
 	{
 		cudaEventDestroy(w->movedEvent);
+		cudaEventDestroy(w->finalizedEvent);
 	}
 	for (int i = 0; i < 2; ++i)
 	{
