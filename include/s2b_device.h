@@ -97,6 +97,7 @@ enum
 	S2B_JOINT_MOUSE = 1,
 	S2B_JOINT_WELD = 2, // never carries S2B_JOINT_ENABLE_LIMIT or S2B_JOINT_ENABLE_MOTOR
 	S2B_JOINT_PRISMATIC = 3,
+	S2B_JOINT_MOTOR = 4, // never carries S2B_JOINT_ENABLE_LIMIT or S2B_JOINT_ENABLE_MOTOR
 };
 
 #define S2B_JOINT_ENABLE_LIMIT 0x10
@@ -122,6 +123,10 @@ typedef struct s2bJointRow
 	// prismatic: the sliding axis in body A's frame (unit length). A prismatic row also reuses the revolute columns:
 	// lowerAngle / upperAngle hold the translation limits (m), maxMotorTorque the maximum motor force (N), impulse[2] the
 	// (perpendicular, angular) block impulse and motorImpulse / lowerImpulse / upperImpulse the axial impulses.
+	// A motor row has no column of its own: localOriginAnchorA holds the linear offset (B's origin in A's frame) and
+	// localOriginAnchorB is (0, 0); referenceAngle holds the angular offset, maxMotorTorque the maximum torque (N-m),
+	// hertz the maximum force (N) and dampingRatio the correction factor; impulse[2] is the linear impulse and
+	// motorImpulse the angular impulse. Its limit impulses stay 0.
 	float localAxisA[2];
 } s2bJointRow;
 
@@ -261,6 +266,12 @@ S2B_API void s2b_upload_forces(s2bWorld* world, const s2bForceRow* rows, int cou
 // Bulk form of s2Body_ApplyForceToCenter (reference src/body.c:206-212): force[k] is ADDED to body bodyIndices[k]. The
 // host arrays are copied into page-locked staging before the call returns; the H2D copy and the add are asynchronous.
 S2B_API void s2b_add_forces(s2bWorld* world, const int32_t* bodyIndices, const float* forcesXY, int count);
+// Bulk re-target of motor joints: offsets[3k .. 3k+2] = (linear offset x, y, angular offset) of joint slot jointIndices[k],
+// written into the device's offset columns only. Like s2b_add_forces it stages through page-locked memory and is
+// asynchronous. It leaves the schedule and a prefetched pair search valid: an offset is read by the solver alone. The caller
+// names live motor joints the device already holds, each at most once per call (entries run in parallel, so for a slot
+// named twice it is unspecified which entry lands); other slots are ignored.
+S2B_API void s2b_set_motor_offsets(s2bWorld* world, const int32_t* jointIndices, const float* offsets, int count);
 // Page-locked host memory for row staging (uploads from it are asynchronous DMA).
 S2B_API void* s2b_host_alloc(size_t bytes);
 S2B_API void s2b_host_free(void* p);

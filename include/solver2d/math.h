@@ -297,6 +297,21 @@ S2_INLINE float s2UnwindAngle(float angle)
 	return angle;
 }
 
+// v scaled back to length maxLength when it is longer, else v itself: the unit vector is formed as s2Normalize forms it
+// (one sqrtf, then a multiply by 1 / length), so host and device agree bit for bit. Caps the motor joint's linear impulse.
+S2_INLINE s2Vec2 s2ClampLength(s2Vec2 v, float maxLength)
+{
+	float lengthSquared = v.x * v.x + v.y * v.y;
+	if (lengthSquared > maxLength * maxLength)
+	{
+		float invLength = 1.0f / sqrtf(lengthSquared);
+		s2Vec2 n = {invLength * v.x, invLength * v.y};
+		s2Vec2 r = {maxLength * n.x, maxLength * n.y};
+		return r;
+	}
+	return v;
+}
+
 S2_INLINE s2Vec2 s2RotateVector(s2Rot q, s2Vec2 v)
 {
 	s2Vec2 r = {q.c * v.x - q.s * v.y, q.s * v.x + q.c * v.y};

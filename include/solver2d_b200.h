@@ -93,6 +93,49 @@ S2B_API float s2PrismaticJoint_GetMotorForce(s2JointId jointId, float inverseTim
 // The current translation (m) along the world axis, from anchor A to anchor B.
 S2B_API float s2PrismaticJoint_GetTranslation(s2JointId jointId);
 
+// Motor joint: drives body B toward a pose relative to body A with bounded effort (DESIGN.md §3.10). Each solver step h it
+// removes the fraction correctionFactor of the pose error, with an impulse of at most h * maxForce (linear) and
+// h * maxTorque (angular). It has no spring and no rigid part. Uses: top-down friction (a joint to the ground with zero
+// offsets and small caps), platforms that a heavy load can stall, force-limited characters and pose controllers.
+// Re-target it every frame with s2World_SetMotorJointOffsets. Destroy it with s2DestroyJoint.
+typedef struct s2MotorJointDef
+{
+	s2BodyId bodyIdA;
+	s2BodyId bodyIdB;
+	s2Vec2 linearOffset;	// target position of body B's origin in body A's frame, relative to A's origin (m)
+	float angularOffset;	// target angle(B) - angle(A) (rad), within [-pi, pi]
+	float maxForce;			// N, >= 0
+	float maxTorque;		// N-m, >= 0
+	float correctionFactor; // in [0, 1]: fraction of the pose error removed per solver step h
+	bool collideConnected;	// keep the contacts the two bodies already have
+} s2MotorJointDef;
+
+S2_INLINE struct s2MotorJointDef s2DefaultMotorJointDef(void)
+{
+	s2MotorJointDef def = S2_ZERO_INIT;
+	def.bodyIdA = s2_nullBodyId;
+	def.bodyIdB = s2_nullBodyId;
+	def.maxForce = 1.0f;
+	def.maxTorque = 1.0f;
+	def.correctionFactor = 0.3f;
+	return def;
+}
+
+// Returns s2_nullJointId (and creates nothing) for a non-finite offset, a negative or non-finite maxForce or maxTorque, or
+// a correctionFactor outside [0, 1]. The setters ignore such input (the joint keeps its value).
+S2B_API s2JointId s2CreateMotorJoint(s2WorldId worldId, const s2MotorJointDef* def);
+S2B_API void s2MotorJoint_SetLinearOffset(s2JointId jointId, s2Vec2 linearOffset);
+S2B_API s2Vec2 s2MotorJoint_GetLinearOffset(s2JointId jointId);
+S2B_API void s2MotorJoint_SetAngularOffset(s2JointId jointId, float angularOffset);
+S2B_API float s2MotorJoint_GetAngularOffset(s2JointId jointId);
+S2B_API void s2MotorJoint_SetMaxForce(s2JointId jointId, float maxForce);
+S2B_API void s2MotorJoint_SetMaxTorque(s2JointId jointId, float maxTorque);
+S2B_API void s2MotorJoint_SetCorrectionFactor(s2JointId jointId, float correctionFactor);
+// The linear impulse of the last step times inverseTimeStep (N); the impulse is per solver step h.
+S2B_API s2Vec2 s2MotorJoint_GetConstraintForce(s2JointId jointId, float inverseTimeStep);
+// The angular impulse of the last step times inverseTimeStep (N-m).
+S2B_API float s2MotorJoint_GetConstraintTorque(s2JointId jointId, float inverseTimeStep);
+
 // Push every pending host-side edit to the device now (s2World_Step does this itself).
 S2B_API void s2World_Flush(s2WorldId worldId);
 
@@ -102,6 +145,13 @@ S2B_API void s2World_Flush(s2WorldId worldId);
 //                                   into out[4 * capacity]; returns the body capacity.
 S2B_API void s2World_ApplyForcesToCenters(s2WorldId worldId, const int32_t* bodyIndices, const float* forcesXY, int32_t count);
 S2B_API int32_t s2World_GetBodyTransforms(s2WorldId worldId, float* out, int32_t capacity);
+// Bulk s2MotorJoint_SetLinearOffset + _SetAngularOffset: offsets[3i .. 3i+2] = (linear x, linear y, angular) for the motor
+// joint in slot jointIndices[i] (its s2JointId.index). All entries are checked first: an index out of range, a free slot, a
+// joint that is not a motor joint or a non-finite value rejects the call, which then changes nothing and returns false.
+// A joint named more than once takes its last entry.
+// Unlike the per-joint setters it writes only the offset columns on the device, asynchronously, and keeps the pair search
+// prefetched behind the last step. Whichever of the two wrote an offset last before a step wins.
+S2B_API bool s2World_SetMotorJointOffsets(s2WorldId worldId, const int32_t* jointIndices, const float* offsets, int32_t count);
 
 // Run `steps` calls of s2World_Step back to back and return the summed device time of the steps in milliseconds, each
 // step bracketed by CUDA events on the world's stream. With flushL2 != 0 the L2 (50 MB on an H100) is evicted between steps

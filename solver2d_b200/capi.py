@@ -172,6 +172,20 @@ class PrismaticJointDef(C.Structure):
     ]
 
 
+class MotorJointDef(C.Structure):
+    """s2MotorJointDef (include/solver2d_b200.h): an extension, absent from the reference."""
+    _fields_ = [
+        ("bodyIdA", BodyId),
+        ("bodyIdB", BodyId),
+        ("linearOffset", Vec2),
+        ("angularOffset", C.c_float),
+        ("maxForce", C.c_float),
+        ("maxTorque", C.c_float),
+        ("correctionFactor", C.c_float),
+        ("collideConnected", C.c_bool),
+    ]
+
+
 class Statistics(C.Structure):
     _fields_ = [
         ("bodyCount", C.c_int32),
@@ -251,6 +265,17 @@ def default_prismatic_def() -> PrismaticJointDef:
     return d
 
 
+def default_motor_def() -> MotorJointDef:
+    """s2DefaultMotorJointDef (include/solver2d_b200.h)."""
+    d = MotorJointDef()
+    d.bodyIdA = BodyId(-1, -1, 0)
+    d.bodyIdB = BodyId(-1, -1, 0)
+    d.maxForce = 1.0
+    d.maxTorque = 1.0
+    d.correctionFactor = 0.3
+    return d
+
+
 def default_mouse_def() -> MouseJointDef:
     """s2DefaultMouseJointDef (reference include/solver2d/joint_types.h:28-37)."""
     d = MouseJointDef()
@@ -309,6 +334,18 @@ _API = {
     "s2PrismaticJoint_SetMotorSpeed": (None, [JointId, C.c_float]),
     "s2PrismaticJoint_GetMotorForce": (C.c_float, [JointId, C.c_float]),
     "s2PrismaticJoint_GetTranslation": (C.c_float, [JointId]),
+    "s2CreateMotorJoint": (JointId, [WorldId, C.POINTER(MotorJointDef)]),
+    "s2MotorJoint_SetLinearOffset": (None, [JointId, Vec2]),
+    "s2MotorJoint_GetLinearOffset": (Vec2, [JointId]),
+    "s2MotorJoint_SetAngularOffset": (None, [JointId, C.c_float]),
+    "s2MotorJoint_GetAngularOffset": (C.c_float, [JointId]),
+    "s2MotorJoint_SetMaxForce": (None, [JointId, C.c_float]),
+    "s2MotorJoint_SetMaxTorque": (None, [JointId, C.c_float]),
+    "s2MotorJoint_SetCorrectionFactor": (None, [JointId, C.c_float]),
+    "s2MotorJoint_GetConstraintForce": (Vec2, [JointId, C.c_float]),
+    "s2MotorJoint_GetConstraintTorque": (C.c_float, [JointId, C.c_float]),
+    # indices (int32 per joint), offsets (x, y, angle per joint), count
+    "s2World_SetMotorJointOffsets": (C.c_bool, [WorldId, C.c_void_p, C.c_void_p, C.c_int32]),
 }
 
 class Transform(C.Structure):

@@ -106,13 +106,18 @@ template <int KIND> __device__ __forceinline__ void s2bPrepareJoint(const SolveA
 	jc.lim[t] = lim;
 	jc.coef[t] = make_float4(a.softJoint.bias, a.softJoint.mass, a.softJoint.impulse, 0.0f);
 
-	if (S2B_JOINT_TYPE(flags) == S2B_JOINT_PRISMATIC)
+	if (S2B_JOINT_TYPE(flags) == S2B_JOINT_PRISMATIC || S2B_JOINT_TYPE(flags) == S2B_JOINT_MOTOR)
 	{
 		// DESIGN.md §3.9: the local axis rides in the motor row's spare zw; every mass is formed fresh in each solve.
 		// Limit and motor impulses are kept only with their flag and a warm start, the block impulse with the warm start.
+		// A motor joint (§3.10) carries its maximum force and correction factor in those zw instead, never has either
+		// flag, and keeps its angular impulse (imp.z) exactly when it keeps its linear one.
+		bool motorJoint = S2B_JOINT_TYPE(flags) == S2B_JOINT_MOTOR;
 		float4 axis = a.joints.target[slot];
-		jc.motor[t] = make_float4(motor.x, motor.y, axis.z, axis.w);
-		jc.d0ax[t] = make_float4(centerDiff0.x, centerDiff0.y, 0.0f, 0.0f);
+		jc.motor[t] = motorJoint ? motor : make_float4(motor.x, motor.y, axis.z, axis.w);
+		// a motor joint's angular row uses the revolute's axial mass, 1 / (iA + iB) (0 when both rotations are fixed)
+		float motorAxialMass = motorJoint && iA + iB > 0.0f ? 1.0f / (iA + iB) : 0.0f;
+		jc.d0ax[t] = make_float4(centerDiff0.x, centerDiff0.y, motorAxialMass, 0.0f);
 		jc.pivot[t] = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
 		if (KIND == JPREP_XPBD || warmStart == false)
 		{
@@ -124,7 +129,7 @@ template <int KIND> __device__ __forceinline__ void s2bPrepareJoint(const SolveA
 			limp.x = 0.0f;
 			limp.y = 0.0f;
 		}
-		if ((flags & S2B_JOINT_ENABLE_MOTOR) == 0)
+		if ((flags & S2B_JOINT_ENABLE_MOTOR) == 0 && motorJoint == false)
 		{
 			imp.z = 0.0f;
 		}
@@ -552,6 +557,135 @@ __device__ __forceinline__ void s2bSolvePrismaticXpbd(const SolveArgs& a, int t)
 }
 
 // ---------------------------------------------------------------------------------------------------------------
+// motor joint (extension, DESIGN.md §3.10; definition: tests/motor_oracle.c). Drives body B toward a pose relative to body
+// A with capped effort: an angular row toward angle(B) - angle(A) = angularOffset, its accumulated impulse clamped to
+// +/- h maxTorque, then a point row that takes B's origin to the linear offset in A's frame, its accumulated impulse scaled
+// back to length h maxForce. Both rows are biased by correctionFactor / h times their position error in every velocity
+// pass: the bias is the drive, and there is no rigid part. Row columns: anchor = (offset - localCenterA, -localCenterB),
+// lim.x = angularOffset, motor = (maxTorque, 0, maxForce, correctionFactor), imp = (linear impulse, angular impulse).
+// The warm start is the revolute's (P = linear impulse at rA / rB, axial = angular impulse).
+// ---------------------------------------------------------------------------------------------------------------
+__device__ __forceinline__ void s2bSolveMotorVelocity(const SolveArgs& a, int t, float h, float inv_h)
+{
+	const JointConstraintView& jc = a.jc;
+	int4 head = jc.head[t];
+	int ia = head.y, ib = head.z;
+	float4 anchor = jc.anchor[t];
+	float4 mass = jc.mass[t];
+	float4 d0 = jc.d0ax[t];
+	float4 motor = jc.motor[t];
+	float angularOffset = jc.lim[t].x;
+	float4 imp = jc.imp[t];
+	float4 velA = a.bodies.vel[ia], velB = a.bodies.vel[ib];
+	float4 poseA = a.bodies.pose[ia], poseB = a.bodies.pose[ib];
+	s2Vec2 vA = V2(velA.x, velA.y), vB = V2(velB.x, velB.y);
+	float wA = velA.z, wB = velB.z;
+	float mA = mass.x, iA = mass.y, mB = mass.z, iB = mass.w;
+	s2Rot qA = R2(poseA.z, poseA.w), qB = R2(poseB.z, poseB.w);
+	float biasScale = motor.w * inv_h;
+
+	if (iA + iB != 0.0f)
+	{
+		float k = 1.0f / (iA + iB);
+		float C = s2UnwindAngle(s2RelativeAngle(qB, qA) - angularOffset);
+		float impulse = -k * (wB - wA + biasScale * C);
+		float oldImpulse = imp.z;
+		float maxImpulse = h * motor.x;
+		imp.z = S2_CLAMP(oldImpulse + impulse, -maxImpulse, maxImpulse);
+		impulse = imp.z - oldImpulse;
+		wA -= iA * impulse;
+		wB += iB * impulse;
+	}
+
+	{
+		s2Vec2 rA = s2RotateVector(qA, V2(anchor.x, anchor.y));
+		s2Vec2 rB = s2RotateVector(qB, V2(anchor.z, anchor.w));
+		s2Vec2 Cdot = s2Sub(s2Add(vB, s2CrossSV(wB, rB)), s2Add(vA, s2CrossSV(wA, rA)));
+		s2Vec2 dcA = V2(poseA.x, poseA.y), dcB = V2(poseB.x, poseB.y);
+		s2Vec2 C = s2Add(s2Add(s2Sub(dcB, dcA), s2Sub(rB, rA)), V2(d0.x, d0.y));
+		s2Mat22 K;
+		K.cx.x = mA + mB + rA.y * rA.y * iA + rB.y * rB.y * iB;
+		K.cy.x = -rA.y * rA.x * iA - rB.y * rB.x * iB;
+		K.cx.y = K.cy.x;
+		K.cy.y = mA + mB + rA.x * rA.x * iA + rB.x * rB.x * iB;
+		s2Vec2 b = s2Solve22(K, s2Add(Cdot, s2MulSV(biasScale, C)));
+		s2Vec2 oldImpulse = V2(imp.x, imp.y);
+		s2Vec2 total = s2ClampLength(s2Sub(oldImpulse, b), h * motor.z);
+		s2Vec2 impulse = s2Sub(total, oldImpulse);
+		imp.x = total.x;
+		imp.y = total.y;
+		vA = s2MulSub(vA, mA, impulse);
+		wA -= iA * s2Cross(rA, impulse);
+		vB = s2MulAdd(vB, mB, impulse);
+		wB += iB * s2Cross(rB, impulse);
+	}
+
+	jc.imp[t] = imp;
+	s2bStoreJointVelocities(a, ia, ib, velA, velB, vA, wA, vB, wB, mA, iA, mB, iB);
+}
+
+// XPBD, zero compliance: the angular row, then the revolute's XPBD row along the current separation. Each removes the
+// fraction correctionFactor of its error, its correction capped at h^2 times the maximum torque or force.
+__device__ __forceinline__ void s2bSolveMotorXpbd(const SolveArgs& a, int t)
+{
+	const JointConstraintView& jc = a.jc;
+	int4 head = jc.head[t];
+	int ia = head.y, ib = head.z;
+	float4 anchor = jc.anchor[t];
+	float4 mass = jc.mass[t];
+	float4 d0 = jc.d0ax[t];
+	float4 motor = jc.motor[t];
+	float4 poseA = a.bodies.pose[ia], poseB = a.bodies.pose[ib];
+	s2Vec2 dcA = V2(poseA.x, poseA.y), dcB = V2(poseB.x, poseB.y);
+	s2Rot qA = R2(poseA.z, poseA.w), qB = R2(poseB.z, poseB.w);
+	float mA = mass.x, iA = mass.y, mB = mass.z, iB = mass.w;
+	float h = a.ctx.h;
+	float cf = motor.w;
+
+	if (iA + iB != 0.0f)
+	{
+		float C = s2UnwindAngle(s2RelativeAngle(qB, qA) - jc.lim[t].x);
+		float maxP = h * h * motor.x;
+		float p = S2_CLAMP(-cf * C / (iA + iB), -maxP, maxP);
+		qA = s2IntegrateRot(qA, -iA * p);
+		qB = s2IntegrateRot(qB, iB * p);
+	}
+
+	if (mA != 0.0f || mB != 0.0f)
+	{
+		s2Vec2 rA = s2RotateVector(qA, V2(anchor.x, anchor.y));
+		s2Vec2 rB = s2RotateVector(qB, V2(anchor.z, anchor.w));
+		s2Vec2 separation = s2Add(s2Add(s2Sub(dcB, dcA), s2Sub(rB, rA)), V2(d0.x, d0.y));
+		float c = s2Length(separation);
+		s2Vec2 n = V2(0.0f, 0.0f);
+		if (c >= 0.001f * 1.1920929e-07f)
+		{
+			float invLength = 1.0f / c;
+			n = V2(invLength * separation.x, invLength * separation.y);
+		}
+		float rnA = s2Cross(rA, n);
+		float rnB = s2Cross(rB, n);
+		float kA = mA + iA * rnA * rnA;
+		float kB = mB + iB * rnB * rnB;
+		float lambda = S2_MAX(-cf * c / (kA + kB), -(h * h * motor.z));
+		s2Vec2 p = s2MulSV(lambda, n);
+		dcA = s2MulSub(dcA, mA, p);
+		qA = s2IntegrateRot(qA, -iA * s2Cross(rA, p));
+		dcB = s2MulAdd(dcB, mB, p);
+		qB = s2IntegrateRot(qB, iB * s2Cross(rB, p));
+	}
+
+	if ((mA != 0.0f) || (iA != 0.0f))
+	{
+		a.bodies.pose[ia] = make_float4(dcA.x, dcA.y, qA.s, qA.c);
+	}
+	if ((mB != 0.0f) || (iB != 0.0f))
+	{
+		a.bodies.pose[ib] = make_float4(dcB.x, dcB.y, qB.s, qB.c);
+	}
+}
+
+// ---------------------------------------------------------------------------------------------------------------
 // warm start: s2WarmStartRevolute (reference src/revolute_joint.c:107-150), s2WarmStartMouse (mouse_joint.c:85-107)
 // ---------------------------------------------------------------------------------------------------------------
 __device__ __forceinline__ void s2bWarmStartJoint(const SolveArgs& a, int t)
@@ -683,7 +817,9 @@ enum JointSolveKind
 	JSOLVE_BAUMGARTE = 1,
 };
 
-template <int KIND> __device__ __forceinline__ void s2bSolveRevoluteVelocity(const SolveArgs& a, int t, float h, float inv_h, bool useBias)
+// MOTOR_ROWS: the soft flavour also solves motor joints (see below); the Baumgarte flavour never does.
+template <int KIND, bool MOTOR_ROWS>
+__device__ __forceinline__ void s2bSolveRevoluteVelocity(const SolveArgs& a, int t, float h, float inv_h, bool useBias)
 {
 	const JointConstraintView& jc = a.jc;
 	int4 head = jc.head[t];
@@ -714,12 +850,18 @@ template <int KIND> __device__ __forceinline__ void s2bSolveRevoluteVelocity(con
 	// limits; the Baumgarte flavour evaluates it where each row needs it. Both give the same bits; each choice is the
 	// one that keeps its kernels' stack frame and spills at what they are without the weld (DESIGN.md §3.8).
 	bool weld = S2B_JOINT_TYPE(head.x) == S2B_JOINT_WELD;
+	// With MOTOR_ROWS the soft flavour also solves the motor joint (DESIGN.md §3.10), whose two rows are this function's
+	// motor row and point row with a drive bias: its angular row is the motor row at the speed -cf / h * C, its point row is
+	// biased by cf / h times the separation in every pass and its accumulated impulse is capped in length. The same bits as
+	// s2bSolveMotorVelocity; sharing the branches keeps TGS_Soft's stack frame and spills where they are without the motor
+	// joint.
+	bool motorJoint = KIND == JSOLVE_SOFT && MOTOR_ROWS && S2B_JOINT_TYPE(head.x) == S2B_JOINT_MOTOR;
 	float jointAngle = 0.0f;
-	if (KIND == JSOLVE_SOFT && (enableLimit || weld) && fixedRotation == false)
+	if (KIND == JSOLVE_SOFT && (enableLimit || weld || motorJoint) && fixedRotation == false)
 	{
 		jointAngle = s2RelativeAngle(qB, qA) - lim.x;
 	}
-	if ((enableMotor || weld) && fixedRotation == false)
+	if ((enableMotor || weld || motorJoint) && fixedRotation == false)
 	{
 		float impulse;
 		if (weld)
@@ -749,7 +891,9 @@ template <int KIND> __device__ __forceinline__ void s2bSolveRevoluteVelocity(con
 		}
 		else
 		{
-			float Cdot = wB - wA - motor.y;
+			// a motor joint's speed -(cf / h * C) makes Cdot = wB - wA + cf / h * C exactly
+			float speed = motorJoint ? -((motor.w * inv_h) * s2UnwindAngle(jointAngle)) : motor.y;
+			float Cdot = wB - wA - speed;
 			impulse = -axialMass * Cdot;
 			float oldImpulse = imp.z;
 			float maxImpulse = h * motor.x;
@@ -847,13 +991,13 @@ template <int KIND> __device__ __forceinline__ void s2bSolveRevoluteVelocity(con
 		float impulseScale = 0.0f;
 		if (KIND == JSOLVE_SOFT)
 		{
-			if (useBias)
+			if (useBias || motorJoint)
 			{
 				s2Vec2 dcA = V2(poseA.x, poseA.y), dcB = V2(poseB.x, poseB.y);
 				s2Vec2 separation = s2Add(s2Add(s2Sub(dcB, dcA), s2Sub(rB, rA)), V2(d0.x, d0.y));
-				bias = s2MulSV(coef.x, separation);
-				massScale = coef.y;
-				impulseScale = coef.z;
+				bias = s2MulSV(motorJoint ? motor.w * inv_h : coef.x, separation);
+				massScale = motorJoint ? 1.0f : coef.y;
+				impulseScale = motorJoint ? 0.0f : coef.z;
 			}
 		}
 		else
@@ -882,8 +1026,18 @@ template <int KIND> __device__ __forceinline__ void s2bSolveRevoluteVelocity(con
 			impulse.x = -b.x;
 			impulse.y = -b.y;
 		}
+		s2Vec2 oldImpulse = V2(imp.x, imp.y);
 		imp.x += impulse.x;
 		imp.y += impulse.y;
+		if (motorJoint)
+		{
+			// the total is formed as oldImpulse - b, as s2bSolveMotorVelocity forms it: oldImpulse + (-1 * b - 0 * imp) has
+			// the same value but can differ in the sign of a zero
+			s2Vec2 total = s2ClampLength(s2Sub(oldImpulse, b), h * motor.z);
+			impulse = s2Sub(total, oldImpulse);
+			imp.x = total.x;
+			imp.y = total.y;
+		}
 
 		vA = s2MulSub(vA, mA, impulse);
 		wA -= iA * s2Cross(rA, impulse);
@@ -896,7 +1050,10 @@ template <int KIND> __device__ __forceinline__ void s2bSolveRevoluteVelocity(con
 	s2bStoreJointVelocities(a, ia, ib, velA, velB, vA, wA, vB, wB, mA, iA, mB, iB);
 }
 
-// s2SolveJoint_Soft dispatch (reference src/joint.c:385-405): the mouse joint is solved only in the biased pass.
+// s2SolveJoint_Soft dispatch (reference src/joint.c:385-405): the mouse joint is solved only in the biased pass. A motor
+// joint is solved in every pass, by the revolute's soft rows when SHARED_MOTOR (the persistent kernels), else by
+// s2bSolveMotorVelocity (the launch-by-launch kernel, whose every-op build spills less that way). Both give the same bits.
+template <bool SHARED_MOTOR>
 __device__ __forceinline__ void s2bSolveJointSoft(const SolveArgs& a, int t, float h, float inv_h, bool useBias)
 {
 	int flags = a.jc.head[t].x;
@@ -913,7 +1070,12 @@ __device__ __forceinline__ void s2bSolveJointSoft(const SolveArgs& a, int t, flo
 		s2bSolvePrismaticVelocity<PSOLVE_SOFT>(a, t, h, inv_h, useBias);
 		return;
 	}
-	s2bSolveRevoluteVelocity<JSOLVE_SOFT>(a, t, h, inv_h, useBias);
+	if (SHARED_MOTOR == false && S2B_JOINT_TYPE(flags) == S2B_JOINT_MOTOR)
+	{
+		s2bSolveMotorVelocity(a, t, h, inv_h);
+		return;
+	}
+	s2bSolveRevoluteVelocity<JSOLVE_SOFT, SHARED_MOTOR>(a, t, h, inv_h, useBias);
 }
 
 // s2SolveJoint_Baumgarte dispatch (reference src/joint.c:409-425)
@@ -930,7 +1092,12 @@ __device__ __forceinline__ void s2bSolveJointBaumgarte(const SolveArgs& a, int t
 		s2bSolvePrismaticVelocity<PSOLVE_BAUMGARTE>(a, t, h, inv_h, useBias);
 		return;
 	}
-	s2bSolveRevoluteVelocity<JSOLVE_BAUMGARTE>(a, t, h, inv_h, useBias);
+	if (S2B_JOINT_TYPE(flags) == S2B_JOINT_MOTOR)
+	{
+		s2bSolveMotorVelocity(a, t, h, inv_h);
+		return;
+	}
+	s2bSolveRevoluteVelocity<JSOLVE_BAUMGARTE, false>(a, t, h, inv_h, useBias);
 }
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -1038,6 +1205,11 @@ __device__ __forceinline__ void s2bSolveJointRigid(const SolveArgs& a, int t, fl
 		s2bSolvePrismaticVelocity<PSOLVE_RIGID>(a, t, h, 0.0f /* inv_h: unused by the rigid rows */, false);
 		return;
 	}
+	if (S2B_JOINT_TYPE(a.jc.head[t].x) == S2B_JOINT_MOTOR)
+	{
+		s2bSolveMotorVelocity(a, t, h, a.ctx.inv_h);
+		return;
+	}
 	s2bSolveRevoluteRigid(a, t, h);
 }
 
@@ -1049,9 +1221,9 @@ __device__ __forceinline__ void s2bSolveJointPosition(const SolveArgs& a, int t)
 {
 	const JointConstraintView& jc = a.jc;
 	int4 head = jc.head[t];
-	if (S2B_JOINT_TYPE(head.x) == S2B_JOINT_MOUSE)
+	if (S2B_JOINT_TYPE(head.x) == S2B_JOINT_MOUSE || S2B_JOINT_TYPE(head.x) == S2B_JOINT_MOTOR)
 	{
-		return;
+		return; // a motor joint, like a mouse joint, has no NGS position row (DESIGN.md §3.10)
 	}
 	if (S2B_JOINT_TYPE(head.x) == S2B_JOINT_PRISMATIC)
 	{
@@ -1141,6 +1313,11 @@ __device__ __forceinline__ void s2bSolveJointXpbd(const SolveArgs& a, int t)
 	if (S2B_JOINT_TYPE(head.x) == S2B_JOINT_PRISMATIC)
 	{
 		s2bSolvePrismaticXpbd(a, t);
+		return;
+	}
+	if (S2B_JOINT_TYPE(head.x) == S2B_JOINT_MOTOR)
+	{
+		s2bSolveMotorXpbd(a, t);
 		return;
 	}
 	const float compliance = 0.0f;

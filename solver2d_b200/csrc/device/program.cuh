@@ -546,13 +546,13 @@ template <int SOLVER> __device__ __forceinline__ void s2bRunJointOpT(int op, con
 		case JOP_SOFT_BIAS:
 			if constexpr (s2bUsesJointOp(SOLVER, JOP_SOFT_BIAS))
 			{
-				s2bSolveJointSoft(a, t, a.ctx.h, a.ctx.inv_h, true);
+				s2bSolveJointSoft<(SOLVER >= 0)>(a, t, a.ctx.h, a.ctx.inv_h, true);
 			}
 			break;
 		case JOP_SOFT_RELAX:
 			if constexpr (s2bUsesJointOp(SOLVER, JOP_SOFT_RELAX))
 			{
-				s2bSolveJointSoft(a, t, a.ctx.h, a.ctx.inv_h, false);
+				s2bSolveJointSoft<(SOLVER >= 0)>(a, t, a.ctx.h, a.ctx.inv_h, false);
 			}
 			break;
 		case JOP_BAUMGARTE_BIAS:

@@ -290,7 +290,8 @@ struct JointConstraintView
 	float4* mass;	// invMassA invIA invMassB invIB
 	float4* d0ax;	// centerDiff0.xy axialMass 0
 	float4* lim;	// referenceAngle lowerAngle upperAngle 0
-	float4* motor;	// maxMotorTorque motorSpeed 0 0 (prismatic: maxMotorForce motorSpeed localAxisA.xy)
+	float4* motor;	// maxMotorTorque motorSpeed 0 0 (prismatic: maxMotorForce motorSpeed localAxisA.xy;
+					// motor joint: maxTorque 0 maxForce correctionFactor)
 	float4* coef;	// biasCoefficient massCoefficient impulseCoefficient 0
 	float4* pivot;	// pivotMass cx.x cx.y cy.x cy.y (mouse, non-fresh revolute)
 	float4* imp;	// impulse.x impulse.y motorImpulse 0        (r/w)

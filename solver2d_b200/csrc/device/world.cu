@@ -841,6 +841,55 @@ extern "C" void s2b_add_forces(s2bWorld* w, const int32_t* bodyIndices, const fl
 			   bodyView(w));
 }
 
+// one thread per entry: a motor joint's linear offset (anchors.xy) and angular offset (lim.x), nothing else of the row.
+// Entries that do not name a live motor joint are skipped; the host validates before it calls.
+__global__ void s2bSetMotorOffsetsKernel(const int* __restrict__ indices, const float* __restrict__ offsets, int count, JointView j)
+{
+	int t = blockIdx.x * blockDim.x + threadIdx.x;
+	if (t >= count)
+	{
+		return;
+	}
+	int i = indices[t];
+	if (i < 0 || i >= j.capacity)
+	{
+		return;
+	}
+	int flags = j.head[i].x;
+	if ((flags & S2B_ROW_VALID) == 0 || ((flags >> 1) & 0x7) != S2B_JOINT_MOTOR)
+	{
+		return;
+	}
+	float* anchors = reinterpret_cast<float*>(j.anchors + i);
+	anchors[0] = offsets[3 * t + 0];
+	anchors[1] = offsets[3 * t + 1];
+	reinterpret_cast<float*>(j.lim + i)[0] = offsets[3 * t + 2];
+}
+
+extern "C" void s2b_set_motor_offsets(s2bWorld* w, const int32_t* jointIndices, const float* offsets, int count)
+{
+	S2bEpochFreeze freeze; // transfer buffers are not part of any captured graph
+
+	if (count <= 0)
+	{
+		return;
+	}
+	S2B_CHECK(cudaSetDevice(w->device));
+	// no uploadEpoch bump, no schedDirty and no synchronisation: the offsets are solver inputs only, so the prefetched pair
+	// search and the captured step graph stay valid
+	size_t idxBytes = sizeof(int32_t) * (size_t)count;
+	size_t idxPadded = (idxBytes + 15) & ~(size_t)15;
+	size_t bytes = idxPadded + sizeof(float) * 3 * (size_t)count;
+	char* host = (char*)bulkStaging(w, bytes);
+	memcpy(host, jointIndices, idxBytes);
+	memcpy(host + idxPadded, offsets, sizeof(float) * 3 * (size_t)count);
+	w->dBulk.reserve(bytes, w->stream, false, false);
+	S2B_CHECK(cudaMemcpyAsync(w->dBulk.p, host, bytes, cudaMemcpyHostToDevice, w->stream));
+	S2B_CHECK(cudaEventRecord(w->bulkEvent[w->bulkCurrent], w->stream));
+	S2B_LAUNCH(w, s2bSetMotorOffsetsKernel, gridFor(count, 256), 256, 0, (const int*)w->dBulk.p,
+			   (const float*)(w->dBulk.p + idxPadded), count, jointView(w));
+}
+
 extern "C" void s2b_download_transforms(s2bWorld* w, float* out, int count)
 {
 	S2bEpochFreeze freeze; // transfer / flush buffers are not part of any captured graph

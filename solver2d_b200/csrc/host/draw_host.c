@@ -79,6 +79,13 @@ static void s2DrawJoint(s2DebugDraw* draw, s2World* world, const s2Joint* joint)
 	draw->DrawPoint(pA, 5.0f, s2Rgb(0.3f, 0.3f, 0.9f), draw->context);
 	draw->DrawPoint(pB, 5.0f, s2Rgb(0.4f, 0.4f, 0.4f), draw->context);
 
+	if (joint->type == s2_motorJoint)
+	{
+		// the segment from the target point (A's linear offset) to B's origin: the pose error the motor is removing
+		draw->DrawSegment(pA, pB, s2Rgb(0.8f, 0.5f, 0.9f), draw->context);
+		return;
+	}
+
 	if (joint->type == s2_prismaticJoint)
 	{
 		// the axis through anchor A (drawSize each way), a mark across the axis at each translation limit, and the

@@ -237,6 +237,122 @@ float s2PrismaticJoint_GetMotorForce(s2JointId jointId, float inverseTimeStep)
 	return inverseTimeStep * world->joints[jointId.index].motorImpulse;
 }
 
+// The motor joint has no counterpart in the reference (DESIGN.md §3.10). Its row has no limit or motor flag; its offsets, caps
+// and correction factor sit in the columns s2_host.h lists. Invalid input creates nothing and returns s2_nullJointId.
+s2JointId s2CreateMotorJoint(s2WorldId worldId, const s2MotorJointDef* def)
+{
+	if (s2IsValidVec2(def->linearOffset) == false || s2IsValid(def->angularOffset) == false || s2IsValid(def->maxForce) == false ||
+		def->maxForce < 0.0f || s2IsValid(def->maxTorque) == false || def->maxTorque < 0.0f ||
+		(def->correctionFactor >= 0.0f && def->correctionFactor <= 1.0f) == false)
+	{
+		return s2_nullJointId;
+	}
+
+	s2World* world = s2GetWorldFromId(worldId);
+	s2Body* bodyA = world->bodies + def->bodyIdA.index;
+	s2Body* bodyB = world->bodies + def->bodyIdB.index;
+
+	s2Joint* joint = s2AllocJoint(world, bodyA, bodyB);
+	joint->type = s2_motorJoint;
+	joint->drawSize = 1.0f;
+	joint->localOriginAnchorA = def->linearOffset;
+	joint->localOriginAnchorB = s2Vec2_zero;
+	joint->referenceAngle = def->angularOffset;
+	joint->maxMotorTorque = def->maxTorque;
+	joint->hertz = def->maxForce;
+	joint->dampingRatio = def->correctionFactor;
+	joint->collideConnected = def->collideConnected;
+
+	s2JointId jointId = {joint->object.index, world->index, joint->object.revision};
+	return jointId;
+}
+
+void s2MotorJoint_SetLinearOffset(s2JointId jointId, s2Vec2 linearOffset)
+{
+	if (s2IsValidVec2(linearOffset) == false)
+	{
+		return; // rejected: the joint keeps its offset
+	}
+	s2World* world;
+	s2Joint* joint = s2GetJointForEdit(jointId, &world);
+	joint->localOriginAnchorA = linearOffset;
+	s2MarkJointDirty(world, joint);
+}
+
+s2Vec2 s2MotorJoint_GetLinearOffset(s2JointId jointId)
+{
+	s2World* world = s2GetWorldFromIndex(jointId.world);
+	return world->joints[jointId.index].localOriginAnchorA;
+}
+
+void s2MotorJoint_SetAngularOffset(s2JointId jointId, float angularOffset)
+{
+	if (s2IsValid(angularOffset) == false)
+	{
+		return;
+	}
+	s2World* world;
+	s2Joint* joint = s2GetJointForEdit(jointId, &world);
+	joint->referenceAngle = angularOffset;
+	s2MarkJointDirty(world, joint);
+}
+
+float s2MotorJoint_GetAngularOffset(s2JointId jointId)
+{
+	s2World* world = s2GetWorldFromIndex(jointId.world);
+	return world->joints[jointId.index].referenceAngle;
+}
+
+void s2MotorJoint_SetMaxForce(s2JointId jointId, float maxForce)
+{
+	if (s2IsValid(maxForce) == false || maxForce < 0.0f)
+	{
+		return;
+	}
+	s2World* world;
+	s2Joint* joint = s2GetJointForEdit(jointId, &world);
+	joint->hertz = maxForce;
+	s2MarkJointDirty(world, joint);
+}
+
+void s2MotorJoint_SetMaxTorque(s2JointId jointId, float maxTorque)
+{
+	if (s2IsValid(maxTorque) == false || maxTorque < 0.0f)
+	{
+		return;
+	}
+	s2World* world;
+	s2Joint* joint = s2GetJointForEdit(jointId, &world);
+	joint->maxMotorTorque = maxTorque;
+	s2MarkJointDirty(world, joint);
+}
+
+void s2MotorJoint_SetCorrectionFactor(s2JointId jointId, float correctionFactor)
+{
+	if ((correctionFactor >= 0.0f && correctionFactor <= 1.0f) == false)
+	{
+		return;
+	}
+	s2World* world;
+	s2Joint* joint = s2GetJointForEdit(jointId, &world);
+	joint->dampingRatio = correctionFactor;
+	s2MarkJointDirty(world, joint);
+}
+
+s2Vec2 s2MotorJoint_GetConstraintForce(s2JointId jointId, float inverseTimeStep)
+{
+	s2World* world = s2GetWorldFromIndex(jointId.world);
+	s2SyncStateToHost(world);
+	return s2MulSV(inverseTimeStep, world->joints[jointId.index].impulse);
+}
+
+float s2MotorJoint_GetConstraintTorque(s2JointId jointId, float inverseTimeStep)
+{
+	s2World* world = s2GetWorldFromIndex(jointId.world);
+	s2SyncStateToHost(world);
+	return inverseTimeStep * world->joints[jointId.index].motorImpulse;
+}
+
 float s2PrismaticJoint_GetTranslation(s2JointId jointId)
 {
 	s2World* world = s2GetWorldFromIndex(jointId.world);

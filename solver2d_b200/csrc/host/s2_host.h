@@ -87,6 +87,7 @@ typedef enum s2JointType
 	s2_mouseJoint,
 	s2_weldJoint,
 	s2_prismaticJoint,
+	s2_motorJoint,
 } s2JointType;
 
 typedef struct s2Body
@@ -166,7 +167,9 @@ typedef struct s2Joint
 	float referenceAngle, lowerAngle, upperAngle;
 	// prismatic
 	s2Vec2 localAxisA;
-	// mouse
+	// mouse; a motor joint keeps its maximum force in hertz and its correction factor in dampingRatio, its linear offset
+	// in localOriginAnchorA (localOriginAnchorB is zero), its angular offset in referenceAngle and its maximum torque in
+	// maxMotorTorque, as its device row does
 	float hertz, dampingRatio;
 	s2Vec2 targetA;
 	// accumulated impulses (cache of the device columns)

@@ -254,9 +254,12 @@ static void s2FillJointRow(s2bJointRow* r, const s2Joint* j)
 		case s2_prismaticJoint:
 			type = S2B_JOINT_PRISMATIC;
 			break;
+		case s2_motorJoint:
+			type = S2B_JOINT_MOTOR;
+			break;
 	}
 	r->flags = S2B_ROW_VALID | (type << 1);
-	// a weld is created with enableLimit == enableMotor == false, so its row never carries either flag
+	// welds and motor joints are created with enableLimit == enableMotor == false, so their rows never carry either flag
 	r->flags |= j->enableLimit ? S2B_JOINT_ENABLE_LIMIT : 0;
 	r->flags |= j->enableMotor ? S2B_JOINT_ENABLE_MOTOR : 0;
 	r->flags |= j->collideConnected ? S2B_JOINT_COLLIDE_CONNECTED : 0;
@@ -390,8 +393,8 @@ void s2FlushToDevice(s2World* world)
 		// Two key lists (body pair = lo << 32 | hi):
 		//   block   — every live joint: s2ShouldBodiesCollide (reference src/body.c:386-417) vetoes a new contact between
 		//             jointed bodies and does not look at collideConnected;
-		//   destroy — revolute, weld and prismatic joints created with collideConnected == false: contacts that already
-		//             exist between the two bodies are removed (reference src/joint.c:214-217).
+		//   destroy — revolute, weld, prismatic and motor joints created with collideConnected == false: contacts that
+		//             already exist between the two bodies are removed (reference src/joint.c:214-217).
 		int cap = world->jointPool.capacity;
 		uint64_t* block = (uint64_t*)malloc(sizeof(uint64_t) * (size_t)(cap > 0 ? cap : 1));
 		uint64_t* destroy = (uint64_t*)malloc(sizeof(uint64_t) * (size_t)(cap > 0 ? cap : 1));
@@ -406,7 +409,7 @@ void s2FlushToDevice(s2World* world)
 			uint64_t lo = (uint64_t)(j->bodyIndexA < j->bodyIndexB ? j->bodyIndexA : j->bodyIndexB);
 			uint64_t hi = (uint64_t)(j->bodyIndexA < j->bodyIndexB ? j->bodyIndexB : j->bodyIndexA);
 			block[nBlock++] = (lo << 32) | hi;
-			if ((j->type == s2_revoluteJoint || j->type == s2_weldJoint || j->type == s2_prismaticJoint) && j->collideConnected == false)
+			if (j->type != s2_mouseJoint && j->collideConnected == false)
 			{
 				destroy[nDestroy++] = (lo << 32) | hi;
 			}
@@ -811,6 +814,66 @@ void s2World_ApplyForcesToCenters(s2WorldId worldId, const int32_t* bodyIndices,
 		s2FlushToDevice(world);
 	}
 	s2b_add_forces(world->device, bodyIndices, forcesXY, count);
+}
+
+bool s2World_SetMotorJointOffsets(s2WorldId worldId, const int32_t* jointIndices, const float* offsets, int32_t count)
+{
+	// bulk s2MotorJoint_SetLinearOffset + _SetAngularOffset. Every entry is checked before anything is written: one bad entry
+	// rejects the whole call.
+	s2World* world = s2GetWorldFromId(worldId);
+	for (int32_t k = 0; k < count; ++k)
+	{
+		int32_t i = jointIndices[k];
+		if (i < 0 || i >= world->jointPool.capacity)
+		{
+			return false;
+		}
+		const s2Joint* joint = world->joints + i;
+		if (s2IsFree(&joint->object) || joint->type != s2_motorJoint || s2IsValid(offsets[3 * k]) == false ||
+			s2IsValid(offsets[3 * k + 1]) == false || s2IsValid(offsets[3 * k + 2]) == false)
+		{
+			return false;
+		}
+	}
+	if (count <= 0)
+	{
+		return true;
+	}
+
+	// The host records take the offsets, so the getters and any later row upload agree with the device. A joint whose row is
+	// still dirty has not reached the device yet (or is about to be replaced there): its upload at the next flush carries the
+	// new offsets, and the device write is left to it. Every other entry goes to the device's offset columns directly, with no
+	// row upload, so the prefetched pair search and the captured step graph stay valid. A joint named more than once takes
+	// its last entry, on the host as on the device: the entries are walked from the last, and each joint is sent once, so no
+	// two threads of the scatter write the same row.
+	int32_t* indices = (int32_t*)malloc(sizeof(int32_t) * (size_t)count);
+	float* values = (float*)malloc(sizeof(float) * 3 * (size_t)count);
+	bool* seen = (bool*)calloc((size_t)world->jointPool.capacity, sizeof(bool));
+	int32_t n = 0;
+	for (int32_t k = count - 1; k >= 0; --k)
+	{
+		if (seen[jointIndices[k]])
+		{
+			continue; // a later entry for this joint wins
+		}
+		seen[jointIndices[k]] = true;
+		s2Joint* joint = world->joints + jointIndices[k];
+		joint->localOriginAnchorA = s2MakeVec2(offsets[3 * k], offsets[3 * k + 1]);
+		joint->referenceAngle = offsets[3 * k + 2];
+		if (joint->rowDirty == false)
+		{
+			indices[n] = jointIndices[k];
+			values[3 * n] = offsets[3 * k];
+			values[3 * n + 1] = offsets[3 * k + 1];
+			values[3 * n + 2] = offsets[3 * k + 2];
+			n += 1;
+		}
+	}
+	s2b_set_motor_offsets(world->device, indices, values, n);
+	free(seen);
+	free(indices);
+	free(values);
+	return true;
 }
 
 float s2World_TimedSteps(s2WorldId worldId, int32_t steps, float timeStep, int32_t velIters, int32_t posIters, bool warmStart,

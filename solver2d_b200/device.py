@@ -69,8 +69,10 @@ ROW_VALID = 0x1
 SHAPE_MOVED = 0x10
 JOINT_ENABLE_LIMIT, JOINT_ENABLE_MOTOR, JOINT_COLLIDE_CONNECTED = 0x10, 0x20, 0x40
 # joint types, stored in flags bits 1-3 (a weld keeps its angular impulse in the motorImpulse column; a prismatic row keeps
-# its translation limits in lowerAngle / upperAngle and its maximum motor force in maxMotorTorque)
-JOINT_REVOLUTE, JOINT_MOUSE, JOINT_WELD, JOINT_PRISMATIC = 0, 1, 2, 3
+# its translation limits in lowerAngle / upperAngle and its maximum motor force in maxMotorTorque; a motor row keeps its
+# linear offset in localOriginAnchorA, its angular offset in referenceAngle, its maximum torque in maxMotorTorque, its
+# maximum force in hertz and its correction factor in dampingRatio)
+JOINT_REVOLUTE, JOINT_MOUSE, JOINT_WELD, JOINT_PRISMATIC, JOINT_MOTOR = 0, 1, 2, 3, 4
 
 # symbols declared in include/s2b_device.h (checked by the CPU test-suite against the built library)
 ABI_SYMBOLS = [
@@ -82,7 +84,7 @@ ABI_SYMBOLS = [
     "s2b_download_solve_order", "s2b_download_islands", "s2b_prefetch_pairs", "s2b_get_counters", "s2b_pack_body_state", "s2b_timed_steps", "s2b_last_stage_ms",
     "s2b_flush_l2", "s2b_time_color_kernel", "s2b_version", "s2b_abi_sizes", "s2b_upload_forces", "s2b_host_alloc",
     "s2b_host_free", "s2b_sync_body_state", "s2b_set_warm_gather", "s2b_eval_atan2", "s2b_set_dataflow", "s2b_set_regions", "s2b_set_graph", "s2b_get_stream", "s2b_add_forces", "s2b_download_transforms",
-    "s2b_set_restitution", "s2b_download_neighbour_blocks", "s2b_download_delta_positions",
+    "s2b_set_restitution", "s2b_download_neighbour_blocks", "s2b_download_delta_positions", "s2b_set_motor_offsets",
 ]
 NSYNC_STRIDE = 17  # entries per block of s2b_download_neighbour_blocks
 

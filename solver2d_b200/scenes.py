@@ -15,6 +15,9 @@ Each recipe restates one of the reference's sample scenes or one of the syntheti
 * :func:`welded_structures` — cantilevers, welded assemblies, a welded platform rider and a chain (the weld joint).
 * :func:`sliders`         — pistons, an elevator, an inclined slider, a kinematic carriage, a slider-crank and a mouse
                             joint on a slider (the prismatic joint).
+* :func:`motors`          — top-down friction, a driven platform with a pile, a weak motor under its load, a dynamic
+                            pair, a rider on a kinematic carriage, a drive across the angle seam and a mouse joint
+                            (the motor joint).
 * :func:`kinematic_rigs`  — piles on sliding kinematic platforms and a turntable, joints hanging from moving kinematic
                             carriages (kinematic bodies under every solver variant).
 
@@ -26,6 +29,8 @@ from __future__ import annotations
 import ctypes as C
 import math
 from dataclasses import dataclass, field
+
+import numpy as np
 
 from . import capi
 from .capi import (BodyId, Capsule, Circle, Segment, Vec2, default_body_def, default_mouse_def, default_revolute_def,
@@ -775,6 +780,132 @@ def sliders(lib: capi.Solver2D, solver="TGS_Soft", copies=1, kinematic=True) -> 
             md.dampingRatio = 0.7
             sc.joints.append(lib.s2CreateMouseJoint(world, C.byref(md)))
     return sc
+
+
+MOTORS_PITCH = 30.0  # width of one copy of motors (m)
+
+
+def motors(lib: capi.Solver2D, solver="TGS_Soft", copies=1, kinematic=True) -> Scene:
+    """Motor joint coverage, `copies` side by side (about 25 bodies each). Per copy:
+
+    * top-down friction: six boxes that ignore gravity (gravityScale 0), motor-jointed to the ground at their start
+      position with correctionFactor 0 and small caps, thrown with initial velocities and spins so that the caps brake them;
+    * a dynamic platform driven by a changing linear offset (see :func:`motors_platform_offsets`), carrying a small pile;
+    * a hanging 1 kg box held by a motor whose 4 N cap is below its 10 N weight, so it sinks onto the ground;
+    * a motor joint between two dynamic boxes, the upper one thrown sideways;
+    * with `kinematic`: a box held above a kinematic carriage that moves sideways;
+    * a box started at +3.0 rad, driven to -3.0 rad across the +/-pi seam;
+    * a mouse joint pulling the upper box of the dynamic pair (first copy only).
+
+    On a library without s2CreateMotorJoint (the reference) every motor joint is created as a revolute joint with the same
+    bodies, anchor A at the linear offset, anchor B at B's origin, the angular offset as its reference angle and the same
+    collideConnected: the broad phase treats every joint alike, so both libraries see the same pairs.
+    ``sc.piles["motor"]`` lists the indices into ``sc.joints`` of the motor joints, ``sc.piles["motor_defs"]`` their
+    definitions (dicts of s2MotorJointDef fields) and ``sc.piles["platform"]`` the indices of the platform joints among
+    ``sc.piles["motor"]``, so that a test can turn the stand-in rows into motor rows and drive the platforms."""
+    world = lib.create_world(solver)
+    sc = Scene(lib, world, name=f"motors{copies}")
+    sc.piles["motor"] = []
+    sc.piles["motor_defs"] = []
+    sc.piles["platform"] = []
+    has_motor = "s2CreateMotorJoint" not in lib.missing
+    gid = _ground(lib, world, 0.5 * MOTORS_PITCH * copies + 5.0)
+    sc.bodies.append(gid)
+    sd = default_shape_def()
+
+    def body(kind, x, y, angle=0.0, hx=0.5, hy=0.5, vx=0.0, vy=0.0, w=0.0, gravity_scale=1.0):
+        bd = default_body_def()
+        bd.type = kind
+        bd.position = Vec2(x, y)
+        bd.angle = angle
+        bd.linearVelocity = Vec2(vx, vy)
+        bd.angularVelocity = w
+        bd.gravityScale = gravity_scale
+        bid = lib.s2CreateBody(world, C.byref(bd))
+        box = lib.s2MakeBox(hx, hy)
+        lib.s2CreatePolygonShape(bid, C.byref(sd), C.byref(box))
+        sc.bodies.append(bid)
+        return bid
+
+    def motor(a, b, offset, angle=0.0, max_force=1.0, max_torque=1.0, cf=0.3, collide=False):
+        d = dict(linearOffset=(float(offset[0]), float(offset[1])), angularOffset=angle, maxForce=max_force, maxTorque=max_torque,
+                 correctionFactor=cf, collideConnected=collide)
+        if has_motor:
+            jd = capi.default_motor_def()
+            for name, value in d.items():
+                setattr(jd, name, Vec2(*value) if isinstance(value, tuple) else value)
+            create = lib.s2CreateMotorJoint
+        else:
+            jd = default_revolute_def()
+            jd.localAnchorA = Vec2(*d["linearOffset"])
+            jd.localAnchorB = Vec2(0.0, 0.0)
+            jd.referenceAngle = angle
+            jd.collideConnected = collide
+            create = lib.s2CreateRevoluteJoint
+        jd.bodyIdA = a
+        jd.bodyIdB = b
+        sc.piles["motor"].append(len(sc.joints))
+        sc.piles["motor_defs"].append(d)
+        jid = create(world, C.byref(jd))
+        sc.joints.append(jid)
+        return jid
+
+    D, S, K = capi.DYNAMIC_BODY, capi.STATIC_BODY, capi.KINEMATIC_BODY
+    ground_y = -1.0  # the ground body's origin: offsets to it are relative to (0, -1)
+    for k in range(copies):
+        x0 = -0.5 * MOTORS_PITCH * (copies - 1) + MOTORS_PITCH * k - 14.0
+        # top-down friction: clear of the ground (y = 3), no gravity, braked by the caps alone
+        for i in range(6):
+            x, y = x0 + 1.5 * i, 3.0
+            box = body(D, x, y, hx=0.25, hy=0.25, vx=2.0 - 0.8 * i, vy=0.5 * (i % 3) - 0.5, w=1.0 - 0.4 * i, gravity_scale=0.0)
+            motor(gid, box, (x, y - ground_y), max_force=2.0, max_torque=0.2, cf=0.0)
+        # a dynamic platform, driven sideways by its offset, carrying a pile
+        px, py = x0 + 11.0, 1.0
+        deck = body(D, px, py, hx=2.0, hy=0.125)
+        sc.piles["platform"].append(len(sc.piles["motor"]))
+        motor(gid, deck, (px, py - ground_y), max_force=500.0, max_torque=200.0, cf=0.3)
+        for i in range(3):
+            body(D, px - 0.7 + 0.7 * i, py + 0.375, hx=0.25, hy=0.25)
+        body(D, px - 0.35, py + 0.875, hx=0.25, hy=0.25)
+        # a motor weaker than its hanging load
+        post = body(S, x0 + 15.0, 4.0, hx=0.25, hy=0.25)
+        load = body(D, x0 + 15.0, 2.5)
+        motor(post, load, (0.0, -1.5), max_force=4.0, max_torque=5.0)
+        # a motor between two dynamic bodies
+        lower = body(D, x0 + 18.0, 0.5)
+        upper = body(D, x0 + 18.0, 2.5, hx=0.4, hy=0.2, vx=2.0)
+        motor(lower, upper, (0.0, 1.5), angle=0.3, max_force=30.0, max_torque=10.0)
+        # a box held above a moving kinematic carriage
+        if kinematic:
+            carriage = body(K, x0 + 22.0, 2.0, hx=1.0, hy=0.125, vx=0.5)
+            rider = body(D, x0 + 22.0, 3.0, hx=0.25, hy=0.25)
+            motor(carriage, rider, (0.0, 1.0), max_force=40.0, max_torque=5.0)
+        # an angular offset across the seam: from +3.0 rad to -3.0 rad is 0.28 rad through pi
+        pivot = body(S, x0 + 26.0, 3.0, hx=0.1, hy=0.1)
+        spinner = body(D, x0 + 26.0, 4.0, angle=3.0, hx=0.6, hy=0.1)
+        motor(pivot, spinner, (0.0, 1.0), angle=-3.0, max_force=50.0, max_torque=2.0)
+        if k == 0:
+            md = default_mouse_def()
+            md.bodyIdA = gid
+            md.bodyIdB = upper
+            md.target = Vec2(x0 + 19.0, 3.0)
+            md.hertz = 3.0
+            md.dampingRatio = 0.7
+            sc.joints.append(lib.s2CreateMouseJoint(world, C.byref(md)))
+    return sc
+
+
+def motors_platform_offsets(sc: Scene, step: int, dt: float = 1.0 / 60.0):
+    """(joint slots, offsets) that drive every platform of a :func:`motors` scene at `step`: the deck swings 1.5 m either side
+    of its start with a 4 s period. `offsets` is float32 (x, y, angle) per joint, the layout of
+    s2World_SetMotorJointOffsets."""
+    slots, offsets = [], []
+    t = step * dt
+    for m in sc.piles["platform"]:
+        d = sc.piles["motor_defs"][m]
+        slots.append(sc.joints[sc.piles["motor"][m]].index)
+        offsets.append((d["linearOffset"][0] + 1.5 * math.sin(0.5 * math.pi * t), d["linearOffset"][1], d["angularOffset"]))
+    return np.array(slots, dtype=np.int32), np.array(offsets, dtype=np.float32).reshape(-1, 3)
 
 
 KINEMATIC_RIGS_PITCH = 24.0  # width of one platform of kinematic_rigs (m)
