@@ -200,6 +200,7 @@ typedef struct s2bCounters
 	int32_t recolouredCount; /* constraints moved out of a sparse top colour by Kempe chains so far (colouring, DESIGN.md 3.2) */
 	int32_t neighbourSync;	 // blocks of the persistent kernel whose colour steps wait only for neighbouring blocks; 0 = grid barriers
 	int32_t narrowphaseRowSteps; // solver stages so far whose contact rows the narrow phase wrote (their prepare pass skipped them)
+	int32_t firstTable;			 // blocks of the persistent kernel that warm-start colour 0 from the first-touch table (the others per thread)
 } s2bCounters;
 
 // ---- lifecycle ------------------------------------------------------------------------------------------------

@@ -281,6 +281,107 @@ __device__ __forceinline__ void s2bPrefetchL1(const void* ptr)
 	asm volatile("prefetch.global.L1 [%0];" ::"l"(ptr));
 }
 
+// ---- block-wide first-touch warm start (TGS_Soft bias sweep, colour 0; DESIGN.md §3.1 (d)) -----------------------------
+// Nearly every body is first touched in colour 0, so in that step nearly every thread gathered two bodies after the wait:
+// per body its head, its incidence entries and both 16-byte warm rows of every entry, about 220 KB per block from L2 in every
+// sub-step. Instead, the bodies a block's share of colour 0 first-touches come from a table built with the schedule
+// (ConstraintView::firstTable, solver.cu s2bFirstTable*Kernel), and what the launch does not change is kept in dynamic shared
+// memory for the whole launch: incidence entries, flags, parameters and forces from the start, and the entries' anchors
+// (warmAnchor, which a rebuild step's prepare pass writes) from the first colour-0 step on, behind its synchronisation. After the
+// wait only the velocity and pose of every body and the impulse row of every entry come from L2, and one thread per body runs
+// the unchanged gather, s2bIntegrateVelocityWarmHead: the same operations in the same order, hence the same bits as the
+// per-thread gather, which a block whose copy is over budget keeps (both paths mix in one launch). That memory is otherwise
+// only used by resident regions and the overflow staging, and neither runs with the first-touch warm start.
+#define S2B_FT_SHARED_BYTES (144 * 1024)
+// dynamic shared memory a launch of the persistent kernel may ask for
+#define S2B_SOLVE_SHARED_MAX (S2B_FT_SHARED_BYTES > S2B_DYN_SHARED_BYTES ? S2B_FT_SHARED_BYTES : S2B_DYN_SHARED_BYTES)
+
+struct S2bFirstTableShared
+{
+	float4* prm;
+	float4* frc;
+	int4* info;		 // body, flags, begin, end (entries of the block's copy)
+	float4* anchors; // per entry: warmAnchor of its constraint and side
+	int* entries;
+};
+
+__device__ __forceinline__ S2bFirstTableShared s2bFirstTableLayout(int slots, int entries)
+{
+	extern __shared__ __align__(16) unsigned char s2bFtShared[];
+	S2bFirstTableShared L;
+	L.prm = reinterpret_cast<float4*>(s2bFtShared);
+	L.frc = L.prm + slots;
+	L.info = reinterpret_cast<int4*>(L.frc + slots);
+	L.anchors = reinterpret_cast<float4*>(L.info + slots);
+	L.entries = reinterpret_cast<int*>(L.anchors + entries);
+	return L;
+}
+
+// once per launch (every thread of the block): sFt[0] = the block's slots (-1: it gathers per thread), sFt[1] = its entries,
+// sFt[2] = 0: the anchors are not staged yet
+__device__ __forceinline__ void s2bFirstTableStage(const SolveArgs& a, int* sFt)
+{
+	const int* table = a.cc.firstTable;
+	int4 hd = reinterpret_cast<const int4*>(table)[blockIdx.x];
+	int slots = hd.y;
+	int base = slots >= 0 ? table[hd.z] : 0;
+	int entries = slots >= 0 ? table[hd.z + slots] - base : 0;
+	if (threadIdx.x == 0)
+	{
+		sFt[0] = slots;
+		sFt[1] = entries;
+		sFt[2] = 0;
+	}
+	S2bFirstTableShared L = s2bFirstTableLayout(max(slots, 0), entries);
+	for (int k = threadIdx.x; k < slots; k += blockDim.x)
+	{
+		int i = table[hd.x + k];
+		L.prm[k] = a.bodies.prm[i];
+		L.frc[k] = a.bodies.frc[i];
+		L.info[k] = make_int4(i, (int)a.bodies.flags[i], table[hd.z + k] - base, table[hd.z + k + 1] - base);
+	}
+	for (int j = threadIdx.x; j < entries; j += blockDim.x)
+	{
+		L.entries[j] = table[hd.w + j];
+	}
+}
+
+// after the synchronisation of the bias sweep's colour-0 step: s2IntegrateVelocities + the warm start of every body of the
+// block's table (every thread of the block; ends with the block barrier the solves need)
+__device__ __forceinline__ void s2bFirstTableGather(const SolveArgs& a, int* sFt)
+{
+	int slots = sFt[0], entries = sFt[1];
+	S2bFirstTableShared L = s2bFirstTableLayout(slots, entries);
+	if (sFt[2] == 0)
+	{
+		// (the first colour-0 step of the launch: prepare, if it ran, is behind the grid barrier just taken)
+		for (int j = threadIdx.x; j < entries; j += blockDim.x)
+		{
+			int e = L.entries[j];
+			L.anchors[j] = (e & S2B_INC_CONTACT) ? a.cc.warmAnchor[(size_t)(e >> 2) * 2 + ((e & S2B_INC_SIDE_B) ? 1 : 0)] : make_float4(0.0f, 0.0f, 0.0f, 0.0f);
+		}
+		__syncthreads();
+		if (threadIdx.x == 0)
+		{
+			sFt[2] = 1;
+		}
+	}
+	for (int k = threadIdx.x; k < slots; k += blockDim.x)
+	{
+		int4 info = L.info[k];
+		GatherHead hd;
+		hd.f = (unsigned)info.y;
+		hd.vel = a.bodies.vel[info.x];
+		hd.prm = L.prm[k];
+		hd.frc = L.frc[k];
+		hd.pose = a.bodies.pose[info.x];
+		hd.begin = info.z;
+		hd.end = info.w;
+		s2bIntegrateVelocityWarmHead<false>(a, info.x, a.ctx.h, hd, false, nullptr, L.entries, L.anchors);
+	}
+	__syncthreads();
+}
+
 // the TGS_Soft row of a contact constraint (what s2bLoadContactStream reads)
 __device__ __forceinline__ void s2bTouchContactRow(const SolveArgs& a, int t)
 {
@@ -454,7 +555,8 @@ __device__ __forceinline__ void s2bTouchJoint(const SolveArgs& a, int t, bool bo
 // device-wide groups (cut colours / wavefront levels, a grid barrier before each), then the serial overflow group.
 template <int SOLVER>
 __device__ __forceinline__ void s2bGroupPass(int jointOp, int contactOp, const SolveArgs& a, const PassPtrs& p, const S2bLaunchInfo& li,
-											 S2bSync& sync, const int* sRegJ, const int* sRegC, const int* sGroupJ, const int* sGroupC, int* sNbr)
+											 S2bSync& sync, const int* sRegJ, const int* sRegC, const int* sGroupJ, const int* sGroupC, int* sNbr,
+											 int* sFt)
 {
 	int traceCode = (PASS_GROUP << 8) | contactOp;
 	if (li.regions && li.primary > 0)
@@ -560,9 +662,11 @@ __device__ __forceinline__ void s2bGroupPass(int jointOp, int contactOp, const S
 			bool fold = bias && li.foldPositions;
 			// first-touch warm start: the marked bodies of a row are gathered right before its solve (warm_gather.cuh)
 			int firstMarks = bias && li.firstTouch ? S2B_TOUCH_FIRST_A | S2B_TOUCH_FIRST_B : 0;
+			// ... or, in colour 0, by the whole block from its first-touch table (block-uniform)
+			bool blockWarm = firstMarks != 0 && g == 0 && sFt[0] >= 0;
 			int t = cBegin + u - njAll;
 			ContactStream cs;
-			if (mine)
+			if (mine && blockWarm == false)
 			{
 				cs = s2bLoadContactStream(a, t, store);
 				cs.last = fold ? a.cc.lastTouch[t] : 0;
@@ -584,6 +688,17 @@ __device__ __forceinline__ void s2bGroupPass(int jointOp, int contactOp, const S
 				s2bSyncBeforeGlobal(a, sync);
 			}
 			bool writeWarm = bias ? a.ctx.extraIterations == 0 : true;
+			if (blockWarm)
+			{
+				// (the row is read after the gathers rather than held in registers through them)
+				s2bFirstTableGather(a, sFt);
+				if (mine)
+				{
+					cs = s2bLoadContactStream(a, t, store);
+					cs.last = a.cc.lastTouch[t];
+				}
+				firstMarks = 0;
+			}
 			if (mine)
 			{
 				if (cs.last & firstMarks)
@@ -895,6 +1010,7 @@ template <int SOLVER> __global__ void __launch_bounds__(S2B_BLOCK, SOLVER == S2B
 	__shared__ int sRegJ[S2B_REG_STRIDE], sRegC[S2B_REG_STRIDE];
 	__shared__ int sGroupJ[S2B_MAX_COLORS + 2], sGroupC[S2B_MAX_COLORS + 2];
 	__shared__ int sNbr[S2B_NSYNC_STRIDE + 1];
+	__shared__ int sFt[3]; // the block's first-touch table in dynamic shared memory: slots (-1: none), entries, anchors staged
 
 	S2bSync sync;
 	sync.base = *((volatile unsigned*)(a.barrier + 32));
@@ -936,6 +1052,14 @@ template <int SOLVER> __global__ void __launch_bounds__(S2B_BLOCK, SOLVER == S2B
 	// lastTouch is only handed over with the gather on.)
 	li.firstTouch = li.foldPositions && a.counts[CNT_KINEMATIC_ITEMS] == 0;
 	li.resident = SOLVER == 7 && li.regions && a.bodyLocal != nullptr && a.counts[CNT_RESIDENT] != 0 && a.bodyTicket == nullptr;
+	if (threadIdx.x == 0)
+	{
+		sFt[0] = -1;
+	}
+	if (SOLVER == 7 && li.firstTouch && a.cc.firstTable != nullptr && a.counts[CNT_FIRST_TABLE] == (int)gridDim.x)
+	{
+		s2bFirstTableStage(a, sFt);
+	}
 	li.bodyBegin = li.bodyEnd = 0;
 	if (li.regions)
 	{
@@ -1011,7 +1135,7 @@ template <int SOLVER> __global__ void __launch_bounds__(S2B_BLOCK, SOLVER == S2B
 					else
 					{
 						s2bGroupPass<SOLVER>(pass.jointOp, pass.contactOp, a, p, li, sync, sRegJ, sRegC, groupsInShared ? sGroupJ : nullptr,
-											 groupsInShared ? sGroupC : nullptr, sNbr);
+											 groupsInShared ? sGroupC : nullptr, sNbr, sFt);
 					}
 				}
 				else if (pass.kind == PASS_BODY && li.foldPositions && pass.bodyOp == BOP_INTEGRATE_POSITIONS)

@@ -91,8 +91,10 @@ template <typename T> struct DevArray
 			{
 				S2B_CHECK(cudaMemcpyAsync(q, p, cap * sizeof(T), cudaMemcpyDeviceToDevice, stream));
 			}
-			// stream-ordered release so in-flight kernels reading the old buffer stay valid
-			S2B_CHECK(cudaFreeAsync(p, stream));
+			// The old buffer came from cudaMalloc, so cudaFreeAsync would not order its release behind this stream: another world's
+			// allocation could take it over while the copy above (or a kernel still queued here) reads it. Wait, then free.
+			S2B_CHECK(cudaStreamSynchronize(stream));
+			S2B_CHECK(cudaFree(p));
 		}
 		p = q;
 		cap = newCap;
@@ -221,6 +223,9 @@ struct ConstraintView
 	// itself (the warm-start gather folded into the sweep), one device-wide body pass less each per sub-step (persistent.cuh).
 	// Null: positions are integrated and velocities gathered by their own body passes.
 	const int* lastTouch;
+	// per block of the persistent kernel, the bodies its share of colour 0 first-touches, with their incidence entries
+	// (persistent.cuh, S2B_FT_*); null: every first-touch gather runs in the thread of the body's row
+	const int* firstTable;
 	// sticky extras
 	float4* fanchor[2]; // COM-relative local friction anchors A.xy B.xy
 	float2* tsep[2];	// tangentSeparation, spare
@@ -389,6 +394,9 @@ struct s2bWorld
 						   // (persistent.cuh; S2B_NEIGHBOUR_SYNC=0 keeps a grid barrier before every colour step)
 	int narrowphasePrepare = 1; // while the solve schedule stands, the narrow phase writes the contact rows and the solver's
 								// prepare pass skips them (narrowphase.cu; S2B_NARROWPHASE_PREPARE=0 leaves it all to prepare)
+	int blockWarm = 1;		// TGS_Soft: the bias sweep's colour-0 step warm-starts a block's first-touched bodies together, from a
+							// table built with the schedule (persistent.cuh; S2B_BLOCK_WARM=0 keeps the gather per thread)
+	int blockWarmBytes = 0; // shared-memory budget of one block's table; 0 = the kernel's dynamic shared memory (S2B_BLOCK_WARM_BYTES)
 	int kempeGrid = 0;
 	DevArray<int> dMovedFlag; // [0] = number of proxies moved in last finalize (device counter)
 	int pairPassCount = 0;

@@ -94,6 +94,9 @@ void s2bFreeSolverScratch(s2bWorld* w)
 	s->incWork.release();
 	s->incList.release();
 	s->lastTouch.release();
+	s->firstTable.release();
+	s->ftRowSlot.release();
+	s->ftDegree.release();
 	s->heavyBodies.release();
 	s->ovBodies.release();
 	s->longBodies.release();
@@ -2113,6 +2116,97 @@ __global__ void s2bTouchMarksKernel(int bodyCapacity, const int* incStart, const
 	}
 }
 
+// ---- first-touch table of the bias sweep's colour 0 (ConstraintView::firstTable; persistent.cuh, s2bFirstTableGather) ----
+// Block b runs the b-th share of colour 0 (s2bGroupShare, the mapping of the neighbour tables). The bodies that the share's rows
+// first-touch get consecutive slots in row order (side A before side B), so a block's slots are one range of the table.
+
+// per contact row: how many bodies it first-touches when it lies in colour 0, else 0 (input of the slot running sum)
+__global__ void s2bFirstTableCountKernel(int contactCount, const int* cGroupOff, const int* touchMarks, int* rowSlot)
+{
+	int t = blockIdx.x * blockDim.x + threadIdx.x;
+	if (t > contactCount)
+	{
+		return;
+	}
+	int n = 0;
+	if (t < contactCount && t >= cGroupOff[0] && t < cGroupOff[1])
+	{
+		n = __popc(touchMarks[t] & (S2B_TOUCH_FIRST_A | S2B_TOUCH_FIRST_B));
+	}
+	rowSlot[t] = n;
+}
+
+// per movable body whose first constraint is a colour-0 row (the row s2bTouchMarksKernel marked): its slot's body and degree
+__global__ void s2bFirstTableSlotKernel(int bodyCapacity, const int* incStart, const int* incList, const int* cGroupOff, const int* touchMarks,
+										const int* rowSlot, int* slotBody, int* slotDegree)
+{
+	int i = blockIdx.x * blockDim.x + threadIdx.x;
+	if (i >= bodyCapacity)
+	{
+		return;
+	}
+	int begin = incStart[i], end = incStart[i + 1];
+	if (end == begin)
+	{
+		return;
+	}
+	int e = incList[begin];
+	int t = e >> 2;
+	if ((e & S2B_INC_CONTACT) == 0 || t < cGroupOff[0] || t >= cGroupOff[1])
+	{
+		return;
+	}
+	int slot = rowSlot[t] + (((e & S2B_INC_SIDE_B) != 0 && (touchMarks[t] & S2B_TOUCH_FIRST_A) != 0) ? 1 : 0);
+	slotBody[slot] = i;
+	slotDegree[slot] = end - begin;
+}
+
+// per slot: the body's incidence entries, copied in list order
+__global__ void s2bFirstTableEntriesKernel(int maxSlots, const int* slots, const int* incStart, const int* incList, const int* slotBody,
+										   const int* entryOff, int* entries)
+{
+	int k = blockIdx.x * blockDim.x + threadIdx.x;
+	if (k >= maxSlots || k >= *slots)
+	{
+		return;
+	}
+	int begin = incStart[slotBody[k]];
+	int n = entryOff[k + 1] - entryOff[k];
+	for (int j = 0; j < n; ++j)
+	{
+		entries[entryOff[k] + j] = incList[begin + j];
+	}
+}
+
+// One block of >= `blocks` threads: every block's header. A block whose copy exceeds `budget` bytes of shared memory keeps the
+// per-thread gather (slots -1); the others take the table, both give the same bits. The table is of no use where the bias sweep
+// does not warm-start at the first touch (joints, a constraint on a kinematic body: persistent.cuh, S2bLaunchInfo::firstTouch).
+__global__ void s2bFirstTableHeaderKernel(int* counts, const int* cGroupOff, const int* jGroupOff, const int* rowSlot, int blocks, int budget,
+										  int* table, int slotBase, int offBase, int entryBase)
+{
+	int b = threadIdx.x;
+	bool fits = false;
+	if (b < blocks)
+	{
+		int nj = jGroupOff[1] - jGroupOff[0];
+		int n = nj + cGroupOff[1] - cGroupOff[0];
+		int share = s2bGroupShare(n, blocks);
+		int u0 = min(n, b * share), u1 = min(n, (b + 1) * share);
+		int t0 = cGroupOff[0] + max(u0 - nj, 0), t1 = cGroupOff[0] + max(u1 - nj, 0);
+		int s0 = rowSlot[t0], s1 = rowSlot[t1];
+		int e0 = table[offBase + s0], e1 = table[offBase + s1];
+		fits = (long long)(s1 - s0) * S2B_FT_SLOT_BYTES + (long long)(e1 - e0) * S2B_FT_ENTRY_BYTES <= budget;
+		reinterpret_cast<int4*>(table)[b] = make_int4(slotBase + s0, fits ? s1 - s0 : -1, offBase + s0, entryBase + e0);
+	}
+	int fitting = __syncthreads_count(fits ? 1 : 0);
+	if (threadIdx.x == 0)
+	{
+		bool usable = counts[CNT_JOINTS] == 0 && counts[CNT_KINEMATIC_ITEMS] == 0;
+		counts[CNT_FIRST_TABLE] = usable ? blocks : 0;
+		counts[CNT_FIRST_TABLE_BLOCKS] = usable ? fitting : 0;
+	}
+}
+
 // ---- launch-by-launch kernels (profiling / cross-check path) ----------------------------------------------------
 
 __global__ void __launch_bounds__(S2B_BLOCK) s2bBodyPassKernel(SolveArgs a, int bodyOp)
@@ -2816,6 +2910,8 @@ struct SolvePlan
 	int grid = 1;	 // blocks of the persistent kernel
 	int regions = 0; // region-local schedule: == grid, or 0
 	bool neighbourSync = false; // the schedule builds neighbour tables for the colour steps (the device decides whether to use them)
+	bool firstTouchMarks = false; // TGS_Soft: the bias sweep is handed the touch marks (ConstraintView::lastTouch)
+	bool firstTable = false;	  // ... and the schedule builds the first-touch table of its colour 0 (ConstraintView::firstTable)
 	HostPlan host;	 // launch-by-launch / wavefront modes
 	int hostNC = 0, hostNJ = 0;
 };
@@ -2869,8 +2965,10 @@ static void planSolve(s2bWorld* w, SolverScratch* s, SolvePlan& pl)
 		if (w->solveGrid == 0 || w->solveGridSolver != solverType)
 		{
 			int blocksPerSm = 0;
-			S2B_CHECK(cudaFuncSetAttribute(s2bPersistentKernel(solverType), cudaFuncAttributeMaxDynamicSharedMemorySize, S2B_DYN_SHARED_BYTES));
-			S2B_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&blocksPerSm, s2bPersistentKernel(solverType), S2B_BLOCK, S2B_DYN_SHARED_BYTES));
+			S2B_CHECK(cudaFuncSetAttribute(s2bPersistentKernel(solverType), cudaFuncAttributeMaxDynamicSharedMemorySize, S2B_SOLVE_SHARED_MAX));
+			// (with the shared memory the largest launch of this variant asks for: TGS_Soft's launches with the first-touch table)
+			S2B_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&blocksPerSm, s2bPersistentKernel(solverType), S2B_BLOCK,
+																	solverType == 7 ? S2B_SOLVE_SHARED_MAX : S2B_DYN_SHARED_BYTES));
 			const char* env = getenv("S2B_SOLVE_BLOCKS_PER_SM");
 			int want = env != nullptr ? atoi(env) : 2;
 			w->solveGrid = w->smCount * std::min(std::max(blocksPerSm, 1), std::max(want, 1));
@@ -2965,6 +3063,18 @@ static void planSolve(s2bWorld* w, SolverScratch* s, SolvePlan& pl)
 		s->incList.reserve(2 * nI, st, false);
 		s->lastTouch.reserve(nC + 2, st, false);
 	}
+	pl.firstTouchMarks = pl.gatherWarm && solverType == 7 && w->fusePositions != 0 && pl.dataflow == false;
+	// (not for a launch that may run regions: the kernel warm-starts at the first touch only without them, and the table's launch
+	// asks for more shared memory, which sets the L1 / shared split the region paths lean on)
+	pl.firstTable = pl.firstTouchMarks && w->blockWarm != 0 && w->schedule == S2B_SCHEDULE_COLOR && pl.usePersistent && pl.grid <= 512 &&
+					pl.regions == 0;
+	if (pl.firstTable)
+	{
+		// (at most two slots per row; the entries of distinct bodies are at most all incidence entries)
+		s->firstTable.reserve(S2B_FT_HEADER + 2 * nC + (2 * nC + 1) + 2 * nI, st, false);
+		s->ftRowSlot.reserve(nC + 1, st, false);
+		s->ftDegree.reserve(2 * nC + 1, st, false);
+	}
 	if (pl.dataflow)
 	{
 		s->flow.reserve(2 * nC + 2 * nJ, st, false);
@@ -3041,6 +3151,8 @@ static void planSolve(s2bWorld* w, SolverScratch* s, SolvePlan& pl)
 							   (int)nI, st);
 	tempBytes = std::max(tempBytes, need);
 	cub::DeviceScan::ExclusiveSum(nullptr, need, (int*)nullptr, (int*)nullptr, bodyCap + 1, st);
+	tempBytes = std::max(tempBytes, need);
+	cub::DeviceScan::ExclusiveSum(nullptr, need, (int*)nullptr, (int*)nullptr, (int)(2 * nC + 1), st);
 	tempBytes = std::max(tempBytes, need);
 	cub::DeviceRadixSort::SortPairs(nullptr, need, (unsigned short*)nullptr, (unsigned short*)nullptr, (int*)nullptr, (int*)nullptr, (int)nI, 0,
 									16, st);
@@ -3327,6 +3439,28 @@ static void enqueueSchedule(s2bWorld* w, SolverScratch* s, SolvePlan& pl)
 			{
 				S2B_CHECK(cudaMemsetAsync(s->lastTouch.p, 0, sizeof(int) * (size_t)contactCount, st));
 				S2B_LAUNCH(w, s2bTouchMarksKernel, gridFor(bodyCap, 256), 256, 0, bodyCap, s->adjStart.p, s->incList.p, s->lastTouch.p);
+				if (pl.firstTable)
+				{
+					int maxSlots = 2 * (int)nC;
+					int* table = s->firstTable.p;
+					int slotBase = S2B_FT_HEADER, offBase = slotBase + maxSlots, entryBase = offBase + maxSlots + 1;
+					int budget = w->blockWarmBytes > 0 ? std::min(w->blockWarmBytes, (int)S2B_FT_SHARED_BYTES) : (int)S2B_FT_SHARED_BYTES;
+					// (ftDegree holds the row counts first, then the slots' degrees)
+					S2B_LAUNCH(w, s2bFirstTableCountKernel, gridFor(contactCount + 1, 256), 256, 0, contactCount, s->cGroupOff.p, s->lastTouch.p,
+							   s->ftDegree.p);
+					size_t tb = s->cubTemp.cap;
+					cub::DeviceScan::ExclusiveSum(s->cubTemp.p, tb, s->ftDegree.p, s->ftRowSlot.p, contactCount + 1, st);
+					S2B_CHECK(cudaMemsetAsync(s->ftDegree.p, 0, sizeof(int) * ((size_t)maxSlots + 1), st));
+					S2B_LAUNCH(w, s2bFirstTableSlotKernel, gridFor(bodyCap, 256), 256, 0, bodyCap, s->adjStart.p, s->incList.p, s->cGroupOff.p,
+							   s->lastTouch.p, s->ftRowSlot.p, table + slotBase, s->ftDegree.p);
+					tb = s->cubTemp.cap;
+					cub::DeviceScan::ExclusiveSum(s->cubTemp.p, tb, s->ftDegree.p, table + offBase, maxSlots + 1, st);
+					w->kernelLaunches += 4;
+					S2B_LAUNCH(w, s2bFirstTableEntriesKernel, gridFor(maxSlots, 256), 256, 0, maxSlots, s->ftRowSlot.p + contactCount, s->adjStart.p,
+							   s->incList.p, table + slotBase, table + offBase, table + entryBase);
+					S2B_LAUNCH(w, s2bFirstTableHeaderKernel, 1, 512, 0, s->counts.p, s->cGroupOff.p, s->jGroupOff.p, s->ftRowSlot.p, pl.grid, budget,
+							   table, slotBase, offBase, entryBase);
+				}
 			}
 		}
 	}
@@ -3403,7 +3537,8 @@ static void enqueueIterate(s2bWorld* w, SolverScratch* s, SolvePlan& pl, bool ca
 	a.cc.src = s->src.p;
 	a.cc.warmP = pl.gatherWarm ? s->warmP.p : nullptr;
 	a.cc.warmAnchor = pl.gatherWarm ? s->warmAnchor.p : nullptr;
-	a.cc.lastTouch = (pl.gatherWarm && pl.solverType == 7 && w->fusePositions != 0 && pl.dataflow == false) ? s->lastTouch.p : nullptr;
+	a.cc.lastTouch = pl.firstTouchMarks ? s->lastTouch.p : nullptr;
+	a.cc.firstTable = pl.firstTable ? s->firstTable.p : nullptr;
 	for (int p = 0; p < 2; ++p)
 	{
 		a.cc.anchor[p] = s->anchor[p].p;
@@ -3513,7 +3648,8 @@ static void enqueueIterate(s2bWorld* w, SolverScratch* s, SolvePlan& pl, bool ca
 		// (inside a capture the time stamps become external event-record nodes so that they are taken on every replay)
 		unsigned evFlags = capturing ? cudaEventRecordExternal : cudaEventRecordDefault;
 		S2B_CHECK(cudaEventRecordWithFlags(w->solveKernelStart, st, evFlags));
-		S2B_CHECK(cudaLaunchCooperativeKernel(s2bPersistentKernel(solverType), dim3(pl.grid), dim3(pl.threads), args, S2B_DYN_SHARED_BYTES, st));
+		size_t shared = a.cc.firstTable != nullptr ? S2B_SOLVE_SHARED_MAX : S2B_DYN_SHARED_BYTES;
+		S2B_CHECK(cudaLaunchCooperativeKernel(s2bPersistentKernel(solverType), dim3(pl.grid), dim3(pl.threads), args, shared, st));
 		S2B_CHECK(cudaEventRecordWithFlags(w->solveKernelEnd, st, evFlags));
 		w->solveKernelTimed = true;
 		w->kernelLaunches += 1;
@@ -4004,6 +4140,7 @@ extern "C" void s2b_get_counters(s2bWorld* w, s2bCounters* out)
 		out->regionCount = counts[CNT_REGIONS_ON] != 0 ? w->scratch->regions : 0;
 		out->overflowCount = counts[CNT_OVERFLOW_C] + counts[CNT_OVERFLOW_J];
 		out->neighbourSync = counts[CNT_NSYNC];
+		out->firstTable = counts[CNT_FIRST_TABLE_BLOCKS];
 		if (w->scratch->kempeState.p != nullptr)
 		{
 			int ks[4];

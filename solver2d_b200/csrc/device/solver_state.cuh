@@ -41,8 +41,19 @@ enum
 	CNT_NSYNC = 23,		// grid the neighbour tables were built for: device-wide colour steps wait for neighbouring blocks only; 0 = off
 	CNT_KINEMATIC_ITEMS = 24, // constraints with an endpoint no constraint moves but whose pose changes (kinematic, s2bItemEndpoints -2)
 	CNT_ROWS_READY = 25, // 1: the narrow phase wrote this solve's contact rows, prepare leaves them (narrowphase.cu, s2bScheduleGate)
+	CNT_FIRST_TABLE = 26, // grid the first-touch table (ConstraintView::firstTable) was built for; 0 = none or unusable
+	CNT_FIRST_TABLE_BLOCKS = 27, // blocks whose copy of the table fits the budget (the others gather per thread)
 	CNT_SIZE = 32
 };
+
+// ConstraintView::firstTable, one int array: [4 b, 4 b + 4) = block b's header {index of its first slot's body, slots (-1: over
+// budget, the block gathers per thread), index of its first slot's entry offset, index of its first entry}; then per slot the body, then
+// per slot + 1 the offset of the slot's entries (running sum), then the entries (incidence entries in list order)
+#define S2B_FT_HEADER (4 * 512)
+// shared memory of one slot (body, flags, parameters, forces, entry range) and of one entry (the entry and its side's anchors)
+// of a block's copy (persistent.cuh, S2bFirstTableShared)
+#define S2B_FT_SLOT_BYTES 48
+#define S2B_FT_ENTRY_BYTES 20
 
 // Device-wide group steps: block b runs items [b * share, (b + 1) * share) of a group of n items (its joints, then its
 // contacts). Every block gets work and a warp's rows stay contiguous (coalesced column loads). The neighbour tables
@@ -161,6 +172,8 @@ struct SolverScratch
 	DevArray<unsigned long long> itemVal, incWork; // warm-start gather: per-item sort value, per-body sort scratch
 	DevArray<int> incList;
 	DevArray<int> lastTouch; // ConstraintView::lastTouch
+	DevArray<int> firstTable;		// ConstraintView::firstTable
+	DevArray<int> ftRowSlot, ftDegree; // its build: per colour-0 row its first slot (running sum), per slot the body's degree
 	DevArray<int> heavyBodies;
 	DevArray<int> longBodies;			// [0] count, then bodies whose incidence list is sorted by a whole block
 	DevArray<int> ovBodies, ovBodySlot; // bodies of the serial overflow group (SolveArgs::ovBodies)

@@ -28,8 +28,10 @@ struct GatherTerms
 	s2Vec2 tv0, tv1;
 };
 
+// anchorRow: this side's anchors when the caller holds them (a block's shared-memory copy); null = warmAnchor
 template <bool FIXED>
-__device__ __forceinline__ GatherTerms s2bGatherTermsOf(const SolveArgs& a, int e, s2Rot q, float invMass, float invI)
+__device__ __forceinline__ GatherTerms s2bGatherTermsOf(const SolveArgs& a, int e, s2Rot q, float invMass, float invI,
+														const float4* anchorRow = nullptr)
 {
 	GatherTerms g;
 	g.np = 0;
@@ -41,7 +43,7 @@ __device__ __forceinline__ GatherTerms s2bGatherTermsOf(const SolveArgs& a, int 
 	{
 		// two 16-byte rows: the impulse vectors of both points, this side's anchors (contact_kernels.cuh, s2bWriteWarm*)
 		float4 imp = a.cc.warmP[t];
-		float4 anchors = a.cc.warmAnchor[(size_t)t * 2 + (sideB ? 1 : 0)];
+		float4 anchors = anchorRow != nullptr ? *anchorRow : a.cc.warmAnchor[(size_t)t * 2 + (sideB ? 1 : 0)];
 		g.np = imp.z == imp.z ? 2 : 1;
 #pragma unroll
 		for (int j = 0; j < 2; ++j)
@@ -136,7 +138,8 @@ __device__ __forceinline__ GatherHead s2bLoadGatherHead(const SolveArgs& a, int 
 // v, w in list order (same float operations, same order as the constraint-by-constraint pass, and the same code as the
 // block-wide hub gather below)
 template <bool FIXED>
-__device__ __forceinline__ void s2bGatherFour(const SolveArgs& a, const int (&e)[4], s2Rot q, float invMass, float invI, s2Vec2& v, float& w)
+__device__ __forceinline__ void s2bGatherFour(const SolveArgs& a, const int (&e)[4], s2Rot q, float invMass, float invI, s2Vec2& v, float& w,
+											  const float4* anchors = nullptr)
 {
 	GatherTerms g[4];
 #pragma unroll
@@ -147,7 +150,7 @@ __device__ __forceinline__ void s2bGatherFour(const SolveArgs& a, const int (&e)
 		g[u].tv0 = g[u].tv1 = V2(0.0f, 0.0f);
 		if (e[u] != -1)
 		{
-			g[u] = s2bGatherTermsOf<FIXED>(a, e[u], q, invMass, invI);
+			g[u] = s2bGatherTermsOf<FIXED>(a, e[u], q, invMass, invI, anchors != nullptr ? anchors + u : nullptr);
 		}
 	}
 #pragma unroll
@@ -173,10 +176,14 @@ __device__ __forceinline__ void s2bGatherFour(const SolveArgs& a, const int (&e)
 // between changes either). Only where this pass still runs beside the folded position integration: when a constraint reads
 // a kinematic body (persistent.cuh, S2bLaunchInfo::firstTouch); otherwise the finalize pass sub-steps such bodies.
 // velOut: where the new velocity goes (the region's shared-memory copy in a resident launch); null = the body's row
+// list, listAnchors: where hd.begin / hd.end point, the entries and their side's anchors (a block's shared-memory copy of its
+// first-touched bodies' lists); null = incList, warmAnchor
 template <bool FIXED>
 __device__ __forceinline__ void s2bIntegrateVelocityWarmHead(const SolveArgs& a, int i, float h, const GatherHead& hd, bool alsoPosition = false,
-															 float4* velOut = nullptr)
+															 float4* velOut = nullptr, const int* list = nullptr,
+															 const float4* listAnchors = nullptr)
 {
+	const int* inc = list != nullptr ? list : a.incList;
 	float4* out = velOut != nullptr ? velOut : a.bodies.vel + i;
 	unsigned f = hd.f;
 	if ((f & S2B_BODY_VALID) == 0)
@@ -228,13 +235,13 @@ __device__ __forceinline__ void s2bIntegrateVelocityWarmHead(const SolveArgs& a,
 #pragma unroll
 	for (int u = 0; u < 4; ++u)
 	{
-		e0[u] = begin + u < end ? a.incList[begin + u] : -1;
-		e1[u] = begin + 4 + u < end ? a.incList[begin + 4 + u] : -1;
+		e0[u] = begin + u < end ? inc[begin + u] : -1;
+		e1[u] = begin + 4 + u < end ? inc[begin + 4 + u] : -1;
 	}
-	s2bGatherFour<FIXED>(a, e0, q, invMass, invI, v, w);
+	s2bGatherFour<FIXED>(a, e0, q, invMass, invI, v, w, listAnchors != nullptr ? listAnchors + begin : nullptr);
 	if (end - begin > 4)
 	{
-		s2bGatherFour<FIXED>(a, e1, q, invMass, invI, v, w);
+		s2bGatherFour<FIXED>(a, e1, q, invMass, invI, v, w, listAnchors != nullptr ? listAnchors + begin + 4 : nullptr);
 	}
 	for (int k0 = begin + 8; k0 < end; k0 += 4)
 	{
@@ -242,9 +249,9 @@ __device__ __forceinline__ void s2bIntegrateVelocityWarmHead(const SolveArgs& a,
 #pragma unroll
 		for (int u = 0; u < 4; ++u)
 		{
-			e[u] = k0 + u < end ? a.incList[k0 + u] : -1;
+			e[u] = k0 + u < end ? inc[k0 + u] : -1;
 		}
-		s2bGatherFour<FIXED>(a, e, q, invMass, invI, v, w);
+		s2bGatherFour<FIXED>(a, e, q, invMass, invI, v, w, listAnchors != nullptr ? listAnchors + k0 : nullptr);
 	}
 	*out = make_float4(v.x, v.y, w, invMass);
 }

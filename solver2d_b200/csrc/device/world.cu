@@ -417,6 +417,16 @@ extern "C" s2bWorld* s2b_world_create(int cudaDevice, int solverType)
 		{
 			w->narrowphasePrepare = atoi(env) != 0 ? 1 : 0;
 		}
+		env = getenv("S2B_BLOCK_WARM");
+		if (env != nullptr)
+		{
+			w->blockWarm = atoi(env) != 0 ? 1 : 0;
+		}
+		env = getenv("S2B_BLOCK_WARM_BYTES");
+		if (env != nullptr)
+		{
+			w->blockWarmBytes = atoi(env) < 0 ? 0 : atoi(env);
+		}
 	}
 	w->solverType = solverType;
 	w->sticky = (solverType == 6); // s2_solverTGS_Sticky

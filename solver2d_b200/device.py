@@ -61,7 +61,8 @@ class Counters(C.Structure):
                 ("movedCount", C.c_int32), ("pairPassCount", C.c_int32), ("kernelLaunches", C.c_int32),
                 ("graphReplays", C.c_int32), ("graphCaptures", C.c_int32), ("scratchBytes", C.c_int64),
                 ("regionCount", C.c_int32), ("cutCount", C.c_int32), ("cutGroupCount", C.c_int32), ("recolouredCount", C.c_int32),
-                ("neighbourSync", C.c_int32), ("narrowphaseRowSteps", C.c_int32)]
+                ("neighbourSync", C.c_int32), ("narrowphaseRowSteps", C.c_int32),
+                ("firstTable", C.c_int32)]
 
 
 SCHEDULE_COLOR, SCHEDULE_WAVEFRONT = 0, 1
