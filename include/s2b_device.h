@@ -55,6 +55,9 @@ typedef struct s2bBodyRow
 	float force[2];
 	float torque;
 	float linearDamping, angularDamping, gravityScale;
+	// extents of the body's shapes about its centre of mass (s2ComputeShapeExtent), used by continuous collision
+	// (s2b_set_continuous): minExtent = smallest inner extent (s2_huge without shapes), maxExtent = largest outer extent
+	float minExtent, maxExtent;
 } s2bBodyRow;
 
 // shape kinds, numeric values of s2ShapeType (reference src/shape.h:14-21)
@@ -201,6 +204,8 @@ typedef struct s2bCounters
 	int32_t neighbourSync;	 // blocks of the persistent kernel whose colour steps wait only for neighbouring blocks; 0 = grid barriers
 	int32_t narrowphaseRowSteps; // solver stages so far whose contact rows the narrow phase wrote (their prepare pass skipped them)
 	int32_t firstTable;			 // blocks of the persistent kernel that warm-start colour 0 from the first-touch table (the others per thread)
+	int32_t continuousShapes;	 // shapes of fast bodies swept against static shapes in the last step (s2b_set_continuous)
+	int32_t continuousHits;		 // bodies the last step's continuous pass stopped at a time of impact
 } s2bCounters;
 
 // ---- lifecycle ------------------------------------------------------------------------------------------------
@@ -238,6 +243,12 @@ S2B_API void s2b_set_dataflow(s2bWorld* world, int enable);
 // that drives the normal velocity of every manifold point towards -e * (its approach speed at the start of the stage), for
 // points whose approach was faster than `threshold` (m/s) and which carry a normal impulse (DESIGN.md §3.7).
 S2B_API void s2b_set_restitution(s2bWorld* world, int enable, float threshold);
+// Continuous collision of dynamic bodies against static shapes (DESIGN.md §3.11). enable = 0 (default): nothing runs.
+// enable = 1: s2b_solve records each dynamic body's centre and rotation before the solver stage and, after it, sweeps the
+// shapes of every fast body (moved more than half its minExtent) against the static shapes the pair rules let it collide
+// with, and moves a body that would hit one back to its earliest time of impact. Velocities are kept. Takes effect at the
+// next s2b_solve; the solver stage's graph is not re-captured.
+S2B_API void s2b_set_continuous(s2bWorld* world, int enable);
 
 // ---- host -> device -------------------------------------------------------------------------------------------
 

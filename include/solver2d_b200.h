@@ -3,6 +3,8 @@
 #pragma once
 
 #include "s2b_device.h"
+#include "solver2d/distance.h"
+#include "solver2d/geometry.h"
 #include "solver2d/id.h"
 #include "solver2d/types.h"
 
@@ -135,6 +137,75 @@ S2B_API void s2MotorJoint_SetCorrectionFactor(s2JointId jointId, float correctio
 S2B_API s2Vec2 s2MotorJoint_GetConstraintForce(s2JointId jointId, float inverseTimeStep);
 // The angular impulse of the last step times inverseTimeStep (N-m).
 S2B_API float s2MotorJoint_GetConstraintTorque(s2JointId jointId, float inverseTimeStep);
+
+// Continuous collision of dynamic bodies against static shapes (default off: collision is discrete, as in the reference).
+// When on, a dynamic body that moved more than half its smallest inner extent in a step is swept from its pose at the
+// start of the step to its pose at the end against the static shapes its shapes may collide with, and stopped at the
+// first time of impact, s2_linearSlop short of the surface; its velocity is kept. Bodies that start the step touching a
+// static shape are held back only if a small core inside the shape would hit it, or starts touching it and moves toward
+// it (the body is then already a quarter of its inner extent deep). Not covered: dynamic against dynamic or
+// kinematic bodies (DESIGN.md §3.11). Takes effect at the next s2World_Step.
+S2B_API void s2World_EnableContinuous(s2WorldId worldId, bool enable);
+
+// Motion of a body over one step, for s2TimeOfImpact: the centre of mass moves linearly from c1 to c2 and the rotation is
+// the normalised linear interpolation of q1 and q2.
+typedef struct s2Sweep
+{
+	s2Vec2 localCenter; // centre of mass in the body frame
+	s2Vec2 c1, c2;		// centre of mass in the world at fractions 0 and 1
+	s2Rot q1, q2;		// rotation at fractions 0 and 1
+} s2Sweep;
+
+typedef struct s2TOIInput
+{
+	s2DistanceProxy proxyA; // vertices in body A's frame
+	s2DistanceProxy proxyB; // vertices in body B's frame
+	s2Sweep sweepA;
+	s2Sweep sweepB;
+	float maxFraction; // sweep interval [0, maxFraction], maxFraction <= 1
+} s2TOIInput;
+
+typedef enum s2TOIState
+{
+	s2_toiStateUnknown,
+	s2_toiStateFailed,	   // the iteration cap was reached: fraction is a time the shapes are still apart
+	s2_toiStateOverlapped, // the shapes are within the target separation at fraction 0
+	s2_toiStateHit,		   // the shapes reach the target separation at fraction
+	s2_toiStateSeparated   // the shapes stay apart over the whole interval: fraction = maxFraction
+} s2TOIState;
+
+typedef struct s2TOIOutput
+{
+	s2TOIState state;
+	float fraction;
+	int32_t iterations; // conservative-advancement iterations taken
+} s2TOIOutput;
+
+// The body transform of a sweep at `fraction`.
+S2B_API s2Transform s2GetSweepTransform(const s2Sweep* sweep, float fraction);
+// Time of impact by conservative advancement: the first fraction at which the shapes' separation (radii included) falls to
+// s2_linearSlop, within a tolerance of s2_linearSlop / 4. The same function runs in the device's continuous pass.
+S2B_API s2TOIOutput s2TimeOfImpact(const s2TOIInput* input);
+// iteration cap of s2TimeOfImpact (s2TOIOutput.iterations never exceeds it)
+#define S2_TOI_MAX_ITERATIONS 50
+
+// The extents a body is classified as fast by, for one shape given in polygon form (circle: 1 vertex; capsule:
+// s2MakeCapsule; segment: s2MakeCapsule with radius 0): minExtent = the radius for a circle or capsule, 0 for a segment,
+// the smallest distance from the centroid to an edge plus the radius for a polygon; maxExtent = the largest distance of a
+// vertex from localCenter (the body's centre of mass, body frame) plus the radius. A body's extents are the smallest
+// minExtent and the largest maxExtent of its shapes. center: where the shape's core proxy sits (a circle of radius
+// minExtent / 4 that continuous collision sweeps for a shape that starts a step touching a static shape): the vertex of a
+// circle, the midpoint of a capsule or segment, the centroid of a polygon.
+typedef struct s2ShapeExtent
+{
+	float minExtent, maxExtent;
+	s2Vec2 center;
+} s2ShapeExtent;
+S2B_API s2ShapeExtent s2ComputeShapeExtent(const s2Polygon* polygonForm, s2Vec2 localCenter);
+// The extents of a body with `count` shapes in polygon form about its centre of mass localCenter: the smallest minExtent
+// and the largest maxExtent of the shapes (s2_huge and 0 without shapes), center = localCenter. What the host stores in
+// s2bBodyRow.minExtent / maxExtent whenever a shape is added to a body.
+S2B_API s2ShapeExtent s2ComputeBodyExtent(const s2Polygon* polygonForms, int32_t count, s2Vec2 localCenter);
 
 // Push every pending host-side edit to the device now (s2World_Step does this itself).
 S2B_API void s2World_Flush(s2WorldId worldId);

@@ -371,6 +371,42 @@ class MassData(C.Structure):
     _fields_ = [("mass", C.c_float), ("center", Vec2), ("I", C.c_float)]
 
 
+class DistanceProxy(C.Structure):
+    _fields_ = [("vertices", Vec2 * MAX_POLYGON_VERTICES), ("count", C.c_int32), ("radius", C.c_float)]
+
+
+class DistanceInput(C.Structure):
+    _fields_ = [("proxyA", DistanceProxy), ("proxyB", DistanceProxy), ("transformA", Transform),
+                ("transformB", Transform), ("useRadii", C.c_bool)]
+
+
+class DistanceOutput(C.Structure):
+    _fields_ = [("pointA", Vec2), ("pointB", Vec2), ("distance", C.c_float), ("iterations", C.c_int32)]
+
+
+class Sweep(C.Structure):
+    """s2Sweep (include/solver2d_b200.h): centre c1 -> c2 linearly, rotation q1 -> q2 by normalised lerp."""
+    _fields_ = [("localCenter", Vec2), ("c1", Vec2), ("c2", Vec2), ("q1", Rot), ("q2", Rot)]
+
+
+class TOIInput(C.Structure):
+    _fields_ = [("proxyA", DistanceProxy), ("proxyB", DistanceProxy), ("sweepA", Sweep), ("sweepB", Sweep),
+                ("maxFraction", C.c_float)]
+
+
+class TOIOutput(C.Structure):
+    _fields_ = [("state", C.c_int), ("fraction", C.c_float), ("iterations", C.c_int32)]
+
+
+class ShapeExtent(C.Structure):
+    _fields_ = [("minExtent", C.c_float), ("maxExtent", C.c_float), ("center", Vec2)]
+
+
+# s2TOIState (include/solver2d_b200.h)
+TOI_UNKNOWN, TOI_FAILED, TOI_OVERLAPPED, TOI_HIT, TOI_SEPARATED = range(5)
+TOI_MAX_ITERATIONS = 50  # S2_TOI_MAX_ITERATIONS
+
+
 # host-callable geometry / narrow-phase API (reference include/solver2d/manifold.h, geometry.h)
 _API.update({
     "s2CollideCircles": (Manifold, [C.POINTER(Circle), Transform, C.POINTER(Circle), Transform]),
@@ -391,6 +427,16 @@ _API.update({
     "s2ComputePolygonAABB": (Box, [C.POINTER(Polygon), Transform]),
     "s2PointInPolygon": (C.c_bool, [Vec2, C.POINTER(Polygon)]),
     "s2MakeRoundedBox": (Polygon, [C.c_float, C.c_float, C.c_float]),
+    "s2MakeProxy": (DistanceProxy, [C.POINTER(Vec2), C.c_int32, C.c_float]),
+    "s2ShapeDistance": (DistanceOutput, [C.POINTER(DistanceCache), C.POINTER(DistanceInput)]),
+    # continuous collision (include/solver2d_b200.h): extensions, absent from the reference
+    "s2World_EnableContinuous": (None, [WorldId, C.c_bool]),
+    "s2Body_SetTransform": (None, [BodyId, Vec2, C.c_float]),
+    "s2World_Flush": (None, [WorldId]),
+    "s2GetSweepTransform": (Transform, [C.POINTER(Sweep), C.c_float]),
+    "s2TimeOfImpact": (TOIOutput, [C.POINTER(TOIInput)]),
+    "s2ComputeShapeExtent": (ShapeExtent, [C.POINTER(Polygon), Vec2]),
+    "s2ComputeBodyExtent": (ShapeExtent, [C.POINTER(Polygon), C.c_int32, Vec2]),
 })
 
 QUERY_CALLBACK = C.CFUNCTYPE(C.c_bool, ShapeId, C.c_void_p)

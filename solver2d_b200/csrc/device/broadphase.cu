@@ -15,11 +15,30 @@
 //     sort on the 64-bit shape-pair key and all contact columns are gathered into the other column set.
 // The contact table is therefore always sorted by pair key: the device's natural (wavefront) constraint order.
 #include "s2b_internal.cuh"
+#include "shared/s2_toi.h"
 
 #include <cub/cub.cuh>
 #include <thrust/iterator/counting_iterator.h>
 
 #include <algorithm>
+
+// continuous collision (s2bContinuousSnapshot / s2bContinuousPass); the columns exist only while the feature is on
+struct ContinuousScratch
+{
+	DevArray<float4> start;		  // per body: centre of mass and rotation before the solver stage (c.x c.y q.s q.c)
+	DevArray<unsigned> fraction;  // per body: float bits of the earliest time of impact (1.0f: none)
+	DevArray<int> shapes;		  // shapes of the fast bodies of this step
+	DevArray<int> counters;		  // [0] shapes listed, [1] bodies clamped
+	bool ran = false;			  // the last s2b_solve ran the pass (the counters are its)
+
+	void release()
+	{
+		start.release();
+		fraction.release();
+		shapes.release();
+		counters.release();
+	}
+};
 
 struct BroadScratch
 {
@@ -53,6 +72,7 @@ struct BroadScratch
 	bool treeValid = false;
 	int treeShapeCap = 0;
 	int treeReuses = 0;
+	unsigned long long treeShapeEpoch = 0; // s2bWorld::shapeEpoch at the last refit: every static box in the tree is current
 	// open-addressing hash set of the shape-pair keys of the current contact table ("does this pair already exist?")
 	DevArray<unsigned long long> pairHash;
 	unsigned long long hashMask = 0;
@@ -70,6 +90,7 @@ struct BroadScratch
 	// the counters' copy to the mailbox runs on a stream of its own: on the world's stream the step would wait for it, and on
 	// the transforms' side stream (s2b_download_transforms) the read-back would wait for the whole search
 	cudaStream_t mailStream = nullptr;
+	ContinuousScratch cont;
 };
 
 #define S2B_TREE_REUSE_LIMIT 16
@@ -119,6 +140,7 @@ void s2bFreeBroadScratch(s2bWorld* w)
 	b->cubTemp.release();
 	b->largeShapes.release();
 	b->pairHash.release();
+	b->cont.release();
 	for (int i = 0; i < 2; ++i)
 	{
 		if (b->evSearch[i] != nullptr)
@@ -1059,20 +1081,13 @@ static size_t bpReserve(s2bWorld* w, BroadScratch* B)
 	return tempBytes;
 }
 
-// First half of a pass, no host synchronisation: hierarchy (re-used or rebuilt) and refit, pair-key hash of the current
-// table, queries from the moved proxies -> candidate pairs (newKey / newShapes), survivors of the current table (keepSlots),
-// and the counters of all that copied to the pinned mailbox.
-static void bpSearch(s2bWorld* w, BroadScratch* B)
+// The hierarchy of a pass over every live shape at its current fat box: the topology of the last build is re-used when
+// `reuseTree`, else rebuilt; the refit then brings every box up to date and clears the per-pass counters.
+static void bpTree(s2bWorld* w, BroadScratch* B, bool reuseTree)
 {
 	cudaStream_t st = w->stream;
 	int shapeCap = w->shapeCap;
-	int oldCount = w->contactCount;
 	ShapeView sv = shapeView(w);
-	BodyView bv = bodyView(w);
-	ContactColumns& cur = w->contacts[w->cur];
-	int newCap = B->newPairCap;
-
-	bool reuseTree = B->treeValid && w->pairsDirty == false && B->treeShapeCap == shapeCap && B->treeReuses < S2B_TREE_REUSE_LIMIT;
 	if (reuseTree)
 	{
 		// keep BC_LEAVES and BC_HEIGHT of the build; s2bRefit clears the per-pass counters
@@ -1112,6 +1127,25 @@ static void bpSearch(s2bWorld* w, BroadScratch* B)
 	// ---- refit ----
 	S2B_LAUNCH(w, s2bRefit, gridFor(shapeCap, 256), 256, 0, sv, B->leafShape.p, B->leafOut.p, B->counters.p, B->wideCount.p,
 			   B->wideSlot.p, B->wideBox.p, B->visit.p, B->rootBox.p);
+
+	B->treeShapeEpoch = w->shapeEpoch;
+}
+
+// First half of a pass, no host synchronisation: hierarchy (re-used or rebuilt) and refit, pair-key hash of the current
+// table, queries from the moved proxies -> candidate pairs (newKey / newShapes), survivors of the current table (keepSlots),
+// and the counters of all that copied to the pinned mailbox.
+static void bpSearch(s2bWorld* w, BroadScratch* B)
+{
+	cudaStream_t st = w->stream;
+	int shapeCap = w->shapeCap;
+	int oldCount = w->contactCount;
+	ShapeView sv = shapeView(w);
+	BodyView bv = bodyView(w);
+	ContactColumns& cur = w->contacts[w->cur];
+	int newCap = B->newPairCap;
+
+	bool reuseTree = B->treeValid && w->pairsDirty == false && B->treeShapeCap == shapeCap && B->treeReuses < S2B_TREE_REUSE_LIMIT;
+	bpTree(w, B, reuseTree);
 
 	// ---- pair-key hash set of the current contact table (rebuilt only when the table changed) ----
 	if (B->hashVersion != w->contactTableVersion || B->pairHash.p == nullptr)
@@ -1363,5 +1397,322 @@ void s2bBroadphaseUpdatePairs(s2bWorld* w)
 		w->treeHeight = hc[BC_HEIGHT];
 		bpCommit(w, B, fresh, kept, tempBytes);
 		break;
+	}
+}
+
+// ---------------------------------------------------------------------------------------------------------------
+// continuous collision: dynamic bodies against static shapes (DESIGN.md §3.11)
+// ---------------------------------------------------------------------------------------------------------------
+
+#define S2B_FRACTION_ONE 0x3F800000u // bits of 1.0f
+#define S2B_SWEEP_BLOCK 128
+
+// before the solver stage: each dynamic body's centre and rotation, and no time of impact yet
+__global__ void s2bContinuousStart(BodyView b, float4* start, unsigned* fraction, int* counters)
+{
+	int i = blockIdx.x * blockDim.x + threadIdx.x;
+	if (i == 0)
+	{
+		counters[0] = 0;
+		counters[1] = 0;
+	}
+	if (i >= b.capacity)
+	{
+		return;
+	}
+	fraction[i] = S2B_FRACTION_ONE;
+	unsigned f = b.flags[i];
+	if ((f & S2B_BODY_VALID) != 0 && S2B_BODY_TYPE(f) == S2B_BODY_DYNAMIC)
+	{
+		float4 pos = b.pos[i], pose = b.pose[i];
+		start[i] = make_float4(pos.x, pos.y, pose.z, pose.w);
+	}
+}
+
+__device__ __forceinline__ s2Sweep s2bBodySweep(const BodyView& b, const float4* start, int body)
+{
+	float4 s0 = start[body], pos = b.pos[body], pose = b.pose[body], org = b.org[body];
+	s2Sweep sweep;
+	sweep.localCenter = s2cVec(org.z, org.w);
+	sweep.c1 = s2cVec(s0.x, s0.y);
+	sweep.c2 = s2cVec(pos.x, pos.y);
+	sweep.q1.s = s0.z;
+	sweep.q1.c = s0.w;
+	sweep.q2.s = pose.z;
+	sweep.q2.c = pose.w;
+	return sweep;
+}
+
+// a dynamic body is fast when |c1 - c0| + |dtheta| maxExtent > minExtent / 2
+__device__ __forceinline__ bool s2bIsFast(const s2Sweep& sweep, float2 ext)
+{
+	float moved = s2Distance(sweep.c1, sweep.c2) + S2_ABS(s2RelativeAngle(sweep.q2, sweep.q1)) * ext.y;
+	return moved > 0.5f * ext.x;
+}
+
+// the shapes of fast bodies, compacted (one atomic per block)
+__global__ void s2bContinuousCollect(ShapeView s, BodyView b, const float2* ext, const float4* start, int* list, int* counters)
+{
+	int i = blockIdx.x * blockDim.x + threadIdx.x;
+	bool fast = false;
+	if (i < s.capacity)
+	{
+		int4 head = s.head[i];
+		if (head.x & S2B_ROW_VALID)
+		{
+			int body = head.y;
+			unsigned f = b.flags[body];
+			if (S2B_BODY_TYPE(f) == S2B_BODY_DYNAMIC)
+			{
+				fast = s2bIsFast(s2bBodySweep(b, start, body), ext[body]);
+			}
+		}
+	}
+	s2bBlockAppend(fast, i, list, counters + 0);
+}
+
+__device__ __forceinline__ void s2bLoadShapeVertices(s2Vec2* vertices, const ShapeView& s, int shape, int count)
+{
+#pragma unroll
+	for (int k = 0; k < s2_maxPolygonVertices; ++k)
+	{
+		if (k < count)
+		{
+			float2 v = s.verts[shape * 8 + k];
+			vertices[k] = s2cVec(v.x, v.y);
+		}
+	}
+}
+
+// The time of impact of one fast shape against one static shape (proxy A = the static shape, proxy B = the fast one), 1 for
+// none. A pair that starts within the target is swept again with the shape's core (a circle of a quarter of its inner extent
+// at its centroid): the body is held back only if that core would hit, or starts within the target and moves toward the
+// static shape (s2cCoreApproaches: held at 0). A segment has no interior and so no core: touching at the start, it is let go.
+__device__ __forceinline__ float s2bStaticImpact(const ShapeView& s, const BodyView& b, int other, int bodyO, const s2Vec2* vertices,
+												 int count, float radius, const s2cShapeExtent& extent, const s2Sweep& sweep)
+{
+	float4 pos = b.pos[bodyO], pose = b.pose[bodyO], org = b.org[bodyO];
+	s2Sweep sweepO;
+	sweepO.localCenter = s2cVec(org.z, org.w);
+	sweepO.c1 = s2cVec(pos.x, pos.y);
+	sweepO.c2 = sweepO.c1;
+	sweepO.q1.s = pose.z;
+	sweepO.q1.c = pose.w;
+	sweepO.q2 = sweepO.q1;
+	int4 headO = s.head[other];
+	int countO = headO.w;
+	s2Vec2 verticesO[s2_maxPolygonVertices];
+	s2bLoadShapeVertices(verticesO, s, other, countO);
+	float radiusO = s.fr[other].y;
+	// (one call site for both sweeps: the conservative advancement is inlined once)
+	const s2Vec2* verticesB = vertices;
+	int countB = count;
+	float radiusB = radius;
+	s2TOIOutput out;
+	for (int attempt = 0; attempt < 2; ++attempt)
+	{
+		out = s2cTimeOfImpact(verticesO, countO, radiusO, &sweepO, verticesB, countB, radiusB, &sweep, 1.0f);
+		if (out.state != s2_toiStateOverlapped || extent.inner <= 0.0f)
+		{
+			break; // (a shape without interior, a segment, has no core: touching at the start, it is let go)
+		}
+		verticesB = &extent.core;
+		countB = 1;
+		radiusB = 0.25f * extent.inner;
+	}
+	if (out.state == s2_toiStateOverlapped && countB == 1 && verticesB != vertices &&
+		s2cCoreApproaches(verticesO, countO, &sweepO, extent.core, &sweep))
+	{
+		return 0.0f;
+	}
+	return out.state == s2_toiStateHit || out.state == s2_toiStateFailed ? out.fraction : 1.0f;
+}
+
+// One thread per listed shape: the box it sweeps over the step, a walk of the wide hierarchy with it, the broad phase's pair
+// rules on every static leaf it overlaps, a time of impact against each survivor, and the earliest one to the body (an
+// atomic min on the bits: fractions are non-negative, so their bits order like the floats, whatever the thread order).
+__global__ void __launch_bounds__(S2B_SWEEP_BLOCK) s2bContinuousSweep(ShapeView s, BodyView b, const float4* start, const int* list,
+																		const int* counters, const int* treeCounters, const float4* wideBox,
+																		const int* wideChild, const unsigned long long* jointKeys,
+																		int jointKeyCount, unsigned* fraction)
+{
+	int k = blockIdx.x * blockDim.x + threadIdx.x;
+	if (k >= counters[0] || treeCounters[BC_LEAVES] <= 1)
+	{
+		return;
+	}
+	int shape = list[k];
+	int4 head = s.head[shape];
+	int body = head.y;
+	int count = head.w;
+	int type = (head.x >> 1) & 0x7;
+	int4 filter = s.filter[shape];
+	float radius = s.fr[shape].y;
+	s2Vec2 vertices[s2_maxPolygonVertices], normals[s2_maxPolygonVertices];
+	s2bLoadShapeVertices(vertices, s, shape, count);
+#pragma unroll
+	for (int i = 0; i < s2_maxPolygonVertices; ++i)
+	{
+		if (i < count)
+		{
+			float2 n = s.normals[shape * 8 + i];
+			normals[i] = s2cVec(n.x, n.y);
+		}
+	}
+	s2Sweep sweep = s2bBodySweep(b, start, body);
+	s2cShapeExtent extent = s2cComputeShapeExtent(vertices, normals, count, radius, sweep.localCenter);
+
+	// Swept box: the box of the centre's path plus the box of the vertices about the centre at both rotations, widened by the
+	// radius, by how far the rotation's arc bulges past its chord (r (1 - cos(phi / 2))) and by the target separation and
+	// tolerance. It holds the shape at every fraction, which the union of the end boxes alone does not for a rotating body.
+	float cosPhi = sweep.q1.c * sweep.q2.c + sweep.q1.s * sweep.q2.s;
+	float cosHalf = sqrtf(S2_MAX(0.0f, 0.5f * (1.0f + cosPhi)));
+	float reach = s2cMaxVertexDistance(vertices, count, sweep.localCenter);
+	float pad = radius + reach * (1.0f - cosHalf) + S2C_TOI_TARGET + S2C_TOI_TOLERANCE;
+	s2Vec2 lower = s2Min(sweep.c1, sweep.c2), upper = s2Max(sweep.c1, sweep.c2);
+	s2Vec2 lo = s2RotateVector(sweep.q1, s2Sub(vertices[0], sweep.localCenter)), hi = lo;
+	for (int i = 0; i < count; ++i)
+	{
+		s2Vec2 r = s2Sub(vertices[i], sweep.localCenter);
+		s2Vec2 r1 = s2RotateVector(sweep.q1, r), r2 = s2RotateVector(sweep.q2, r);
+		lo = s2Min(lo, s2Min(r1, r2));
+		hi = s2Max(hi, s2Max(r1, r2));
+	}
+	float4 box = make_float4(lower.x + lo.x - pad, lower.y + lo.y - pad, upper.x + hi.x + pad, upper.y + hi.y + pad);
+
+	float earliest = 1.0f;
+	int stack[S2B_QUERY_STACK];
+	int sp = 0;
+	int node = 0;
+	while (node >= 0)
+	{
+		const float4* boxes = wideBox + node * S2B_WIDE;
+		const int* refs = wideChild + node * S2B_WIDE;
+		int next = -1;
+		for (int i = 0; i < S2B_WIDE; ++i)
+		{
+			int c = refs[i];
+			if (c == S2B_WIDE_EMPTY || s2bBoxesOverlap(box, boxes[i]) == false)
+			{
+				continue;
+			}
+			if (c >= 0)
+			{
+				if (next < 0)
+				{
+					next = c;
+				}
+				else
+				{
+					stack[sp++] = c;
+				}
+				continue;
+			}
+			int other = ~c;
+			int4 headO = s.head[other];
+			int bodyO = headO.y;
+			// static shapes only, under the broad phase's own rules: filter, joint override, a manifold for the pair
+			if ((headO.x & S2B_ROW_VALID) == 0 || S2B_BODY_TYPE((unsigned)b.flags[bodyO]) != S2B_BODY_STATIC)
+			{
+				continue;
+			}
+			if (s2bShouldShapesCollide(filter, s.filter[other]) == false || s2bJointOverride(jointKeys, jointKeyCount, body, bodyO) ||
+				s2bPairKind(type, (headO.x >> 1) & 0x7) == 0)
+			{
+				continue;
+			}
+			earliest = S2_MIN(earliest, s2bStaticImpact(s, b, other, bodyO, vertices, count, radius, extent, sweep));
+		}
+		node = next >= 0 ? next : (sp > 0 ? stack[--sp] : -1);
+	}
+	if (earliest < 1.0f)
+	{
+		atomicMin(fraction + body, __float_as_uint(earliest));
+	}
+}
+
+// a body with a time of impact takes the sweep's pose at it (its velocity stays); finalize then derives its origin and boxes
+__global__ void s2bContinuousClamp(BodyView b, const float4* start, const unsigned* fraction, int* counters)
+{
+	int i = blockIdx.x * blockDim.x + threadIdx.x;
+	if (i >= b.capacity || fraction[i] >= S2B_FRACTION_ONE)
+	{
+		return;
+	}
+	s2Sweep sweep = s2bBodySweep(b, start, i);
+	s2Vec2 c;
+	s2Rot q;
+	s2cSweepPose(&sweep, __uint_as_float(fraction[i]), &c, &q);
+	float4 pos = b.pos[i], pose = b.pose[i];
+	b.pos[i] = make_float4(c.x, c.y, pos.z, pos.w);
+	b.pose[i] = make_float4(pose.x, pose.y, q.s, q.c);
+	atomicAdd(counters + 1, 1);
+}
+
+void s2bContinuousSnapshot(s2bWorld* w)
+{
+	S2bEpochFreeze freeze; // none of these columns is part of the solver stage's graph
+	BroadScratch* B = getBroad(w);
+	ContinuousScratch& C = B->cont;
+	cudaStream_t st = w->stream;
+	if (w->bodyCap == 0)
+	{
+		return;
+	}
+	C.start.reserve((size_t)w->bodyCap, st, false, false);
+	C.fraction.reserve((size_t)w->bodyCap, st, false, false);
+	C.counters.reserve(2, st, false);
+	S2B_LAUNCH(w, s2bContinuousStart, gridFor(w->bodyCap, 256), 256, 0, bodyView(w), C.start.p, C.fraction.p, C.counters.p);
+}
+
+void s2bContinuousPass(s2bWorld* w)
+{
+	S2bEpochFreeze freeze;
+	if (w->continuous == 0)
+	{
+		if (w->broad != nullptr && w->broad->cont.start.p != nullptr)
+		{
+			S2B_CHECK(cudaStreamSynchronize(w->stream));
+			w->broad->cont.release();
+		}
+		if (w->broad != nullptr)
+		{
+			w->broad->cont.ran = false;
+		}
+		return;
+	}
+	BroadScratch* B = getBroad(w);
+	ContinuousScratch& C = B->cont;
+	cudaStream_t st = w->stream;
+	C.ran = false;
+	if (w->bodyCap == 0 || w->shapeCap == 0 || C.start.p == nullptr)
+	{
+		return;
+	}
+	// The hierarchy has to hold every live static shape at its current box. A pair pass leaves it so, and static boxes change
+	// only by uploads, which mark the pairs dirty; a world whose pair pass never ran since its last shape upload (or ever)
+	// builds it here. A search prefetched behind the previous step would share the counters, so it is dropped.
+	if (B->treeValid == false || B->treeShapeCap != w->shapeCap || B->treeShapeEpoch != w->shapeEpoch)
+	{
+		B->prefetched = false;
+		bpReserve(w, B);
+		bpTree(w, B, false);
+	}
+	C.shapes.reserve((size_t)w->shapeCap, st, false, false);
+	ShapeView sv = shapeView(w);
+	BodyView bv = bodyView(w);
+	S2B_LAUNCH(w, s2bContinuousCollect, gridFor(w->shapeCap, 256), 256, 0, sv, bv, w->bExt.p, C.start.p, C.shapes.p, C.counters.p);
+	S2B_LAUNCH(w, s2bContinuousSweep, gridFor(w->shapeCap, S2B_SWEEP_BLOCK), S2B_SWEEP_BLOCK, 0, sv, bv, C.start.p, C.shapes.p,
+			   C.counters.p, B->counters.p, B->wideBox.p, B->wideChild.p, w->jointPairKeys.p, w->jointPairCount, C.fraction.p);
+	S2B_LAUNCH(w, s2bContinuousClamp, gridFor(w->bodyCap, 256), 256, 0, bv, C.start.p, C.fraction.p, C.counters.p);
+	C.ran = true;
+}
+
+void s2bContinuousCounters(s2bWorld* w, int out[2])
+{
+	out[0] = out[1] = 0;
+	if (w->broad != nullptr && w->broad->cont.ran)
+	{
+		S2B_CHECK(cudaMemcpy(out, w->broad->cont.counters.p, sizeof(int) * 2, cudaMemcpyDeviceToHost));
 	}
 }

@@ -329,6 +329,7 @@ struct s2bWorld
 						// s2b_set_dataflow / S2B_DATAFLOW=1 enable it
 	int restitution = 0;			   // s2b_set_restitution: end the solver stage with the restitution pass
 	float restitutionThreshold = 1.0f; // approach speed (m/s) below which a contact does not bounce
+	int continuous = 0;				   // s2b_set_continuous: sweep fast bodies against static shapes after the solver stage
 	int gatherWarm = 1; // per-body warm-start gather (warm_gather.cuh); s2b_set_warm_gather / S2B_WARM_GATHER=0 disable it
 	int smCount = 132;
 	int coopSupported = 0;
@@ -343,6 +344,7 @@ struct s2bWorld
 	int bodyCap = 0;
 	DevArray<float4> bVel, bPose, bPos, bOrg, bFrc, bPrm, bAux0, bAux1;
 	DevArray<uint8_t> bFlags;
+	DevArray<float2> bExt; // minExtent maxExtent (continuous collision; kept out of BodyView, which the solver kernels take)
 
 	// shapes
 	int shapeCap = 0;
@@ -384,6 +386,7 @@ struct s2bWorld
 	// broad phase
 	bool pairsDirty = true; // host-side structural change
 	unsigned long long uploadEpoch = 0; // bumped by every row upload: a pair search started before it is stale
+	unsigned long long shapeEpoch = 0;	// bumped by every shape upload: a hierarchy refitted before it may miss static boxes
 	int prefetchPairs = 1;	// start the pair search of the next step behind finalize (S2B_PREFETCH_PAIRS=0: off)
 	int kempe = 1;		// empty a sparse top colour by Kempe chains after colouring (S2B_KEMPE=0 disables)
 	int wholeIslandBodies = 1200; // regions: islands up to this size are never cut (S2B_WHOLE_ISLAND)
@@ -516,3 +519,7 @@ void s2bSolve(s2bWorld* w, int solverType, const s2bStepContext* ctx);
 void s2bFinalize(s2bWorld* w);
 void s2bFreeSolverScratch(s2bWorld* w);
 void s2bFreeBroadScratch(s2bWorld* w);
+// continuous collision (broadphase.cu, DESIGN.md §3.11): the start poses before the solver stage, the sweep and clamp after it
+void s2bContinuousSnapshot(s2bWorld* w);
+void s2bContinuousPass(s2bWorld* w);
+void s2bContinuousCounters(s2bWorld* w, int out[2]);

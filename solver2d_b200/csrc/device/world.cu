@@ -10,7 +10,7 @@
 // scatter kernels
 // ---------------------------------------------------------------------------------------------------------------
 
-__global__ void s2bScatterBodies(const s2bBodyRow* __restrict__ rows, int count, BodyView b, int* schedDirty)
+__global__ void s2bScatterBodies(const s2bBodyRow* __restrict__ rows, int count, BodyView b, float2* ext, int* schedDirty)
 {
 	int t = blockIdx.x * blockDim.x + threadIdx.x;
 	if (t >= count)
@@ -47,6 +47,7 @@ __global__ void s2bScatterBodies(const s2bBodyRow* __restrict__ rows, int count,
 	}
 	b.prm[i] = make_float4(r.linearDamping, r.angularDamping, r.gravityScale, r.invI);
 	b.flags[i] = (uint8_t)(r.flags & 0x7);
+	ext[i] = make_float2(r.minExtent, r.maxExtent);
 }
 
 __global__ void s2bScatterShapes(const s2bShapeRow* __restrict__ rows, int count, ShapeView s)
@@ -150,7 +151,7 @@ __global__ void s2bScatterContacts(const s2bContactRow* __restrict__ rows, int c
 // gather kernels
 // ---------------------------------------------------------------------------------------------------------------
 
-__global__ void s2bGatherBodies(s2bBodyRow* rows, int count, BodyView b, int useRowIndex)
+__global__ void s2bGatherBodies(s2bBodyRow* rows, int count, BodyView b, const float2* ext, int useRowIndex)
 {
 	int t = blockIdx.x * blockDim.x + threadIdx.x;
 	if (t >= count)
@@ -183,6 +184,9 @@ __global__ void s2bGatherBodies(s2bBodyRow* rows, int count, BodyView b, int use
 	r.linearDamping = prm.x;
 	r.angularDamping = prm.y;
 	r.gravityScale = prm.z;
+	float2 e = ext[i];
+	r.minExtent = e.x;
+	r.maxExtent = e.y;
 	rows[t] = r;
 }
 
@@ -467,6 +471,7 @@ extern "C" void s2b_world_destroy(s2bWorld* w)
 	w->bAux0.release();
 	w->bAux1.release();
 	w->bFlags.release();
+	w->bExt.release();
 	w->sHead.release();
 	w->sFilter.release();
 	w->sAabb.release();
@@ -601,6 +606,12 @@ extern "C" void s2b_set_restitution(s2bWorld* w, int enable, float threshold)
 	w->restitution = enable != 0 ? 1 : 0;
 }
 
+extern "C" void s2b_set_continuous(s2bWorld* w, int enable)
+{
+	// no scheduleEpoch bump: the pass runs outside the solver stage's graph
+	w->continuous = enable != 0 ? 1 : 0;
+}
+
 static void reserveBodies(s2bWorld* w, int cap)
 {
 	if (cap <= w->bodyCap)
@@ -617,6 +628,7 @@ static void reserveBodies(s2bWorld* w, int cap)
 	w->bAux0.reserve(cap, s);
 	w->bAux1.reserve(cap, s);
 	w->bFlags.reserve(cap, s);
+	w->bExt.reserve(cap, s);
 	w->bodyCap = (int)w->bVel.cap;
 }
 
@@ -667,7 +679,7 @@ extern "C" void s2b_upload_bodies(s2bWorld* w, const s2bBodyRow* rows, int count
 	}
 	w->uploadEpoch += 1; // rows changed: a pair search started behind the previous step is stale now
 	s2bBodyRow* d = (s2bBodyRow*)stageRows(w, rows, sizeof(s2bBodyRow) * (size_t)count);
-	S2B_LAUNCH(w, s2bScatterBodies, gridFor(count, 128), 128, 0, d, count, bodyView(w), w->schedDirty.p);
+	S2B_LAUNCH(w, s2bScatterBodies, gridFor(count, 128), 128, 0, d, count, bodyView(w), w->bExt.p, w->schedDirty.p);
 	S2B_CHECK(cudaFreeAsync(d, w->stream));
 	// the staging copy reads pageable host memory: make sure it is consumed before the caller reuses the buffer
 	S2B_CHECK(cudaStreamSynchronize(w->stream));
@@ -687,6 +699,7 @@ extern "C" void s2b_upload_shapes(s2bWorld* w, const s2bShapeRow* rows, int coun
 	S2B_CHECK(cudaFreeAsync(d, w->stream));
 	S2B_CHECK(cudaStreamSynchronize(w->stream));
 	w->pairsDirty = true;
+	w->shapeEpoch += 1;
 }
 
 extern "C" void s2b_upload_joints(s2bWorld* w, const s2bJointRow* rows, int count, int jointCapacity)
@@ -1041,7 +1054,7 @@ extern "C" void s2b_download_bodies(s2bWorld* w, s2bBodyRow* rows, int count)
 	}
 	S2B_CHECK(cudaSetDevice(w->device));
 	s2bBodyRow* d = (s2bBodyRow*)stageRows(w, rows, sizeof(s2bBodyRow) * (size_t)count);
-	S2B_LAUNCH(w, s2bGatherBodies, gridFor(count, 128), 128, 0, d, count, bodyView(w), 1);
+	S2B_LAUNCH(w, s2bGatherBodies, gridFor(count, 128), 128, 0, d, count, bodyView(w), w->bExt.p, 1);
 	S2B_CHECK(cudaMemcpyAsync(rows, d, sizeof(s2bBodyRow) * (size_t)count, cudaMemcpyDeviceToHost, w->stream));
 	S2B_CHECK(cudaFreeAsync(d, w->stream));
 	S2B_CHECK(cudaStreamSynchronize(w->stream));
@@ -1060,7 +1073,7 @@ extern "C" void s2b_download_all_bodies(s2bWorld* w, s2bBodyRow* rows, int capac
 	}
 	s2bBodyRow* d = nullptr;
 	S2B_CHECK(cudaMallocAsync((void**)&d, sizeof(s2bBodyRow) * (size_t)capacity, w->stream));
-	S2B_LAUNCH(w, s2bGatherBodies, gridFor(capacity, 128), 128, 0, d, capacity, bodyView(w), 0);
+	S2B_LAUNCH(w, s2bGatherBodies, gridFor(capacity, 128), 128, 0, d, capacity, bodyView(w), w->bExt.p, 0);
 	S2B_CHECK(cudaMemcpyAsync(rows, d, sizeof(s2bBodyRow) * (size_t)capacity, cudaMemcpyDeviceToHost, w->stream));
 	S2B_CHECK(cudaFreeAsync(d, w->stream));
 	S2B_CHECK(cudaStreamSynchronize(w->stream));
@@ -1206,7 +1219,14 @@ extern "C" void s2b_solve(s2bWorld* w, int solverType, const s2bStepContext* con
 	S2B_CHECK(cudaSetDevice(w->device));
 	w->xfSeq += 1;
 	S2B_CHECK(cudaEventRecord(w->timer.ev[2], w->stream));
+	// continuous collision brackets the solver stage (and its graph): start poses after this step's uploads, the sweep
+	// and the clamp before finalize derives origins and boxes from the poses
+	if (w->continuous)
+	{
+		s2bContinuousSnapshot(w);
+	}
 	s2bSolve(w, solverType, context);
+	s2bContinuousPass(w);
 }
 
 extern "C" void s2b_finalize(s2bWorld* w)

@@ -3,6 +3,9 @@
 // uploads the row. Reads of simulation state first make the host copy current (s2SyncStateToHost).
 #include "s2_host.h"
 
+#include "solver2d_b200.h"
+
+#include <stdlib.h>
 #include <string.h>
 
 s2Body* s2GetBody(s2World* world, s2BodyId id)
@@ -38,6 +41,8 @@ s2BodyId s2CreateBody(s2WorldId worldId, const s2BodyDef* def)
 	slot->localCenter = slot->force = s2Vec2_zero;
 	slot->torque = 0.0f;
 	slot->mass = slot->invMass = slot->I = slot->invI = 0.0f;
+	slot->minExtent = s2_huge;
+	slot->maxExtent = 0.0f;
 	slot->shapeList = S2_NULL_INDEX;
 	slot->jointCount = 0;
 	// device mirror: not there yet (rowDirty / forceDirty keep their value — a reused slot may already sit in the dirty list)
@@ -132,6 +137,51 @@ s2MassData s2Shape_ComputeMass(const s2Shape* shape)
 		return s2_shapeMass[shape->type](&shape->capsule, shape->density);
 	}
 	return (s2MassData){0};
+}
+
+s2Polygon s2Shape_PolygonForm(const s2Shape* shape)
+{
+	s2Polygon poly;
+	switch (shape->type)
+	{
+		case s2_circleShape:
+			memset(&poly, 0, sizeof(poly));
+			poly.vertices[0] = shape->circle.point;
+			poly.count = 1;
+			poly.radius = shape->circle.radius;
+			break;
+		case s2_capsuleShape:
+			poly = s2MakeCapsule(shape->capsule.point1, shape->capsule.point2, shape->capsule.radius);
+			break;
+		case s2_segmentShape:
+			poly = s2MakeCapsule(shape->segment.point1, shape->segment.point2, 0.0f);
+			break;
+		default:
+			poly = shape->polygon;
+			break;
+	}
+	return poly;
+}
+
+// The extents continuous collision classifies the body by (s2ComputeBodyExtent over its shapes, about the centre of mass).
+// Called whenever a shape is added.
+static void s2UpdateBodyExtents(s2World* world, s2Body* b)
+{
+	int32_t count = 0;
+	for (int32_t next = b->shapeList; next != S2_NULL_INDEX; next = world->shapes[next].nextShapeIndex)
+	{
+		count += 1;
+	}
+	s2Polygon* forms = (s2Polygon*)malloc(sizeof(s2Polygon) * (size_t)(count > 0 ? count : 1));
+	int32_t i = 0;
+	for (int32_t next = b->shapeList; next != S2_NULL_INDEX; next = world->shapes[next].nextShapeIndex)
+	{
+		forms[i++] = s2Shape_PolygonForm(world->shapes + next);
+	}
+	s2ShapeExtent e = s2ComputeBodyExtent(forms, count, b->localCenter);
+	free(forms);
+	b->minExtent = e.minExtent;
+	b->maxExtent = e.maxExtent;
 }
 
 // Mass, centre of mass and inertia about it of a body from the shapes attached to it (behaviour of reference
@@ -257,6 +307,7 @@ static s2ShapeId s2CreateShape(s2BodyId bodyId, const s2ShapeDef* def, const voi
 	{
 		s2UpdateBodyMass(world, body);
 	}
+	s2UpdateBodyExtents(world, body);
 
 	s2MarkShapeDirty(world, shape);
 	s2MarkBodyDirty(world, body);

@@ -5,6 +5,7 @@
 #include "s2_host.h"
 
 #include "shared/s2_collide.h"
+#include "shared/s2_toi.h"
 
 #include <float.h>
 #include <string.h>
@@ -659,4 +660,37 @@ s2Manifold s2CollideSegmentAndPolygon(const s2Segment* segmentA, s2Transform xfA
 {
 	s2Polygon polyA = s2MakeCapsule(segmentA->point1, segmentA->point2, 0.0f);
 	return s2CollidePolygons(&polyA, xfA, polygonB, xfB, cache);
+}
+
+// ---- continuous collision (shared implementation, csrc/shared/s2_toi.h) --------------------------------------------
+
+s2Transform s2GetSweepTransform(const s2Sweep* sweep, float fraction)
+{
+	return s2cGetSweepTransform(sweep, fraction);
+}
+
+s2TOIOutput s2TimeOfImpact(const s2TOIInput* input)
+{
+	return s2cTimeOfImpact(input->proxyA.vertices, input->proxyA.count, input->proxyA.radius, &input->sweepA, input->proxyB.vertices,
+						   input->proxyB.count, input->proxyB.radius, &input->sweepB, input->maxFraction);
+}
+
+s2ShapeExtent s2ComputeShapeExtent(const s2Polygon* polygonForm, s2Vec2 localCenter)
+{
+	s2cShapeExtent e = s2cComputeShapeExtent(polygonForm->vertices, polygonForm->normals, polygonForm->count, polygonForm->radius,
+											 localCenter);
+	s2ShapeExtent out = {e.inner, e.outer, e.core};
+	return out;
+}
+
+s2ShapeExtent s2ComputeBodyExtent(const s2Polygon* polygonForms, int32_t count, s2Vec2 localCenter)
+{
+	s2ShapeExtent out = {s2_huge, 0.0f, localCenter};
+	for (int32_t i = 0; i < count; ++i)
+	{
+		s2ShapeExtent e = s2ComputeShapeExtent(polygonForms + i, localCenter);
+		out.minExtent = S2_MIN(out.minExtent, e.minExtent);
+		out.maxExtent = S2_MAX(out.maxExtent, e.maxExtent);
+	}
+	return out;
 }

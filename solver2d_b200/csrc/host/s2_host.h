@@ -111,6 +111,7 @@ typedef struct s2Body
 	float linearDamping;
 	float angularDamping;
 	float gravityScale;
+	float minExtent, maxExtent; // continuous collision: smallest inner / largest outer extent of the shapes (s2UpdateBodyExtents)
 
 	int32_t shapeList;
 	int32_t jointCount;
@@ -216,6 +217,9 @@ typedef struct s2World
 	bool enableRestitution;
 	float restitutionThreshold;
 	bool restitutionDirty;
+	// continuous collision (include/solver2d_b200.h): pushed to the device by the next flush when continuousDirty
+	bool enableContinuous;
+	bool continuousDirty;
 	bool stateFresh;	 // host body / joint state mirrors the device
 	bool boxesFresh;	 // host shape AABBs mirror the device
 	uint64_t stepId;
@@ -262,6 +266,8 @@ void s2FreeProxyId(s2ProxyIds* ids, int32_t proxyId);
 
 s2Box s2Shape_ComputeAABB(const s2Shape* shape, s2Transform xf);
 s2MassData s2Shape_ComputeMass(const s2Shape* shape);
+// the shape as the device stores it: circle = 1 vertex + radius, capsule / segment = s2MakeCapsule, polygon as is
+s2Polygon s2Shape_PolygonForm(const s2Shape* shape);
 
 // per-variant solver entry points (names and shape of reference src/solvers.h:70-79); each enqueues the variant's
 // kernel schedule on the world's device

@@ -173,6 +173,8 @@ static void s2FillBodyRow(s2bBodyRow* r, const s2Body* b)
 	r->linearDamping = b->linearDamping;
 	r->angularDamping = b->angularDamping;
 	r->gravityScale = b->gravityScale;
+	r->minExtent = b->minExtent;
+	r->maxExtent = b->maxExtent;
 }
 
 static void s2FillShapeRow(s2bShapeRow* r, const s2Shape* s)
@@ -201,25 +203,7 @@ static void s2FillShapeRow(s2bShapeRow* r, const s2Shape* s)
 	r->fatAABB[3] = s->fatAABB.upperBound.y;
 
 	// polygon form of every shape kind (see s2b_device.h)
-	s2Polygon poly;
-	switch (s->type)
-	{
-		case s2_circleShape:
-			memset(&poly, 0, sizeof(poly));
-			poly.vertices[0] = s->circle.point;
-			poly.count = 1;
-			poly.radius = s->circle.radius;
-			break;
-		case s2_capsuleShape:
-			poly = s2MakeCapsule(s->capsule.point1, s->capsule.point2, s->capsule.radius);
-			break;
-		case s2_segmentShape:
-			poly = s2MakeCapsule(s->segment.point1, s->segment.point2, 0.0f);
-			break;
-		default:
-			poly = s->polygon;
-			break;
-	}
+	s2Polygon poly = s2Shape_PolygonForm(s);
 	r->radius = poly.radius;
 	r->count = poly.count;
 	for (int i = 0; i < poly.count && i < s2_maxPolygonVertices; ++i)
@@ -386,6 +370,12 @@ void s2FlushToDevice(s2World* world)
 	{
 		s2b_set_restitution(dev, world->enableRestitution ? 1 : 0, world->restitutionThreshold);
 		world->restitutionDirty = false;
+	}
+
+	if (world->continuousDirty)
+	{
+		s2b_set_continuous(dev, world->enableContinuous ? 1 : 0);
+		world->continuousDirty = false;
 	}
 
 	if (world->jointPairsDirty)
@@ -797,6 +787,13 @@ void s2World_SetRestitutionThreshold(s2WorldId worldId, float threshold)
 	}
 	world->restitutionThreshold = threshold;
 	world->restitutionDirty = true;
+}
+
+void s2World_EnableContinuous(s2WorldId worldId, bool enable)
+{
+	s2World* world = s2GetWorldFromId(worldId);
+	world->enableContinuous = enable;
+	world->continuousDirty = true;
 }
 
 void s2World_Flush(s2WorldId worldId)

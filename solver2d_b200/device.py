@@ -18,7 +18,8 @@ BODY_ROW = np.dtype([
     ("index", "<i4"), ("flags", "<i4"), ("origin", "<f4", 2), ("position", "<f4", 2), ("rot", "<f4", 2),
     ("linearVelocity", "<f4", 2), ("angularVelocity", "<f4"), ("localCenter", "<f4", 2), ("mass", "<f4"),
     ("invMass", "<f4"), ("I", "<f4"), ("invI", "<f4"), ("force", "<f4", 2), ("torque", "<f4"),
-    ("linearDamping", "<f4"), ("angularDamping", "<f4"), ("gravityScale", "<f4"),
+    ("linearDamping", "<f4"), ("angularDamping", "<f4"), ("gravityScale", "<f4"), ("minExtent", "<f4"),
+    ("maxExtent", "<f4"),
 ], align=True)
 
 SHAPE_ROW = np.dtype([
@@ -62,7 +63,7 @@ class Counters(C.Structure):
                 ("graphReplays", C.c_int32), ("graphCaptures", C.c_int32), ("scratchBytes", C.c_int64),
                 ("regionCount", C.c_int32), ("cutCount", C.c_int32), ("cutGroupCount", C.c_int32), ("recolouredCount", C.c_int32),
                 ("neighbourSync", C.c_int32), ("narrowphaseRowSteps", C.c_int32),
-                ("firstTable", C.c_int32)]
+                ("firstTable", C.c_int32), ("continuousShapes", C.c_int32), ("continuousHits", C.c_int32)]
 
 
 SCHEDULE_COLOR, SCHEDULE_WAVEFRONT = 0, 1
@@ -86,6 +87,7 @@ ABI_SYMBOLS = [
     "s2b_flush_l2", "s2b_time_color_kernel", "s2b_version", "s2b_abi_sizes", "s2b_upload_forces", "s2b_host_alloc",
     "s2b_host_free", "s2b_sync_body_state", "s2b_set_warm_gather", "s2b_eval_atan2", "s2b_set_dataflow", "s2b_set_regions", "s2b_set_graph", "s2b_get_stream", "s2b_add_forces", "s2b_download_transforms",
     "s2b_set_restitution", "s2b_download_neighbour_blocks", "s2b_download_delta_positions", "s2b_set_motor_offsets",
+    "s2b_set_continuous",
 ]
 NSYNC_STRIDE = 17  # entries per block of s2b_download_neighbour_blocks
 
@@ -125,6 +127,7 @@ class Device:
         L.s2b_world_destroy.argtypes = [vp]
         L.s2b_set_gravity.argtypes = [vp, C.c_float, C.c_float]
         L.s2b_set_restitution.argtypes = [vp, C.c_int, C.c_float]
+        L.s2b_set_continuous.argtypes = [vp, C.c_int]
         for name in ("s2b_set_schedule", "s2b_set_max_colors", "s2b_set_persistent", "s2b_set_warm_gather", "s2b_set_dataflow", "s2b_set_regions", "s2b_set_graph"):
             getattr(L, name).argtypes = [vp, C.c_int]
         for name in ("s2b_upload_bodies", "s2b_upload_shapes", "s2b_upload_joints"):
@@ -243,6 +246,11 @@ class DeviceWorld:
         """Restitution pass at the end of the solver stage (off by default; DESIGN.md §3.7). `threshold`: approach speed
         (m/s) below which a contact does not bounce; a negative or non-finite value is ignored."""
         self.L.s2b_set_restitution(self.h, 1 if enable else 0, threshold)
+
+    def set_continuous(self, enable: bool):
+        """Continuous collision of dynamic bodies against static shapes after the solver stage (off by default;
+        DESIGN.md §3.11)."""
+        self.L.s2b_set_continuous(self.h, 1 if enable else 0)
 
     def set_warm_gather(self, enable: bool):
         self.L.s2b_set_warm_gather(self.h, 1 if enable else 0)

@@ -20,6 +20,8 @@ Each recipe restates one of the reference's sample scenes or one of the syntheti
                             (the motor joint).
 * :func:`kinematic_rigs`  — piles on sliding kinematic platforms and a turntable, joints hanging from moving kinematic
                             carriages (kinematic bodies under every solver variant).
+* :func:`projectiles`     — circles, capsules, boxes and hulls fired at 30-200 m/s at thin static boxes and segments
+                            (continuous collision).
 
 All scenes are deterministic lattices (no RNG). A recipe returns a :class:`Scene` holding the world id and the
 body ids in creation order.
@@ -1142,3 +1144,106 @@ def pyramid_field(lib: capi.Solver2D, solver="TGS_Soft", count=256, base_count=4
                 lib.s2CreatePolygonShape(bid, C.byref(sd), C.byref(box))
                 sc.bodies.append(bid)
     return sc
+
+
+PROJECTILE_SPEEDS = (30.0, 55.0, 90.0, 140.0, 200.0)  # m/s
+PROJECTILE_TILTS = (0.0, 0.3, -0.45)  # rad: wall turned away from facing the projectile head-on
+PROJECTILE_WALL_HALF_LENGTH = 2.0
+PROJECTILE_WALL_HALF_THICKNESS = 0.025  # a 0.05 m thick box
+
+
+def projectiles(lib: capi.Solver2D, solver="TGS_Soft", copies=1, excluded=True) -> Scene:
+    """Continuous-collision coverage: lanes on a grid, each a static wall (its own body: a box 0.05 m thick or a segment,
+    4 m long, tilted by one of PROJECTILE_TILTS) and a projectile without gravity fired at it along +x (a circle, capsule,
+    box or hexagon at each of PROJECTILE_SPEEDS). At 60 Hz a projectile moves 0.5-3.3 m per step, so without continuous
+    collision many pass through. With `excluded`, four more lanes whose projectile must pass: two whose filter excludes the
+    wall and two jointed to the wall's body by a prismatic joint along the flight (the joint rule creates no contact; the
+    reference has no prismatic joint and builds these lanes without it). `copies` repeats the lane set.
+
+    sc.piles["lanes"]: per lane a dict with the projectile's and the wall's body ids, the wall's centre, unit normal
+    (pointing away from the projectile's side) and half length, `passes` (the projectile is meant to pass), `exclusion`
+    ("filter", "joint" or None) and both shapes in polygon form (`form`, `wall_form`)."""
+    world = lib.create_world(solver)
+    sc = Scene(lib, world, name=f"projectiles{copies}")
+    specs = [(kind, v, wall, tilt, None) for kind in range(4) for v in PROJECTILE_SPEEDS for wall in ("box", "segment")
+             for tilt in PROJECTILE_TILTS] * copies
+    if excluded:
+        specs += [(0, 90.0, "box", 0.0, "filter"), (2, 140.0, "segment", 0.0, "filter"), (1, 90.0, "box", 0.0, "joint"),
+                  (3, 140.0, "segment", 0.0, "joint")]
+    cols = int(math.ceil(math.sqrt(len(specs))))
+    lanes = []
+    hexagon = lib.s2MakePolygon(C.byref(lib.s2ComputeHull(
+        (Vec2 * 6)(*[Vec2(0.12 * math.cos(math.pi * m / 3.0), 0.12 * math.sin(math.pi * m / 3.0)) for m in range(6)]), 6)))
+    for n, (kind, speed, wall, tilt, exclusion) in enumerate(specs):
+        i, j = divmod(n, cols)
+        cx, cy = 12.0 * j + 6.0 * (i % 2), 10.0 * i
+        bd = default_body_def()
+        bd.position = Vec2(cx, cy)
+        bd.angle = tilt
+        wid = lib.s2CreateBody(world, C.byref(bd))
+        sd = default_shape_def()
+        if exclusion == "filter":
+            sd.filter = capi.Filter(0x0002, 0xFFFFFFFF, 0)
+        if wall == "box":
+            wall_form = lib.s2MakeBox(PROJECTILE_WALL_HALF_THICKNESS, PROJECTILE_WALL_HALF_LENGTH)
+            lib.s2CreatePolygonShape(wid, C.byref(sd), C.byref(wall_form))
+        else:
+            seg = Segment(Vec2(0.0, -PROJECTILE_WALL_HALF_LENGTH), Vec2(0.0, PROJECTILE_WALL_HALF_LENGTH))
+            lib.s2CreateSegmentShape(wid, C.byref(sd), C.byref(seg))
+            wall_form = lib.s2MakeCapsule(seg.point1, seg.point2, 0.0)
+
+        pd = default_body_def()
+        pd.type = capi.DYNAMIC_BODY
+        start = Vec2(cx - 2.5 - 0.17 * (n % 5), cy)
+        pd.position = start
+        pd.gravityScale = 0.0
+        pd.linearVelocity = Vec2(speed, 0.0)
+        pd.angle = 0.3 * (n % 4)
+        pd.angularVelocity = 2.0 if n % 3 == 0 else 0.0
+        pid = lib.s2CreateBody(world, C.byref(pd))
+        ps = default_shape_def()
+        if exclusion == "filter":
+            ps.filter = capi.Filter(0x0001, 0xFFFFFFFF & ~0x0002, 0)
+        if kind == 0:
+            lib.s2CreateCircleShape(pid, C.byref(ps), C.byref(Circle(Vec2(0.0, 0.0), 0.1)))
+            form = capi.Polygon()
+            form.count, form.radius = 1, 0.1
+        elif kind == 1:
+            lib.s2CreateCapsuleShape(pid, C.byref(ps), C.byref(Capsule(Vec2(-0.15, 0.0), Vec2(0.15, 0.0), 0.05)))
+            form = lib.s2MakeCapsule(Vec2(-0.15, 0.0), Vec2(0.15, 0.0), 0.05)
+        elif kind == 2:
+            form = lib.s2MakeBox(0.1, 0.1)
+            lib.s2CreatePolygonShape(pid, C.byref(ps), C.byref(form))
+        else:
+            form = hexagon
+            lib.s2CreatePolygonShape(pid, C.byref(ps), C.byref(hexagon))
+        if exclusion == "joint" and "s2CreatePrismaticJoint" not in lib.missing:
+            jd = capi.default_prismatic_def()
+            jd.bodyIdA = wid
+            jd.bodyIdB = pid
+            jd.localAnchorA = lib.s2Body_GetLocalPoint(wid, start)
+            jd.localAnchorB = Vec2(0.0, 0.0)
+            jd.localAxisA = Vec2(math.cos(tilt), -math.sin(tilt))
+            jd.referenceAngle = pd.angle - tilt
+            sc.joints.append(lib.s2CreatePrismaticJoint(world, C.byref(jd)))
+        sc.bodies.append(pid)
+        lanes.append(dict(body=pid, wall=wid, center=(cx, cy), normal=(math.cos(tilt), math.sin(tilt)),
+                          half_length=PROJECTILE_WALL_HALF_LENGTH, passes=exclusion is not None, exclusion=exclusion,
+                          form=form, wall_form=wall_form))
+    sc.piles["lanes"] = lanes
+    return sc
+
+
+def projectiles_behind(lib: capi.Solver2D, sc: Scene) -> np.ndarray:
+    """Per lane of a :func:`projectiles` scene: True where the projectile's centre of mass is past its wall's mid-plane
+    within the wall's span, half a metre in from either end."""
+    out = []
+    for lane in sc.piles["lanes"]:
+        p = lib.s2Body_GetPosition(lane["body"])
+        dx, dy = p.x - lane["center"][0], p.y - lane["center"][1]
+        nx, ny = lane["normal"]
+        depth = dx * nx + dy * ny
+        along = -dx * ny + dy * nx
+        # (half a metre in from the ends: a projectile that slides off a tilted wall and rounds its end is not through it)
+        out.append(depth > 0.0 and abs(along) <= lane["half_length"] - 0.5)
+    return np.array(out, dtype=bool)
