@@ -33,17 +33,21 @@ S2C_FN s2Transform s2cGetSweepTransform(const s2Sweep* sweep, float t)
 }
 
 // Bound on the angular speed d(theta)/dt of the normalised lerp from q1 to q2 over t in [0, 1] (DESIGN.md §3.11):
-// 2 |sin phi| / (1 + cos phi) = 2 tan(|phi| / 2), phi the angle from q1 to q2. Unbounded for a half turn.
+// |q1 - q2|^2 / |cross(q1, q2)|, which is 2 tan(|phi| / 2) for unit rotations (phi the angle from q1 to q2) and stays an
+// upper bound for rotations a few ulp off unit length (as s2IntegrateRot leaves them). Unbounded for a half turn. (The
+// form 2 |sin phi| / (1 + cos phi) is not: at a half turn of rotations shorter than unit, 1 + cos phi is a few ulp and
+// sin phi round-off, and the bound came out near 0.)
 S2C_FN float s2cSweepAngularBound(const s2Sweep* sweep)
 {
 	float sinPhi = sweep->q1.c * sweep->q2.s - sweep->q1.s * sweep->q2.c;
 	float cosPhi = sweep->q1.c * sweep->q2.c + sweep->q1.s * sweep->q2.s;
-	float denom = 1.0f + cosPhi;
-	if (denom < FLT_EPSILON)
+	float dc = sweep->q1.c - sweep->q2.c, ds = sweep->q1.s - sweep->q2.s;
+	float chordSq = dc * dc + ds * ds;
+	if (sinPhi == 0.0f)
 	{
-		return FLT_MAX;
+		return cosPhi > 0.0f ? 0.0f : FLT_MAX;
 	}
-	return 2.0f * S2_ABS(sinPhi) / denom;
+	return S2_MIN(chordSq / S2_ABS(sinPhi), FLT_MAX);
 }
 
 // largest distance of a vertex from the body's centre of mass (vertices in the body frame)
