@@ -22,6 +22,9 @@ Each recipe restates one of the reference's sample scenes or one of the syntheti
                             carriages (kinematic bodies under every solver variant).
 * :func:`projectiles`     — circles, capsules, boxes and hulls fired at 30-200 m/s at thin static boxes and segments
                             (continuous collision).
+* :func:`hub_trays`       — trays carrying spaced riders of 1-60 shapes, and riders on the ground: hub bodies with exact
+                            contact counts (the solver's hub-body capacity limits).
+* :func:`hub_beam`        — a beam hanging N pendulums: a hub body with exact joint counts.
 
 All scenes are deterministic lattices (no RNG). A recipe returns a :class:`Scene` holding the world id and the
 body ids in creation order.
@@ -1247,3 +1250,171 @@ def projectiles_behind(lib: capi.Solver2D, sc: Scene) -> np.ndarray:
         # (half a metre in from the ends: a projectile that slides off a tilted wall and rounds its end is not through it)
         out.append(depth > 0.0 and abs(along) <= lane["half_length"] - 0.5)
     return np.array(out, dtype=bool)
+
+
+HUB_RIDER_PITCH = 0.25  # m between the shapes of one rider
+HUB_RIDER_GAP = 0.4     # m between neighbouring riders: their fat boxes (0.1 m margin) stay apart, so they never touch
+HUB_LANE_LENGTH = 150.0  # m of riders on one ground lane (on_ground)
+
+
+def hub_trays(lib: capi.Solver2D, solver="TGS_Soft", trays=(), on_ground=()) -> Scene:
+    """Hub bodies with contact counts set exactly, on static ground lanes 4 m apart (each lane its own static box, top face
+    at y = -4 * lane), so that no coordinate grows past about half the longest tray:
+
+    * one lane per entry of `trays`: a dynamic tray (a 0.5 m thick box) resting on the lane, with one spaced layer of
+      riders on top. An entry lists the riders' shape counts: a rider with k shapes is one body with k shapes in a row,
+      0.25 m apart, so it touches its tray k times and nothing else. Riders at even positions are 0.1 m circles created after
+      their tray; riders at odd positions are 0.2 m boxes created before it, so the tray is body A of some contacts and
+      body B of others. A tray's incidence list is then 1 (its lane) + the sum of its entry.
+    * then `on_ground`: one rider per entry resting on the lanes themselves (up to HUB_LANE_LENGTH per lane), each a body
+      with exactly that many incident contacts (the static lane does not count).
+
+    ``sc.piles["trays"]`` holds the trays' body ids, ``sc.piles["riders"]`` per tray the riders' ids and
+    ``sc.piles["on_ground"]`` those of `on_ground`."""
+    world = lib.create_world(solver)
+    sc = Scene(lib, world, name="hub_trays")
+    r, thick = 0.1, 0.25
+    sc.piles["trays"], sc.piles["riders"], sc.piles["on_ground"] = [], [], []
+
+    def width(k):
+        return HUB_RIDER_PITCH * (k - 1) + 2.0 * r
+
+    def lane(n, length):
+        bd = default_body_def()
+        bd.position = Vec2(0.0, -4.0 * n - 1.0)
+        gid = lib.s2CreateBody(world, C.byref(bd))
+        sd = default_shape_def()
+        lib.s2CreatePolygonShape(gid, C.byref(sd), C.byref(lib.s2MakeBox(0.5 * length + 1.0, 1.0)))
+        sc.bodies.append(gid)
+
+    def rider(x_left, y, k, box):
+        bd = default_body_def()
+        bd.type = capi.DYNAMIC_BODY
+        bd.position = Vec2(x_left + 0.5 * width(k), y + r)
+        bid = lib.s2CreateBody(world, C.byref(bd))
+        sd = default_shape_def()
+        for m in range(k):
+            cx = -0.5 * width(k) + r + HUB_RIDER_PITCH * m
+            if box:
+                poly = lib.s2MakeOffsetBox(r, r, Vec2(cx, 0.0), 0.0)
+                lib.s2CreatePolygonShape(bid, C.byref(sd), C.byref(poly))
+            else:
+                lib.s2CreateCircleShape(bid, C.byref(sd), C.byref(Circle(Vec2(cx, 0.0), r)))
+        sc.bodies.append(bid)
+        return bid
+
+    n = 0
+    for entry in trays:
+        span = sum(width(k) + HUB_RIDER_GAP for k in entry) + HUB_RIDER_GAP
+        lane(n, span)
+        y0 = -4.0 * n
+        lefts = []
+        cursor = -0.5 * span + HUB_RIDER_GAP
+        for k in entry:
+            lefts.append(cursor)
+            cursor += width(k) + HUB_RIDER_GAP
+        ids = [None] * len(entry)
+        for m in range(1, len(entry), 2):
+            ids[m] = rider(lefts[m], y0 + 2.0 * thick, entry[m], True)
+        bd = default_body_def()
+        bd.type = capi.DYNAMIC_BODY
+        bd.position = Vec2(0.0, y0 + thick)
+        tid = lib.s2CreateBody(world, C.byref(bd))
+        sd = default_shape_def()
+        sd.density = 5.0
+        lib.s2CreatePolygonShape(tid, C.byref(sd), C.byref(lib.s2MakeBox(0.5 * span, thick)))
+        sc.bodies.append(tid)
+        for m in range(0, len(entry), 2):
+            ids[m] = rider(lefts[m], y0 + 2.0 * thick, entry[m], False)
+        sc.piles["trays"].append(tid)
+        sc.piles["riders"].append(ids)
+        n += 1
+    rows, row = [], []
+    for k in on_ground:
+        if row and sum(width(j) + HUB_RIDER_GAP for j in row) + width(k) > HUB_LANE_LENGTH:
+            rows.append(row)
+            row = []
+        row.append(k)
+    if row:
+        rows.append(row)
+    for row in rows:
+        span = sum(width(k) + HUB_RIDER_GAP for k in row) + HUB_RIDER_GAP
+        lane(n, span)
+        cursor = -0.5 * span + HUB_RIDER_GAP
+        for k in row:
+            sc.piles["on_ground"].append(rider(cursor, -4.0 * n, k, False))
+            cursor += width(k) + HUB_RIDER_GAP
+        n += 1
+    return sc
+
+
+def hub_beam(lib: capi.Solver2D, solver="TGS_Soft", pendulums=8, limits_motor=False, mouse=True) -> Scene:
+    """A dynamic beam hung from a static anchor by a revolute joint at each end, with `pendulums` boxes hanging 1 m below it
+    on revolute joints, 0.5 m apart (the beam is body A of the even ones and body B of the odd ones), and with `mouse` a
+    mouse joint pulling the beam. The beam's incidence list is pendulums + 2 (+ 1); nothing touches anything. No two bobs
+    share mass, inertia and centre of mass (half sizes 0.05-0.08 m, densities 0.5-2, centres up to 0.02 m off the origin;
+    neighbours stay 0.3 m apart, so their fat boxes never overlap),
+    and the beam is created after them, so a row that reads another body's columns reads different values. With
+    `limits_motor` the pendulum joints have angle limits and a motor. ``sc.piles["pendulum"]`` holds the indices into
+    ``sc.joints`` of the pendulum joints, ``sc.piles["beam"]`` the beam's id."""
+    world = lib.create_world(solver)
+    sc = Scene(lib, world, name=f"hub_beam{pendulums}")
+    bd = default_body_def()
+    anchor = lib.s2CreateBody(world, C.byref(bd))
+    sc.bodies.append(anchor)
+    half = 0.25 * pendulums + 0.5
+    y = 10.0
+    bobs, xs = [], []
+    for n in range(pendulums):
+        px = -half + 0.5 + 0.5 * n
+        bd = default_body_def()
+        bd.type = capi.DYNAMIC_BODY
+        bd.position = Vec2(px, y - 1.0)
+        bob = lib.s2CreateBody(world, C.byref(bd))
+        sd = default_shape_def()
+        sd.density = 0.5 + 0.25 * (n % 7)
+        h = 0.05 + 0.01 * (n % 4)
+        lib.s2CreatePolygonShape(bob, C.byref(sd), C.byref(lib.s2MakeOffsetBox(h, h, Vec2(0.01 * (n % 5 - 2), 0.0), 0.0)))
+        sc.bodies.append(bob)
+        bobs.append(bob)
+        xs.append(px)
+    bd = default_body_def()
+    bd.type = capi.DYNAMIC_BODY
+    bd.position = Vec2(0.0, y)
+    beam = lib.s2CreateBody(world, C.byref(bd))
+    sd = default_shape_def()
+    lib.s2CreatePolygonShape(beam, C.byref(sd), C.byref(lib.s2MakeBox(half, 0.1)))
+    sc.bodies.append(beam)
+    sc.piles["beam"] = beam
+    for end, (a, b) in ((-1.0, (anchor, beam)), (1.0, (beam, anchor))):
+        jd = default_revolute_def()
+        pivot = Vec2(end * half, y)
+        jd.bodyIdA, jd.bodyIdB = a, b
+        jd.localAnchorA = lib.s2Body_GetLocalPoint(a, pivot)
+        jd.localAnchorB = lib.s2Body_GetLocalPoint(b, pivot)
+        sc.joints.append(lib.s2CreateRevoluteJoint(world, C.byref(jd)))
+    sc.piles["pendulum"] = []
+    for n, (bob, px) in enumerate(zip(bobs, xs)):
+        a, b = (beam, bob) if n % 2 == 0 else (bob, beam)
+        jd = default_revolute_def()
+        pivot = Vec2(px, y)
+        jd.bodyIdA, jd.bodyIdB = a, b
+        jd.localAnchorA = lib.s2Body_GetLocalPoint(a, pivot)
+        jd.localAnchorB = lib.s2Body_GetLocalPoint(b, pivot)
+        if limits_motor:
+            jd.enableLimit = True
+            jd.lowerAngle, jd.upperAngle = -0.05, 0.05
+            jd.enableMotor = True
+            jd.motorSpeed = 0.5 if n % 3 == 0 else -0.25
+            jd.maxMotorTorque = 0.5
+        sc.piles["pendulum"].append(len(sc.joints))
+        sc.joints.append(lib.s2CreateRevoluteJoint(world, C.byref(jd)))
+    if mouse:
+        md = default_mouse_def()
+        md.bodyIdA = anchor
+        md.bodyIdB = beam
+        md.target = Vec2(0.5, y + 0.25)
+        md.hertz = 4.0
+        md.dampingRatio = 0.7
+        sc.joints.append(lib.s2CreateMouseJoint(world, C.byref(md)))
+    return sc
