@@ -38,6 +38,10 @@ typedef struct s2bWorld s2bWorld;
 // body's delta position on the device (XPBD leaves a kinematic body's growing from step to step, DESIGN.md §3.8); any
 // other row starts the body at zero
 #define S2B_BODY_TELEPORT 0x10
+// body rows only: the body is a bullet (s2Body_SetBullet). While continuous collision is on (s2b_set_continuous), a fast
+// dynamic bullet is swept after finalize against static, kinematic and non-bullet dynamic shapes at their final poses
+// (DESIGN.md §3.12). No effect on static and kinematic bodies. The device keeps the bit in its flags column.
+#define S2B_BODY_BULLET 0x20
 
 // One rigid body; mirrors the solver-relevant fields of s2Body (reference src/body.h:16-76).
 typedef struct s2bBodyRow
@@ -206,6 +210,8 @@ typedef struct s2bCounters
 	int32_t firstTable;			 // blocks of the persistent kernel that warm-start colour 0 from the first-touch table (the others per thread)
 	int32_t continuousShapes;	 // shapes of fast bodies swept against static shapes in the last step (s2b_set_continuous)
 	int32_t continuousHits;		 // bodies the last step's continuous pass stopped at a time of impact
+	int32_t bulletShapes;		 // shapes of fast bullets swept in the last step's bullet pass (S2B_BODY_BULLET)
+	int32_t bulletHits;			 // bullets the last step's bullet pass stopped at a time of impact
 } s2bCounters;
 
 // ---- lifecycle ------------------------------------------------------------------------------------------------

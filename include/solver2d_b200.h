@@ -143,9 +143,18 @@ S2B_API float s2MotorJoint_GetConstraintTorque(s2JointId jointId, float inverseT
 // start of the step to its pose at the end against the static shapes its shapes may collide with, and stopped at the
 // first time of impact, s2_linearSlop short of the surface; its velocity is kept. Bodies that start the step touching a
 // static shape are held back only if a small core inside the shape would hit it, or starts touching it and moves toward
-// it (the body is then already a quarter of its inner extent deep). Not covered: dynamic against dynamic or
-// kinematic bodies (DESIGN.md §3.11). Takes effect at the next s2World_Step.
+// it (the body is then already a quarter of its inner extent deep). Dynamic against dynamic or kinematic bodies is swept
+// only for bullets (s2Body_SetBullet). Takes effect at the next s2World_Step.
 S2B_API void s2World_EnableContinuous(s2WorldId worldId, bool enable);
+
+// Bullets (DESIGN.md §3.12; default off). While continuous collision is on, a fast dynamic bullet (fast by the rule above)
+// is swept once every other body has its final pose for the step: against the shapes of static, kinematic and non-bullet
+// dynamic bodies, each held still at that final pose, under the same pair rules. It stops at the first time of impact,
+// s2_linearSlop short of the surface, and keeps its velocity, so the next step's contact does the stopping. Bullet against
+// bullet is not swept, and a target's own motion within the step is not swept either. No effect on static and kinematic
+// bodies, nor while continuous collision is off. Takes effect at the next s2World_Step.
+S2B_API void s2Body_SetBullet(s2BodyId bodyId, bool flag);
+S2B_API bool s2Body_IsBullet(s2BodyId bodyId);
 
 // Motion of a body over one step, for s2TimeOfImpact: the centre of mass moves linearly from c1 to c2 and the rotation is
 // the normalised linear interpolation of q1 and q2.

@@ -437,6 +437,9 @@ _API.update({
     "s2TimeOfImpact": (TOIOutput, [C.POINTER(TOIInput)]),
     "s2ComputeShapeExtent": (ShapeExtent, [C.POINTER(Polygon), Vec2]),
     "s2ComputeBodyExtent": (ShapeExtent, [C.POINTER(Polygon), C.c_int32, Vec2]),
+    # bullets (include/solver2d_b200.h): extensions, absent from the reference
+    "s2Body_SetBullet": (None, [BodyId, C.c_bool]),
+    "s2Body_IsBullet": (C.c_bool, [BodyId]),
 })
 
 QUERY_CALLBACK = C.CFUNCTYPE(C.c_bool, ShapeId, C.c_void_p)

@@ -22,20 +22,24 @@
 
 #include <algorithm>
 
-// continuous collision (s2bContinuousSnapshot / s2bContinuousPass); the columns exist only while the feature is on
+// continuous collision (s2bContinuousSnapshot / s2bContinuousPass / s2bBulletPass); the columns exist only while the
+// feature is on
 struct ContinuousScratch
 {
 	DevArray<float4> start;		  // per body: centre of mass and rotation before the solver stage (c.x c.y q.s q.c)
 	DevArray<unsigned> fraction;  // per body: float bits of the earliest time of impact (1.0f: none)
-	DevArray<int> shapes;		  // shapes of the fast bodies of this step
-	DevArray<int> counters;		  // [0] shapes listed, [1] bodies clamped
+	DevArray<int> shapes;		  // shapes of the fast non-bullet bodies of this step
+	DevArray<int> bulletShapes;	  // shapes of the fast bullets of this step
+	DevArray<int> counters;		  // [0] shapes listed, [1] bodies clamped, [2] bullet shapes listed, [3] bullets clamped
 	bool ran = false;			  // the last s2b_solve ran the pass (the counters are its)
+	bool bulletRan = false;		  // the last finalize ran the bullet pass
 
 	void release()
 	{
 		start.release();
 		fraction.release();
 		shapes.release();
+		bulletShapes.release();
 		counters.release();
 	}
 };
@@ -1404,7 +1408,6 @@ void s2bBroadphaseUpdatePairs(s2bWorld* w)
 // continuous collision: dynamic bodies against static shapes (DESIGN.md §3.11)
 // ---------------------------------------------------------------------------------------------------------------
 
-#define S2B_FRACTION_ONE 0x3F800000u // bits of 1.0f
 #define S2B_SWEEP_BLOCK 128
 
 // before the solver stage: each dynamic body's centre and rotation, and no time of impact yet
@@ -1450,7 +1453,7 @@ __device__ __forceinline__ bool s2bIsFast(const s2Sweep& sweep, float2 ext)
 	return moved > 0.5f * ext.x;
 }
 
-// the shapes of fast bodies, compacted (one atomic per block)
+// the shapes of fast bodies, compacted (one atomic per block); bullets are left to the bullet pass
 __global__ void s2bContinuousCollect(ShapeView s, BodyView b, const float2* ext, const float4* start, int* list, int* counters)
 {
 	int i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -1462,7 +1465,7 @@ __global__ void s2bContinuousCollect(ShapeView s, BodyView b, const float2* ext,
 		{
 			int body = head.y;
 			unsigned f = b.flags[body];
-			if (S2B_BODY_TYPE(f) == S2B_BODY_DYNAMIC)
+			if (S2B_BODY_TYPE(f) == S2B_BODY_DYNAMIC && (f & S2B_BODY_BULLET) == 0)
 			{
 				fast = s2bIsFast(s2bBodySweep(b, start, body), ext[body]);
 			}
@@ -1528,9 +1531,19 @@ __device__ __forceinline__ float s2bStaticImpact(const ShapeView& s, const BodyV
 	return out.state == s2_toiStateHit || out.state == s2_toiStateFailed ? out.fraction : 1.0f;
 }
 
+// which leaves a sweep takes as candidates
+enum
+{
+	S2B_SWEEP_STATIC = 0, // the non-bullet pass: shapes of static bodies
+	S2B_SWEEP_BULLET = 1, // the bullet pass: shapes of other bodies that are static, kinematic, or dynamic and not bullets
+};
+
 // One thread per listed shape: the box it sweeps over the step, a walk of the wide hierarchy with it, the broad phase's pair
-// rules on every static leaf it overlaps, a time of impact against each survivor, and the earliest one to the body (an
-// atomic min on the bits: fractions are non-negative, so their bits order like the floats, whatever the thread order).
+// rules on every candidate leaf it overlaps, a time of impact against each survivor (held still at its current pose), and
+// the earliest one to the body (an atomic min on the bits: fractions are non-negative, so their bits order like the floats,
+// whatever the thread order). Both passes launch this kernel; they differ only in the candidate rule, fixed at compile time:
+// s2bContinuousSweep<S2B_SWEEP_STATIC> and s2bContinuousSweep<S2B_SWEEP_BULLET>.
+template <int mode>
 __global__ void __launch_bounds__(S2B_SWEEP_BLOCK) s2bContinuousSweep(ShapeView s, BodyView b, const float4* start, const int* list,
 																		const int* counters, const int* treeCounters, const float4* wideBox,
 																		const int* wideChild, const unsigned long long* jointKeys,
@@ -1611,10 +1624,22 @@ __global__ void __launch_bounds__(S2B_SWEEP_BLOCK) s2bContinuousSweep(ShapeView 
 			int other = ~c;
 			int4 headO = s.head[other];
 			int bodyO = headO.y;
-			// static shapes only, under the broad phase's own rules: filter, joint override, a manifold for the pair
-			if ((headO.x & S2B_ROW_VALID) == 0 || S2B_BODY_TYPE((unsigned)b.flags[bodyO]) != S2B_BODY_STATIC)
+			// the mode's candidates, under the broad phase's own rules: filter, joint override, a manifold for the pair
+			if (mode == S2B_SWEEP_STATIC)
 			{
-				continue;
+				if ((headO.x & S2B_ROW_VALID) == 0 || S2B_BODY_TYPE((unsigned)b.flags[bodyO]) != S2B_BODY_STATIC)
+				{
+					continue;
+				}
+			}
+			else
+			{
+				unsigned fO = b.flags[bodyO];
+				if ((headO.x & S2B_ROW_VALID) == 0 || bodyO == body ||
+					(S2B_BODY_TYPE(fO) == S2B_BODY_DYNAMIC && (fO & S2B_BODY_BULLET) != 0))
+				{
+					continue;
+				}
 			}
 			if (s2bShouldShapesCollide(filter, s.filter[other]) == false || s2bJointOverride(jointKeys, jointKeyCount, body, bodyO) ||
 				s2bPairKind(type, (headO.x >> 1) & 0x7) == 0)
@@ -1649,6 +1674,88 @@ __global__ void s2bContinuousClamp(BodyView b, const float4* start, const unsign
 	atomicAdd(counters + 1, 1);
 }
 
+// ---------------------------------------------------------------------------------------------------------------
+// bullets: fast dynamic bullets against every other non-bullet shape at its final pose, after finalize (DESIGN.md §3.12)
+// ---------------------------------------------------------------------------------------------------------------
+
+// the shapes of fast bullets, compacted like s2bContinuousCollect's
+__global__ void s2bBulletCollect(ShapeView s, BodyView b, const float2* ext, const float4* start, int* list, int* counters)
+{
+	int i = blockIdx.x * blockDim.x + threadIdx.x;
+	bool fast = false;
+	if (i < s.capacity)
+	{
+		int4 head = s.head[i];
+		if (head.x & S2B_ROW_VALID)
+		{
+			int body = head.y;
+			unsigned f = b.flags[body];
+			if (S2B_BODY_TYPE(f) == S2B_BODY_DYNAMIC && (f & S2B_BODY_BULLET) != 0)
+			{
+				fast = s2bIsFast(s2bBodySweep(b, start, body), ext[body]);
+			}
+		}
+	}
+	s2bBlockAppend(fast, i, list, counters + 2);
+}
+
+// a bullet with a time of impact takes the sweep's pose at it (its velocity stays) and the origin finalize derives for that
+// pose; the bodies the non-bullet pass clamped are not bullets and were finalized as they are
+__global__ void s2bBulletClamp(BodyView b, const float4* start, const unsigned* fraction, int* counters)
+{
+	int i = blockIdx.x * blockDim.x + threadIdx.x;
+	if (i >= b.capacity || fraction[i] >= S2B_FRACTION_ONE || (b.flags[i] & S2B_BODY_BULLET) == 0)
+	{
+		return;
+	}
+	s2Sweep sweep = s2bBodySweep(b, start, i);
+	s2Vec2 c;
+	s2Rot q;
+	s2cSweepPose(&sweep, __uint_as_float(fraction[i]), &c, &q);
+	float4 pos = b.pos[i], pose = b.pose[i], org = b.org[i];
+	b.pos[i] = make_float4(c.x, c.y, pos.z, pos.w);
+	b.pose[i] = make_float4(pose.x, pose.y, q.s, q.c);
+	// origin = position - R * localCenter, as s2bFinalizeBodies
+	s2Vec2 lc = {org.z, org.w};
+	s2Vec2 o = s2Sub(c, s2RotateVector(q, lc));
+	b.org[i] = make_float4(o.x, o.y, org.z, org.w);
+	atomicAdd(counters + 3, 1);
+}
+
+// Inside finalize, after its kernels. The hierarchy holds the fat boxes of this step's pair pass, and dynamic shapes have
+// moved since: it is refitted (same topology, every box from the fat column, which now holds each non-static shape's final
+// box) before the bullets are swept. The refit leaves the hierarchy as the next search's own refit would, and is not
+// counted toward the rebuild cadence (S2B_TREE_REUSE_LIMIT).
+void s2bBulletPass(s2bWorld* w)
+{
+	S2bEpochFreeze freeze;
+	BroadScratch* B = w->broad;
+	if (B == nullptr)
+	{
+		return;
+	}
+	ContinuousScratch& C = B->cont;
+	C.bulletRan = false;
+	if (C.ran == false)
+	{
+		return;
+	}
+	cudaStream_t st = w->stream;
+	ShapeView sv = shapeView(w);
+	BodyView bv = bodyView(w);
+	// (the non-bullet pass just made sure the hierarchy holds every live shape: C.ran)
+	S2B_LAUNCH(w, s2bRefit, gridFor(w->shapeCap, 256), 256, 0, sv, B->leafShape.p, B->leafOut.p, B->counters.p, B->wideCount.p,
+			   B->wideSlot.p, B->wideBox.p, B->visit.p, B->rootBox.p);
+	C.bulletShapes.reserve((size_t)w->shapeCap, st, false, false);
+	S2B_CHECK(cudaMemsetAsync(C.counters.p + 2, 0, sizeof(int) * 2, st));
+	S2B_LAUNCH(w, s2bBulletCollect, gridFor(w->shapeCap, 256), 256, 0, sv, bv, w->bExt.p, C.start.p, C.bulletShapes.p, C.counters.p);
+	S2B_LAUNCH(w, s2bContinuousSweep<S2B_SWEEP_BULLET>, gridFor(w->shapeCap, S2B_SWEEP_BLOCK), S2B_SWEEP_BLOCK, 0, sv, bv, C.start.p,
+			   C.bulletShapes.p, C.counters.p + 2, B->counters.p, B->wideBox.p, B->wideChild.p, w->jointPairKeys.p, w->jointPairCount, C.fraction.p);
+	S2B_LAUNCH(w, s2bBulletClamp, gridFor(w->bodyCap, 256), 256, 0, bv, C.start.p, C.fraction.p, C.counters.p);
+	s2bRefinalizeBulletShapes(w, C.bulletShapes.p, C.counters.p + 2, C.fraction.p);
+	C.bulletRan = true;
+}
+
 void s2bContinuousSnapshot(s2bWorld* w)
 {
 	S2bEpochFreeze freeze; // none of these columns is part of the solver stage's graph
@@ -1661,7 +1768,7 @@ void s2bContinuousSnapshot(s2bWorld* w)
 	}
 	C.start.reserve((size_t)w->bodyCap, st, false, false);
 	C.fraction.reserve((size_t)w->bodyCap, st, false, false);
-	C.counters.reserve(2, st, false);
+	C.counters.reserve(4, st, false);
 	S2B_LAUNCH(w, s2bContinuousStart, gridFor(w->bodyCap, 256), 256, 0, bodyView(w), C.start.p, C.fraction.p, C.counters.p);
 }
 
@@ -1678,6 +1785,7 @@ void s2bContinuousPass(s2bWorld* w)
 		if (w->broad != nullptr)
 		{
 			w->broad->cont.ran = false;
+			w->broad->cont.bulletRan = false;
 		}
 		return;
 	}
@@ -1685,6 +1793,7 @@ void s2bContinuousPass(s2bWorld* w)
 	ContinuousScratch& C = B->cont;
 	cudaStream_t st = w->stream;
 	C.ran = false;
+	C.bulletRan = false;
 	if (w->bodyCap == 0 || w->shapeCap == 0 || C.start.p == nullptr)
 	{
 		return;
@@ -1702,17 +1811,18 @@ void s2bContinuousPass(s2bWorld* w)
 	ShapeView sv = shapeView(w);
 	BodyView bv = bodyView(w);
 	S2B_LAUNCH(w, s2bContinuousCollect, gridFor(w->shapeCap, 256), 256, 0, sv, bv, w->bExt.p, C.start.p, C.shapes.p, C.counters.p);
-	S2B_LAUNCH(w, s2bContinuousSweep, gridFor(w->shapeCap, S2B_SWEEP_BLOCK), S2B_SWEEP_BLOCK, 0, sv, bv, C.start.p, C.shapes.p,
-			   C.counters.p, B->counters.p, B->wideBox.p, B->wideChild.p, w->jointPairKeys.p, w->jointPairCount, C.fraction.p);
+	S2B_LAUNCH(w, s2bContinuousSweep<S2B_SWEEP_STATIC>, gridFor(w->shapeCap, S2B_SWEEP_BLOCK), S2B_SWEEP_BLOCK, 0, sv, bv, C.start.p,
+			   C.shapes.p, C.counters.p, B->counters.p, B->wideBox.p, B->wideChild.p, w->jointPairKeys.p, w->jointPairCount, C.fraction.p);
 	S2B_LAUNCH(w, s2bContinuousClamp, gridFor(w->bodyCap, 256), 256, 0, bv, C.start.p, C.fraction.p, C.counters.p);
 	C.ran = true;
 }
 
-void s2bContinuousCounters(s2bWorld* w, int out[2])
+void s2bContinuousCounters(s2bWorld* w, int out[4])
 {
-	out[0] = out[1] = 0;
+	out[0] = out[1] = out[2] = out[3] = 0;
 	if (w->broad != nullptr && w->broad->cont.ran)
 	{
-		S2B_CHECK(cudaMemcpy(out, w->broad->cont.counters.p, sizeof(int) * 2, cudaMemcpyDeviceToHost));
+		S2B_CHECK(cudaMemcpy(out, w->broad->cont.counters.p, sizeof(int) * (w->broad->cont.bulletRan ? 4 : 2),
+							 cudaMemcpyDeviceToHost));
 	}
 }

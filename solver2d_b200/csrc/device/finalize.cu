@@ -33,24 +33,13 @@ __global__ void s2bFinalizeBodies(BodyView b)
 // All four shape kinds are stored in polygon form (count vertices + radius), for which the per-kind AABB functions of
 // the reference (src/geometry.c:288-341) reduce to the same float operations: min/max over the transformed
 // vertices, then -/+ radius.
-__global__ void s2bFinalizeShapes(ShapeView s, BodyView b, int* movedCounter)
+//
+// Once finalize has run, the bullet pass (DESIGN.md §3.12) redoes a clamped bullet's shapes with `again`: a shape that is
+// already flagged MOVED is not counted a second time.
+template <bool again> __device__ __forceinline__ void s2bFinalizeShape(const ShapeView& s, const BodyView& b, int i, int4 head,
+																		 int* movedCounter)
 {
-	int i = blockIdx.x * blockDim.x + threadIdx.x;
-	if (i >= s.capacity)
-	{
-		return;
-	}
-	int4 head = s.head[i];
-	if ((head.x & S2B_ROW_VALID) == 0)
-	{
-		return;
-	}
 	int body = head.y;
-	unsigned f = b.flags[body];
-	if (S2B_BODY_TYPE(f) == S2B_BODY_STATIC)
-	{
-		return;
-	}
 	float4 org = b.org[body];
 	float4 pose = b.pose[body];
 	s2Transform xf;
@@ -97,8 +86,56 @@ __global__ void s2bFinalizeShapes(ShapeView s, BodyView b, int* movedCounter)
 		s.fat[i] = make_float4(aabb.lowerBound.x - s2_aabbMargin, aabb.lowerBound.y - s2_aabbMargin,
 							   aabb.upperBound.x + s2_aabbMargin, aabb.upperBound.y + s2_aabbMargin);
 		s.head[i] = make_int4(head.x | S2B_SHAPE_MOVED, head.y, head.z, head.w);
-		atomicAdd(movedCounter, 1);
+		if (again == false || (head.x & S2B_SHAPE_MOVED) == 0)
+		{
+			atomicAdd(movedCounter, 1);
+		}
 	}
+}
+
+__global__ void s2bFinalizeShapes(ShapeView s, BodyView b, int* movedCounter)
+{
+	int i = blockIdx.x * blockDim.x + threadIdx.x;
+	if (i >= s.capacity)
+	{
+		return;
+	}
+	int4 head = s.head[i];
+	if ((head.x & S2B_ROW_VALID) == 0)
+	{
+		return;
+	}
+	unsigned f = b.flags[head.y];
+	if (S2B_BODY_TYPE(f) == S2B_BODY_STATIC)
+	{
+		return;
+	}
+	s2bFinalizeShape<false>(s, b, i, head, movedCounter);
+}
+
+// The listed shapes (list[0, count[0])) of the bodies the bullet pass clamped (fraction below 1): boxes and fat-box moves
+// for the clamped pose, as finalize derives them.
+__global__ void s2bRefinalizeShapes(ShapeView s, BodyView b, const int* list, const int* count, const unsigned* fraction,
+									int* movedCounter)
+{
+	int k = blockIdx.x * blockDim.x + threadIdx.x;
+	if (k >= count[0])
+	{
+		return;
+	}
+	int i = list[k];
+	int4 head = s.head[i];
+	if (fraction[head.y] >= S2B_FRACTION_ONE) // (not clamped)
+	{
+		return;
+	}
+	s2bFinalizeShape<true>(s, b, i, head, movedCounter);
+}
+
+void s2bRefinalizeBulletShapes(s2bWorld* w, const int* list, const int* count, const unsigned* fraction)
+{
+	S2B_LAUNCH(w, s2bRefinalizeShapes, gridFor(w->shapeCap, 256), 256, 0, shapeView(w), bodyView(w), list, count, fraction,
+			   w->dMovedFlag.p);
 }
 
 void s2bFinalize(s2bWorld* w)
@@ -112,6 +149,12 @@ void s2bFinalize(s2bWorld* w)
 	if (w->shapeCap > 0)
 	{
 		S2B_LAUNCH(w, s2bFinalizeShapes, gridFor(w->shapeCap, 256), 256, 0, shapeView(w), bodyView(w), w->dMovedFlag.p);
+	}
+	// bullets are swept once every other body is final, and their boxes and moves redone where they were clamped: all of it
+	// before the moved counter is copied, so that the transform read-back and the pair search behind it see the clamped poses
+	if (w->continuous != 0 && w->bulletCount > 0)
+	{
+		s2bBulletPass(w);
 	}
 	// publish the moved-proxy counter to the pinned mailbox; the next step reads it after this step has drained. The copy
 	// runs on the side stream, behind finalize only: on the world's stream the device-to-host copy (and the counter memset

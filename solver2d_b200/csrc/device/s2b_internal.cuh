@@ -345,6 +345,10 @@ struct s2bWorld
 	DevArray<float4> bVel, bPose, bPos, bOrg, bFrc, bPrm, bAux0, bAux1;
 	DevArray<uint8_t> bFlags;
 	DevArray<float2> bExt; // minExtent maxExtent (continuous collision; kept out of BodyView, which the solver kernels take)
+	// per body slot: the last uploaded row was valid, dynamic and a bullet (S2B_BODY_BULLET); the bullet pass runs only while
+	// bulletCount > 0, so a world without bullets launches nothing for it
+	std::vector<uint8_t> bulletSlot;
+	int bulletCount = 0;
 
 	// shapes
 	int shapeCap = 0;
@@ -520,6 +524,13 @@ void s2bFinalize(s2bWorld* w);
 void s2bFreeSolverScratch(s2bWorld* w);
 void s2bFreeBroadScratch(s2bWorld* w);
 // continuous collision (broadphase.cu, DESIGN.md §3.11): the start poses before the solver stage, the sweep and clamp after it
+// the bits of 1.0f: a per-body time of impact of "none" (a fraction is non-negative, so its bits order like the float)
+#define S2B_FRACTION_ONE 0x3F800000u
 void s2bContinuousSnapshot(s2bWorld* w);
 void s2bContinuousPass(s2bWorld* w);
-void s2bContinuousCounters(s2bWorld* w, int out[2]);
+// the bullet pass (broadphase.cu, DESIGN.md §3.12): inside finalize, after its kernels and before the moved counter's copy
+void s2bBulletPass(s2bWorld* w);
+// (finalize.cu) boxes and fat-box moves of the listed shapes whose body has a fraction below 1, for its clamped pose
+void s2bRefinalizeBulletShapes(s2bWorld* w, const int* list, const int* count, const unsigned* fraction);
+// [0] continuousShapes [1] continuousHits [2] bulletShapes [3] bulletHits of the last step
+void s2bContinuousCounters(s2bWorld* w, int out[4]);

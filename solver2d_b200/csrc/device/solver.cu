@@ -4168,10 +4168,12 @@ extern "C" void s2b_get_counters(s2bWorld* w, s2bCounters* out)
 	{
 		S2B_CHECK(cudaMemcpy(&out->narrowphaseRowSteps, w->schedDirty.p + S2B_SCHED_ROW_STEPS, sizeof(int), cudaMemcpyDeviceToHost));
 	}
-	int continuous[2];
+	int continuous[4];
 	s2bContinuousCounters(w, continuous);
 	out->continuousShapes = continuous[0];
 	out->continuousHits = continuous[1];
+	out->bulletShapes = continuous[2];
+	out->bulletHits = continuous[3];
 }
 
 extern "C" void s2b_set_solve_trace(s2bWorld* w, int capacity)

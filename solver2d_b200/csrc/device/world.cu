@@ -46,7 +46,7 @@ __global__ void s2bScatterBodies(const s2bBodyRow* __restrict__ rows, int count,
 		b.frc[i] = make_float4(r.force[0], r.force[1], r.torque, r.mass);
 	}
 	b.prm[i] = make_float4(r.linearDamping, r.angularDamping, r.gravityScale, r.invI);
-	b.flags[i] = (uint8_t)(r.flags & 0x7);
+	b.flags[i] = (uint8_t)(r.flags & (0x7 | S2B_BODY_BULLET));
 	ext[i] = make_float2(r.minExtent, r.maxExtent);
 }
 
@@ -678,6 +678,19 @@ extern "C" void s2b_upload_bodies(s2bWorld* w, const s2bBodyRow* rows, int count
 		return;
 	}
 	w->uploadEpoch += 1; // rows changed: a pair search started behind the previous step is stale now
+	// bullets per slot, so that a world without one adds no launch to its steps (s2bFinalize)
+	if (w->bulletSlot.size() < (size_t)w->bodyCap)
+	{
+		w->bulletSlot.resize((size_t)w->bodyCap, 0);
+	}
+	for (int t = 0; t < count; ++t)
+	{
+		int32_t f = rows[t].flags;
+		uint8_t bullet = (f & S2B_ROW_VALID) != 0 && ((f >> 1) & 0x3) == (int32_t)S2B_BODY_DYNAMIC && (f & S2B_BODY_BULLET) != 0;
+		uint8_t& slot = w->bulletSlot[(size_t)rows[t].index];
+		w->bulletCount += (int)bullet - (int)slot;
+		slot = bullet;
+	}
 	s2bBodyRow* d = (s2bBodyRow*)stageRows(w, rows, sizeof(s2bBodyRow) * (size_t)count);
 	S2B_LAUNCH(w, s2bScatterBodies, gridFor(count, 128), 128, 0, d, count, bodyView(w), w->bExt.p, w->schedDirty.p);
 	S2B_CHECK(cudaFreeAsync(d, w->stream));

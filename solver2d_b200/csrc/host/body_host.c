@@ -43,6 +43,7 @@ s2BodyId s2CreateBody(s2WorldId worldId, const s2BodyDef* def)
 	slot->mass = slot->invMass = slot->I = slot->invI = 0.0f;
 	slot->minExtent = s2_huge;
 	slot->maxExtent = 0.0f;
+	slot->isBullet = false;
 	slot->shapeList = S2_NULL_INDEX;
 	slot->jointCount = 0;
 	// device mirror: not there yet (rowDirty / forceDirty keep their value — a reused slot may already sit in the dirty list)
@@ -79,6 +80,7 @@ void s2DestroyBody(s2BodyId bodyId)
 	}
 	s2FreeObject(&world->bodyPool, &body->object);
 	body->onDevice = false;
+	body->isBullet = false;
 	s2MarkBodyDirty(world, body);
 }
 
@@ -443,6 +445,27 @@ void s2Body_ApplyLinearImpulse(s2BodyId bodyId, s2Vec2 impulse, s2Vec2 point)
 	body->linearVelocity = s2MulAdd(body->linearVelocity, body->invMass, impulse);
 	body->angularVelocity += body->invI * s2Cross(s2Sub(point, body->position), impulse);
 	s2MarkBodyDirty(world, body);
+}
+
+// Bullets (DESIGN.md §3.12): the flag travels in the body row; the device sweeps a fast dynamic bullet against non-bullet
+// shapes while continuous collision is on. The whole row is re-uploaded, so the host copy of the state is made current first.
+void s2Body_SetBullet(s2BodyId bodyId, bool flag)
+{
+	s2World* world = s2GetWorldFromIndex(bodyId.world);
+	s2Body* body = s2GetBody(world, bodyId);
+	if (body->isBullet == flag)
+	{
+		return;
+	}
+	s2SyncStateToHost(world);
+	body->isBullet = flag;
+	s2MarkBodyDirty(world, body);
+}
+
+bool s2Body_IsBullet(s2BodyId bodyId)
+{
+	s2World* world = s2GetWorldFromIndex(bodyId.world);
+	return s2GetBody(world, bodyId)->isBullet;
 }
 
 s2BodyType s2Body_GetType(s2BodyId bodyId)

@@ -112,6 +112,7 @@ typedef struct s2Body
 	float angularDamping;
 	float gravityScale;
 	float minExtent, maxExtent; // continuous collision: smallest inner / largest outer extent of the shapes (s2UpdateBodyExtents)
+	bool isBullet;				// s2Body_SetBullet: the row carries S2B_BODY_BULLET
 
 	int32_t shapeList;
 	int32_t jointCount;

@@ -151,7 +151,7 @@ static void s2FillBodyRow(s2bBodyRow* r, const s2Body* b)
 {
 	r->index = b->object.index;
 	r->flags = s2IsFree(&b->object) ? 0 : (S2B_ROW_VALID | ((int32_t)b->type << 1) | (b->onDevice ? S2B_BODY_ADD_FORCE : 0) |
-											 (b->teleported ? S2B_BODY_TELEPORT : 0));
+											 (b->teleported ? S2B_BODY_TELEPORT : 0) | (b->isBullet ? S2B_BODY_BULLET : 0));
 	r->origin[0] = b->origin.x;
 	r->origin[1] = b->origin.y;
 	r->position[0] = b->position.x;

@@ -1252,6 +1252,134 @@ def projectiles_behind(lib: capi.Solver2D, sc: Scene) -> np.ndarray:
     return np.array(out, dtype=bool)
 
 
+BULLET_TARGETS = ("plank", "kinematic", "block")
+BULLET_PLANK_HALF_LENGTH = 2.0
+BULLET_PLANK_HALF_THICKNESS = 0.025  # a 0.05 m thick plank
+BULLET_PLANK_DENSITY = 2000.0        # 400 kg: a projectile (at most 0.15 kg) stopped at it moves it by mm/s
+BULLET_KINEMATIC_SPEED = 0.5         # m/s along the kinematic plank's own length
+BULLET_BLOCK_HALF = 0.15             # boxes of the block: 0.3 m, 3 deep and 5 high, touching
+BULLET_BLOCK_DENSITY = 2000.0
+BULLET_LANE_PITCH = 6.0              # m between lanes: each lane has a row of its own, free past its target
+
+
+def bullets(lib: capi.Solver2D, solver="TGS_Soft", copies=1, flagged=True, excluded=True) -> Scene:
+    """Bullet coverage (s2Body_SetBullet, DESIGN.md §3.12): lanes stacked along y, each a projectile without gravity fired
+    along +x (a circle, capsule, box or hexagon at each of PROJECTILE_SPEEDS) at a non-static target, in the manner of
+    :func:`projectiles`. Targets (BULLET_TARGETS): a heavy dynamic plank 0.05 m thick without gravity; a kinematic plank of
+    the same shape sliding slowly along its own length; a small block of heavy boxes without gravity (3 deep, 5 high), the
+    projectile aimed at its middle row. With `flagged` every projectile is a bullet. With `excluded`, three more lanes
+    whose projectile must pass its plank in both modes: the plank is itself a bullet (bullet against bullet is not swept), a filter excludes
+    the plank, or the projectile is jointed to the plank by a prismatic joint along the flight (the reference has no
+    prismatic joint and builds that lane without it). `copies` repeats the lane set.
+
+    sc.piles["lanes"]: per lane a dict with the projectile's body and shape ids (`body`, `shape`), its target's body id
+    (`target`; the back middle box of a block), every (body id, shape id) of the target (`targets`), `kind` (one of
+    BULLET_TARGETS), `passes`, `exclusion` ("bullet", "filter", "joint" or None),
+    `span` (half the extent of the target face that counts, in the target's frame) and the shapes in polygon form (`form`,
+    `target_form`)."""
+    world = lib.create_world(solver)
+    sc = Scene(lib, world, name=f"bullets{copies}")
+    specs = [(kind, v, target, None) for target in BULLET_TARGETS for kind in range(4) for v in PROJECTILE_SPEEDS] * copies
+    if excluded:
+        specs += [(0, 140.0, "plank", "bullet"), (2, 140.0, "plank", "filter"), (1, 140.0, "plank", "joint")]
+    hexagon = lib.s2MakePolygon(C.byref(lib.s2ComputeHull(
+        (Vec2 * 6)(*[Vec2(0.12 * math.cos(math.pi * m / 3.0), 0.12 * math.sin(math.pi * m / 3.0)) for m in range(6)]), 6)))
+    lanes = []
+    for n, (kind, speed, target, exclusion) in enumerate(specs):
+        cy = BULLET_LANE_PITCH * n
+        tilt = 0.2 if n % 2 else 0.0
+        sd = default_shape_def()
+        if exclusion == "filter":
+            sd.filter = capi.Filter(0x0002, 0xFFFFFFFF, 0)
+        td = default_body_def()
+        td.gravityScale = 0.0
+        if target == "block":
+            td.type = capi.DYNAMIC_BODY
+            sd.density = BULLET_BLOCK_DENSITY
+            target_form = lib.s2MakeBox(BULLET_BLOCK_HALF, BULLET_BLOCK_HALF)
+            tid, targets = None, []
+            for col in range(3):
+                for row in range(-2, 3):
+                    td.position = Vec2(2.0 * BULLET_BLOCK_HALF * col, cy + 2.0 * BULLET_BLOCK_HALF * row)
+                    bid = lib.s2CreateBody(world, C.byref(td))
+                    targets.append((bid, lib.s2CreatePolygonShape(bid, C.byref(sd), C.byref(target_form))))
+                    sc.bodies.append(bid)
+                    if col == 2 and row == 0:
+                        tid = bid  # (the back middle box: a projectile past it went through the whole block)
+            span = BULLET_BLOCK_HALF
+        else:
+            td.position = Vec2(0.0, cy)
+            td.angle = tilt
+            if target == "plank":
+                td.type = capi.DYNAMIC_BODY
+                sd.density = BULLET_PLANK_DENSITY
+            else:
+                td.type = capi.KINEMATIC_BODY
+                td.linearVelocity = Vec2(-math.sin(tilt) * BULLET_KINEMATIC_SPEED, math.cos(tilt) * BULLET_KINEMATIC_SPEED)
+            tid = lib.s2CreateBody(world, C.byref(td))
+            target_form = lib.s2MakeBox(BULLET_PLANK_HALF_THICKNESS, BULLET_PLANK_HALF_LENGTH)
+            targets = [(tid, lib.s2CreatePolygonShape(tid, C.byref(sd), C.byref(target_form)))]
+            sc.bodies.append(tid)
+            # (half a metre in from the ends: a projectile that slides off a tilted plank and rounds its end is not through it)
+            span = BULLET_PLANK_HALF_LENGTH - 0.5
+        if exclusion == "bullet" and "s2Body_SetBullet" not in lib.missing:
+            lib.s2Body_SetBullet(tid, True)
+
+        pd = default_body_def()
+        pd.type = capi.DYNAMIC_BODY
+        # far enough from the target that no step starts with the two within contact reach: 1.2 m, or more for slow shots
+        start = Vec2(-1.2 - 0.17 * (n % 5), cy)
+        pd.position = start
+        pd.gravityScale = 0.0
+        pd.linearVelocity = Vec2(speed, 0.0)
+        pd.angle = 0.3 * (n % 4)
+        pd.angularVelocity = 2.0 if n % 3 == 0 else 0.0
+        pid = lib.s2CreateBody(world, C.byref(pd))
+        ps = default_shape_def()
+        if exclusion == "filter":
+            ps.filter = capi.Filter(0x0001, 0xFFFFFFFF & ~0x0002, 0)
+        if kind == 0:
+            shape = lib.s2CreateCircleShape(pid, C.byref(ps), C.byref(Circle(Vec2(0.0, 0.0), 0.1)))
+            form = capi.Polygon()
+            form.count, form.radius = 1, 0.1
+        elif kind == 1:
+            shape = lib.s2CreateCapsuleShape(pid, C.byref(ps), C.byref(Capsule(Vec2(-0.15, 0.0), Vec2(0.15, 0.0), 0.05)))
+            form = lib.s2MakeCapsule(Vec2(-0.15, 0.0), Vec2(0.15, 0.0), 0.05)
+        elif kind == 2:
+            form = lib.s2MakeBox(0.1, 0.1)
+            shape = lib.s2CreatePolygonShape(pid, C.byref(ps), C.byref(form))
+        else:
+            form = hexagon
+            shape = lib.s2CreatePolygonShape(pid, C.byref(ps), C.byref(hexagon))
+        if flagged and "s2Body_SetBullet" not in lib.missing:
+            lib.s2Body_SetBullet(pid, True)
+        if exclusion == "joint" and "s2CreatePrismaticJoint" not in lib.missing:
+            jd = capi.default_prismatic_def()
+            jd.bodyIdA = tid
+            jd.bodyIdB = pid
+            jd.localAnchorA = lib.s2Body_GetLocalPoint(tid, start)
+            jd.localAnchorB = Vec2(0.0, 0.0)
+            jd.localAxisA = Vec2(math.cos(tilt), -math.sin(tilt))
+            jd.referenceAngle = pd.angle - tilt
+            sc.joints.append(lib.s2CreatePrismaticJoint(world, C.byref(jd)))
+        sc.bodies.append(pid)
+        lanes.append(dict(body=pid, shape=shape, target=tid, targets=targets, kind=target, passes=exclusion is not None,
+                          exclusion=exclusion, span=span, form=form, target_form=target_form))
+    sc.piles["lanes"] = lanes
+    return sc
+
+
+def bullets_behind(lib: capi.Solver2D, sc: Scene) -> np.ndarray:
+    """Per lane of a :func:`bullets` scene: True where the projectile's centre of mass is past the mid-plane of its target
+    at the target's current pose, within the lane's span of that plane."""
+    out = []
+    for lane in sc.piles["lanes"]:
+        p = lib.s2Body_GetPosition(lane["body"])
+        local = lib.s2Body_GetLocalPoint(lane["target"], p)
+        out.append(local.x > 0.0 and abs(local.y) <= lane["span"])
+    return np.array(out, dtype=bool)
+
+
 HUB_RIDER_PITCH = 0.25  # m between the shapes of one rider
 HUB_RIDER_GAP = 0.4     # m between neighbouring riders: their fat boxes (0.1 m margin) stay apart, so they never touch
 HUB_LANE_LENGTH = 150.0  # m of riders on one ground lane (on_ground)
