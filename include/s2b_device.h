@@ -212,6 +212,8 @@ typedef struct s2bCounters
 	int32_t continuousHits;		 // bodies the last step's continuous pass stopped at a time of impact
 	int32_t bulletShapes;		 // shapes of fast bullets swept in the last step's bullet pass (S2B_BODY_BULLET)
 	int32_t bulletHits;			 // bullets the last step's bullet pass stopped at a time of impact
+	int32_t residentRegions;	 // 1: the last solve ran its regions with their bodies in shared memory (TGS_Soft, DESIGN.md §3.1)
+	int32_t maxRegionBodies;	 // bodies in the largest region of the last schedule (static bodies a region owns included), 0 = no regions
 } s2bCounters;
 
 // ---- lifecycle ------------------------------------------------------------------------------------------------

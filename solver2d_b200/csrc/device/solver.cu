@@ -4141,6 +4141,8 @@ extern "C" void s2b_get_counters(s2bWorld* w, s2bCounters* out)
 		out->overflowCount = counts[CNT_OVERFLOW_C] + counts[CNT_OVERFLOW_J];
 		out->neighbourSync = counts[CNT_NSYNC];
 		out->firstTable = counts[CNT_FIRST_TABLE_BLOCKS];
+		out->residentRegions = counts[CNT_REGIONS_ON] != 0 && counts[CNT_RESIDENT] != 0 ? 1 : 0;
+		out->maxRegionBodies = counts[CNT_MAX_REGION];
 		if (w->scratch->kempeState.p != nullptr)
 		{
 			int ks[4];

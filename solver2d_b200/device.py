@@ -64,7 +64,8 @@ class Counters(C.Structure):
                 ("regionCount", C.c_int32), ("cutCount", C.c_int32), ("cutGroupCount", C.c_int32), ("recolouredCount", C.c_int32),
                 ("neighbourSync", C.c_int32), ("narrowphaseRowSteps", C.c_int32),
                 ("firstTable", C.c_int32), ("continuousShapes", C.c_int32), ("continuousHits", C.c_int32),
-                ("bulletShapes", C.c_int32), ("bulletHits", C.c_int32)]
+                ("bulletShapes", C.c_int32), ("bulletHits", C.c_int32), ("residentRegions", C.c_int32),
+                ("maxRegionBodies", C.c_int32)]
 
 
 SCHEDULE_COLOR, SCHEDULE_WAVEFRONT = 0, 1
