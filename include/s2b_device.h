@@ -214,6 +214,7 @@ typedef struct s2bCounters
 	int32_t bulletHits;			 // bullets the last step's bullet pass stopped at a time of impact
 	int32_t residentRegions;	 // 1: the last solve ran its regions with their bodies in shared memory (TGS_Soft, DESIGN.md §3.1)
 	int32_t maxRegionBodies;	 // bodies in the largest region of the last schedule (static bodies a region owns included), 0 = no regions
+	int32_t finalizeRefits;		 // pair passes so far whose refit and moved proxies ran inside the finalize before them (DESIGN.md §3.3)
 } s2bCounters;
 
 // ---- lifecycle ------------------------------------------------------------------------------------------------

@@ -14,7 +14,7 @@
 //   * existing contacts whose fat AABBs stopped overlapping are dropped, survivors and new pairs are merged by a radix
 //     sort on the 64-bit shape-pair key and all contact columns are gathered into the other column set.
 // The contact table is therefore always sorted by pair key: the device's natural (wavefront) constraint order.
-#include "s2b_internal.cuh"
+#include "finalize.cuh"
 #include "shared/s2_toi.h"
 
 #include <cub/cub.cuh>
@@ -50,6 +50,8 @@ struct BroadScratch
 	DevArray<int> leafShape;	   // compacted valid shapes
 	DevArray<unsigned> mortonIn, mortonOut;
 	DevArray<int> leafIn, leafOut; // sorted leaf -> index into leafShape
+	DevArray<int> sortedShape;	   // sorted leaf -> shape (leafShape[leafOut[k]]), set by the build
+	DevArray<int> shapeLeaf;	   // shape -> sorted leaf, set by the build for the shapes in the hierarchy
 	DevArray<int> counters;		   // [0] leaf count [1] new pair count [2] kept count [3] bounds ready ...
 	DevArray<int> boundsBits;	   // 4 ordered-int encoded floats: min.x min.y max.x max.y
 	DevArray<int2> children;	   // binary internal nodes
@@ -60,7 +62,7 @@ struct BroadScratch
 	DevArray<int> wideCount;	   // children per wide node
 	DevArray<int> wideSlot;		   // per binary node: slot (wide parent * S2B_WIDE + i) it occupies, -1 for the root
 	DevArray<int> visit;		   // refit arrival counters (wide nodes); the last arriver resets its counter
-	DevArray<float4> rootBox;	   // box of the whole scene
+	DevArray<float4> rootBox;	   // box of the whole scene: two slots, the last refit's is rootBox[rootSlot]
 	DevArray<int> movedLeaves;	   // sorted-leaf indices of moved proxies
 	DevArray<int> movedFlag;
 	DevArray<int> largeShapes;	   // shapes of moved proxies with scene-sized boxes
@@ -77,6 +79,13 @@ struct BroadScratch
 	int treeShapeCap = 0;
 	int treeReuses = 0;
 	unsigned long long treeShapeEpoch = 0; // s2bWorld::shapeEpoch at the last refit: every static box in the tree is current
+	int rootSlot = 0;
+	// the per-pass counters (BC_NEW_PAIRS ...) are zero on the stream: nothing has appended to them since they were cleared
+	bool countersClean = false;
+	// finalize refitted the hierarchy and collected the moved proxies of the next search (s2bFinalizeRefit), at uploadEpoch
+	// fusedEpoch; the search that takes them over clears it, and searchFused says whether the last search did
+	bool fusedReady = false, searchFused = false;
+	unsigned long long fusedEpoch = 0;
 	// open-addressing hash set of the shape-pair keys of the current contact table ("does this pair already exist?")
 	DevArray<unsigned long long> pairHash;
 	unsigned long long hashMask = 0;
@@ -121,6 +130,8 @@ void s2bFreeBroadScratch(s2bWorld* w)
 	b->mortonOut.release();
 	b->leafIn.release();
 	b->leafOut.release();
+	b->sortedShape.release();
+	b->shapeLeaf.release();
 	b->counters.release();
 	b->boundsBits.release();
 	b->children.release();
@@ -516,10 +527,17 @@ __device__ __forceinline__ void s2bWideChildren(int wide, int node, int n, const
 // S2B_WIDE_LEVELS levels down, or the leaves met before. The binary height (deepest leaf) is taken here once per build:
 // the refit no longer visits the binary tree.
 __global__ void s2bBuildWide(const int* leafShape, const int* sortedLeaf, int* counters, const int2* children, const int* parent,
-							 int* wideChild, int* wideCount, int* wideSlot)
+							 int* wideChild, int* wideCount, int* wideSlot, int* sortedShape, int* shapeLeaf)
 {
 	int n = counters[BC_LEAVES];
 	int u = blockIdx.x * blockDim.x + threadIdx.x;
+	if (u < n)
+	{
+		// (the leaf columns of the finalize that refits this hierarchy, s2bFinalizeRefit, and of the bullet pass after it)
+		int shape = leafShape[sortedLeaf[u]];
+		sortedShape[u] = shape;
+		shapeLeaf[shape] = u;
+	}
 	if (u >= n - 1)
 	{
 		return;
@@ -554,25 +572,9 @@ __global__ void s2bBuildWide(const int* leafShape, const int* sortedLeaf, int* c
 
 // Boxes bottom-up: a leaf thread writes its fat box into its slot in the parent wide node and counts its arrival; the last
 // child to arrive resets the counter for the next pass, unions the node's child boxes and carries that box one level up.
-// The refit is the first kernel of every search, and nothing before it in the pass touches the per-pass counters, so it clears
-// them (a memset on the stream in its place cost more than the refit's leaf threads wait for it).
-__global__ void s2bRefit(ShapeView s, const int* leafShape, const int* sortedLeaf, int* counters, const int* wideCount,
-						 const int* wideSlot, float4* wideBox, int* visit, float4* rootBox)
+__device__ __forceinline__ void s2bRefitClimb(int n, int k, float4 box, const int* wideCount, const int* wideSlot, float4* wideBox,
+											 int* visit, float4* rootBox)
 {
-	int n = counters[BC_LEAVES];
-	int k = blockIdx.x * blockDim.x + threadIdx.x;
-	if (k == 0)
-	{
-		for (int c = BC_NEW_PAIRS; c < BC_SIZE; ++c)
-		{
-			counters[c] = 0;
-		}
-	}
-	if (k >= n)
-	{
-		return;
-	}
-	float4 box = s.fat[leafShape[sortedLeaf[k]]];
 	if (n == 1)
 	{
 		rootBox[0] = box;
@@ -609,6 +611,29 @@ __global__ void s2bRefit(ShapeView s, const int* leafShape, const int* sortedLea
 			return;
 		}
 	}
+}
+
+// Every leaf's fat box, climbed. The search's own refit is the first kernel of its pass, and nothing before it in the pass
+// touches the per-pass counters, so it clears them (`clearCounters`; a memset on the stream in its place cost more than
+// the refit's leaf threads wait for it). The bullet pass's refit leaves them alone: finalize may have collected the next
+// search's moved proxies into them already (s2bFinalizeRefit).
+__global__ void s2bRefit(ShapeView s, const int* leafShape, const int* sortedLeaf, int* counters, const int* wideCount,
+						 const int* wideSlot, float4* wideBox, int* visit, float4* rootBox, int clearCounters)
+{
+	int n = counters[BC_LEAVES];
+	int k = blockIdx.x * blockDim.x + threadIdx.x;
+	if (k == 0 && clearCounters != 0)
+	{
+		for (int c = BC_NEW_PAIRS; c < BC_SIZE; ++c)
+		{
+			counters[c] = 0;
+		}
+	}
+	if (k >= n)
+	{
+		return;
+	}
+	s2bRefitClimb(n, k, s.fat[leafShape[sortedLeaf[k]]], wideCount, wideSlot, wideBox, visit, rootBox);
 }
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -682,6 +707,56 @@ __global__ void s2bCollectMovers(ShapeView s, const int* leafShape, const int* s
 		}
 	}
 	s2bBlockAppend(moved, k, movedLeaves, counters + BC_MOVED);
+}
+
+// Finalize's shapes, the refit and s2bCollectMovers in one launch, for a pass that reuses the hierarchy's topology: its leaves
+// are then exactly the live shapes. One thread per sorted leaf finalizes a non-static shape (s2bFinalizeShape, as
+// s2bFinalizeShapes), appends the leaf to the moved proxies when its MOVED flag is set (by finalize or by an upload) and
+// climbs with the box it holds; a static shape's box only climbs. The per-pass counters must be zero before the launch
+// (s2bClearMovedFlags clears them). A large mover is judged against `lastRoot`, the root box of the previous refit: this
+// launch's own root box is final only at its end. The path a moved proxy takes never changes the pairs it finds.
+__global__ void s2bFinalizeRefitKernel(ShapeView s, BodyView b, const int* sortedShape, int* counters, const int* wideCount,
+									   const int* wideSlot, float4* wideBox, int* visit, const float4* lastRoot, float4* rootBox,
+									   int* movedLeaves, int* largeShapes, int* movedCounter)
+{
+	int n = counters[BC_LEAVES];
+	int k = blockIdx.x * blockDim.x + threadIdx.x;
+	bool moved = false;
+	float4 box;
+	if (k < n)
+	{
+		int shape = sortedShape[k];
+		int4 head = s.head[shape];
+		if (S2B_BODY_TYPE(b.flags[head.y]) != S2B_BODY_STATIC)
+		{
+			box = s2bFinalizeShape<false>(s, b, shape, head, movedCounter);
+		}
+		else
+		{
+			box = s.fat[shape];
+		}
+		moved = (head.x & S2B_SHAPE_MOVED) != 0;
+		if (moved && n >= 256)
+		{
+			float4 root = lastRoot[0];
+			float area = (box.z - box.x) * (box.w - box.y);
+			float sceneArea = (root.z - root.x) * (root.w - root.y);
+			if (area * 256.0f > sceneArea)
+			{
+				int slot = atomicAdd(counters + BC_LARGE, 1);
+				if (slot < S2B_MAX_LARGE_MOVERS)
+				{
+					largeShapes[slot] = shape;
+					moved = false;
+				}
+			}
+		}
+	}
+	s2bBlockAppend(moved, k, movedLeaves, counters + BC_MOVED);
+	if (k < n)
+	{
+		s2bRefitClimb(n, k, box, wideCount, wideSlot, wideBox, visit, rootBox);
+	}
 }
 
 // what the query of proxy Q does with an overlapping proxy `other` (reference s2PairQueryCallback, src/broad_phase.c:166-258)
@@ -792,12 +867,81 @@ __device__ __forceinline__ bool s2bMakeQuery(PairQuery& q, int shapeQ, const Sha
 #define S2B_QUERY_BATCH 16
 #define S2B_QUERY_BLOCK 128
 
-// moved proxies with ordinary boxes: one thread walks the wide hierarchy
+// every leaf against the short list of large movers (s2bCollectMovers). Same rules, same pairs; the order new pairs are
+// emitted in never matters (they are sorted).
+__device__ __forceinline__ void s2bFindPairsLarge(int k, const ShapeView& s, const BodyView& b, const int* leafShape, int* counters,
+												  const int* largeShapes, const unsigned long long* pairHash, unsigned long long hashMask,
+												  const unsigned long long* jointKeys, int jointKeyCount, unsigned long long* newKey,
+												  int2* newShapes, int newCap)
+{
+	int n = counters[BC_LEAVES];
+	int large = min(counters[BC_LARGE], S2B_MAX_LARGE_MOVERS);
+	if (k >= n || large == 0)
+	{
+		return;
+	}
+	int other = leafShape[k];
+	float4 boxO = s.fat[other];
+	for (int i = 0; i < large; ++i)
+	{
+		int shapeQ = largeShapes[i];
+		if (s2bBoxesOverlap(s.fat[shapeQ], boxO) == false)
+		{
+			continue;
+		}
+		PairQuery q;
+		if (s2bMakeQuery(q, shapeQ, s, b))
+		{
+			s2bConsiderPair(q, other, s, b, counters, pairHash, hashMask, jointKeys, jointKeyCount, newKey, newShapes, newCap);
+		}
+	}
+}
+
+// survivors: both shapes alive and not re-created, fat AABBs still overlap (reference src/world.c:149-166), and no joint
+// created since forbids the pair (reference src/joint.c:214-217)
+// The survivors' slots are appended to keepSlots (BC_KEPT): their order does not matter, the merged table is sorted by pair key.
+// Every thread of the block calls this (s2bBlockAppend).
+__device__ __forceinline__ void s2bCollectKeptContacts(int i, const int2* contactShapes, int contactCount, const ShapeView& s,
+													   const unsigned long long* jointKeys, int jointKeyCount, int* keepSlots, int* counters)
+{
+	bool keep = false;
+	if (i < contactCount)
+	{
+		int2 sh = contactShapes[i];
+		int4 ha = s.head[sh.x], hb = s.head[sh.y];
+		bool alive = (ha.x & S2B_ROW_VALID) && (hb.x & S2B_ROW_VALID) && (ha.x & S2B_SHAPE_FRESH) == 0 && (hb.x & S2B_SHAPE_FRESH) == 0;
+		keep = alive && s2bBoxesOverlap(s.fat[sh.x], s.fat[sh.y]) && s2bJointOverride(jointKeys, jointKeyCount, ha.y, hb.y) == false;
+	}
+	s2bBlockAppend(keep, i, keepSlots, counters + BC_KEPT);
+}
+
+
+// The queries of a pass in one launch, three kinds of block: the first `walkBlocks` walk the wide hierarchy, one thread per
+// moved proxy with an ordinary box; the next `keptBlocks` collect the survivors of the contact table (one thread per
+// contact); the rest test every leaf against the large movers (one thread per leaf). The survivors and the large movers
+// need nothing of the walk, so their blocks run beside it instead of queued behind it.
 __global__ void __launch_bounds__(S2B_QUERY_BLOCK) s2bFindPairs(ShapeView s, BodyView b, const int* leafShape, const int* sortedLeaf, int* counters,
 								 const int* movedLeaves, const float4* wideBox, const int* wideChild,
 								 const unsigned long long* pairHash, unsigned long long hashMask, const unsigned long long* jointKeys,
-								 int jointKeyCount, unsigned long long* newKey, int2* newShapes, int newCap)
+								 int jointKeyCount, unsigned long long* newKey, int2* newShapes, int newCap, int walkBlocks,
+								 int keptBlocks, const int2* contactShapes, int contactCount, const unsigned long long* destroyKeys,
+								 int destroyKeyCount, int* keepSlots, const int* largeShapes)
 {
+	if ((int)blockIdx.x >= walkBlocks)
+	{
+		int block = (int)blockIdx.x - walkBlocks;
+		if (block < keptBlocks)
+		{
+			s2bCollectKeptContacts(block * blockDim.x + threadIdx.x, contactShapes, contactCount, s, destroyKeys, destroyKeyCount,
+								   keepSlots, counters);
+		}
+		else
+		{
+			s2bFindPairsLarge((block - keptBlocks) * blockDim.x + threadIdx.x, s, b, leafShape, counters, largeShapes, pairHash,
+							  hashMask, jointKeys, jointKeyCount, newKey, newShapes, newCap);
+		}
+		return;
+	}
 	// overlapping LEAVES are only collected during the walk and examined in batches afterwards: the walk (box tests) and the
 	// pair rules (shape header, hash probe, filters) are two different instruction streams, and a warp whose lanes hit
 	// leaves at different moments would otherwise execute both serially for every lane
@@ -876,54 +1020,6 @@ __global__ void __launch_bounds__(S2B_QUERY_BLOCK) s2bFindPairs(ShapeView s, Bod
 		}
 		nFound = 0;
 	}
-}
-
-// every leaf against the short list of large movers (s2bCollectMovers). Same rules, same pairs; the order new pairs are
-// emitted in never matters (they are sorted).
-__global__ void s2bFindPairsLarge(ShapeView s, BodyView b, const int* leafShape, int* counters, const int* largeShapes,
-								  const unsigned long long* pairHash, unsigned long long hashMask, const unsigned long long* jointKeys,
-								  int jointKeyCount, unsigned long long* newKey, int2* newShapes, int newCap)
-{
-	int n = counters[BC_LEAVES];
-	int large = min(counters[BC_LARGE], S2B_MAX_LARGE_MOVERS);
-	int k = blockIdx.x * blockDim.x + threadIdx.x;
-	if (k >= n || large == 0)
-	{
-		return;
-	}
-	int other = leafShape[k];
-	float4 boxO = s.fat[other];
-	for (int i = 0; i < large; ++i)
-	{
-		int shapeQ = largeShapes[i];
-		if (s2bBoxesOverlap(s.fat[shapeQ], boxO) == false)
-		{
-			continue;
-		}
-		PairQuery q;
-		if (s2bMakeQuery(q, shapeQ, s, b))
-		{
-			s2bConsiderPair(q, other, s, b, counters, pairHash, hashMask, jointKeys, jointKeyCount, newKey, newShapes, newCap);
-		}
-	}
-}
-
-// survivors: both shapes alive and not re-created, fat AABBs still overlap (reference src/world.c:149-166), and no joint
-// created since forbids the pair (reference src/joint.c:214-217)
-// The survivors' slots are appended to keepSlots (BC_KEPT): their order does not matter, the merged table is sorted by pair key.
-__global__ void s2bCollectKeptContacts(ContactView c, int contactCount, ShapeView s, const unsigned long long* jointKeys, int jointKeyCount,
-									   int* keepSlots, int* counters)
-{
-	int i = blockIdx.x * blockDim.x + threadIdx.x;
-	bool keep = false;
-	if (i < contactCount)
-	{
-		int2 sh = c.shapes[i];
-		int4 ha = s.head[sh.x], hb = s.head[sh.y];
-		bool alive = (ha.x & S2B_ROW_VALID) && (hb.x & S2B_ROW_VALID) && (ha.x & S2B_SHAPE_FRESH) == 0 && (hb.x & S2B_SHAPE_FRESH) == 0;
-		keep = alive && s2bBoxesOverlap(s.fat[sh.x], s.fat[sh.y]) && s2bJointOverride(jointKeys, jointKeyCount, ha.y, hb.y) == false;
-	}
-	s2bBlockAppend(keep, i, keepSlots, counters + BC_KEPT);
 }
 
 // The sort key is the pair key squeezed to 2 x shapeBits bits (lo << shapeBits | hi) so the radix sort runs only over
@@ -1016,7 +1112,9 @@ __global__ void s2bGatherContactsSorted(const int* counters, const unsigned long
 	}
 }
 
-__global__ void s2bClearMovedFlags(ShapeView s, int* movedCounter)
+// Also clears the per-pass counters of the search (the host has read them): finalize may append the next search's moved
+// proxies to them (s2bFinalizeRefit).
+__global__ void s2bClearMovedFlags(ShapeView s, int* movedCounter, int* passCounters)
 {
 	int i = blockIdx.x * blockDim.x + threadIdx.x;
 	if (i < s.capacity)
@@ -1030,6 +1128,10 @@ __global__ void s2bClearMovedFlags(ShapeView s, int* movedCounter)
 	if (i == 0)
 	{
 		movedCounter[0] = 0;
+		for (int c = BC_NEW_PAIRS; c < BC_SIZE; ++c)
+		{
+			passCounters[c] = 0;
+		}
 	}
 }
 
@@ -1053,6 +1155,8 @@ static size_t bpReserve(s2bWorld* w, BroadScratch* B)
 	B->mortonOut.reserve(nS, st, false);
 	B->leafIn.reserve(nS, st, false);
 	B->leafOut.reserve(nS, st, false);
+	B->sortedShape.reserve(nS, st, false, false);
+	B->shapeLeaf.reserve(nS, st, false, false);
 	B->counters.reserve(BC_SIZE, st, false);
 	B->boundsBits.reserve(4, st, false);
 	B->children.reserve(nS, st, false);
@@ -1062,7 +1166,7 @@ static size_t bpReserve(s2bWorld* w, BroadScratch* B)
 	B->wideCount.reserve(nS, st, false, false);
 	B->wideSlot.reserve(2 * nS, st, false, false);
 	B->visit.reserve(nS, st, false); // zeroed once here: from then on every refit leaves its counters at zero
-	B->rootBox.reserve(1, st, false);
+	B->rootBox.reserve(2, st, false);
 	B->movedLeaves.reserve(nS, st, false);
 	B->movedFlag.reserve(nS, st, false);
 	B->largeShapes.reserve(S2B_MAX_LARGE_MOVERS, st, false);
@@ -1122,7 +1226,7 @@ static void bpTree(s2bWorld* w, BroadScratch* B, bool reuseTree)
 		// ---- hierarchy ----
 		S2B_LAUNCH(w, s2bBuildRadixTree, gridFor(shapeCap, 256), 256, 0, B->mortonOut.p, B->counters.p, B->children.p, B->parent.p);
 		S2B_LAUNCH(w, s2bBuildWide, gridFor(shapeCap, 256), 256, 0, B->leafShape.p, B->leafOut.p, B->counters.p, B->children.p,
-				   B->parent.p, B->wideChild.p, B->wideCount.p, B->wideSlot.p);
+				   B->parent.p, B->wideChild.p, B->wideCount.p, B->wideSlot.p, B->sortedShape.p, B->shapeLeaf.p);
 		B->treeValid = true;
 		B->treeShapeCap = shapeCap;
 		B->treeReuses = 0;
@@ -1130,9 +1234,41 @@ static void bpTree(s2bWorld* w, BroadScratch* B, bool reuseTree)
 
 	// ---- refit ----
 	S2B_LAUNCH(w, s2bRefit, gridFor(shapeCap, 256), 256, 0, sv, B->leafShape.p, B->leafOut.p, B->counters.p, B->wideCount.p,
-			   B->wideSlot.p, B->wideBox.p, B->visit.p, B->rootBox.p);
+			   B->wideSlot.p, B->wideBox.p, B->visit.p, B->rootBox.p + B->rootSlot, 1);
 
 	B->treeShapeEpoch = w->shapeEpoch;
+	B->countersClean = true;
+}
+
+// On a pass that will reuse the hierarchy's topology (the decision bpSearch would take, taken here on the same state),
+// finalize's shapes, the refit and the moved proxies of the next search run as one launch (s2bFinalizeRefitKernel) and the
+// search skips its own refit and s2bCollectMovers (DESIGN.md §3.3). The per-pass counters have to be clear: they are after
+// a pass's commit, so this holds in a scene in motion; otherwise (a search that was never committed, a finalize with no
+// pass since the last one) finalize runs the old way.
+bool s2bFinalizeRefit(s2bWorld* w)
+{
+	S2bEpochFreeze freeze;
+	BroadScratch* B = w->broad;
+	if (B == nullptr)
+	{
+		return false;
+	}
+	B->fusedReady = false;
+	bool reuseTree = B->treeValid && w->pairsDirty == false && B->treeShapeCap == w->shapeCap && B->treeReuses < S2B_TREE_REUSE_LIMIT;
+	if (reuseTree == false || B->countersClean == false || w->fusedRefit == 0)
+	{
+		return false;
+	}
+	int last = B->rootSlot;
+	B->rootSlot ^= 1;
+	S2B_LAUNCH(w, s2bFinalizeRefitKernel, gridFor(w->shapeCap, 256), 256, 0, shapeView(w), bodyView(w), B->sortedShape.p,
+			   B->counters.p, B->wideCount.p, B->wideSlot.p, B->wideBox.p, B->visit.p, B->rootBox.p + last,
+			   B->rootBox.p + B->rootSlot, B->movedLeaves.p, B->largeShapes.p, w->dMovedFlag.p);
+	B->treeShapeEpoch = w->shapeEpoch;
+	B->countersClean = false;
+	B->fusedReady = true;
+	B->fusedEpoch = w->uploadEpoch;
+	return true;
 }
 
 // First half of a pass, no host synchronisation: hierarchy (re-used or rebuilt) and refit, pair-key hash of the current
@@ -1148,8 +1284,22 @@ static void bpSearch(s2bWorld* w, BroadScratch* B)
 	ContactColumns& cur = w->contacts[w->cur];
 	int newCap = B->newPairCap;
 
-	bool reuseTree = B->treeValid && w->pairsDirty == false && B->treeShapeCap == shapeCap && B->treeReuses < S2B_TREE_REUSE_LIMIT;
-	bpTree(w, B, reuseTree);
+	// the hierarchy and the moved proxies came with finalize unless something was uploaded since (a body moved by the host,
+	// shapes created or destroyed), or another search took them over already
+	bool fused = B->fusedReady && B->fusedEpoch == w->uploadEpoch && w->pairsDirty == false;
+	B->fusedReady = false;
+	B->searchFused = fused;
+	if (fused)
+	{
+		// counted per search that reuses the topology, as bpTree counts it: a finalize whose refit no search takes over (nothing
+		// moved) does not bring the next rebuild closer
+		B->treeReuses += 1;
+	}
+	else
+	{
+		bool reuseTree = B->treeValid && w->pairsDirty == false && B->treeShapeCap == shapeCap && B->treeReuses < S2B_TREE_REUSE_LIMIT;
+		bpTree(w, B, reuseTree);
+	}
 
 	// ---- pair-key hash set of the current contact table (rebuilt only when the table changed) ----
 	if (B->hashVersion != w->contactTableVersion || B->pairHash.p == nullptr)
@@ -1169,21 +1319,18 @@ static void bpSearch(s2bWorld* w, BroadScratch* B)
 		B->hashVersion = w->contactTableVersion;
 	}
 
-	// ---- queries from moved proxies ----
-	S2B_LAUNCH(w, s2bCollectMovers, gridFor(shapeCap, 256), 256, 0, sv, B->leafShape.p, B->leafOut.p, B->counters.p, B->rootBox.p,
-			   B->movedLeaves.p, B->largeShapes.p);
-	S2B_LAUNCH(w, s2bFindPairs, gridFor(shapeCap, S2B_QUERY_BLOCK), S2B_QUERY_BLOCK, 0, sv, bv, B->leafShape.p, B->leafOut.p,
-			   B->counters.p, B->movedLeaves.p, B->wideBox.p, B->wideChild.p, B->pairHash.p, B->hashMask, w->jointPairKeys.p,
-			   w->jointPairCount, B->newKey.p, B->newShapes.p, newCap);
-	S2B_LAUNCH(w, s2bFindPairsLarge, gridFor(shapeCap, 256), 256, 0, sv, bv, B->leafShape.p, B->counters.p, B->largeShapes.p,
-			   B->pairHash.p, B->hashMask, w->jointPairKeys.p, w->jointPairCount, B->newKey.p, B->newShapes.p, newCap);
-
-	// ---- survivors ----
-	if (oldCount > 0)
+	// ---- queries from moved proxies, survivors, large movers: one launch ----
+	if (fused == false)
 	{
-		S2B_LAUNCH(w, s2bCollectKeptContacts, gridFor(oldCount, 256), 256, 0, makeView(cur), oldCount, sv, w->jointDestroyKeys.p,
-				   w->jointDestroyCount, B->keepSlots.p, B->counters.p);
+		S2B_LAUNCH(w, s2bCollectMovers, gridFor(shapeCap, 256), 256, 0, sv, B->leafShape.p, B->leafOut.p, B->counters.p,
+				   B->rootBox.p + B->rootSlot, B->movedLeaves.p, B->largeShapes.p);
 	}
+	int walkBlocks = gridFor(shapeCap, S2B_QUERY_BLOCK), keptBlocks = gridFor(oldCount, S2B_QUERY_BLOCK);
+	S2B_LAUNCH(w, s2bFindPairs, walkBlocks + keptBlocks + gridFor(shapeCap, S2B_QUERY_BLOCK), S2B_QUERY_BLOCK, 0, sv, bv,
+			   B->leafShape.p, B->leafOut.p, B->counters.p, B->movedLeaves.p, B->wideBox.p, B->wideChild.p, B->pairHash.p,
+			   B->hashMask, w->jointPairKeys.p, w->jointPairCount, B->newKey.p, B->newShapes.p, newCap, walkBlocks, keptBlocks,
+			   cur.shapes.p, oldCount, w->jointDestroyKeys.p, w->jointDestroyCount, B->keepSlots.p, B->largeShapes.p);
+	B->countersClean = false;
 	// The counters go to the mailbox on mailStream, behind the search's kernels only, so that the world's stream does not
 	// wait for the copy. searchDone passes once they have arrived, and the moved-proxy counter's copy too (s2bFinalize):
 	// whoever waits for this pass's counters has that one behind it as well. The next pass clears the counters only after
@@ -1273,10 +1420,12 @@ static void bpCommit(s2bWorld* w, BroadScratch* B, int fresh, int kept, size_t t
 			B->pairHash.reserve((size_t)size, st, false, false);
 		}
 	}
-	S2B_LAUNCH(w, s2bClearMovedFlags, gridFor(shapeCap, 256), 256, 0, sv, w->dMovedFlag.p);
+	S2B_LAUNCH(w, s2bClearMovedFlags, gridFor(shapeCap, 256), 256, 0, sv, w->dMovedFlag.p, B->counters.p);
+	B->countersClean = true;
 	w->hostMail[MAIL_MOVED] = 0;
 	w->pairsDirty = false;
 	w->pairPassCount += 1;
+	w->finalizeRefits += B->searchFused ? 1 : 0;
 }
 
 // Start the pair search of the NEXT step behind this one (called after finalize): its inputs — fat AABBs, MOVED flags, the
@@ -1726,6 +1875,9 @@ __global__ void s2bBulletClamp(BodyView b, const float4* start, const unsigned* 
 // moved since: it is refitted (same topology, every box from the fat column, which now holds each non-static shape's final
 // box) before the bullets are swept. The refit leaves the hierarchy as the next search's own refit would, and is not
 // counted toward the rebuild cadence (S2B_TREE_REUSE_LIMIT).
+// When finalize refitted the hierarchy itself (s2bFinalizeRefit), the sweep walks that, and the refit runs after the clamped
+// bullets' shapes are redone instead, for the search that will not refit; a shape that escapes its fat box only then joins
+// the moved proxies finalize collected. Either way the pass adds five launches.
 void s2bBulletPass(s2bWorld* w)
 {
 	S2bEpochFreeze freeze;
@@ -1744,15 +1896,29 @@ void s2bBulletPass(s2bWorld* w)
 	ShapeView sv = shapeView(w);
 	BodyView bv = bodyView(w);
 	// (the non-bullet pass just made sure the hierarchy holds every live shape: C.ran)
-	S2B_LAUNCH(w, s2bRefit, gridFor(w->shapeCap, 256), 256, 0, sv, B->leafShape.p, B->leafOut.p, B->counters.p, B->wideCount.p,
-			   B->wideSlot.p, B->wideBox.p, B->visit.p, B->rootBox.p);
+	bool fused = B->fusedReady;
+	if (fused == false)
+	{
+		S2B_LAUNCH(w, s2bRefit, gridFor(w->shapeCap, 256), 256, 0, sv, B->leafShape.p, B->leafOut.p, B->counters.p, B->wideCount.p,
+				   B->wideSlot.p, B->wideBox.p, B->visit.p, B->rootBox.p + B->rootSlot, 0);
+	}
 	C.bulletShapes.reserve((size_t)w->shapeCap, st, false, false);
 	S2B_CHECK(cudaMemsetAsync(C.counters.p + 2, 0, sizeof(int) * 2, st));
 	S2B_LAUNCH(w, s2bBulletCollect, gridFor(w->shapeCap, 256), 256, 0, sv, bv, w->bExt.p, C.start.p, C.bulletShapes.p, C.counters.p);
 	S2B_LAUNCH(w, s2bContinuousSweep<S2B_SWEEP_BULLET>, gridFor(w->shapeCap, S2B_SWEEP_BLOCK), S2B_SWEEP_BLOCK, 0, sv, bv, C.start.p,
 			   C.bulletShapes.p, C.counters.p + 2, B->counters.p, B->wideBox.p, B->wideChild.p, w->jointPairKeys.p, w->jointPairCount, C.fraction.p);
 	S2B_LAUNCH(w, s2bBulletClamp, gridFor(w->bodyCap, 256), 256, 0, bv, C.start.p, C.fraction.p, C.counters.p);
-	s2bRefinalizeBulletShapes(w, C.bulletShapes.p, C.counters.p + 2, C.fraction.p);
+	if (fused == false)
+	{
+		s2bRefinalizeBulletShapes(w, C.bulletShapes.p, C.counters.p + 2, C.fraction.p, nullptr, nullptr, nullptr);
+	}
+	else
+	{
+		s2bRefinalizeBulletShapes(w, C.bulletShapes.p, C.counters.p + 2, C.fraction.p, B->shapeLeaf.p, B->movedLeaves.p,
+								  B->counters.p + BC_MOVED);
+		S2B_LAUNCH(w, s2bRefit, gridFor(w->shapeCap, 256), 256, 0, sv, B->leafShape.p, B->leafOut.p, B->counters.p, B->wideCount.p,
+				   B->wideSlot.p, B->wideBox.p, B->visit.p, B->rootBox.p + B->rootSlot, 0);
+	}
 	C.bulletRan = true;
 }
 

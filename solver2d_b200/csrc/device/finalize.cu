@@ -3,7 +3,7 @@
 //
 // Both kernels are pure streaming passes (bandwidth-bound): bodies 64 B read + 32 B written, shapes ~190 B read
 // (geometry) + 16-32 B written.
-#include "s2b_internal.cuh"
+#include "finalize.cuh"
 
 __global__ void s2bFinalizeBodies(BodyView b)
 {
@@ -30,69 +30,6 @@ __global__ void s2bFinalizeBodies(BodyView b)
 	b.frc[i] = make_float4(0.0f, 0.0f, 0.0f, frc.w);
 }
 
-// All four shape kinds are stored in polygon form (count vertices + radius), for which the per-kind AABB functions of
-// the reference (src/geometry.c:288-341) reduce to the same float operations: min/max over the transformed
-// vertices, then -/+ radius.
-//
-// Once finalize has run, the bullet pass (DESIGN.md §3.12) redoes a clamped bullet's shapes with `again`: a shape that is
-// already flagged MOVED is not counted a second time.
-template <bool again> __device__ __forceinline__ void s2bFinalizeShape(const ShapeView& s, const BodyView& b, int i, int4 head,
-																		 int* movedCounter)
-{
-	int body = head.y;
-	float4 org = b.org[body];
-	float4 pose = b.pose[body];
-	s2Transform xf;
-	xf.p.x = org.x;
-	xf.p.y = org.y;
-	xf.q.s = pose.z;
-	xf.q.c = pose.w;
-
-	int count = head.w;
-	float radius = s.fr[i].y;
-	float2 v0 = s.verts[i * 8];
-	s2Vec2 p0 = {v0.x, v0.y};
-	s2Vec2 lower = s2TransformPoint(xf, p0);
-	s2Vec2 upper = lower;
-	for (int k = 1; k < count; ++k)
-	{
-		float2 vk = s.verts[i * 8 + k];
-		s2Vec2 pk = {vk.x, vk.y};
-		s2Vec2 v = s2TransformPoint(xf, pk);
-		lower = s2Min(lower, v);
-		upper = s2Max(upper, v);
-	}
-	s2Vec2 r = {radius, radius};
-	lower = s2Sub(lower, r);
-	upper = s2Add(upper, r);
-
-	s2Box aabb;
-	aabb.lowerBound.x = lower.x - s2_speculativeDistance;
-	aabb.lowerBound.y = lower.y - s2_speculativeDistance;
-	aabb.upperBound.x = upper.x + s2_speculativeDistance;
-	aabb.upperBound.y = upper.y + s2_speculativeDistance;
-	s.aabb[i] = make_float4(aabb.lowerBound.x, aabb.lowerBound.y, aabb.upperBound.x, aabb.upperBound.y);
-
-	float4 fat4 = s.fat[i];
-	s2Box fat;
-	fat.lowerBound.x = fat4.x;
-	fat.lowerBound.y = fat4.y;
-	fat.upperBound.x = fat4.z;
-	fat.upperBound.y = fat4.w;
-	if (s2AABB_Contains(fat, aabb) == false)
-	{
-		// the proxy escaped its fat box: re-centre it and buffer a move for the next pair update
-		// (reference src/world.c:291-296 -> s2BroadPhase_EnlargeProxy -> s2BufferMove)
-		s.fat[i] = make_float4(aabb.lowerBound.x - s2_aabbMargin, aabb.lowerBound.y - s2_aabbMargin,
-							   aabb.upperBound.x + s2_aabbMargin, aabb.upperBound.y + s2_aabbMargin);
-		s.head[i] = make_int4(head.x | S2B_SHAPE_MOVED, head.y, head.z, head.w);
-		if (again == false || (head.x & S2B_SHAPE_MOVED) == 0)
-		{
-			atomicAdd(movedCounter, 1);
-		}
-	}
-}
-
 __global__ void s2bFinalizeShapes(ShapeView s, BodyView b, int* movedCounter)
 {
 	int i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -114,9 +51,11 @@ __global__ void s2bFinalizeShapes(ShapeView s, BodyView b, int* movedCounter)
 }
 
 // The listed shapes (list[0, count[0])) of the bodies the bullet pass clamped (fraction below 1): boxes and fat-box moves
-// for the clamped pose, as finalize derives them.
+// for the clamped pose, as finalize derives them. When finalize has already collected this pass's moved proxies
+// (s2bFinalizeRefit), `movedLeaves` is set: a shape that escapes its fat box only now (the one that is counted) is appended to
+// them, at its sorted leaf (`shapeLeaf`).
 __global__ void s2bRefinalizeShapes(ShapeView s, BodyView b, const int* list, const int* count, const unsigned* fraction,
-									int* movedCounter)
+									int* movedCounter, const int* shapeLeaf, int* movedLeaves, int* movedLeafCount)
 {
 	int k = blockIdx.x * blockDim.x + threadIdx.x;
 	if (k >= count[0])
@@ -129,13 +68,19 @@ __global__ void s2bRefinalizeShapes(ShapeView s, BodyView b, const int* list, co
 	{
 		return;
 	}
+	int before = head.x;
 	s2bFinalizeShape<true>(s, b, i, head, movedCounter);
+	if (movedLeaves != nullptr && (head.x & S2B_SHAPE_MOVED) != 0 && (before & S2B_SHAPE_MOVED) == 0)
+	{
+		movedLeaves[atomicAdd(movedLeafCount, 1)] = shapeLeaf[i];
+	}
 }
 
-void s2bRefinalizeBulletShapes(s2bWorld* w, const int* list, const int* count, const unsigned* fraction)
+void s2bRefinalizeBulletShapes(s2bWorld* w, const int* list, const int* count, const unsigned* fraction, const int* shapeLeaf,
+							   int* movedLeaves, int* movedLeafCount)
 {
 	S2B_LAUNCH(w, s2bRefinalizeShapes, gridFor(w->shapeCap, 256), 256, 0, shapeView(w), bodyView(w), list, count, fraction,
-			   w->dMovedFlag.p);
+			   w->dMovedFlag.p, shapeLeaf, movedLeaves, movedLeafCount);
 }
 
 void s2bFinalize(s2bWorld* w)
@@ -146,7 +91,9 @@ void s2bFinalize(s2bWorld* w)
 	{
 		S2B_LAUNCH(w, s2bFinalizeBodies, gridFor(w->bodyCap, 256), 256, 0, bodyView(w));
 	}
-	if (w->shapeCap > 0)
+	// when the next pair search will reuse the hierarchy's topology, the shapes are finalized by the kernel that also refits
+	// it and collects the search's moved proxies (DESIGN.md §3.3)
+	if (w->shapeCap > 0 && s2bFinalizeRefit(w) == false)
 	{
 		S2B_LAUNCH(w, s2bFinalizeShapes, gridFor(w->shapeCap, 256), 256, 0, shapeView(w), bodyView(w), w->dMovedFlag.p);
 	}

@@ -404,9 +404,12 @@ struct s2bWorld
 	int blockWarm = 1;		// TGS_Soft: the bias sweep's colour-0 step warm-starts a block's first-touched bodies together, from a
 							// table built with the schedule (persistent.cuh; S2B_BLOCK_WARM=0 keeps the gather per thread)
 	int blockWarmBytes = 0; // shared-memory budget of one block's table; 0 = the kernel's dynamic shared memory (S2B_BLOCK_WARM_BYTES)
+	int fusedRefit = 1; // finalize refits the pair search's hierarchy and collects its moved proxies when the search will
+						// reuse the topology (broadphase.cu s2bFinalizeRefit; S2B_FINALIZE_REFIT=0: the search does both)
 	int kempeGrid = 0;
 	DevArray<int> dMovedFlag; // [0] = number of proxies moved in last finalize (device counter)
 	int pairPassCount = 0;
+	int finalizeRefits = 0; // pair passes whose refit and moved proxies came from finalize (s2bFinalizeRefit)
 	int treeHeight = 0;
 
 	// solve-order hint (validation)
@@ -530,7 +533,12 @@ void s2bContinuousSnapshot(s2bWorld* w);
 void s2bContinuousPass(s2bWorld* w);
 // the bullet pass (broadphase.cu, DESIGN.md §3.12): inside finalize, after its kernels and before the moved counter's copy
 void s2bBulletPass(s2bWorld* w);
-// (finalize.cu) boxes and fat-box moves of the listed shapes whose body has a fraction below 1, for its clamped pose
-void s2bRefinalizeBulletShapes(s2bWorld* w, const int* list, const int* count, const unsigned* fraction);
+// (finalize.cu) boxes and fat-box moves of the listed shapes whose body has a fraction below 1, for its clamped pose; with
+// `movedLeaves`, a shape that escapes its fat box only now is appended to the moved proxies finalize collected
+void s2bRefinalizeBulletShapes(s2bWorld* w, const int* list, const int* count, const unsigned* fraction, const int* shapeLeaf,
+							   int* movedLeaves, int* movedLeafCount);
+// (broadphase.cu) finalize's shapes, the refit and the moved proxies of the next pair search in one launch, when that search
+// will reuse the hierarchy's topology; false: nothing launched, finalize runs s2bFinalizeShapes (DESIGN.md §3.3)
+bool s2bFinalizeRefit(s2bWorld* w);
 // [0] continuousShapes [1] continuousHits [2] bulletShapes [3] bulletHits of the last step
 void s2bContinuousCounters(s2bWorld* w, int out[4]);

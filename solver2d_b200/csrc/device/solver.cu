@@ -4163,6 +4163,7 @@ extern "C" void s2b_get_counters(s2bWorld* w, s2bCounters* out)
 	out->treeHeight = w->treeHeight;
 	out->movedCount = w->hostMail[MAIL_MOVED];
 	out->pairPassCount = w->pairPassCount;
+	out->finalizeRefits = w->finalizeRefits;
 	out->kernelLaunches = w->kernelLaunches;
 	out->graphReplays = w->scratch != nullptr ? w->scratch->graphReplays : 0;
 	out->graphCaptures = w->scratch != nullptr ? w->scratch->graphCaptures : 0;

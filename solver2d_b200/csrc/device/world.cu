@@ -431,6 +431,11 @@ extern "C" s2bWorld* s2b_world_create(int cudaDevice, int solverType)
 		{
 			w->blockWarmBytes = atoi(env) < 0 ? 0 : atoi(env);
 		}
+		env = getenv("S2B_FINALIZE_REFIT");
+		if (env != nullptr)
+		{
+			w->fusedRefit = atoi(env) != 0 ? 1 : 0;
+		}
 	}
 	w->solverType = solverType;
 	w->sticky = (solverType == 6); // s2_solverTGS_Sticky

@@ -21,9 +21,11 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
 # kernels of a pair-search pass, in launch order; the cub kernels of the Morton sort and the leaf selection run between
-# s2bFlagValidShapes and the tree build
-SEARCH_PREFIXES = ("s2bFlagValidShapes", "s2bSceneBounds", "s2bMortonCodes", "s2bBuildRadixTree", "s2bBuildWide", "s2bRefit",
-                   "s2bBuildPairHash", "s2bCollectMovers", "s2bFindPairsLarge", "s2bFindPairs", "s2bCollectKeptContacts")
+# s2bFlagValidShapes and the tree build. On a pass that reuses the hierarchy, the refit and the moved proxies ran inside
+# finalize (s2bFinalizeRefitKernel, which also finalizes the shapes); the query launch s2bFindPairs also holds the survivor
+# and large-mover scans.
+SEARCH_PREFIXES = ("s2bFlagValidShapes", "s2bSceneBounds", "s2bMortonCodes", "s2bBuildRadixTree", "s2bBuildWide",
+                   "s2bFinalizeRefitKernel", "s2bRefit", "s2bBuildPairHash", "s2bCollectMovers", "s2bFindPairs")
 
 
 def _short(name: str) -> str:
@@ -35,14 +37,14 @@ def _short(name: str) -> str:
 
 def collect_passes(kernels):
     """kernels: [(start_us, end_us, name)] sorted by start. A pass opens at s2bFlagValidShapes (rebuild) or at a refit
-    kernel that is not preceded by a build in the same pass, and closes at s2bCollectKeptContacts."""
+    kernel (s2bRefit, s2bFinalizeRefitKernel) that is not preceded by a build in the same pass, and closes at s2bFindPairs."""
     passes, cur, in_build = [], None, False
     for t0, t1, name in kernels:
         short = _short(name)
         if short == "s2bFlagValidShapes":
             cur = {"kernels": [], "rebuild": True, "t0": t0}
             in_build = True
-        elif short == "s2bRefit" and (cur is None or not in_build):
+        elif short in ("s2bRefit", "s2bFinalizeRefitKernel") and (cur is None or not in_build):
             cur = {"kernels": [], "rebuild": False, "t0": t0}
         if cur is None:
             continue
@@ -51,7 +53,7 @@ def collect_passes(kernels):
             cur["t1"] = t1
         if short.startswith("s2bRefit"):
             in_build = False
-        if short == "s2bCollectKeptContacts":
+        if short == "s2bFindPairs":
             passes.append(cur)
             cur = None
     return passes
@@ -74,8 +76,8 @@ def report(passes, label):
           f"first-to-last kernel span {np.mean(span):7.1f} us")
     for k, v in sorted(per.items(), key=lambda kv: -np.mean(kv[1])):
         print(f"    {k:40s} {np.mean(v):7.2f} us  (min {min(v):6.2f} max {max(v):6.2f}, in {len(v)} passes)")
-    tree = sum(np.mean(per.get(k, [0.0])) for k in ("s2bRefit", "s2bFindPairs"))
-    print(f"    refit + tree queries (s2bRefit* + s2bFindPairs): {tree:.1f} us per pass")
+    tree = sum(np.mean(per.get(k, [0.0])) for k in ("s2bRefit", "s2bFinalizeRefitKernel", "s2bFindPairs"))
+    print(f"    refit + queries (s2bRefit or s2bFinalizeRefitKernel, which finalizes the shapes too, + s2bFindPairs): {tree:.1f} us per pass")
 
 
 def main():

@@ -5,9 +5,10 @@
 Scenes and step parameters are those of tools/pair_search_probe.py (TGS_Soft, dt = 1/60, 4 sub-steps, 2 relax
 iterations). After the warm-up the steps are recorded under torch.profiler (CUDA activities). Every window that opens at
 the end of an s2bPersistentSolveT launch and closes at the start of the next s2bUpdateContactsKernel launch holds
-finalize (s2bFinalizeBodies, s2bFinalizeShapes, the moved-counter copy), the pair search queued behind it for the next
-step (refit, movers, the tree walk and the pair rules, survivors, the mailbox copy) and the commit of that search at the
-start of the next step (merge, s2bClearMovedFlags). For each kernel, copy and memset the script prints its mean device
+finalize (s2bFinalizeBodies, then s2bFinalizeShapes or, on a pass that reuses the hierarchy, s2bFinalizeRefitKernel, which
+also refits and collects the moved proxies; the moved-counter copy), the pair search queued behind it for the next step
+(refit and movers where finalize did not do them, then one s2bFindPairs launch: the tree walk and the pair rules, survivors,
+large movers; the mailbox copy) and the commit of that search at the start of the next step (merge, s2bClearMovedFlags). For each kernel, copy and memset the script prints its mean device
 time per window and the mean idle gap in front of it; the gap in front of the first event of the next step includes the
 host's per-step synchronisation and the counter read-back of this script. Also printed: the mean moved-proxy count per
 step, the pair passes and the contact count.
