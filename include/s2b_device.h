@@ -215,6 +215,10 @@ typedef struct s2bCounters
 	int32_t residentRegions;	 // 1: the last solve ran its regions with their bodies in shared memory (TGS_Soft, DESIGN.md §3.1)
 	int32_t maxRegionBodies;	 // bodies in the largest region of the last schedule (static bodies a region owns included), 0 = no regions
 	int32_t finalizeRefits;		 // pair passes so far whose refit and moved proxies ran inside the finalize before them (DESIGN.md §3.3)
+	int32_t pairRetries;		 // pair searches so far whose candidate pairs overflowed the pair buffer and were run again
+	int32_t prefetchRetries;	 // the part of pairRetries whose overflowing search was started behind the previous step
+	int32_t largeMovers;		 // moved proxies with scene-sized boxes in the last committed pass, before the cap of 64 (DESIGN.md §3.3)
+	int32_t treeBuilds;			 // pair-search hierarchies built from scratch so far (the others were refitted)
 } s2bCounters;
 
 // ---- lifecycle ------------------------------------------------------------------------------------------------

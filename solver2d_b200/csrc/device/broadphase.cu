@@ -1174,7 +1174,7 @@ static size_t bpReserve(s2bWorld* w, BroadScratch* B)
 	B->keepSlots.reserve((size_t)std::max(oldCount, 1), st, false);
 	if (B->newPairCap == 0)
 	{
-		B->newPairCap = 8 * shapeCap + 1024;
+		B->newPairCap = w->pairBuffer > 0 ? w->pairBuffer : 8 * shapeCap + 1024;
 	}
 	size_t need = 0, tempBytes = 0;
 	cub::DeviceSelect::Flagged(nullptr, need, thrust::counting_iterator<int>(0), (int*)nullptr, (int*)nullptr, (int*)nullptr,
@@ -1230,6 +1230,7 @@ static void bpTree(s2bWorld* w, BroadScratch* B, bool reuseTree)
 		B->treeValid = true;
 		B->treeShapeCap = shapeCap;
 		B->treeReuses = 0;
+		w->treeBuilds += 1;
 	}
 
 	// ---- refit ----
@@ -1500,11 +1501,14 @@ void s2bBroadphaseUpdatePairs(s2bWorld* w)
 			if (fresh <= B->newPairCap)
 			{
 				w->treeHeight = hc[BC_HEIGHT];
+				w->largeMovers = hc[BC_LARGE];
 				B->lastPassRan = hc[BC_MOVED] > 0 || hc[BC_LARGE] > 0;
 				bpCommit(w, B, fresh, kept, B->prefetchTempBytes);
 				return;
 			}
 			B->newPairCap = fresh + fresh / 2 + 1024; // rare: redo the pass below with a larger pair buffer
+			w->pairRetries += 1;
+			w->prefetchRetries += 1;
 		}
 		// (something was uploaded since: the search is stale — e.g. new shapes — and is redone)
 	}
@@ -1545,9 +1549,11 @@ void s2bBroadphaseUpdatePairs(s2bWorld* w)
 		if (fresh > B->newPairCap)
 		{
 			B->newPairCap = fresh + fresh / 2 + 1024;
+			w->pairRetries += 1;
 			continue; // rare: redo the pass with a larger pair buffer
 		}
 		w->treeHeight = hc[BC_HEIGHT];
+		w->largeMovers = hc[BC_LARGE];
 		bpCommit(w, B, fresh, kept, tempBytes);
 		break;
 	}

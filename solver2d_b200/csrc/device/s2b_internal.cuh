@@ -410,6 +410,11 @@ struct s2bWorld
 	DevArray<int> dMovedFlag; // [0] = number of proxies moved in last finalize (device counter)
 	int pairPassCount = 0;
 	int finalizeRefits = 0; // pair passes whose refit and moved proxies came from finalize (s2bFinalizeRefit)
+	int pairRetries = 0;	// pair searches run again because their candidate pairs overflowed the pair buffer
+	int prefetchRetries = 0; // ... of which the overflowing search was the prefetched one
+	int largeMovers = 0;	// BC_LARGE of the last committed pass (uncapped)
+	int treeBuilds = 0;		// pair-search hierarchies built from scratch
+	int pairBuffer = 0;		// initial candidate-pair capacity; 0 = 8 per shape slot + 1024 (S2B_PAIR_BUFFER)
 	int treeHeight = 0;
 
 	// solve-order hint (validation)

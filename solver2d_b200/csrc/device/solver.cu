@@ -4164,6 +4164,10 @@ extern "C" void s2b_get_counters(s2bWorld* w, s2bCounters* out)
 	out->movedCount = w->hostMail[MAIL_MOVED];
 	out->pairPassCount = w->pairPassCount;
 	out->finalizeRefits = w->finalizeRefits;
+	out->pairRetries = w->pairRetries;
+	out->prefetchRetries = w->prefetchRetries;
+	out->largeMovers = w->largeMovers;
+	out->treeBuilds = w->treeBuilds;
 	out->kernelLaunches = w->kernelLaunches;
 	out->graphReplays = w->scratch != nullptr ? w->scratch->graphReplays : 0;
 	out->graphCaptures = w->scratch != nullptr ? w->scratch->graphCaptures : 0;

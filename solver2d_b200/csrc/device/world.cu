@@ -436,6 +436,11 @@ extern "C" s2bWorld* s2b_world_create(int cudaDevice, int solverType)
 		{
 			w->fusedRefit = atoi(env) != 0 ? 1 : 0;
 		}
+		env = getenv("S2B_PAIR_BUFFER");
+		if (env != nullptr)
+		{
+			w->pairBuffer = atoi(env) < 0 ? 0 : atoi(env);
+		}
 	}
 	w->solverType = solverType;
 	w->sticky = (solverType == 6); // s2_solverTGS_Sticky

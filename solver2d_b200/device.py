@@ -65,7 +65,8 @@ class Counters(C.Structure):
                 ("neighbourSync", C.c_int32), ("narrowphaseRowSteps", C.c_int32),
                 ("firstTable", C.c_int32), ("continuousShapes", C.c_int32), ("continuousHits", C.c_int32),
                 ("bulletShapes", C.c_int32), ("bulletHits", C.c_int32), ("residentRegions", C.c_int32),
-                ("maxRegionBodies", C.c_int32), ("finalizeRefits", C.c_int32)]
+                ("maxRegionBodies", C.c_int32), ("finalizeRefits", C.c_int32), ("pairRetries", C.c_int32),
+                ("prefetchRetries", C.c_int32), ("largeMovers", C.c_int32), ("treeBuilds", C.c_int32)]
 
 
 SCHEDULE_COLOR, SCHEDULE_WAVEFRONT = 0, 1
