@@ -135,6 +135,9 @@ typedef struct s2bJointRow
 	// hertz the maximum force (N) and dampingRatio the correction factor; impulse[2] is the linear impulse and
 	// motorImpulse the angular impulse. Its limit impulses stay 0.
 	float localAxisA[2];
+	// break thresholds (N, N-m) of the reaction pass (DESIGN.md §3.13); 0 = none. A row with either set is checked after every
+	// finalize; a row without them is never checked.
+	float breakForce, breakTorque;
 } s2bJointRow;
 
 // One contact (shape pair) with its persistent manifold; mirrors s2Contact + s2Manifold + s2DistanceCache
@@ -219,6 +222,8 @@ typedef struct s2bCounters
 	int32_t prefetchRetries;	 // the part of pairRetries whose overflowing search was started behind the previous step
 	int32_t largeMovers;		 // moved proxies with scene-sized boxes in the last committed pass, before the cap of 64 (DESIGN.md §3.3)
 	int32_t treeBuilds;			 // pair-search hierarchies built from scratch so far (the others were refitted)
+	int32_t jointsChecked;		 // joint slots the last step's reaction pass checked against their thresholds (0: it did not run)
+	int32_t jointsBroken;		 // joints over a threshold at the end of the last step (s2b_download_broken_joints)
 } s2bCounters;
 
 // ---- lifecycle ------------------------------------------------------------------------------------------------
@@ -327,6 +332,17 @@ S2B_API void s2b_prefetch_pairs(s2bWorld* world);
 S2B_API void s2b_step(s2bWorld* world, int solverType, const s2bStepContext* context);
 
 // ---- device -> host (synchronising) ---------------------------------------------------------------------------
+
+// Joint reactions (DESIGN.md §3.13). While at least one live joint row has breakForce or breakTorque set, s2b_finalize ends
+// with the reaction pass: every joint's force and torque on body B (s2MakeJointReaction in include/solver2d_b200.h, at the
+// rate of the last s2b_solve) compared with its thresholds, and the joints over one listed. Breaking is only reported here:
+// a caller of s2b_step removes a broken joint itself (the host library does it at the start of the next s2World_Step).
+// s2b_download_joint_reactions runs the same pass without the test: {fx, fy, torque} of joint slots [0, capacity) into
+// out[3 * capacity], zero for free slots. Synchronises.
+S2B_API void s2b_download_joint_reactions(s2bWorld* world, float* out, int capacity);
+// The joint slots over a threshold at the end of the last step, ascending; returns their count and writes at most `capacity`.
+// Zero when the last step had no thresholds to check. Synchronises.
+S2B_API int s2b_download_broken_joints(s2bWorld* world, int32_t* slots, int capacity);
 
 S2B_API void s2b_sync(s2bWorld* world);
 // The CUDA stream (cudaStream_t, returned as an opaque pointer) every operation of this world is enqueued on: lets a

@@ -138,6 +138,76 @@ S2B_API s2Vec2 s2MotorJoint_GetConstraintForce(s2JointId jointId, float inverseT
 // The angular impulse of the last step times inverseTimeStep (N-m).
 S2B_API float s2MotorJoint_GetConstraintTorque(s2JointId jointId, float inverseTimeStep);
 
+// ---- joint reactions and breakable joints (DESIGN.md §3.13) --------------------------------------------------------
+
+// What a joint exerts on body B over the last step: force (N, world frame) and torque (N-m).
+typedef struct s2JointReaction
+{
+	s2Vec2 force;
+	float torque;
+} s2JointReaction;
+
+// The one definition of a joint's reaction, used by the device's reaction pass, the host getters and the tests. `type` is
+// an S2B_JOINT_* value; the impulses are the columns of s2bJointRow; qA is body A's rotation at the end of the step (only the
+// prismatic joint reads it, with localAxisA). `rate` is 1 / (the interval the solver variant accumulates the impulses over):
+// 1 / dt under TGS_Sticky, 1 / h under every other variant (h = dt for the variants that do not sub-step).
+//   revolute   force = rate impulse    torque = rate (motorImpulse + lowerImpulse - upperImpulse)
+//   mouse, weld, motor                 force = rate impulse    torque = rate motorImpulse
+//   prismatic  force = rate (impulse.x perp + (motorImpulse + lowerImpulse - upperImpulse) axis), torque = rate impulse.y,
+//              axis = qA localAxisA, perp = leftPerp(axis)
+// Every operation is a separate float32 rounding, so the host and the device (built without contraction) agree bit for bit.
+S2_INLINE s2JointReaction s2MakeJointReaction(int32_t type, s2Vec2 impulse, float motorImpulse, float lowerImpulse,
+											  float upperImpulse, s2Rot qA, s2Vec2 localAxisA, float rate)
+{
+	s2JointReaction r;
+	s2Vec2 f = impulse;
+	float t = motorImpulse;
+	if (type == S2B_JOINT_REVOLUTE)
+	{
+		t = motorImpulse + lowerImpulse - upperImpulse;
+	}
+	else if (type == S2B_JOINT_PRISMATIC)
+	{
+		s2Vec2 axis = s2RotateVector(qA, localAxisA);
+		s2Vec2 perp = s2LeftPerp(axis);
+		float axial = motorImpulse + lowerImpulse - upperImpulse;
+		f.x = impulse.x * perp.x + axial * axis.x;
+		f.y = impulse.x * perp.y + axial * axis.y;
+		t = impulse.y;
+	}
+	r.force.x = rate * f.x;
+	r.force.y = rate * f.y;
+	r.torque = rate * t;
+	return r;
+}
+
+// s2MakeJointReaction as an exported host function, for bindings and CPU tests that evaluate oracle rows with the same
+// arithmetic.
+S2B_API s2JointReaction s2ComputeJointReaction(int32_t type, s2Vec2 impulse, float motorImpulse, float lowerImpulse,
+											   float upperImpulse, s2Rot qA, s2Vec2 localAxisA, float rate);
+
+// The reaction of the last s2World_Step (zero before the first step), from the same impulses and rate the break test used.
+// Every joint type. XPBD keeps no impulses for its revolute, weld, prismatic and motor rows, so they read zero under XPBD.
+// Under XPBD a mouse joint reads its running impulse (carried across steps without a warm start or reset) times 1 / h:
+// not a measured load, since XPBD's mouse joint does not hold a load at rest (DESIGN.md §3.13).
+S2B_API s2Vec2 s2Joint_GetReactionForce(s2JointId jointId);
+S2B_API float s2Joint_GetReactionTorque(s2JointId jointId);
+// Break thresholds (default: none). A positive finite value sets one, 0 removes it, a negative or NaN value is ignored (the
+// joint keeps its value). A joint breaks when |force| > breakForce or |torque| > breakTorque, each test applying only when
+// its threshold is set. A joint that exceeds a threshold at the end of a step acted in that step; the next s2World_Step
+// destroys it, exactly as s2DestroyJoint, before it pushes edits to the device. Until then it exists, its getters report the
+// load that broke it, and it may be destroyed by the caller.
+S2B_API void s2Joint_SetBreakForce(s2JointId jointId, float breakForce);
+S2B_API float s2Joint_GetBreakForce(s2JointId jointId);
+S2B_API void s2Joint_SetBreakTorque(s2JointId jointId, float breakTorque);
+S2B_API float s2Joint_GetBreakTorque(s2JointId jointId);
+// The joints that went over a threshold in the last step, in slot order, with the ids they had then. Returns the count and
+// writes at most `capacity` ids.
+S2B_API int32_t s2World_GetBrokenJoints(s2WorldId worldId, s2JointId* out, int32_t capacity);
+// Bulk s2Joint_GetReactionForce + _GetReactionTorque, computed on the device: {fx, fy, torque} for joint slots
+// [0, min(capacity, joint capacity)) into out[3 * capacity]; free slots read zero. Returns the joint capacity.
+S2B_API int32_t s2World_GetJointReactions(s2WorldId worldId, float* out, int32_t capacity);
+
 // Continuous collision of dynamic bodies against static shapes (default off: collision is discrete, as in the reference).
 // When on, a dynamic body that moved more than half its smallest inner extent in a step is swept from its pose at the
 // start of the step to its pose at the end against the static shapes its shapes may collide with, and stopped at the

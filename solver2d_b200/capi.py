@@ -442,6 +442,26 @@ _API.update({
     "s2Body_IsBullet": (C.c_bool, [BodyId]),
 })
 
+class JointReaction(C.Structure):
+    """s2JointReaction (include/solver2d_b200.h): force on body B (N, world frame) and torque on B (N-m)."""
+    _fields_ = [("force", Vec2), ("torque", C.c_float)]
+
+
+# breakable joints (include/solver2d_b200.h, DESIGN.md §3.13): extensions, absent from the reference
+_API.update({
+    "s2ComputeJointReaction": (JointReaction, [C.c_int32, Vec2, C.c_float, C.c_float, C.c_float, Rot, Vec2, C.c_float]),
+    "s2Joint_GetReactionForce": (Vec2, [JointId]),
+    "s2Joint_GetReactionTorque": (C.c_float, [JointId]),
+    "s2Joint_SetBreakForce": (None, [JointId, C.c_float]),
+    "s2Joint_GetBreakForce": (C.c_float, [JointId]),
+    "s2Joint_SetBreakTorque": (None, [JointId, C.c_float]),
+    "s2Joint_GetBreakTorque": (C.c_float, [JointId]),
+    # out (s2JointId per entry), capacity; returns the count
+    "s2World_GetBrokenJoints": (C.c_int32, [WorldId, C.c_void_p, C.c_int32]),
+    # out (fx, fy, torque per slot), capacity; returns the joint capacity
+    "s2World_GetJointReactions": (C.c_int32, [WorldId, C.c_void_p, C.c_int32]),
+})
+
 QUERY_CALLBACK = C.CFUNCTYPE(C.c_bool, ShapeId, C.c_void_p)
 
 

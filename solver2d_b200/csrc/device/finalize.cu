@@ -126,4 +126,15 @@ void s2bFinalize(s2bWorld* w)
 	}
 	S2B_CHECK(cudaMemcpyAsync(w->hostMail + MAIL_MOVED, w->dMovedFlag.p, sizeof(int), cudaMemcpyDeviceToHost, cs));
 	S2B_CHECK(cudaEventRecord(w->movedEvent, cs));
+	// joint reactions against their break thresholds, on the impulses just solved and the final poses; a world without
+	// thresholds launches nothing here (DESIGN.md §3.13)
+	if (w->breakCount > 0 && w->jointCap > 0)
+	{
+		s2bJointBreakPass(w, cs);
+	}
+	else
+	{
+		w->brokenPending = false;
+		w->jointsChecked = 0;
+	}
 }

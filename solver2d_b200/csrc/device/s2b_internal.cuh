@@ -362,6 +362,20 @@ struct s2bWorld
 	DevArray<int4> jHead;
 	DevArray<float4> jAnchors, jLim, jMotor, jTarget, jImp, jLimp;
 	DevArray<int> jColor;
+	// breakForce breakTorque per joint slot (0 = no threshold). Kept out of JointView, which SolveArgs carries into every solver
+	// kernel: only the scatter, the gather and the reaction pass read it
+	DevArray<float2> jBreak;
+	// per joint slot: the last uploaded row was valid and had a threshold; the reaction pass runs after finalize only while
+	// breakCount > 0, so a world without thresholds launches nothing for it (DESIGN.md §3.13)
+	std::vector<uint8_t> breakSlot;
+	int breakCount = 0;
+	float reactionRate = 0.0f; // 1 / the interval the last s2b_solve accumulated joint impulses over (s2MakeJointReaction)
+	DevArray<int> dBroken;	   // [0] count, then the slots over a threshold (device order)
+	int* hostBroken = nullptr; // pinned copy of dBroken, jointCap + 1 ints
+	int hostBrokenCap = 0;
+	cudaEvent_t brokenEvent = nullptr; // recorded behind the copy into hostBroken
+	bool brokenPending = false;		   // the last finalize ran the pass: hostBroken is valid once brokenEvent has passed
+	int jointsChecked = 0;			   // slots the last finalize's pass checked (0: it did not run)
 	DevArray<unsigned long long> jointPairKeys; // every jointed body pair: blocks new contacts
 	int jointPairCount = 0;
 	DevArray<unsigned long long> jointDestroyKeys; // pairs whose existing contacts are removed
@@ -545,5 +559,7 @@ void s2bRefinalizeBulletShapes(s2bWorld* w, const int* list, const int* count, c
 // (broadphase.cu) finalize's shapes, the refit and the moved proxies of the next pair search in one launch, when that search
 // will reuse the hierarchy's topology; false: nothing launched, finalize runs s2bFinalizeShapes (DESIGN.md §3.3)
 bool s2bFinalizeRefit(s2bWorld* w);
+// (reactions.cu, DESIGN.md §3.13) the reaction pass at the end of finalize, when some joint has a threshold
+void s2bJointBreakPass(s2bWorld* w, cudaStream_t copyStream);
 // [0] continuousShapes [1] continuousHits [2] bulletShapes [3] bulletHits of the last step
 void s2bContinuousCounters(s2bWorld* w, int out[4]);

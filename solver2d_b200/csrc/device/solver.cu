@@ -4168,6 +4168,12 @@ extern "C" void s2b_get_counters(s2bWorld* w, s2bCounters* out)
 	out->prefetchRetries = w->prefetchRetries;
 	out->largeMovers = w->largeMovers;
 	out->treeBuilds = w->treeBuilds;
+	out->jointsChecked = w->jointsChecked;
+	if (w->brokenPending)
+	{
+		S2B_CHECK(cudaEventSynchronize(w->brokenEvent)); // the broken list's copy (s2bJointBreakPass)
+		out->jointsBroken = w->hostBroken[0];
+	}
 	out->kernelLaunches = w->kernelLaunches;
 	out->graphReplays = w->scratch != nullptr ? w->scratch->graphReplays : 0;
 	out->graphCaptures = w->scratch != nullptr ? w->scratch->graphCaptures : 0;

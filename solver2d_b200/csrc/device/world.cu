@@ -72,7 +72,7 @@ __global__ void s2bScatterShapes(const s2bShapeRow* __restrict__ rows, int count
 	}
 }
 
-__global__ void s2bScatterJoints(const s2bJointRow* __restrict__ rows, int count, JointView j, int* schedDirty)
+__global__ void s2bScatterJoints(const s2bJointRow* __restrict__ rows, int count, JointView j, float2* brk, int* schedDirty)
 {
 	int t = blockIdx.x * blockDim.x + threadIdx.x;
 	if (t >= count)
@@ -99,6 +99,7 @@ __global__ void s2bScatterJoints(const s2bJointRow* __restrict__ rows, int count
 	j.target[i] = make_float4(r->target[0], r->target[1], r->localAxisA[0], r->localAxisA[1]);
 	j.imp[i] = make_float4(r->impulse[0], r->impulse[1], r->motorImpulse, 0.0f);
 	j.limp[i] = make_float4(r->lowerImpulse, r->upperImpulse, 0.0f, 0.0f);
+	brk[i] = make_float2(r->breakForce, r->breakTorque);
 }
 
 __device__ __forceinline__ int s2bPackCache(const s2bContactRow* r)
@@ -190,7 +191,7 @@ __global__ void s2bGatherBodies(s2bBodyRow* rows, int count, BodyView b, const f
 	rows[t] = r;
 }
 
-__global__ void s2bGatherJoints(s2bJointRow* rows, int count, JointView j)
+__global__ void s2bGatherJoints(s2bJointRow* rows, int count, JointView j, const float2* brk)
 {
 	int i = blockIdx.x * blockDim.x + threadIdx.x;
 	if (i >= count)
@@ -224,6 +225,9 @@ __global__ void s2bGatherJoints(s2bJointRow* rows, int count, JointView j)
 	r.motorImpulse = imp.z;
 	r.lowerImpulse = limp.x;
 	r.upperImpulse = limp.y;
+	float2 b = brk[i];
+	r.breakForce = b.x;
+	r.breakTorque = b.y;
 	rows[i] = r;
 }
 
@@ -498,6 +502,12 @@ extern "C" void s2b_world_destroy(s2bWorld* w)
 	w->jImp.release();
 	w->jLimp.release();
 	w->jColor.release();
+	w->jBreak.release();
+	w->dBroken.release();
+	if (w->brokenEvent != nullptr)
+	{
+		cudaEventDestroy(w->brokenEvent);
+	}
 	w->jointPairKeys.release();
 	w->jointDestroyKeys.release();
 	w->dState.release();
@@ -551,6 +561,10 @@ extern "C" void s2b_world_destroy(s2bWorld* w)
 	w->dXf.release();
 	cudaFreeHost(w->hostMail);
 	cudaFree(w->devMail);
+	if (w->hostBroken != nullptr)
+	{
+		cudaFreeHost(w->hostBroken);
+	}
 	for (int i = 0; i < 5; ++i)
 	{
 		cudaEventDestroy(w->timer.ev[i]);
@@ -675,6 +689,7 @@ static void reserveJoints(s2bWorld* w, int cap)
 	w->jImp.reserve(cap, s);
 	w->jLimp.reserve(cap, s);
 	w->jColor.reserve(cap, s);
+	w->jBreak.reserve(cap, s);
 	w->jointCap = (int)w->jHead.cap;
 }
 
@@ -734,8 +749,20 @@ extern "C" void s2b_upload_joints(s2bWorld* w, const s2bJointRow* rows, int coun
 		return;
 	}
 	w->uploadEpoch += 1; // rows changed: a pair search started behind the previous step is stale now
+	// rows with a break threshold per slot, so that a world without one adds no launch to its steps (s2bFinalize)
+	if (w->breakSlot.size() < (size_t)w->jointCap)
+	{
+		w->breakSlot.resize((size_t)w->jointCap, 0);
+	}
+	for (int t = 0; t < count; ++t)
+	{
+		uint8_t has = (rows[t].flags & S2B_ROW_VALID) != 0 && (rows[t].breakForce > 0.0f || rows[t].breakTorque > 0.0f);
+		uint8_t& slot = w->breakSlot[(size_t)rows[t].index];
+		w->breakCount += (int)has - (int)slot;
+		slot = has;
+	}
 	s2bJointRow* d = (s2bJointRow*)stageRows(w, rows, sizeof(s2bJointRow) * (size_t)count);
-	S2B_LAUNCH(w, s2bScatterJoints, gridFor(count, 128), 128, 0, d, count, jointView(w), w->schedDirty.p);
+	S2B_LAUNCH(w, s2bScatterJoints, gridFor(count, 128), 128, 0, d, count, jointView(w), w->jBreak.p, w->schedDirty.p);
 	S2B_CHECK(cudaFreeAsync(d, w->stream));
 	S2B_CHECK(cudaStreamSynchronize(w->stream));
 }
@@ -1176,7 +1203,7 @@ extern "C" void s2b_download_joints(s2bWorld* w, s2bJointRow* rows, int capacity
 	}
 	s2bJointRow* d = nullptr;
 	S2B_CHECK(cudaMallocAsync((void**)&d, sizeof(s2bJointRow) * (size_t)capacity, w->stream));
-	S2B_LAUNCH(w, s2bGatherJoints, gridFor(capacity, 128), 128, 0, d, capacity, jointView(w));
+	S2B_LAUNCH(w, s2bGatherJoints, gridFor(capacity, 128), 128, 0, d, capacity, jointView(w), w->jBreak.p);
 	S2B_CHECK(cudaMemcpyAsync(rows, d, sizeof(s2bJointRow) * (size_t)capacity, cudaMemcpyDeviceToHost, w->stream));
 	S2B_CHECK(cudaFreeAsync(d, w->stream));
 	S2B_CHECK(cudaStreamSynchronize(w->stream));
@@ -1250,6 +1277,9 @@ extern "C" void s2b_solve(s2bWorld* w, int solverType, const s2bStepContext* con
 	}
 	s2bSolve(w, solverType, context);
 	s2bContinuousPass(w);
+	// TGS_Sticky prepares its joints once per step and accumulates their impulses over all sub-steps; every other variant
+	// warm starts each solver step h from the impulse, which is therefore the impulse of one step h
+	w->reactionRate = solverType == 6 ? context->inv_dt : context->inv_h; // 6: s2_solverTGS_Sticky
 }
 
 extern "C" void s2b_finalize(s2bWorld* w)

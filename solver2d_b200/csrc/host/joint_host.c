@@ -3,10 +3,12 @@
 #include "s2_host.h"
 #include "solver2d_b200.h"
 
+#include <float.h>
 #include <string.h>
 
 static s2Joint* s2AllocJoint(s2World* world, s2Body* bodyA, s2Body* bodyB)
 {
+	s2FetchBrokenJoints(world); // (the slot may be one the last step broke)
 	s2Joint* joint = (s2Joint*)s2AllocObject(&world->jointPool);
 	world->joints = (s2Joint*)world->jointPool.memory;
 	bool rowDirty = joint->rowDirty;
@@ -99,7 +101,12 @@ s2JointId s2CreateWeldJoint(s2WorldId worldId, const s2WeldJointDef* def)
 void s2DestroyJoint(s2JointId jointId)
 {
 	s2World* world = s2GetWorldFromIndex(jointId.world);
+	s2FetchBrokenJoints(world); // (the slot may be one the last step broke)
 	s2Joint* joint = world->joints + jointId.index;
+	if (joint->breakForce > 0.0f || joint->breakTorque > 0.0f)
+	{
+		world->breakableCount -= 1;
+	}
 	world->bodies[joint->bodyIndexA].jointCount -= 1;
 	world->bodies[joint->bodyIndexB].jointCount -= 1;
 	s2FreeObject(&world->jointPool, &joint->object);
@@ -366,4 +373,82 @@ float s2PrismaticJoint_GetTranslation(s2JointId jointId)
 	s2Vec2 pB = s2TransformPoint(xfB, joint->localOriginAnchorB);
 	s2Vec2 axis = s2RotateVector(bodyA->rot, joint->localAxisA);
 	return s2Dot(axis, s2Sub(pB, pA));
+}
+
+// ---- reactions and break thresholds (DESIGN.md §3.13) -----------------------------------------------------------------
+
+// s2JointType and the device's S2B_JOINT_* number the joint types alike
+_Static_assert((int)s2_revoluteJoint == S2B_JOINT_REVOLUTE && (int)s2_mouseJoint == S2B_JOINT_MOUSE &&
+				   (int)s2_weldJoint == S2B_JOINT_WELD && (int)s2_prismaticJoint == S2B_JOINT_PRISMATIC &&
+				   (int)s2_motorJoint == S2B_JOINT_MOTOR,
+			   "joint type numbering");
+
+s2JointReaction s2ComputeJointReaction(int32_t type, s2Vec2 impulse, float motorImpulse, float lowerImpulse, float upperImpulse,
+									   s2Rot qA, s2Vec2 localAxisA, float rate)
+{
+	return s2MakeJointReaction(type, impulse, motorImpulse, lowerImpulse, upperImpulse, qA, localAxisA, rate);
+}
+
+// from the lazily synced impulses and body A's rotation, at the rate of the last step: the numbers the device's pass tested
+static s2JointReaction s2GetJointReaction(s2JointId jointId)
+{
+	s2World* world = s2GetWorldFromIndex(jointId.world);
+	s2SyncStateToHost(world);
+	const s2Joint* joint = world->joints + jointId.index;
+	S2_ASSERT(s2ObjectValid(&joint->object) && joint->object.revision == jointId.revision);
+	return s2MakeJointReaction((int32_t)joint->type, joint->impulse, joint->motorImpulse, joint->lowerImpulse, joint->upperImpulse,
+							   world->bodies[joint->bodyIndexA].rot, joint->localAxisA, world->reactionRate);
+}
+
+s2Vec2 s2Joint_GetReactionForce(s2JointId jointId)
+{
+	return s2GetJointReaction(jointId).force;
+}
+
+float s2Joint_GetReactionTorque(s2JointId jointId)
+{
+	return s2GetJointReaction(jointId).torque;
+}
+
+// a positive finite threshold sets it, 0 removes it; anything else is ignored
+static void s2SetBreakThreshold(s2JointId jointId, float value, bool torque)
+{
+	if ((value >= 0.0f && value <= FLT_MAX) == false)
+	{
+		return; // rejected (negative, NaN or infinite): the joint keeps its threshold
+	}
+	s2World* world;
+	s2Joint* joint = s2GetJointForEdit(jointId, &world);
+	bool had = joint->breakForce > 0.0f || joint->breakTorque > 0.0f;
+	if (torque)
+	{
+		joint->breakTorque = value;
+	}
+	else
+	{
+		joint->breakForce = value;
+	}
+	bool has = joint->breakForce > 0.0f || joint->breakTorque > 0.0f;
+	world->breakableCount += (int32_t)has - (int32_t)had;
+	s2MarkJointDirty(world, joint);
+}
+
+void s2Joint_SetBreakForce(s2JointId jointId, float breakForce)
+{
+	s2SetBreakThreshold(jointId, breakForce, false);
+}
+
+float s2Joint_GetBreakForce(s2JointId jointId)
+{
+	return s2GetWorldFromIndex(jointId.world)->joints[jointId.index].breakForce;
+}
+
+void s2Joint_SetBreakTorque(s2JointId jointId, float breakTorque)
+{
+	s2SetBreakThreshold(jointId, breakTorque, true);
+}
+
+float s2Joint_GetBreakTorque(s2JointId jointId)
+{
+	return s2GetWorldFromIndex(jointId.world)->joints[jointId.index].breakTorque;
 }

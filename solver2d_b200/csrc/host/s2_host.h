@@ -177,6 +177,8 @@ typedef struct s2Joint
 	// accumulated impulses (cache of the device columns)
 	s2Vec2 impulse;
 	float motorImpulse, lowerImpulse, upperImpulse;
+	// break thresholds (s2Joint_SetBreakForce / _SetBreakTorque), 0 = none
+	float breakForce, breakTorque;
 
 	bool rowDirty;
 } s2Joint;
@@ -221,6 +223,14 @@ typedef struct s2World
 	// continuous collision (include/solver2d_b200.h): pushed to the device by the next flush when continuousDirty
 	bool enableContinuous;
 	bool continuousDirty;
+	// breakable joints (include/solver2d_b200.h): the rate of the last step's solve (s2MakeJointReaction), the live joints with
+	// a threshold, and the joints the last step's reaction pass found over one, fetched once per step (s2FetchBrokenJoints)
+	float reactionRate;
+	int32_t breakableCount;
+	bool brokenPending; // the last step ran the reaction pass and its list has not been fetched yet
+	s2JointId* broken;
+	int32_t* brokenSlots; // the device's list, read into this buffer (brokenCapacity entries, as broken)
+	int32_t brokenCount, brokenCapacity;
 	bool stateFresh;	 // host body / joint state mirrors the device
 	bool boxesFresh;	 // host shape AABBs mirror the device
 	uint64_t stepId;
@@ -260,6 +270,9 @@ void s2MarkBodyDirty(s2World* world, s2Body* body);
 void s2MarkBodyForceDirty(s2World* world, s2Body* body);
 void s2MarkShapeDirty(s2World* world, s2Shape* shape);
 void s2MarkJointDirty(s2World* world, s2Joint* joint);
+// the ids of the joints the last step broke, read from the device while they still name those joints: before any slot is
+// freed or reused, and before the next step destroys them
+void s2FetchBrokenJoints(s2World* world);
 void s2IndexListPush(s2IndexList* list, int32_t value);
 
 int32_t s2AllocProxyId(s2ProxyIds* ids);

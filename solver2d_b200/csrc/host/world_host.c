@@ -269,6 +269,8 @@ static void s2FillJointRow(s2bJointRow* r, const s2Joint* j)
 	r->upperImpulse = j->upperImpulse;
 	r->localAxisA[0] = j->localAxisA.x;
 	r->localAxisA[1] = j->localAxisA.y;
+	r->breakForce = j->breakForce;
+	r->breakTorque = j->breakTorque;
 }
 
 static int s2CompareU64(const void* a, const void* b)
@@ -460,6 +462,30 @@ void s2SyncStateToHost(s2World* world)
 	world->stateFresh = true;
 }
 
+void s2FetchBrokenJoints(s2World* world)
+{
+	if (world->brokenPending == false)
+	{
+		return;
+	}
+	world->brokenPending = false;
+	int32_t cap = world->jointPool.capacity;
+	if (world->brokenCapacity < cap)
+	{
+		world->brokenCapacity = cap;
+		world->broken = (s2JointId*)realloc(world->broken, sizeof(s2JointId) * (size_t)cap);
+		world->brokenSlots = (int32_t*)realloc(world->brokenSlots, sizeof(int32_t) * (size_t)cap);
+	}
+	int32_t n = s2b_download_broken_joints(world->device, world->brokenSlots, cap);
+	world->brokenCount = n < cap ? n : cap;
+	for (int32_t k = 0; k < world->brokenCount; ++k)
+	{
+		int32_t slot = world->brokenSlots[k];
+		s2JointId id = {slot, world->index, world->joints[slot].object.revision};
+		world->broken[k] = id;
+	}
+}
+
 void s2SyncBoxesToHost(s2World* world)
 {
 	if (world->boxesFresh)
@@ -556,6 +582,8 @@ void s2DestroyWorld(s2WorldId id)
 	s2IndexListFree(&world->dirtyForces);
 	s2IndexListFree(&world->dirtyShapes);
 	s2IndexListFree(&world->dirtyJoints);
+	free(world->broken);
+	free(world->brokenSlots);
 	for (int i = 0; i < s2_bodyTypeCount; ++i)
 	{
 		free(world->proxyIds[i].freeStack);
@@ -577,6 +605,20 @@ void s2World_Step(s2WorldId worldId, float timeStep, int32_t velIters, int32_t p
 {
 	s2World* world = s2GetWorldFromId(worldId);
 	world->stepId += 1;
+
+	// joints the last step found over a threshold acted in that step and are destroyed now, as s2DestroyJoint, unless the
+	// caller destroyed them first (a freed or reused slot fails the revision check)
+	s2FetchBrokenJoints(world);
+	for (int32_t k = 0; k < world->brokenCount; ++k)
+	{
+		s2JointId id = world->broken[k];
+		const s2Joint* joint = world->joints + id.index;
+		if (s2ObjectValid(&joint->object) && joint->object.revision == id.revision)
+		{
+			s2DestroyJoint(id);
+		}
+	}
+	world->brokenCount = 0;
 
 	s2FlushToDevice(world);
 
@@ -603,6 +645,9 @@ void s2World_Step(s2WorldId worldId, float timeStep, int32_t velIters, int32_t p
 	}
 	context.bodies = world->bodies;
 	context.bodyCapacity = world->bodyPool.capacity;
+	// the rate joint reactions are read at, as the device keeps it (s2b_solve): TGS_Sticky accumulates its joint impulses over
+	// the whole step, every other variant over one solver step h
+	world->reactionRate = world->solverType == s2_solverTGS_Sticky ? context.inv_dt : context.inv_h;
 
 	// solver dispatch through the per-variant entry points (reference src/world.c:206-256)
 	switch (world->solverType)
@@ -646,6 +691,8 @@ void s2World_Step(s2WorldId worldId, float timeStep, int32_t velIters, int32_t p
 	// the pair search of the NEXT step (reference src/broad_phase.c:309-367: s2UpdateBroadPhasePairs) only needs what finalize
 	// has just produced: start it now, so that the next step finds its counters waiting instead of stopping mid-pass
 	s2b_prefetch_pairs(world->device);
+	// the device ran the reaction pass behind finalize when some live joint has a threshold (its rows are all uploaded now)
+	world->brokenPending = world->breakableCount > 0;
 
 	// forces are consumed by the step (reference src/world.c:275-276)
 	world->stateFresh = false;
@@ -904,6 +951,30 @@ int32_t s2World_GetBodyTransforms(s2WorldId worldId, float* out, int32_t capacit
 	int32_t n = world->bodyHighWater < capacity ? world->bodyHighWater : capacity;
 	s2b_download_transforms(world->device, out, n);
 	return world->bodyPool.capacity;
+}
+
+int32_t s2World_GetBrokenJoints(s2WorldId worldId, s2JointId* out, int32_t capacity)
+{
+	s2World* world = s2GetWorldFromId(worldId);
+	s2FetchBrokenJoints(world);
+	for (int32_t k = 0; k < world->brokenCount && k < capacity; ++k)
+	{
+		out[k] = world->broken[k];
+	}
+	return world->brokenCount;
+}
+
+int32_t s2World_GetJointReactions(s2WorldId worldId, float* out, int32_t capacity)
+{
+	// on the device, from the same columns and rate as the reaction pass; rows edited since the last step are pushed first so
+	// that the bulk read agrees with the per-joint getters
+	s2World* world = s2GetWorldFromId(worldId);
+	if (world->dirtyJoints.count > 0 || world->dirtyBodies.count > 0)
+	{
+		s2FlushToDevice(world);
+	}
+	s2b_download_joint_reactions(world->device, out, capacity);
+	return world->jointPool.capacity;
 }
 
 float s2Atan2Device(float y, float x)

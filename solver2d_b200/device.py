@@ -33,7 +33,7 @@ JOINT_ROW = np.dtype([
     ("localOriginAnchorB", "<f4", 2), ("referenceAngle", "<f4"), ("lowerAngle", "<f4"), ("upperAngle", "<f4"),
     ("maxMotorTorque", "<f4"), ("motorSpeed", "<f4"), ("hertz", "<f4"), ("dampingRatio", "<f4"), ("target", "<f4", 2),
     ("impulse", "<f4", 2), ("motorImpulse", "<f4"), ("lowerImpulse", "<f4"), ("upperImpulse", "<f4"),
-    ("localAxisA", "<f4", 2),
+    ("localAxisA", "<f4", 2), ("breakForce", "<f4"), ("breakTorque", "<f4"),
 ], align=True)
 
 CONTACT_POINT = np.dtype([
@@ -66,7 +66,8 @@ class Counters(C.Structure):
                 ("firstTable", C.c_int32), ("continuousShapes", C.c_int32), ("continuousHits", C.c_int32),
                 ("bulletShapes", C.c_int32), ("bulletHits", C.c_int32), ("residentRegions", C.c_int32),
                 ("maxRegionBodies", C.c_int32), ("finalizeRefits", C.c_int32), ("pairRetries", C.c_int32),
-                ("prefetchRetries", C.c_int32), ("largeMovers", C.c_int32), ("treeBuilds", C.c_int32)]
+                ("prefetchRetries", C.c_int32), ("largeMovers", C.c_int32), ("treeBuilds", C.c_int32),
+                ("jointsChecked", C.c_int32), ("jointsBroken", C.c_int32)]
 
 
 SCHEDULE_COLOR, SCHEDULE_WAVEFRONT = 0, 1
@@ -90,7 +91,7 @@ ABI_SYMBOLS = [
     "s2b_flush_l2", "s2b_time_color_kernel", "s2b_version", "s2b_abi_sizes", "s2b_upload_forces", "s2b_host_alloc",
     "s2b_host_free", "s2b_sync_body_state", "s2b_set_warm_gather", "s2b_eval_atan2", "s2b_set_dataflow", "s2b_set_regions", "s2b_set_graph", "s2b_get_stream", "s2b_add_forces", "s2b_download_transforms",
     "s2b_set_restitution", "s2b_download_neighbour_blocks", "s2b_download_delta_positions", "s2b_set_motor_offsets",
-    "s2b_set_continuous",
+    "s2b_set_continuous", "s2b_download_joint_reactions", "s2b_download_broken_joints",
 ]
 NSYNC_STRIDE = 17  # entries per block of s2b_download_neighbour_blocks
 
@@ -148,6 +149,9 @@ class Device:
         L.s2b_download_shape_boxes.argtypes = [vp, vp, vp, vp, C.c_int]
         L.s2b_download_delta_positions.argtypes = [vp, vp, C.c_int]
         L.s2b_download_joints.argtypes = [vp, vp, C.c_int]
+        L.s2b_download_joint_reactions.argtypes = [vp, vp, C.c_int]
+        L.s2b_download_broken_joints.restype = C.c_int
+        L.s2b_download_broken_joints.argtypes = [vp, vp, C.c_int]
         L.s2b_download_contacts.restype = C.c_int
         L.s2b_download_contacts.argtypes = [vp, vp, C.c_int]
         L.s2b_download_solve_order.restype = C.c_int
@@ -309,6 +313,21 @@ class DeviceWorld:
         rows = np.zeros(cap, dtype=JOINT_ROW)
         self.L.s2b_download_joints(self.h, rows.ctypes.data, cap)
         return rows
+
+    def download_joint_reactions(self, capacity: int | None = None) -> np.ndarray:
+        """(capacity, 3) float32 {fx, fy, torque} of every joint slot from the reaction pass (DESIGN.md §3.13); zero for
+        free slots."""
+        cap = self.joint_cap if capacity is None else capacity
+        out = np.zeros((max(cap, 1), 3), dtype=np.float32)
+        self.L.s2b_download_joint_reactions(self.h, out.ctypes.data, cap)
+        return out[:cap]
+
+    def download_broken_joints(self) -> np.ndarray:
+        """Joint slots over a break threshold at the end of the last step, ascending."""
+        n = self.L.s2b_download_broken_joints(self.h, None, 0)
+        slots = np.zeros(max(n, 1), dtype=np.int32)
+        self.L.s2b_download_broken_joints(self.h, slots.ctypes.data, n)
+        return slots[:n]
 
     def download_contacts(self, max_count: int) -> np.ndarray:
         rows = np.zeros(max(max_count, 1), dtype=CONTACT_ROW)

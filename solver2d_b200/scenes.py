@@ -1546,3 +1546,159 @@ def hub_beam(lib: capi.Solver2D, solver="TGS_Soft", pendulums=8, limits_motor=Fa
         md.dampingRatio = 0.7
         sc.joints.append(lib.s2CreateMouseJoint(world, C.byref(md)))
     return sc
+
+
+def breakables(lib: capi.Solver2D, solver="TGS_Soft", parts=("weld", "prismatic", "motor")) -> Scene:
+    """Breakable joints (DESIGN.md §3.13), about 40 bodies:
+
+    * a plank bridge: ten planks on revolute joints (collideConnected false) between two static posts, a heavy ball
+      (15.7 kg) dropped on its middle; breakForce 400 N on every bridge joint;
+    * a shelf welded to a static wall (breakTorque 25 N-m), loaded by a growing pile of boxes that rain onto it;
+    * a piston on a vertical prismatic joint, thrown up at 20 m/s into its upper limit (breakForce 200 N);
+    * a motor joint with a 500 N cap driving its box towards a pose 5 m away (breakForce 100 N: under TGS_Sticky the cap
+      holds for the whole step, so the reading is a quarter of it), and a mouse joint whose 5 Hz spring is pulled 5 m off
+      its box (breakForce 300 N);
+    * one joint of each type holding a box at rest, with thresholds it never reaches (1e6).
+
+    `parts` names the extension joint types the scene contains (the shelf, the piston and the motor joints with their
+    held boxes); the revolute and mouse joints are always there. On a library without the extensions (the reference) each weld, prismatic and motor joint is a revolute joint with the
+    same bodies, anchors and collideConnected, as in :func:`sliders` and :func:`motors`, so both libraries see the same pairs.
+    Thresholds are not applied here: ``sc.piles["break"]`` lists (index into ``sc.joints``, breakForce, breakTorque) and
+    :func:`apply_break_thresholds` sets them; ``sc.piles["never"]`` lists the indices of the joints that must hold;
+    ``sc.piles["types"]`` names the type of every joint and ``sc.piles["defs"]`` maps the index of each prismatic and motor
+    joint to its definition (dicts of s2PrismaticJointDef / s2MotorJointDef fields), so that a test can turn the stand-in
+    rows into rows of their own type."""
+    world = lib.create_world(solver)
+    sc = Scene(lib, world, name="breakables")
+    sc.piles.update({"break": [], "never": [], "types": [], "defs": {}})
+    has_ext = "s2CreateWeldJoint" not in lib.missing
+    gid = _ground(lib, world, 40.0)
+    sc.bodies.append(gid)
+    sd = default_shape_def()
+    sd.density = 1.0
+
+    def body(x, y, hx=0.5, hy=0.5, vy=0.0, radius=0.0, density=1.0, kind=capi.DYNAMIC_BODY):
+        bd = default_body_def()
+        bd.type = kind
+        bd.position = Vec2(x, y)
+        bd.linearVelocity = Vec2(0.0, vy)
+        bid = lib.s2CreateBody(world, C.byref(bd))
+        d = default_shape_def()
+        d.density = density
+        if radius > 0.0:
+            lib.s2CreateCircleShape(bid, C.byref(d), C.byref(Circle(Vec2(0.0, 0.0), radius)))
+        else:
+            lib.s2CreatePolygonShape(bid, C.byref(d), C.byref(lib.s2MakeBox(hx, hy)))
+        sc.bodies.append(bid)
+        return bid
+
+    def add(kind, jid, force=0.0, torque=0.0, never=False):
+        sc.piles["types"].append(kind)
+        if never:
+            sc.piles["never"].append(len(sc.joints))
+        sc.piles["break"].append((len(sc.joints), force, torque))
+        sc.joints.append(jid)
+
+    def revolute(a, b, anchor_a, anchor_b, collide=False):
+        jd = default_revolute_def()
+        jd.bodyIdA, jd.bodyIdB = a, b
+        jd.localAnchorA, jd.localAnchorB = Vec2(*anchor_a), Vec2(*anchor_b)
+        jd.collideConnected = collide
+        return lib.s2CreateRevoluteJoint(world, C.byref(jd))
+
+    def weld(a, b, anchor_a, anchor_b):
+        if not has_ext:
+            return revolute(a, b, anchor_a, anchor_b)
+        jd = capi.default_weld_def()
+        jd.bodyIdA, jd.bodyIdB = a, b
+        jd.localAnchorA, jd.localAnchorB = Vec2(*anchor_a), Vec2(*anchor_b)
+        return lib.s2CreateWeldJoint(world, C.byref(jd))
+
+    def prismatic(a, b, anchor_a, lower, upper):
+        sc.piles["defs"][len(sc.joints)] = dict(lowerTranslation=lower, upperTranslation=upper, localAxisA=(0.0, 1.0))
+        if not has_ext:
+            return revolute(a, b, anchor_a, (0.0, 0.0))
+        jd = capi.default_prismatic_def()
+        jd.bodyIdA, jd.bodyIdB = a, b
+        jd.localAnchorA = Vec2(*anchor_a)
+        jd.localAxisA = Vec2(0.0, 1.0)
+        jd.enableLimit = True
+        jd.lowerTranslation, jd.upperTranslation = lower, upper
+        return lib.s2CreatePrismaticJoint(world, C.byref(jd))
+
+    def motor(a, b, offset, max_force):
+        sc.piles["defs"][len(sc.joints)] = dict(linearOffset=offset, maxForce=max_force, maxTorque=max_force)
+        if not has_ext:
+            return revolute(a, b, offset, (0.0, 0.0))
+        jd = capi.default_motor_def()
+        jd.bodyIdA, jd.bodyIdB = a, b
+        jd.linearOffset = Vec2(*offset)
+        jd.maxForce, jd.maxTorque = max_force, max_force
+        return lib.s2CreateMotorJoint(world, C.byref(jd))
+
+    def mouse(b, at, target):
+        # a mouse joint is anchored where it is created: created on the box, then pulled to its target
+        jd = default_mouse_def()
+        jd.bodyIdA, jd.bodyIdB = gid, b
+        jd.target = Vec2(*at)
+        jd.hertz, jd.dampingRatio = 5.0, 0.7
+        jid = lib.s2CreateMouseJoint(world, C.byref(jd))
+        lib.s2MouseJoint_SetTarget(jid, Vec2(*target))
+        return jid
+
+    # the plank bridge between two posts: post tops at y = 4, planks 1 m long
+    left, right = body(-16.5, 2.0, 0.5, 2.0, kind=capi.STATIC_BODY), body(-5.5, 2.0, 0.5, 2.0, kind=capi.STATIC_BODY)
+    prev, prev_anchor = left, (0.5, 2.0)
+    for k in range(10):
+        plank = body(-15.5 + k, 4.0, 0.5, 0.125)
+        add("revolute", revolute(prev, plank, prev_anchor, (-0.5, 0.0)), force=400.0)
+        prev, prev_anchor = plank, (0.5, 0.0)
+    add("revolute", revolute(prev, right, prev_anchor, (-0.5, 2.0)), force=400.0)
+    body(-11.0, 9.0, radius=0.5, density=20.0)
+
+    if "weld" in parts:
+        # the welded shelf on a wall, and its pile
+        wall = body(-1.0, 3.0, 0.25, 3.0, kind=capi.STATIC_BODY)
+        shelf = body(0.75, 3.0, 1.5, 0.1)
+        add("weld", weld(wall, shelf, (0.25, 0.0), (-1.5, 0.0)), torque=25.0)
+        for k in range(6):
+            body(1.25, 4.0 + 1.5 * k, 0.3, 0.3, density=2.0)
+
+    if "prismatic" in parts:
+        # the piston: a static guide, a 1 kg block thrown up into its upper limit
+        guide = body(5.0, 1.0, 0.25, 1.0, kind=capi.STATIC_BODY)
+        block = body(6.0, 1.0, 0.5, 0.5, vy=20.0)
+        add("prismatic", prismatic(guide, block, (1.0, 0.0), -0.5, 1.5), force=200.0)
+
+    if "motor" in parts:
+        # the motor joint driving its box 5 m off
+        post = body(10.0, 1.0, 0.25, 1.0, kind=capi.STATIC_BODY)
+        driven = body(11.0, 3.0, 0.5, 0.5)
+        add("motor", motor(post, driven, (6.0, 2.0), 500.0), force=100.0)
+    # the mouse joint pulled 5 m off its box
+    pulled = body(14.0, 2.0, 0.5, 0.5)
+    add("mouse", mouse(pulled, (14.0, 2.0), (19.0, 2.0)), force=300.0)
+
+    # one joint of each type holding a box at rest, far below its thresholds
+    hanger = body(25.0, 8.0, 4.0, 0.25, kind=capi.STATIC_BODY)
+    boxes = [body(22.0 + 1.5 * k, 6.5, 0.25, 0.25) for k in range(5)]
+    add("revolute", revolute(hanger, boxes[0], (-3.0, -1.5), (0.0, 0.0)), force=1e6, torque=1e6, never=True)
+    if "weld" in parts:
+        add("weld", weld(hanger, boxes[1], (-1.5, -1.5), (0.0, 0.0)), force=1e6, torque=1e6, never=True)
+    if "prismatic" in parts:
+        add("prismatic", prismatic(hanger, boxes[2], (0.0, -1.5), -0.5, 0.5), force=1e6, torque=1e6, never=True)
+    if "motor" in parts:
+        add("motor", motor(hanger, boxes[3], (1.5, -1.5), 100.0), force=1e6, torque=1e6, never=True)
+    add("mouse", mouse(boxes[4], (28.0, 6.5), (28.0, 6.5)), force=1e6, torque=1e6, never=True)
+    return sc
+
+
+def apply_break_thresholds(sc: Scene):
+    """Sets the thresholds :func:`breakables` recorded (a library without s2Joint_SetBreakForce is left as it is)."""
+    if "s2Joint_SetBreakForce" in sc.lib.missing:
+        return
+    for index, force, torque in sc.piles["break"]:
+        if force > 0.0:
+            sc.lib.s2Joint_SetBreakForce(sc.joints[index], force)
+        if torque > 0.0:
+            sc.lib.s2Joint_SetBreakTorque(sc.joints[index], torque)
