@@ -110,6 +110,8 @@ enum
 #define S2B_JOINT_ENABLE_LIMIT 0x10
 #define S2B_JOINT_ENABLE_MOTOR 0x20
 #define S2B_JOINT_COLLIDE_CONNECTED 0x40
+// revolute and prismatic rows only: a spring on the joint's axis (DESIGN.md §3.14), stiffness hertz, damping dampingRatio
+#define S2B_JOINT_ENABLE_SPRING 0x80
 
 // One joint; mirrors s2Joint / s2RevoluteJoint / s2MouseJoint (reference src/joint.h:28-102).
 typedef struct s2bJointRow
@@ -138,6 +140,10 @@ typedef struct s2bJointRow
 	// break thresholds (N, N-m) of the reaction pass (DESIGN.md §3.13); 0 = none. A row with either set is checked after every
 	// finalize; a row without them is never checked.
 	float breakForce, breakTorque;
+	// the spring's accumulated impulse (S2B_JOINT_ENABLE_SPRING; DESIGN.md §3.14): angular for a revolute row, along the axis
+	// for a prismatic row. A revolute or prismatic row with the spring flag carries the spring's stiffness (Hz) in hertz and
+	// its damping ratio in dampingRatio.
+	float springImpulse;
 } s2bJointRow;
 
 // One contact (shape pair) with its persistent manifold; mirrors s2Contact + s2Manifold + s2DistanceCache

@@ -51,9 +51,9 @@ S2_INLINE struct s2WeldJointDef s2DefaultWeldJointDef(void)
 S2B_API s2JointId s2CreateWeldJoint(s2WorldId worldId, const s2WeldJointDef* def);
 
 // Prismatic (slider) joint: body B slides along an axis fixed in body A, keeps angle(B) - angle(A) at referenceAngle and
-// may have translation limits and a linear motor (DESIGN.md §3.9). Anchors are relative to each body's origin; the
-// translation is measured along the axis from anchor A to anchor B. Under XPBD the motor is not applied. Destroy it with
-// s2DestroyJoint.
+// may have translation limits, a linear motor (DESIGN.md §3.9) and a spring toward translation 0 (DESIGN.md §3.14). Anchors
+// are relative to each body's origin; the translation is measured along the axis from anchor A to anchor B. Under XPBD the
+// motor is not applied. Destroy it with s2DestroyJoint.
 typedef struct s2PrismaticJointDef
 {
 	s2BodyId bodyIdA;
@@ -70,6 +70,9 @@ typedef struct s2PrismaticJointDef
 	float maxMotorForce; // N
 	float drawSize;
 	bool collideConnected; // keep the contacts the two bodies already have
+	bool enableSpring;	   // a spring along the axis that pulls the translation toward 0
+	float hertz;		   // the spring's stiffness as a frequency (Hz), >= 0; 0 exerts nothing
+	float dampingRatio;	   // the spring's damping ratio, >= 0 (1 = critical)
 } s2PrismaticJointDef;
 
 S2_INLINE struct s2PrismaticJointDef s2DefaultPrismaticJointDef(void)
@@ -82,8 +85,8 @@ S2_INLINE struct s2PrismaticJointDef s2DefaultPrismaticJointDef(void)
 	return def;
 }
 
-// Returns s2_nullJointId (and creates nothing) for an axis of zero length or with a non-finite component, or for
-// lowerTranslation > upperTranslation.
+// Returns s2_nullJointId (and creates nothing) for an axis of zero length or with a non-finite component, for
+// lowerTranslation > upperTranslation, or for a negative or non-finite hertz or dampingRatio.
 S2B_API s2JointId s2CreatePrismaticJoint(s2WorldId worldId, const s2PrismaticJointDef* def);
 S2B_API void s2PrismaticJoint_EnableLimit(s2JointId jointId, bool enableLimit);
 // Ignored when lower > upper (the joint keeps its limits).
@@ -94,6 +97,18 @@ S2B_API void s2PrismaticJoint_SetMotorSpeed(s2JointId jointId, float motorSpeed)
 S2B_API float s2PrismaticJoint_GetMotorForce(s2JointId jointId, float inverseTimeStep);
 // The current translation (m) along the world axis, from anchor A to anchor B.
 S2B_API float s2PrismaticJoint_GetTranslation(s2JointId jointId);
+// The spring (DESIGN.md §3.14). A negative or non-finite hertz or damping ratio is ignored (the joint keeps its value).
+S2B_API void s2PrismaticJoint_EnableSpring(s2JointId jointId, bool enableSpring);
+S2B_API void s2PrismaticJoint_SetSpringHertz(s2JointId jointId, float hertz);
+S2B_API void s2PrismaticJoint_SetSpringDampingRatio(s2JointId jointId, float dampingRatio);
+
+// Revolute joint spring (DESIGN.md §3.14): pulls angle(B) - angle(A) toward referenceAngle with stiffness hertz (Hz) and
+// damping ratio dampingRatio, before the motor and the limits. s2RevoluteJointDef is the reference's and has no spring
+// fields: a revolute joint starts without a spring (hertz 0, damping ratio 0). A negative or non-finite hertz or damping
+// ratio is ignored (the joint keeps its value). A spring on a joint whose two rotations are fixed exerts nothing.
+S2B_API void s2RevoluteJoint_EnableSpring(s2JointId jointId, bool enableSpring);
+S2B_API void s2RevoluteJoint_SetSpringHertz(s2JointId jointId, float hertz);
+S2B_API void s2RevoluteJoint_SetSpringDampingRatio(s2JointId jointId, float dampingRatio);
 
 // Motor joint: drives body B toward a pose relative to body A with bounded effort (DESIGN.md §3.10). Each solver step h it
 // removes the fraction correctionFactor of the pose error, with an impulse of at most h * maxForce (linear) and
@@ -151,6 +166,9 @@ typedef struct s2JointReaction
 // an S2B_JOINT_* value; the impulses are the columns of s2bJointRow; qA is body A's rotation at the end of the step (only the
 // prismatic joint reads it, with localAxisA). `rate` is 1 / (the interval the solver variant accumulates the impulses over):
 // 1 / dt under TGS_Sticky, 1 / h under every other variant (h = dt for the variants that do not sub-step).
+// A revolute or prismatic joint with its spring enabled passes motorImpulse + springImpulse as `motorImpulse` (the spring
+// acts on the same axis: the revolute's torque, the prismatic's axial force), so its reaction and break test include the
+// spring's load; every other joint passes motorImpulse.
 //   revolute   force = rate impulse    torque = rate (motorImpulse + lowerImpulse - upperImpulse)
 //   mouse, weld, motor                 force = rate impulse    torque = rate motorImpulse
 //   prismatic  force = rate (impulse.x perp + (motorImpulse + lowerImpulse - upperImpulse) axis), torque = rate impulse.y,

@@ -169,6 +169,9 @@ class PrismaticJointDef(C.Structure):
         ("maxMotorForce", C.c_float),
         ("drawSize", C.c_float),
         ("collideConnected", C.c_bool),
+        ("enableSpring", C.c_bool),
+        ("hertz", C.c_float),
+        ("dampingRatio", C.c_float),
     ]
 
 
@@ -334,6 +337,13 @@ _API = {
     "s2PrismaticJoint_SetMotorSpeed": (None, [JointId, C.c_float]),
     "s2PrismaticJoint_GetMotorForce": (C.c_float, [JointId, C.c_float]),
     "s2PrismaticJoint_GetTranslation": (C.c_float, [JointId]),
+    # joint springs (DESIGN.md §3.14)
+    "s2PrismaticJoint_EnableSpring": (None, [JointId, C.c_bool]),
+    "s2PrismaticJoint_SetSpringHertz": (None, [JointId, C.c_float]),
+    "s2PrismaticJoint_SetSpringDampingRatio": (None, [JointId, C.c_float]),
+    "s2RevoluteJoint_EnableSpring": (None, [JointId, C.c_bool]),
+    "s2RevoluteJoint_SetSpringHertz": (None, [JointId, C.c_float]),
+    "s2RevoluteJoint_SetSpringDampingRatio": (None, [JointId, C.c_float]),
     "s2CreateMotorJoint": (JointId, [WorldId, C.POINTER(MotorJointDef)]),
     "s2MotorJoint_SetLinearOffset": (None, [JointId, Vec2]),
     "s2MotorJoint_GetLinearOffset": (Vec2, [JointId]),

@@ -7,6 +7,10 @@
 #include "contact_kernels.cuh"
 
 #define S2B_JOINT_TYPE(flags) (((flags) >> 1) & 0x7)
+// row flags of the joint-constraint stream only (jc.head.x): an XPBD spring row's body A / B is static, so its sub-step start
+// pose is its pose (a static body's aux0 row is never written)
+#define S2B_JC_STATIC_A 0x100
+#define S2B_JC_STATIC_B 0x200
 
 struct JointBodies
 {
@@ -41,7 +45,7 @@ enum JointPrepareKind
 
 // Builds row t of the joint-constraint stream from joint slot `slot`. `warmStart` is the flag the *variant* passes
 // (TGS_Soft and SoftStep pass true regardless of the step flag, TGS_Sticky false; SURVEY §8a N3).
-template <int KIND> __device__ __forceinline__ void s2bPrepareJoint(const SolveArgs& a, int t, int slot, bool warmStart)
+template <int KIND> __device__ __forceinline__ void s2bPrepareJointRows(const SolveArgs& a, int t, int slot, bool warmStart)
 {
 	const JointConstraintView& jc = a.jc;
 	int4 head = a.joints.head[slot];
@@ -202,6 +206,72 @@ __device__ __forceinline__ void s2bStoreJointImpulses(const SolveArgs& a, int t)
 }
 
 // ---------------------------------------------------------------------------------------------------------------
+// joint spring (extension, DESIGN.md §3.14; definition: tests/spring_oracle.c). One soft row on the joint's axis toward zero
+// error, solved before the joint's own rows in every velocity pass of every variant: the revolute's relative angle, the
+// prismatic's translation. XPBD solves it as a compliant position row with damping instead. The spring is kept in functions
+// of its own, run ahead of the joint's rows through memory (the bodies' velocity and pose rows, jc.imp.w), so the joint
+// rows' code and register allocation stay as they are without it.
+// Stream lanes: jc.coef.w = bias, jc.lim.w = mass scale, jc.d0ax.w = impulse scale (XPBD: 2 pi hertz h, damping ratio);
+// jc.imp.w = accumulated spring impulse.
+// ---------------------------------------------------------------------------------------------------------------
+
+// the spring's part of prepare. A spring acts only on a revolute or prismatic row with a positive hertz and, on a revolute
+// row, a rotation to act on; every other row loses the flag in jc.head, so no solve or warm start evaluates a spring term
+// for it, and gets a zero spring impulse.
+template <int KIND> __device__ __forceinline__ void s2bPrepareSpring(const SolveArgs& a, int t, int slot, bool warmStart)
+{
+	const JointConstraintView& jc = a.jc;
+	float* lambda = reinterpret_cast<float*>(jc.imp + t) + 3;
+	int4 head = jc.head[t];
+	int flags = head.x;
+	if ((flags & S2B_JOINT_ENABLE_SPRING) == 0)
+	{
+		*lambda = 0.0f;
+		return;
+	}
+	float4 motor = a.joints.motor[slot]; // hertz, damping ratio in zw
+	float iA = a.bodies.pos[head.y].z, iB = a.bodies.pos[head.z].z;
+	int type = S2B_JOINT_TYPE(flags);
+	if ((type != S2B_JOINT_REVOLUTE && type != S2B_JOINT_PRISMATIC) || (motor.z > 0.0f) == false ||
+		(type == S2B_JOINT_REVOLUTE && iA + iB == 0.0f))
+	{
+		jc.head[t] = make_int4(flags & ~S2B_JOINT_ENABLE_SPRING, head.y, head.z, head.w);
+		*lambda = 0.0f;
+		return;
+	}
+	// the mouse joint's coefficients and expression order, for the step h every variant passes to its joint solve
+	float h = a.ctx.h;
+	float zeta = motor.w;
+	float omega = 2.0f * s2_pi * motor.z;
+	if (KIND == JPREP_XPBD)
+	{
+		flags |= (S2B_BODY_TYPE(a.bodies.flags[head.y]) == S2B_BODY_STATIC ? S2B_JC_STATIC_A : 0) |
+				 (S2B_BODY_TYPE(a.bodies.flags[head.z]) == S2B_BODY_STATIC ? S2B_JC_STATIC_B : 0);
+		jc.head[t] = make_int4(flags, head.y, head.z, head.w);
+		reinterpret_cast<float*>(jc.coef + t)[3] = omega * h;
+		reinterpret_cast<float*>(jc.lim + t)[3] = zeta;
+		*lambda = 0.0f;
+		return;
+	}
+	float biasCoefficient = omega / (2.0f * zeta + h * omega);
+	float c = h * omega * (2.0f * zeta + h * omega);
+	float impulseCoefficient = 1.0f / (1.0f + c);
+	float massCoefficient = c * impulseCoefficient;
+	reinterpret_cast<float*>(jc.coef + t)[3] = biasCoefficient;
+	reinterpret_cast<float*>(jc.lim + t)[3] = massCoefficient;
+	reinterpret_cast<float*>(jc.d0ax + t)[3] = impulseCoefficient;
+	// kept exactly when the variant's warm-start flag keeps the point impulse
+	*lambda = warmStart ? a.joints.imp[slot].w : 0.0f;
+}
+
+// Builds row t of the joint-constraint stream from joint slot `slot`: the joint's rows, then its spring.
+template <int KIND> __device__ __forceinline__ void s2bPrepareJoint(const SolveArgs& a, int t, int slot, bool warmStart)
+{
+	s2bPrepareJointRows<KIND>(a, t, slot, warmStart);
+	s2bPrepareSpring<KIND>(a, t, slot, warmStart);
+}
+
+// ---------------------------------------------------------------------------------------------------------------
 // prismatic joint (extension, DESIGN.md §3.9; definition: tests/prismatic_oracle.c). Body B slides along an axis fixed
 // in body A: rows motor, lower limit, upper limit (along the axis), then a 2x2 block holding the perpendicular
 // separation and the relative angle. Every mass depends on the current separation d, so each solve forms it fresh.
@@ -246,7 +316,8 @@ __device__ __forceinline__ PrismaticWarm s2bPrismaticWarmTerms(const SolveArgs& 
 										 V2(poseB.x, poseB.y), R2(poseB.z, poseB.w));
 	s2Vec2 perp = s2LeftPerp(f.axis);
 	s2Vec2 dA = s2Add(f.d, f.rA);
-	float axialImpulse = imp.z + limp.x - limp.y;
+	// axial = spring + motor + lower - upper (DESIGN.md §3.14); a row without a spring adds no spring term
+	float axialImpulse = ((head.x & S2B_JOINT_ENABLE_SPRING) != 0 ? imp.w + imp.z : imp.z) + limp.x - limp.y;
 	PrismaticWarm w;
 	w.P = s2Add(s2MulSV(axialImpulse, f.axis), s2MulSV(imp.x, perp));
 	w.LA = axialImpulse * s2Cross(dA, f.axis) + imp.x * s2Cross(dA, perp) + imp.y;
@@ -686,6 +757,136 @@ __device__ __forceinline__ void s2bSolveMotorXpbd(const SolveArgs& a, int t)
 }
 
 // ---------------------------------------------------------------------------------------------------------------
+// joint spring rows (DESIGN.md §3.14), run ahead of the joint's own rows by the dispatchers below
+// ---------------------------------------------------------------------------------------------------------------
+
+// the velocity row, the same in every velocity flavour (a force law, not an error correction):
+// impulse = -k massScale (Cdot + bias C) - impulseScale lambda, k the axis's effective mass
+__device__ __forceinline__ void s2bSolveSpringVelocity(const SolveArgs& a, int t)
+{
+	const JointConstraintView& jc = a.jc;
+	int4 head = jc.head[t];
+	int ia = head.y, ib = head.z;
+	float4 mass = jc.mass[t];
+	float4 d0 = jc.d0ax[t];
+	float4 lim = jc.lim[t];
+	float bias = jc.coef[t].w, massScale = lim.w, impulseScale = d0.w;
+	float4 imp = jc.imp[t];
+	float4 velA = a.bodies.vel[ia], velB = a.bodies.vel[ib];
+	float4 poseA = a.bodies.pose[ia], poseB = a.bodies.pose[ib];
+	s2Vec2 vA = V2(velA.x, velA.y), vB = V2(velB.x, velB.y);
+	float wA = velA.z, wB = velB.z;
+	float mA = mass.x, iA = mass.y, mB = mass.z, iB = mass.w;
+	s2Rot qA = R2(poseA.z, poseA.w), qB = R2(poseB.z, poseB.w);
+	if (S2B_JOINT_TYPE(head.x) == S2B_JOINT_REVOLUTE)
+	{
+		// C = the weld's angular error (§3.8), k = 1 / (iA + iB)
+		float k = 1.0f / (iA + iB);
+		float C = s2UnwindAngle(s2RelativeAngle(qB, qA) - lim.x);
+		float impulse = -k * massScale * (wB - wA + bias * C) - impulseScale * imp.w;
+		imp.w += impulse;
+		wA -= iA * impulse;
+		wB += iB * impulse;
+	}
+	else
+	{
+		// C = the translation, k = the axial mass §3.9 forms in every solve
+		PrismaticFrame f = s2bPrismaticFrame(jc.anchor[t], d0, jc.motor[t], V2(poseA.x, poseA.y), qA, V2(poseB.x, poseB.y), qB);
+		s2Vec2 dA = s2Add(f.d, f.rA);
+		float a1 = s2Cross(dA, f.axis), a2 = s2Cross(f.rB, f.axis);
+		float k = mA + mB + iA * a1 * a1 + iB * a2 * a2;
+		float axialMass = k > 0.0f ? 1.0f / k : 0.0f;
+		float Cdot = s2Dot(f.axis, s2Sub(vB, vA)) + a2 * wB - a1 * wA;
+		float impulse = -axialMass * massScale * (Cdot + bias * s2Dot(f.axis, f.d)) - impulseScale * imp.w;
+		imp.w += impulse;
+		s2Vec2 P = s2MulSV(impulse, f.axis);
+		vA = s2MulSub(vA, mA, P);
+		wA -= iA * (impulse * a1);
+		vB = s2MulAdd(vB, mB, P);
+		wB += iB * (impulse * a2);
+	}
+	reinterpret_cast<float*>(jc.imp + t)[3] = imp.w;
+	s2bStoreJointVelocities(a, ia, ib, velA, velB, vA, wA, vB, wB, mA, iA, mB, iB);
+}
+
+// XPBD with damping (Macklin et al. 2016), one solve per sub-step from a zero multiplier: w = the axis's generalized inverse
+// mass, C and C0 the error now and at the sub-step's start pose (aux0: dp0, q0; a static body's own pose), omegaH = 2 pi
+// hertz h. A rotation is integrated only where it can change (s2IntegrateRot renormalizes even by a zero angle).
+__device__ __forceinline__ void s2bSolveSpringXpbd(const SolveArgs& a, int t)
+{
+	const JointConstraintView& jc = a.jc;
+	int4 head = jc.head[t];
+	int ia = head.y, ib = head.z;
+	float4 mass = jc.mass[t];
+	float4 lim = jc.lim[t];
+	float omegaH = jc.coef[t].w, zeta = lim.w;
+	float4 poseA = a.bodies.pose[ia], poseB = a.bodies.pose[ib];
+	float4 p0A = (head.x & S2B_JC_STATIC_A) != 0 ? poseA : a.bodies.aux0[ia];
+	float4 p0B = (head.x & S2B_JC_STATIC_B) != 0 ? poseB : a.bodies.aux0[ib];
+	s2Vec2 dcA = V2(poseA.x, poseA.y), dcB = V2(poseB.x, poseB.y);
+	s2Rot qA = R2(poseA.z, poseA.w), qB = R2(poseB.z, poseB.w);
+	float mA = mass.x, iA = mass.y, mB = mass.z, iB = mass.w;
+	float w, C, C0, LA, LB;
+	s2Vec2 axis = V2(0.0f, 0.0f);
+	if (S2B_JOINT_TYPE(head.x) == S2B_JOINT_REVOLUTE)
+	{
+		w = iA + iB;
+		C = s2UnwindAngle(s2RelativeAngle(qB, qA) - lim.x);
+		C0 = s2UnwindAngle(s2RelativeAngle(R2(p0B.z, p0B.w), R2(p0A.z, p0A.w)) - lim.x);
+		LA = 1.0f;
+		LB = 1.0f;
+	}
+	else
+	{
+		float4 anchor = jc.anchor[t], d0 = jc.d0ax[t], motor = jc.motor[t];
+		PrismaticFrame f0 = s2bPrismaticFrame(anchor, d0, motor, V2(p0A.x, p0A.y), R2(p0A.z, p0A.w), V2(p0B.x, p0B.y), R2(p0B.z, p0B.w));
+		PrismaticFrame f = s2bPrismaticFrame(anchor, d0, motor, dcA, qA, dcB, qB);
+		axis = f.axis;
+		LA = s2Cross(s2Add(f.d, f.rA), f.axis);
+		LB = s2Cross(f.rB, f.axis);
+		w = mA + mB + iA * LA * LA + iB * LB * LB;
+		C = s2Dot(f.axis, f.d);
+		C0 = s2Dot(f0.axis, f0.d);
+		if ((w > 0.0f) == false)
+		{
+			return;
+		}
+	}
+	float alphaTilde = w / (omegaH * omegaH);
+	float gamma = 2.0f * zeta / omegaH;
+	float p = -(C + gamma * (C - C0)) / ((1.0f + gamma) * w + alphaTilde);
+	if (S2B_JOINT_TYPE(head.x) == S2B_JOINT_PRISMATIC)
+	{
+		s2Vec2 P = s2MulSV(p, axis);
+		dcA = s2MulSub(dcA, mA, P);
+		dcB = s2MulAdd(dcB, mB, P);
+		LA = p * LA;
+		LB = p * LB;
+	}
+	else
+	{
+		LA = p;
+		LB = p;
+	}
+	if (iA != 0.0f)
+	{
+		qA = s2IntegrateRot(qA, -iA * LA);
+	}
+	if (iB != 0.0f)
+	{
+		qB = s2IntegrateRot(qB, iB * LB);
+	}
+	if ((mA != 0.0f) || (iA != 0.0f))
+	{
+		a.bodies.pose[ia] = make_float4(dcA.x, dcA.y, qA.s, qA.c);
+	}
+	if ((mB != 0.0f) || (iB != 0.0f))
+	{
+		a.bodies.pose[ib] = make_float4(dcB.x, dcB.y, qB.s, qB.c);
+	}
+}
+
+// ---------------------------------------------------------------------------------------------------------------
 // warm start: s2WarmStartRevolute (reference src/revolute_joint.c:107-150), s2WarmStartMouse (mouse_joint.c:85-107)
 // ---------------------------------------------------------------------------------------------------------------
 __device__ __forceinline__ void s2bWarmStartJoint(const SolveArgs& a, int t)
@@ -736,7 +937,8 @@ __device__ __forceinline__ void s2bWarmStartJoint(const SolveArgs& a, int t)
 	s2Vec2 rB = s2RotateVector(R2(poseB.z, poseB.w), V2(anchor.z, anchor.w));
 	float mA = mass.x, iA = mass.y, mB = mass.z, iB = mass.w;
 
-	float axialImpulse = imp.z + limp.x - limp.y;
+	// axial = spring + motor + lower - upper (DESIGN.md §3.14); a row without a spring adds no spring term
+	float axialImpulse = ((head.x & S2B_JOINT_ENABLE_SPRING) != 0 ? imp.w + imp.z : imp.z) + limp.x - limp.y;
 	s2Vec2 P = V2(imp.x, imp.y);
 
 	vA = s2MulSub(vA, mA, P);
@@ -1057,6 +1259,10 @@ template <bool SHARED_MOTOR>
 __device__ __forceinline__ void s2bSolveJointSoft(const SolveArgs& a, int t, float h, float inv_h, bool useBias)
 {
 	int flags = a.jc.head[t].x;
+	if (flags & S2B_JOINT_ENABLE_SPRING)
+	{
+		s2bSolveSpringVelocity(a, t);
+	}
 	if (S2B_JOINT_TYPE(flags) == S2B_JOINT_MOUSE)
 	{
 		if (useBias)
@@ -1082,6 +1288,10 @@ __device__ __forceinline__ void s2bSolveJointSoft(const SolveArgs& a, int t, flo
 __device__ __forceinline__ void s2bSolveJointBaumgarte(const SolveArgs& a, int t, float h, float inv_h, bool useBias)
 {
 	int flags = a.jc.head[t].x;
+	if (flags & S2B_JOINT_ENABLE_SPRING)
+	{
+		s2bSolveSpringVelocity(a, t);
+	}
 	if (S2B_JOINT_TYPE(flags) == S2B_JOINT_MOUSE)
 	{
 		s2bSolveMouse(a, t);
@@ -1195,6 +1405,10 @@ __device__ __forceinline__ void s2bSolveRevoluteRigid(const SolveArgs& a, int t,
 // s2SolveJoint dispatch (reference src/joint.c:329-345)
 __device__ __forceinline__ void s2bSolveJointRigid(const SolveArgs& a, int t, float h)
 {
+	if (a.jc.head[t].x & S2B_JOINT_ENABLE_SPRING)
+	{
+		s2bSolveSpringVelocity(a, t);
+	}
 	if (S2B_JOINT_TYPE(a.jc.head[t].x) == S2B_JOINT_MOUSE)
 	{
 		s2bSolveMouse(a, t);
@@ -1304,6 +1518,10 @@ __device__ __forceinline__ void s2bSolveJointPosition(const SolveArgs& a, int t)
 __device__ __forceinline__ void s2bSolveJointXpbd(const SolveArgs& a, int t)
 {
 	const JointConstraintView& jc = a.jc;
+	if (jc.head[t].x & S2B_JOINT_ENABLE_SPRING)
+	{
+		s2bSolveSpringXpbd(a, t);
+	}
 	int4 head = jc.head[t];
 	if (S2B_JOINT_TYPE(head.x) == S2B_JOINT_MOUSE)
 	{

@@ -40,7 +40,9 @@ __global__ void s2bJointReactionKernel(JointView j, const float2* __restrict__ b
 	float4 imp = j.imp[i], limp = j.limp[i], target = j.target[i];
 	float4 qa = pose[head.y];
 	s2Rot qA = {qa.z, qa.w};
-	s2JointReaction r = s2MakeJointReaction((head.x >> 1) & 0x7, s2MakeVec2(imp.x, imp.y), imp.z, limp.x, limp.y, qA,
+	// a spring acts on the motor's axis: its impulse joins the motor argument (DESIGN.md §3.14)
+	float motorImpulse = (head.x & S2B_JOINT_ENABLE_SPRING) != 0 ? imp.z + imp.w : imp.z;
+	s2JointReaction r = s2MakeJointReaction((head.x >> 1) & 0x7, s2MakeVec2(imp.x, imp.y), motorImpulse, limp.x, limp.y, qA,
 											s2MakeVec2(target.z, target.w), rate);
 	if (reactions != nullptr)
 	{

@@ -281,7 +281,7 @@ struct JointView
 	float4* lim;	// referenceAngle lowerAngle upperAngle 0
 	float4* motor;	// maxMotorTorque motorSpeed hertz dampingRatio
 	float4* target; // mouse target.xy, prismatic localAxisA.xy
-	float4* imp;	// impulse.x impulse.y motorImpulse 0
+	float4* imp;	// impulse.x impulse.y motorImpulse springImpulse
 	float4* limp;	// lowerImpulse upperImpulse 0 0
 	int* color;		// colour the joint was last solved with (-1: none)
 	int capacity;
@@ -290,16 +290,17 @@ struct JointView
 // per-step joint-constraint columns in solve order
 struct JointConstraintView
 {
-	int4* head;		// flags(type, limit, motor), bodyA, bodyB, source joint slot
+	int4* head;		// flags(type, limit, motor, spring), bodyA, bodyB, source joint slot. The spring flag stays only on rows
+					// whose spring acts (DESIGN.md §3.14); XPBD spring rows add S2B_JC_STATIC_A / _B.
 	float4* anchor; // COM-relative local anchors A.xy B.xy
 	float4* mass;	// invMassA invIA invMassB invIB
-	float4* d0ax;	// centerDiff0.xy axialMass 0
-	float4* lim;	// referenceAngle lowerAngle upperAngle 0
+	float4* d0ax;	// centerDiff0.xy axialMass springImpulseScale
+	float4* lim;	// referenceAngle lowerAngle upperAngle springMassScale (XPBD: spring dampingRatio)
 	float4* motor;	// maxMotorTorque motorSpeed 0 0 (prismatic: maxMotorForce motorSpeed localAxisA.xy;
 					// motor joint: maxTorque 0 maxForce correctionFactor)
-	float4* coef;	// biasCoefficient massCoefficient impulseCoefficient 0
+	float4* coef;	// biasCoefficient massCoefficient impulseCoefficient springBias (XPBD: 2 pi hertz h)
 	float4* pivot;	// pivotMass cx.x cx.y cy.x cy.y (mouse, non-fresh revolute)
-	float4* imp;	// impulse.x impulse.y motorImpulse 0        (r/w)
+	float4* imp;	// impulse.x impulse.y motorImpulse springImpulse (r/w)
 	float4* limp;	// lowerImpulse upperImpulse 0 0              (r/w)
 };
 

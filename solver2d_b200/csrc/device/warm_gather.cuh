@@ -93,7 +93,8 @@ __device__ __forceinline__ GatherTerms s2bGatherTermsOf(const SolveArgs& a, int 
 		else
 		{
 			float4 limp = a.jc.limp[t];
-			float axialImpulse = imp.z + limp.x - limp.y;
+			// as s2bWarmStartJoint: the spring impulse joins the axial sum only on a spring row (DESIGN.md §3.14)
+			float axialImpulse = ((head.x & S2B_JOINT_ENABLE_SPRING) != 0 ? imp.w + imp.z : imp.z) + limp.x - limp.y;
 			if (sideB)
 			{
 				s2Vec2 rB = s2RotateVector(q, V2(anchor.z, anchor.w));

@@ -97,7 +97,7 @@ __global__ void s2bScatterJoints(const s2bJointRow* __restrict__ rows, int count
 	j.lim[i] = make_float4(r->referenceAngle, r->lowerAngle, r->upperAngle, 0.0f);
 	j.motor[i] = make_float4(r->maxMotorTorque, r->motorSpeed, r->hertz, r->dampingRatio);
 	j.target[i] = make_float4(r->target[0], r->target[1], r->localAxisA[0], r->localAxisA[1]);
-	j.imp[i] = make_float4(r->impulse[0], r->impulse[1], r->motorImpulse, 0.0f);
+	j.imp[i] = make_float4(r->impulse[0], r->impulse[1], r->motorImpulse, r->springImpulse);
 	j.limp[i] = make_float4(r->lowerImpulse, r->upperImpulse, 0.0f, 0.0f);
 	brk[i] = make_float2(r->breakForce, r->breakTorque);
 }
@@ -225,6 +225,7 @@ __global__ void s2bGatherJoints(s2bJointRow* rows, int count, JointView j, const
 	r.motorImpulse = imp.z;
 	r.lowerImpulse = limp.x;
 	r.upperImpulse = limp.y;
+	r.springImpulse = imp.w;
 	float2 b = brk[i];
 	r.breakForce = b.x;
 	r.breakTorque = b.y;

@@ -165,14 +165,88 @@ float s2RevoluteJoint_GetMotorTorque(s2JointId jointId, float inverseTimeStep)
 	return inverseTimeStep * world->joints[jointId.index].motorImpulse;
 }
 
+// ---- joint springs (DESIGN.md §3.14): revolute and prismatic joints; hertz and dampingRatio carry the spring ---------------
+
+static bool s2IsValidSpringValue(float value)
+{
+	return s2IsValid(value) && value >= 0.0f;
+}
+
+static void s2EnableJointSpring(s2JointId jointId, s2JointType type, bool enableSpring)
+{
+	s2World* world;
+	s2Joint* joint = s2GetJointForEdit(jointId, &world);
+	if (joint->type != type)
+	{
+		return; // only revolute and prismatic joints have a spring
+	}
+	joint->enableSpring = enableSpring;
+	s2MarkJointDirty(world, joint);
+}
+
+static void s2SetJointSpringValue(s2JointId jointId, s2JointType type, float value, bool dampingRatio)
+{
+	if (s2IsValidSpringValue(value) == false)
+	{
+		return; // rejected: the joint keeps its value
+	}
+	s2World* world;
+	s2Joint* joint = s2GetJointForEdit(jointId, &world);
+	if (joint->type != type)
+	{
+		return; // only revolute and prismatic joints have a spring
+	}
+	if (dampingRatio)
+	{
+		joint->dampingRatio = value;
+	}
+	else
+	{
+		joint->hertz = value;
+	}
+	s2MarkJointDirty(world, joint);
+}
+
+void s2RevoluteJoint_EnableSpring(s2JointId jointId, bool enableSpring)
+{
+	s2EnableJointSpring(jointId, s2_revoluteJoint, enableSpring);
+}
+
+void s2RevoluteJoint_SetSpringHertz(s2JointId jointId, float hertz)
+{
+	s2SetJointSpringValue(jointId, s2_revoluteJoint, hertz, false);
+}
+
+void s2RevoluteJoint_SetSpringDampingRatio(s2JointId jointId, float dampingRatio)
+{
+	s2SetJointSpringValue(jointId, s2_revoluteJoint, dampingRatio, true);
+}
+
+void s2PrismaticJoint_EnableSpring(s2JointId jointId, bool enableSpring)
+{
+	s2EnableJointSpring(jointId, s2_prismaticJoint, enableSpring);
+}
+
+void s2PrismaticJoint_SetSpringHertz(s2JointId jointId, float hertz)
+{
+	s2SetJointSpringValue(jointId, s2_prismaticJoint, hertz, false);
+}
+
+void s2PrismaticJoint_SetSpringDampingRatio(s2JointId jointId, float dampingRatio)
+{
+	s2SetJointSpringValue(jointId, s2_prismaticJoint, dampingRatio, true);
+}
+
 // The prismatic joint has no counterpart in the reference (DESIGN.md §3.9). Degenerate input creates nothing and returns
-// s2_nullJointId: an axis that cannot be normalized, or lowerTranslation > upperTranslation.
+// s2_nullJointId: an axis that cannot be normalized, lowerTranslation > upperTranslation, or a spring hertz or damping ratio
+// that is negative or not finite.
 s2JointId s2CreatePrismaticJoint(s2WorldId worldId, const s2PrismaticJointDef* def)
 {
 	s2Vec2 axis = def->localAxisA;
 	float length = s2Length(axis);
 	if (s2IsValidVec2(axis) == false || s2IsValid(length) == false || length == 0.0f ||
-		(def->lowerTranslation <= def->upperTranslation) == false)
+		(def->lowerTranslation <= def->upperTranslation) == false || s2IsValidSpringValue(def->hertz) == false ||
+		s2IsValidSpringValue(def->dampingRatio) == false)
 	{
 		return s2_nullJointId;
 	}
@@ -195,6 +269,9 @@ s2JointId s2CreatePrismaticJoint(s2WorldId worldId, const s2PrismaticJointDef* d
 	joint->enableLimit = def->enableLimit;
 	joint->enableMotor = def->enableMotor;
 	joint->collideConnected = def->collideConnected;
+	joint->enableSpring = def->enableSpring;
+	joint->hertz = def->hertz;
+	joint->dampingRatio = def->dampingRatio;
 
 	s2JointId jointId = {joint->object.index, world->index, joint->object.revision};
 	return jointId;
@@ -396,7 +473,11 @@ static s2JointReaction s2GetJointReaction(s2JointId jointId)
 	s2SyncStateToHost(world);
 	const s2Joint* joint = world->joints + jointId.index;
 	S2_ASSERT(s2ObjectValid(&joint->object) && joint->object.revision == jointId.revision);
-	return s2MakeJointReaction((int32_t)joint->type, joint->impulse, joint->motorImpulse, joint->lowerImpulse, joint->upperImpulse,
+	// a spring acts on the motor's axis: its impulse joins the motor argument (DESIGN.md §3.14). The flag is the one of the
+	// row the device last solved, so the getters read what the device's reaction and break pass read for that step even
+	// after s2*Joint_EnableSpring has changed the joint and before the next step uploads it.
+	float motorImpulse = joint->springUploaded ? joint->motorImpulse + joint->springImpulse : joint->motorImpulse;
+	return s2MakeJointReaction((int32_t)joint->type, joint->impulse, motorImpulse, joint->lowerImpulse, joint->upperImpulse,
 							   world->bodies[joint->bodyIndexA].rot, joint->localAxisA, world->reactionRate);
 }
 

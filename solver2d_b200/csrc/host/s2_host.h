@@ -171,12 +171,17 @@ typedef struct s2Joint
 	s2Vec2 localAxisA;
 	// mouse; a motor joint keeps its maximum force in hertz and its correction factor in dampingRatio, its linear offset
 	// in localOriginAnchorA (localOriginAnchorB is zero), its angular offset in referenceAngle and its maximum torque in
-	// maxMotorTorque, as its device row does
+	// maxMotorTorque, as its device row does. A revolute or prismatic joint keeps its spring's stiffness (Hz) and damping
+	// ratio here (DESIGN.md §3.14).
 	float hertz, dampingRatio;
+	bool enableSpring;
+	// enableSpring as the device's last uploaded row has it: the reaction getters pair it with the synced impulses, which
+	// that row produced (a setter call between steps changes enableSpring but not yet the row)
+	bool springUploaded;
 	s2Vec2 targetA;
 	// accumulated impulses (cache of the device columns)
 	s2Vec2 impulse;
-	float motorImpulse, lowerImpulse, upperImpulse;
+	float motorImpulse, lowerImpulse, upperImpulse, springImpulse;
 	// break thresholds (s2Joint_SetBreakForce / _SetBreakTorque), 0 = none
 	float breakForce, breakTorque;
 

@@ -247,6 +247,8 @@ static void s2FillJointRow(s2bJointRow* r, const s2Joint* j)
 	r->flags |= j->enableLimit ? S2B_JOINT_ENABLE_LIMIT : 0;
 	r->flags |= j->enableMotor ? S2B_JOINT_ENABLE_MOTOR : 0;
 	r->flags |= j->collideConnected ? S2B_JOINT_COLLIDE_CONNECTED : 0;
+	// only revolute and prismatic joints have a spring setter, so no other row carries the flag
+	r->flags |= j->enableSpring ? S2B_JOINT_ENABLE_SPRING : 0;
 	r->bodyA = j->bodyIndexA;
 	r->bodyB = j->bodyIndexB;
 	r->localOriginAnchorA[0] = j->localOriginAnchorA.x;
@@ -267,6 +269,7 @@ static void s2FillJointRow(s2bJointRow* r, const s2Joint* j)
 	r->motorImpulse = j->motorImpulse;
 	r->lowerImpulse = j->lowerImpulse;
 	r->upperImpulse = j->upperImpulse;
+	r->springImpulse = j->springImpulse;
 	r->localAxisA[0] = j->localAxisA.x;
 	r->localAxisA[1] = j->localAxisA.y;
 	r->breakForce = j->breakForce;
@@ -362,6 +365,7 @@ void s2FlushToDevice(s2World* world)
 		{
 			s2Joint* j = world->joints + world->dirtyJoints.data[i];
 			s2FillJointRow(rows + i, j);
+			j->springUploaded = j->enableSpring;
 			j->rowDirty = false;
 		}
 		s2b_upload_joints(dev, rows, n, world->jointPool.capacity);
@@ -456,6 +460,7 @@ void s2SyncStateToHost(s2World* world)
 			j->motorImpulse = rows[i].motorImpulse;
 			j->lowerImpulse = rows[i].lowerImpulse;
 			j->upperImpulse = rows[i].upperImpulse;
+			j->springImpulse = rows[i].springImpulse;
 		}
 		free(rows);
 	}

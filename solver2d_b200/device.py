@@ -33,7 +33,7 @@ JOINT_ROW = np.dtype([
     ("localOriginAnchorB", "<f4", 2), ("referenceAngle", "<f4"), ("lowerAngle", "<f4"), ("upperAngle", "<f4"),
     ("maxMotorTorque", "<f4"), ("motorSpeed", "<f4"), ("hertz", "<f4"), ("dampingRatio", "<f4"), ("target", "<f4", 2),
     ("impulse", "<f4", 2), ("motorImpulse", "<f4"), ("lowerImpulse", "<f4"), ("upperImpulse", "<f4"),
-    ("localAxisA", "<f4", 2), ("breakForce", "<f4"), ("breakTorque", "<f4"),
+    ("localAxisA", "<f4", 2), ("breakForce", "<f4"), ("breakTorque", "<f4"), ("springImpulse", "<f4"),
 ], align=True)
 
 CONTACT_POINT = np.dtype([
@@ -73,7 +73,7 @@ class Counters(C.Structure):
 SCHEDULE_COLOR, SCHEDULE_WAVEFRONT = 0, 1
 ROW_VALID = 0x1
 SHAPE_MOVED = 0x10
-JOINT_ENABLE_LIMIT, JOINT_ENABLE_MOTOR, JOINT_COLLIDE_CONNECTED = 0x10, 0x20, 0x40
+JOINT_ENABLE_LIMIT, JOINT_ENABLE_MOTOR, JOINT_COLLIDE_CONNECTED, JOINT_ENABLE_SPRING = 0x10, 0x20, 0x40, 0x80
 # joint types, stored in flags bits 1-3 (a weld keeps its angular impulse in the motorImpulse column; a prismatic row keeps
 # its translation limits in lowerAngle / upperAngle and its maximum motor force in maxMotorTorque; a motor row keeps its
 # linear offset in localOriginAnchorA, its angular offset in referenceAngle, its maximum torque in maxMotorTorque, its

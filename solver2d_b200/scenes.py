@@ -787,6 +787,157 @@ def sliders(lib: capi.Solver2D, solver="TGS_Soft", copies=1, kinematic=True) -> 
     return sc
 
 
+SPRINGS_PITCH = 40.0  # width of one copy of springs (m)
+
+
+def springs(lib: capi.Solver2D, solver="TGS_Soft", copies=1, kinematic=True) -> Scene:
+    """Joint spring coverage (DESIGN.md §3.14), `copies` side by side (about 25 bodies each). Per copy:
+
+    * a car driving over bumps: a chassis on two prismatic suspension springs with limits (axis up, 4 Hz, damping ratio
+      0.7), each holding an axle, and a circular wheel on each axle on a motorised revolute joint (the car's parts share a
+      negative collision group, so only the wheels and the chassis touch the world);
+    * a soft chain of six links on revolute springs (3 Hz, 0.3), hung from a post, falling onto a pile of boxes;
+    * a flipper: a revolute joint with a spring (5 Hz, 0.2), limits and a weak motor on one plank;
+    * with `kinematic`: a box on a prismatic spring (2 Hz, 0.1) along a kinematic carriage that moves sideways;
+    * a revolute spring (2 Hz, 0.5) whose rest angle, pi - 0.05, sits at the seam: its body starts at -pi + 0.1, so the
+      spring turns it back across the seam;
+    * a box pulled by a mouse joint (first copy only).
+
+    On a library without s2CreatePrismaticJoint (the reference) every prismatic joint is created as a revolute joint with
+    limits and motor off, and no spring is set, as ``sliders`` does. ``sc.piles["prismatic"]``, ``["prismatic_defs"]`` and
+    ``["prismatic_bodies"]`` describe the prismatic joints as in ``sliders``; ``sc.piles["springs"]`` lists
+    (index into ``sc.joints``, hertz, dampingRatio) of every sprung joint, so that a test can give the stand-in rows their
+    springs."""
+    world = lib.create_world(solver)
+    sc = Scene(lib, world, name=f"springs{copies}")
+    sc.piles["prismatic"] = []
+    sc.piles["prismatic_defs"] = []
+    sc.piles["prismatic_bodies"] = []
+    sc.piles["springs"] = []
+    has_prismatic = "s2CreatePrismaticJoint" not in lib.missing
+    gid = _ground(lib, world, 0.5 * SPRINGS_PITCH * copies + 5.0)
+    sc.bodies.append(gid)
+
+    def body(kind, x, y, angle=0.0, hx=0.5, hy=0.125, vx=0.0, vy=0.0, radius=None, group=0):
+        bd = default_body_def()
+        bd.type = kind
+        bd.position = Vec2(x, y)
+        bd.angle = angle
+        bd.linearVelocity = Vec2(vx, vy)
+        bid = lib.s2CreateBody(world, C.byref(bd))
+        sd = default_shape_def()
+        sd.filter.groupIndex = group
+        if radius is not None:
+            lib.s2CreateCircleShape(bid, C.byref(sd), C.byref(Circle(Vec2(0.0, 0.0), radius)))
+        else:
+            lib.s2CreatePolygonShape(bid, C.byref(sd), C.byref(lib.s2MakeBox(hx, hy)))
+        sc.bodies.append(bid)
+        return bid
+
+    def spring(jid, hertz, zeta, prismatic_joint):
+        sc.piles["springs"].append((len(sc.joints) - 1, hertz, zeta))
+        if not has_prismatic:
+            return  # the reference has no spring
+        if prismatic_joint:
+            return  # set in the definition
+        lib.s2RevoluteJoint_EnableSpring(jid, True)
+        lib.s2RevoluteJoint_SetSpringHertz(jid, hertz)
+        lib.s2RevoluteJoint_SetSpringDampingRatio(jid, zeta)
+
+    def prismatic(a, b, pivot, axis, limit=None, hertz=0.0, zeta=0.0):
+        d = dict(localAnchorA=tuple(lib.s2Body_GetLocalPoint(a, pivot)), localAnchorB=tuple(lib.s2Body_GetLocalPoint(b, pivot)),
+                 localAxisA=axis, referenceAngle=0.0, enableLimit=limit is not None,
+                 lowerTranslation=limit[0] if limit else 0.0, upperTranslation=limit[1] if limit else 0.0,
+                 enableMotor=False, motorSpeed=0.0, maxMotorForce=0.0, collideConnected=False)
+        if has_prismatic:
+            jd = capi.default_prismatic_def()
+            for name, value in d.items():
+                setattr(jd, name, Vec2(*value) if isinstance(value, tuple) else value)
+            jd.enableSpring, jd.hertz, jd.dampingRatio = True, hertz, zeta
+            create = lib.s2CreatePrismaticJoint
+        else:
+            jd = default_revolute_def()
+            jd.localAnchorA = Vec2(*d["localAnchorA"])
+            jd.localAnchorB = Vec2(*d["localAnchorB"])
+            create = lib.s2CreateRevoluteJoint
+        jd.bodyIdA = a
+        jd.bodyIdB = b
+        sc.piles["prismatic"].append(len(sc.joints))
+        sc.piles["prismatic_defs"].append(d)
+        sc.piles["prismatic_bodies"].append((a, b))
+        jid = create(world, C.byref(jd))
+        sc.joints.append(jid)
+        spring(jid, hertz, zeta, True)
+        return jid
+
+    def revolute(a, b, pivot, reference_angle=0.0, motor=None, limit=None, hertz=None, zeta=0.0):
+        jd = default_revolute_def()
+        jd.bodyIdA = a
+        jd.bodyIdB = b
+        jd.localAnchorA = lib.s2Body_GetLocalPoint(a, pivot)
+        jd.localAnchorB = lib.s2Body_GetLocalPoint(b, pivot)
+        jd.referenceAngle = reference_angle
+        if motor is not None:
+            jd.enableMotor = True
+            jd.motorSpeed, jd.maxMotorTorque = motor
+        if limit is not None:
+            jd.enableLimit = True
+            jd.lowerAngle, jd.upperAngle = limit
+        jid = lib.s2CreateRevoluteJoint(world, C.byref(jd))
+        sc.joints.append(jid)
+        if hertz is not None:
+            spring(jid, hertz, zeta, False)
+        return jid
+
+    D, S, K = capi.DYNAMIC_BODY, capi.STATIC_BODY, capi.KINEMATIC_BODY
+    up = (0.0, 1.0)
+    for k in range(copies):
+        x0 = -0.5 * SPRINGS_PITCH * (copies - 1) + SPRINGS_PITCH * k - 18.0
+        # bumps on the ground, then the car
+        for i in range(4):
+            body(S, x0 + 4.0 + 2.5 * i, 0.05, hx=0.4, hy=0.05 + 0.05 * (i % 2))
+        group = -(k + 1)
+        chassis = body(D, x0, 1.5, hx=1.2, hy=0.2, group=group)
+        for dx in (-0.9, 0.9):
+            axle = body(D, x0 + dx, 0.9, hx=0.1, hy=0.1, group=group)
+            prismatic(chassis, axle, Vec2(x0 + dx, 0.9), up, limit=(-0.25, 0.25), hertz=4.0, zeta=0.7)
+            wheel = body(D, x0 + dx, 0.9, radius=0.4, group=group)
+            revolute(axle, wheel, Vec2(x0 + dx, 0.9), motor=(-8.0, 12.0))
+        # a soft chain falling onto a pile
+        post = body(S, x0 + 16.0, 6.0, hx=0.1, hy=0.1)
+        prev = post
+        for i in range(6):
+            link = body(D, x0 + 16.5 + 1.0 * i, 6.0, hx=0.5, hy=0.1)
+            revolute(prev, link, Vec2(x0 + 16.0 + 1.0 * i, 6.0), hertz=3.0, zeta=0.3)
+            prev = link
+        for i in range(3):
+            for j in range(3 - i):
+                body(D, x0 + 18.0 + 0.55 * j + 0.275 * i, 0.25 + 0.5 * i, hx=0.25, hy=0.25)
+        # a flipper: spring, limits and a weak motor together
+        hinge = body(S, x0 + 25.0, 1.0, hx=0.1, hy=0.1)
+        plank = body(D, x0 + 26.0, 1.0, hx=1.0, hy=0.1)
+        revolute(hinge, plank, Vec2(x0 + 25.0, 1.0), motor=(1.0, 2.0), limit=(-0.5, 0.5), hertz=5.0, zeta=0.2)
+        # a box on a prismatic spring along a kinematic carriage
+        if kinematic:
+            carriage = body(K, x0 + 30.0, 3.0, hx=1.0, hy=0.125, vx=0.7)
+            rider = body(D, x0 + 30.5, 3.375, hx=0.25, hy=0.25)
+            prismatic(carriage, rider, Vec2(x0 + 30.5, 3.375), (1.0, 0.0), limit=(-0.75, 0.75), hertz=2.0, zeta=0.1)
+        # a revolute spring whose rest angle sits at the seam
+        pin = body(S, x0 + 34.0, 4.0, hx=0.1, hy=0.1)
+        arm = body(D, x0 + 34.0, 4.0, angle=-math.pi + 0.1, hx=0.6, hy=0.1)
+        revolute(pin, arm, Vec2(x0 + 34.0, 4.0), reference_angle=math.pi - 0.05, hertz=2.0, zeta=0.5)
+        if k == 0:
+            dragged = body(D, x0 + 37.0, 0.25, hx=0.25, hy=0.25)
+            md = default_mouse_def()
+            md.bodyIdA = gid
+            md.bodyIdB = dragged
+            md.target = Vec2(x0 + 37.5, 1.5)
+            md.hertz = 3.0
+            md.dampingRatio = 0.7
+            sc.joints.append(lib.s2CreateMouseJoint(world, C.byref(md)))
+    return sc
+
+
 MOTORS_PITCH = 30.0  # width of one copy of motors (m)
 
 
