@@ -136,6 +136,9 @@ typedef struct s2bJointRow
 	// localOriginAnchorB is (0, 0); referenceAngle holds the angular offset, maxMotorTorque the maximum torque (N-m),
 	// hertz the maximum force (N) and dampingRatio the correction factor; impulse[2] is the linear impulse and
 	// motorImpulse the angular impulse. Its limit impulses stay 0.
+	// A weld row (which never carries the limit, motor or spring flag) holds its soft parts (DESIGN.md §3.15): the anchor
+	// spring's stiffness (Hz) in hertz and its damping ratio in dampingRatio, the angle spring's stiffness (Hz) in
+	// maxMotorTorque and its damping ratio in motorSpeed. A hertz of 0 makes that part rigid.
 	float localAxisA[2];
 	// break thresholds (N, N-m) of the reaction pass (DESIGN.md §3.13); 0 = none. A row with either set is checked after every
 	// finalize; a row without them is never checked.

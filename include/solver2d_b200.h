@@ -25,9 +25,10 @@ S2B_API void s2World_EnableRestitution(s2WorldId worldId, bool enable);
 // s2World_Step.
 S2B_API void s2World_SetRestitutionThreshold(s2WorldId worldId, float threshold);
 
-// Weld joint: holds body B rigidly to body A, the anchor points together and angle(B) - angle(A) at referenceAngle.
-// It is as rigid as the solver variant makes a revolute joint's point constraint (DESIGN.md §3.8). Anchors are relative
-// to each body's origin. Destroy it with s2DestroyJoint.
+// Weld joint: holds body B to body A, the anchor points together and angle(B) - angle(A) at referenceAngle. With both
+// hertz at 0 it is rigid: as rigid as the solver variant makes a revolute joint's point constraint (DESIGN.md §3.8). A
+// positive linearHertz makes the anchor constraint a spring, a positive angularHertz the angle constraint (a soft weld,
+// DESIGN.md §3.15). Anchors are relative to each body's origin. Destroy it with s2DestroyJoint.
 typedef struct s2WeldJointDef
 {
 	s2BodyId bodyIdA;
@@ -36,7 +37,11 @@ typedef struct s2WeldJointDef
 	s2Vec2 localAnchorB;
 	float referenceAngle; // angle(B) - angle(A) at rest
 	float drawSize;
-	bool collideConnected; // keep the contacts the two bodies already have
+	bool collideConnected;	   // keep the contacts the two bodies already have
+	float linearHertz;		   // the anchor spring's stiffness as a frequency (Hz), >= 0; 0 = rigid
+	float linearDampingRatio;  // the anchor spring's damping ratio, >= 0 (1 = critical)
+	float angularHertz;		   // the angle spring's stiffness as a frequency (Hz), >= 0; 0 = rigid
+	float angularDampingRatio; // the angle spring's damping ratio, >= 0 (1 = critical)
 } s2WeldJointDef;
 
 S2_INLINE struct s2WeldJointDef s2DefaultWeldJointDef(void)
@@ -48,7 +53,18 @@ S2_INLINE struct s2WeldJointDef s2DefaultWeldJointDef(void)
 	return def;
 }
 
+// Returns s2_nullJointId (and creates nothing) for a negative or non-finite hertz or damping ratio.
 S2B_API s2JointId s2CreateWeldJoint(s2WorldId worldId, const s2WeldJointDef* def);
+// The soft weld (DESIGN.md §3.15). A setter ignores a negative or non-finite value (the joint keeps its value) and a joint
+// that is not a weld; a change takes effect at the next step. A getter returns 0 for a joint that is not a weld.
+S2B_API void s2WeldJoint_SetLinearHertz(s2JointId jointId, float hertz);
+S2B_API void s2WeldJoint_SetLinearDampingRatio(s2JointId jointId, float dampingRatio);
+S2B_API void s2WeldJoint_SetAngularHertz(s2JointId jointId, float hertz);
+S2B_API void s2WeldJoint_SetAngularDampingRatio(s2JointId jointId, float dampingRatio);
+S2B_API float s2WeldJoint_GetLinearHertz(s2JointId jointId);
+S2B_API float s2WeldJoint_GetLinearDampingRatio(s2JointId jointId);
+S2B_API float s2WeldJoint_GetAngularHertz(s2JointId jointId);
+S2B_API float s2WeldJoint_GetAngularDampingRatio(s2JointId jointId);
 
 // Prismatic (slider) joint: body B slides along an axis fixed in body A, keeps angle(B) - angle(A) at referenceAngle and
 // may have translation limits, a linear motor (DESIGN.md §3.9) and a spring toward translation 0 (DESIGN.md §3.14). Anchors

@@ -149,6 +149,10 @@ class WeldJointDef(C.Structure):
         ("referenceAngle", C.c_float),
         ("drawSize", C.c_float),
         ("collideConnected", C.c_bool),
+        ("linearHertz", C.c_float),
+        ("linearDampingRatio", C.c_float),
+        ("angularHertz", C.c_float),
+        ("angularDampingRatio", C.c_float),
     ]
 
 
@@ -255,6 +259,8 @@ def default_weld_def() -> WeldJointDef:
     d.bodyIdA = BodyId(-1, -1, 0)
     d.bodyIdB = BodyId(-1, -1, 0)
     d.drawSize = 1.0
+    # a rigid weld: hertz 0 on both parts (DESIGN.md §3.15)
+    d.linearHertz = d.linearDampingRatio = d.angularHertz = d.angularDampingRatio = 0.0
     return d
 
 
@@ -330,6 +336,15 @@ _API = {
     "s2World_EnableRestitution": (None, [WorldId, C.c_bool]),
     "s2World_SetRestitutionThreshold": (None, [WorldId, C.c_float]),
     "s2CreateWeldJoint": (JointId, [WorldId, C.POINTER(WeldJointDef)]),
+    # soft weld (DESIGN.md §3.15)
+    "s2WeldJoint_SetLinearHertz": (None, [JointId, C.c_float]),
+    "s2WeldJoint_SetLinearDampingRatio": (None, [JointId, C.c_float]),
+    "s2WeldJoint_SetAngularHertz": (None, [JointId, C.c_float]),
+    "s2WeldJoint_SetAngularDampingRatio": (None, [JointId, C.c_float]),
+    "s2WeldJoint_GetLinearHertz": (C.c_float, [JointId]),
+    "s2WeldJoint_GetLinearDampingRatio": (C.c_float, [JointId]),
+    "s2WeldJoint_GetAngularHertz": (C.c_float, [JointId]),
+    "s2WeldJoint_GetAngularDampingRatio": (C.c_float, [JointId]),
     "s2CreatePrismaticJoint": (JointId, [WorldId, C.POINTER(PrismaticJointDef)]),
     "s2PrismaticJoint_EnableLimit": (None, [JointId, C.c_bool]),
     "s2PrismaticJoint_SetLimits": (None, [JointId, C.c_float, C.c_float]),

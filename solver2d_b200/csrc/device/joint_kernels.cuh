@@ -11,6 +11,11 @@
 // pose is its pose (a static body's aux0 row is never written)
 #define S2B_JC_STATIC_A 0x100
 #define S2B_JC_STATIC_B 0x200
+// row flags of the joint-constraint stream only: a weld row's angle / anchor constraint is a spring (DESIGN.md §3.15). XPBD
+// soft weld rows also carry S2B_JC_STATIC_A / _B.
+#define S2B_JC_SOFT_ANGULAR 0x400
+#define S2B_JC_SOFT_LINEAR 0x800
+#define S2B_JC_SOFT_WELD (S2B_JC_SOFT_ANGULAR | S2B_JC_SOFT_LINEAR)
 
 struct JointBodies
 {
@@ -42,6 +47,9 @@ enum JointPrepareKind
 	JPREP_SOFT = 1,	 // s2PrepareRevolute_Soft  (reference src/revolute_joint.c:421-506)
 	JPREP_XPBD = 2,	 // s2PrepareRevolute_XPBD  (reference src/revolute_joint.c:792-823)
 };
+
+// a weld row's soft parts (DESIGN.md §3.15), run at the end of the weld's prepare; defined with the soft weld below
+template <int KIND> __device__ __forceinline__ void s2bPrepareSoftWeld(const SolveArgs& a, int t, int slot);
 
 // Builds row t of the joint-constraint stream from joint slot `slot`. `warmStart` is the flag the *variant* passes
 // (TGS_Soft and SoftStep pass true regardless of the step flag, TGS_Sticky false; SURVEY §8a N3).
@@ -149,6 +157,7 @@ template <int KIND> __device__ __forceinline__ void s2bPrepareJointRows(const So
 		jc.pivot[t] = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
 		jc.imp[t] = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
 		jc.limp[t] = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
+		s2bPrepareSoftWeld<KIND>(a, t, slot);
 		return;
 	}
 
@@ -195,6 +204,10 @@ template <int KIND> __device__ __forceinline__ void s2bPrepareJointRows(const So
 	}
 	jc.imp[t] = imp;
 	jc.limp[t] = limp;
+	if (weld)
+	{
+		s2bPrepareSoftWeld<KIND>(a, t, slot);
+	}
 }
 
 // write the accumulated joint impulses back to the persistent joint columns
@@ -264,7 +277,79 @@ template <int KIND> __device__ __forceinline__ void s2bPrepareSpring(const Solve
 	*lambda = warmStart ? a.joints.imp[slot].w : 0.0f;
 }
 
-// Builds row t of the joint-constraint stream from joint slot `slot`: the joint's rows, then its spring.
+// ---------------------------------------------------------------------------------------------------------------
+// soft weld (extension, DESIGN.md §3.15; definition: tests/soft_weld_oracle.c). A weld row whose anchor or angle constraint
+// has a positive hertz replaces the rigid form of that row with a force law, the same in every velocity flavour and pass;
+// the NGS position pass skips a soft part and XPBD solves it as a compliant row with damping. Its impulse columns and warm
+// start are the weld's (angular imp.z, point imp.xy). A weld row with both hertz at 0 gets no marker and takes the weld's
+// own rows. Row lanes (s2bJointRow): the linear pair in hertz / dampingRatio, the angular pair in maxMotorTorque /
+// motorSpeed, so joints.motor = (angularHertz, angularDampingRatio, linearHertz, linearDampingRatio).
+// Stream lanes: jc.motor.xyz = the angular part's bias, mass scale, impulse scale (XPBD: 2 pi hertz h, damping ratio in
+// xy); jc.lim.yzw = the linear part's (XPBD: yz).
+// ---------------------------------------------------------------------------------------------------------------
+
+template <int KIND> __device__ __forceinline__ void s2bPrepareSoftWeld(const SolveArgs& a, int t, int slot)
+{
+	const JointConstraintView& jc = a.jc;
+	int4 head = jc.head[t];
+	if (S2B_JOINT_TYPE(head.x) != S2B_JOINT_WELD)
+	{
+		return;
+	}
+	float4 motor = a.joints.motor[slot];
+	bool softAngular = motor.x > 0.0f, softLinear = motor.z > 0.0f;
+	if (softAngular == false && softLinear == false)
+	{
+		return;
+	}
+	// the mouse joint's coefficients and expression order, for the step h every variant passes to its joint solve
+	float h = a.ctx.h;
+	float4 lim = jc.lim[t];
+	float4 coefA = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
+	int flags = head.x | (softAngular ? S2B_JC_SOFT_ANGULAR : 0) | (softLinear ? S2B_JC_SOFT_LINEAR : 0);
+	for (int part = 0; part < 2; ++part)
+	{
+		float hertz = part == 0 ? motor.x : motor.z;
+		float zeta = part == 0 ? motor.y : motor.w;
+		if ((hertz > 0.0f) == false)
+		{
+			continue;
+		}
+		float omega = 2.0f * s2_pi * hertz;
+		float x, y, z = 0.0f;
+		if (KIND == JPREP_XPBD)
+		{
+			x = omega * h;
+			y = zeta;
+		}
+		else
+		{
+			x = omega / (2.0f * zeta + h * omega);
+			float c = h * omega * (2.0f * zeta + h * omega);
+			z = 1.0f / (1.0f + c);
+			y = c * z;
+		}
+		if (part == 0)
+		{
+			coefA = make_float4(x, y, z, 0.0f);
+		}
+		else
+		{
+			lim = make_float4(lim.x, x, y, z);
+		}
+	}
+	if (KIND == JPREP_XPBD)
+	{
+		flags |= (S2B_BODY_TYPE(a.bodies.flags[head.y]) == S2B_BODY_STATIC ? S2B_JC_STATIC_A : 0) |
+				 (S2B_BODY_TYPE(a.bodies.flags[head.z]) == S2B_BODY_STATIC ? S2B_JC_STATIC_B : 0);
+	}
+	jc.head[t] = make_int4(flags, head.y, head.z, head.w);
+	jc.motor[t] = coefA;
+	jc.lim[t] = lim;
+}
+
+// Builds row t of the joint-constraint stream from joint slot `slot`: the joint's rows (a weld's with its soft parts), then
+// its spring.
 template <int KIND> __device__ __forceinline__ void s2bPrepareJoint(const SolveArgs& a, int t, int slot, bool warmStart)
 {
 	s2bPrepareJointRows<KIND>(a, t, slot, warmStart);
@@ -1074,7 +1159,14 @@ __device__ __forceinline__ void s2bSolveRevoluteVelocity(const SolveArgs& a, int
 			float impulseScale = 0.0f;
 			if (KIND == JSOLVE_SOFT)
 			{
-				if (useBias)
+				if (head.x & S2B_JC_SOFT_ANGULAR)
+				{
+					// a soft weld's angle spring (DESIGN.md §3.15): its own coefficients, in every pass
+					bias = motor.x * C;
+					massScale = motor.y;
+					impulseScale = motor.z;
+				}
+				else if (useBias)
 				{
 					bias = coef.x * C;
 					massScale = coef.y;
@@ -1193,13 +1285,15 @@ __device__ __forceinline__ void s2bSolveRevoluteVelocity(const SolveArgs& a, int
 		float impulseScale = 0.0f;
 		if (KIND == JSOLVE_SOFT)
 		{
-			if (useBias || motorJoint)
+			// a soft weld's anchor spring (DESIGN.md §3.15) takes its own coefficients in every pass
+			bool softLinear = (head.x & S2B_JC_SOFT_LINEAR) != 0;
+			if (useBias || motorJoint || softLinear)
 			{
 				s2Vec2 dcA = V2(poseA.x, poseA.y), dcB = V2(poseB.x, poseB.y);
 				s2Vec2 separation = s2Add(s2Add(s2Sub(dcB, dcA), s2Sub(rB, rA)), V2(d0.x, d0.y));
-				bias = s2MulSV(motorJoint ? motor.w * inv_h : coef.x, separation);
-				massScale = motorJoint ? 1.0f : coef.y;
-				impulseScale = motorJoint ? 0.0f : coef.z;
+				bias = s2MulSV(softLinear ? lim.y : (motorJoint ? motor.w * inv_h : coef.x), separation);
+				massScale = softLinear ? lim.z : (motorJoint ? 1.0f : coef.y);
+				impulseScale = softLinear ? lim.w : (motorJoint ? 0.0f : coef.z);
 			}
 		}
 		else
@@ -1252,6 +1346,286 @@ __device__ __forceinline__ void s2bSolveRevoluteVelocity(const SolveArgs& a, int
 	s2bStoreJointVelocities(a, ia, ib, velA, velB, vA, wA, vB, wB, mA, iA, mB, iB);
 }
 
+// ---------------------------------------------------------------------------------------------------------------
+// soft weld rows (DESIGN.md §3.15): a weld row with S2B_JC_SOFT_ANGULAR or S2B_JC_SOFT_LINEAR. The angular row, then the
+// point row, as the weld's; a soft part is the force law impulse = -k massScale (Cdot + bias C) - impulseScale lambda in
+// every velocity pass, a rigid part is the flavour's weld row, op for op. k is the weld's axial mass for the angular row
+// and, for the point row, the 2x2 effective mass the flavour's point row uses: fresh in the Baumgarte flavour, the
+// prepare-time pivot in the rigid flavour. The soft flavour needs no function of its own: its weld rows already have the
+// force law's form, and s2bSolveRevoluteVelocity gives them the soft parts' coefficients. The other two are kept apart
+// from s2bSolveRevoluteVelocity / s2bSolveRevoluteRigid, whose weld rows have another form, so that those rows' code
+// stays as it is.
+// ---------------------------------------------------------------------------------------------------------------
+enum SoftWeldForm
+{
+	SWELD_BAUMGARTE = 1, // PGS, TGS_Sticky
+	SWELD_RIGID = 2,	 // PGS_NGS, PGS_NGS_Block, TGS_NGS
+};
+
+template <int FORM> __device__ __forceinline__ void s2bSolveSoftWeldVelocity(const SolveArgs& a, int t, float inv_h)
+{
+	const JointConstraintView& jc = a.jc;
+	int4 head = jc.head[t];
+	int ia = head.y, ib = head.z;
+	float4 anchor = jc.anchor[t];
+	float4 mass = jc.mass[t];
+	float4 d0 = jc.d0ax[t];
+	float4 lim = jc.lim[t];
+	float4 imp = jc.imp[t];
+	float4 velA = a.bodies.vel[ia], velB = a.bodies.vel[ib];
+	float4 poseA = a.bodies.pose[ia], poseB = a.bodies.pose[ib];
+	s2Vec2 vA = V2(velA.x, velA.y), vB = V2(velB.x, velB.y);
+	float wA = velA.z, wB = velB.z;
+	float mA = mass.x, iA = mass.y, mB = mass.z, iB = mass.w;
+	float axialMass = d0.z;
+	s2Rot qA = R2(poseA.z, poseA.w), qB = R2(poseB.z, poseB.w);
+	bool softLinear = (head.x & S2B_JC_SOFT_LINEAR) != 0;
+
+	// angular row
+	if (iA + iB != 0.0f)
+	{
+		float impulse;
+		if (head.x & S2B_JC_SOFT_ANGULAR)
+		{
+			float4 sc = jc.motor[t]; // bias, mass scale, impulse scale
+			float C = s2UnwindAngle(s2RelativeAngle(qB, qA) - lim.x);
+			float Cdot = wB - wA;
+			impulse = -axialMass * sc.y * (Cdot + sc.x * C) - sc.z * imp.z;
+		}
+		else if (FORM == SWELD_BAUMGARTE)
+		{
+			float C = s2UnwindAngle(s2RelativeAngle(qB, qA) - lim.x);
+			float bias = s2_baumgarte * inv_h * C;
+			float Cdot = wB - wA;
+			impulse = -axialMass * (Cdot + bias);
+		}
+		else
+		{
+			impulse = -axialMass * (wB - wA);
+		}
+		imp.z += impulse;
+		wA -= iA * impulse;
+		wB += iB * impulse;
+	}
+
+	// point row
+	{
+		s2Vec2 rA = s2RotateVector(qA, V2(anchor.x, anchor.y));
+		s2Vec2 rB = s2RotateVector(qB, V2(anchor.z, anchor.w));
+		s2Vec2 Cdot = s2Sub(s2Add(vB, s2CrossSV(wB, rB)), s2Add(vA, s2CrossSV(wA, rA)));
+		s2Vec2 bias = V2(0.0f, 0.0f);
+		float massScale = 1.0f;
+		float impulseScale = 0.0f;
+		if (softLinear || FORM == SWELD_BAUMGARTE)
+		{
+			s2Vec2 dcA = V2(poseA.x, poseA.y), dcB = V2(poseB.x, poseB.y);
+			s2Vec2 separation = s2Add(s2Add(s2Sub(dcB, dcA), s2Sub(rB, rA)), V2(d0.x, d0.y));
+			if (softLinear)
+			{
+				bias = s2MulSV(lim.y, separation);
+				massScale = lim.z;
+				impulseScale = lim.w;
+			}
+			else
+			{
+				bias = s2MulSV(s2_baumgarte * inv_h, separation);
+			}
+		}
+
+		s2Vec2 b;
+		if (FORM == SWELD_RIGID)
+		{
+			float4 pv = jc.pivot[t];
+			s2Mat22 pivot;
+			pivot.cx = V2(pv.x, pv.y);
+			pivot.cy = V2(pv.z, pv.w);
+			b = s2MulMV(pivot, softLinear ? s2Add(Cdot, bias) : s2Neg(Cdot));
+		}
+		else
+		{
+			s2Mat22 K;
+			K.cx.x = mA + mB + rA.y * rA.y * iA + rB.y * rB.y * iB;
+			K.cy.x = -rA.y * rA.x * iA - rB.y * rB.x * iB;
+			K.cx.y = K.cy.x;
+			K.cy.y = mA + mB + rA.x * rA.x * iA + rB.x * rB.x * iB;
+			b = s2Solve22(K, s2Add(Cdot, bias));
+		}
+
+		s2Vec2 impulse;
+		if (softLinear)
+		{
+			impulse.x = -massScale * b.x - impulseScale * imp.x;
+			impulse.y = -massScale * b.y - impulseScale * imp.y;
+		}
+		else if (FORM == SWELD_BAUMGARTE)
+		{
+			impulse.x = -b.x;
+			impulse.y = -b.y;
+		}
+		else
+		{
+			impulse = b; // pivot (-Cdot)
+		}
+		imp.x += impulse.x;
+		imp.y += impulse.y;
+		vA = s2MulSub(vA, mA, impulse);
+		wA -= iA * s2Cross(rA, impulse);
+		vB = s2MulAdd(vB, mB, impulse);
+		wB += iB * s2Cross(rB, impulse);
+	}
+
+	jc.imp[t] = imp;
+	s2bStoreJointVelocities(a, ia, ib, velA, velB, vA, wA, vB, wB, mA, iA, mB, iB);
+}
+
+// The NGS position pass: a soft part has no position row (as the mouse joint and the springs); a rigid part is the weld's
+// correction (s2bSolveJointPosition), the angle first.
+__device__ __forceinline__ void s2bSolveSoftWeldPosition(const SolveArgs& a, int t)
+{
+	const JointConstraintView& jc = a.jc;
+	int4 head = jc.head[t];
+	if ((head.x & S2B_JC_SOFT_WELD) == S2B_JC_SOFT_WELD)
+	{
+		return;
+	}
+	int ia = head.y, ib = head.z;
+	float4 anchor = jc.anchor[t];
+	float4 mass = jc.mass[t];
+	float4 d0 = jc.d0ax[t];
+	float4 poseA = a.bodies.pose[ia], poseB = a.bodies.pose[ib];
+	s2Vec2 dcA = V2(poseA.x, poseA.y), dcB = V2(poseB.x, poseB.y);
+	s2Rot qA = R2(poseA.z, poseA.w), qB = R2(poseB.z, poseB.w);
+	float mA = mass.x, iA = mass.y, mB = mass.z, iB = mass.w;
+
+	// at least one part is soft: a rigid angle (then the anchor is soft) or a rigid anchor (then the angle is soft)
+	if ((head.x & S2B_JC_SOFT_ANGULAR) == 0)
+	{
+		if (iA + iB != 0.0f)
+		{
+			float C = s2UnwindAngle(s2RelativeAngle(qB, qA) - jc.lim[t].x);
+			float p = -d0.z * S2_CLAMP(C, -s2_maxAngularCorrection, s2_maxAngularCorrection);
+			qA = s2IntegrateRot(qA, -iA * p);
+			qB = s2IntegrateRot(qB, iB * p);
+		}
+	}
+	else
+	{
+		s2Vec2 rA = s2RotateVector(qA, V2(anchor.x, anchor.y));
+		s2Vec2 rB = s2RotateVector(qB, V2(anchor.z, anchor.w));
+		s2Vec2 C = s2Add(s2Add(s2Sub(dcB, dcA), s2Sub(rB, rA)), V2(d0.x, d0.y));
+		s2Mat22 K;
+		K.cx.x = mA + mB + iA * rA.y * rA.y + iB * rB.y * rB.y;
+		K.cx.y = -iA * rA.x * rA.y - iB * rB.x * rB.y;
+		K.cy.x = K.cx.y;
+		K.cy.y = mA + mB + iA * rA.x * rA.x + iB * rB.x * rB.x;
+		s2Vec2 impulse = s2Solve22(K, s2Neg(C));
+		dcA = s2MulSub(dcA, mA, impulse);
+		qA = s2IntegrateRot(qA, -iA * s2Cross(rA, impulse));
+		dcB = s2MulAdd(dcB, mB, impulse);
+		qB = s2IntegrateRot(qB, iB * s2Cross(rB, impulse));
+	}
+
+	if ((mA != 0.0f) || (iA != 0.0f))
+	{
+		a.bodies.pose[ia] = make_float4(dcA.x, dcA.y, qA.s, qA.c);
+	}
+	if ((mB != 0.0f) || (iB != 0.0f))
+	{
+		a.bodies.pose[ib] = make_float4(dcB.x, dcB.y, qB.s, qB.c);
+	}
+}
+
+// XPBD with damping (Macklin et al. 2016), as the springs' (§3.14): w the row's generalized inverse mass, C and C0 the error
+// now and at the sub-step's start pose, omegaH = 2 pi hertz h
+__device__ __forceinline__ float s2bSoftWeldXpbdImpulse(float w, float C, float C0, float omegaH, float zeta)
+{
+	float alphaTilde = w / (omegaH * omegaH);
+	float gamma = 2.0f * zeta / omegaH;
+	return -(C + gamma * (C - C0)) / ((1.0f + gamma) * w + alphaTilde);
+}
+
+// XPBD: the weld's rows (s2bSolveJointXpbd), a soft part compliant with damping. The start pose is aux0 (dp0, q0), or a
+// static body's own pose. The linear row acts along n = separation / |separation| with C = |separation| and C0 = n . the
+// separation at the start pose.
+__device__ __forceinline__ void s2bSolveSoftWeldXpbd(const SolveArgs& a, int t)
+{
+	const float compliance = 0.0f;
+	const JointConstraintView& jc = a.jc;
+	int4 head = jc.head[t];
+	int ia = head.y, ib = head.z;
+	float4 anchor = jc.anchor[t];
+	float4 mass = jc.mass[t];
+	float4 d0 = jc.d0ax[t];
+	float4 lim = jc.lim[t];
+	float4 poseA = a.bodies.pose[ia], poseB = a.bodies.pose[ib];
+	float4 p0A = (head.x & S2B_JC_STATIC_A) != 0 ? poseA : a.bodies.aux0[ia];
+	float4 p0B = (head.x & S2B_JC_STATIC_B) != 0 ? poseB : a.bodies.aux0[ib];
+	s2Vec2 dcA = V2(poseA.x, poseA.y), dcB = V2(poseB.x, poseB.y);
+	s2Rot qA = R2(poseA.z, poseA.w), qB = R2(poseB.z, poseB.w);
+	s2Rot q0A = R2(p0A.z, p0A.w), q0B = R2(p0B.z, p0B.w);
+	float mA = mass.x, iA = mass.y, mB = mass.z, iB = mass.w;
+	if (iA + iB != 0.0f)
+	{
+		float C = s2UnwindAngle(s2RelativeAngle(qB, qA) - lim.x);
+		float p;
+		if (head.x & S2B_JC_SOFT_ANGULAR)
+		{
+			float4 sc = jc.motor[t]; // 2 pi hertz h, damping ratio
+			float C0 = s2UnwindAngle(s2RelativeAngle(q0B, q0A) - lim.x);
+			p = s2bSoftWeldXpbdImpulse(iA + iB, C, C0, sc.x, sc.y);
+		}
+		else
+		{
+			p = -C / (iA + iB);
+		}
+		qA = s2IntegrateRot(qA, -iA * p);
+		qB = s2IntegrateRot(qB, iB * p);
+	}
+	s2Vec2 rA = s2RotateVector(qA, V2(anchor.x, anchor.y));
+	s2Vec2 rB = s2RotateVector(qB, V2(anchor.z, anchor.w));
+	s2Vec2 separation = s2Add(s2Add(s2Sub(dcB, dcA), s2Sub(rB, rA)), V2(d0.x, d0.y));
+	float c = s2Length(separation);
+	s2Vec2 n = V2(0.0f, 0.0f);
+	if (c >= 0.001f * 1.1920929e-07f)
+	{
+		float invLength = 1.0f / c;
+		n = V2(invLength * separation.x, invLength * separation.y);
+	}
+	if (mA == 0.0f && mB == 0.0f)
+	{
+		return;
+	}
+	float rnA = s2Cross(rA, n);
+	float rnB = s2Cross(rB, n);
+	float kA = mA + iA * rnA * rnA;
+	float kB = mB + iB * rnB * rnB;
+	float lambda;
+	if (head.x & S2B_JC_SOFT_LINEAR)
+	{
+		s2Vec2 rA0 = s2RotateVector(q0A, V2(anchor.x, anchor.y));
+		s2Vec2 rB0 = s2RotateVector(q0B, V2(anchor.z, anchor.w));
+		s2Vec2 separation0 = s2Add(s2Add(s2Sub(V2(p0B.x, p0B.y), V2(p0A.x, p0A.y)), s2Sub(rB0, rA0)), V2(d0.x, d0.y));
+		lambda = s2bSoftWeldXpbdImpulse(kA + kB, c, s2Dot(n, separation0), lim.y, lim.z);
+	}
+	else
+	{
+		lambda = -c / (kA + kB + compliance);
+	}
+	s2Vec2 p = s2MulSV(lambda, n);
+	dcA = s2MulSub(dcA, mA, p);
+	qA = s2IntegrateRot(qA, -iA * s2Cross(rA, p));
+	dcB = s2MulAdd(dcB, mB, p);
+	qB = s2IntegrateRot(qB, iB * s2Cross(rB, p));
+	if ((mA != 0.0f) || (iA != 0.0f))
+	{
+		a.bodies.pose[ia] = make_float4(dcA.x, dcA.y, qA.s, qA.c);
+	}
+	if ((mB != 0.0f) || (iB != 0.0f))
+	{
+		a.bodies.pose[ib] = make_float4(dcB.x, dcB.y, qB.s, qB.c);
+	}
+}
+
 // s2SolveJoint_Soft dispatch (reference src/joint.c:385-405): the mouse joint is solved only in the biased pass. A motor
 // joint is solved in every pass, by the revolute's soft rows when SHARED_MOTOR (the persistent kernels), else by
 // s2bSolveMotorVelocity (the launch-by-launch kernel, whose every-op build spills less that way). Both give the same bits.
@@ -1281,6 +1655,7 @@ __device__ __forceinline__ void s2bSolveJointSoft(const SolveArgs& a, int t, flo
 		s2bSolveMotorVelocity(a, t, h, inv_h);
 		return;
 	}
+	// a soft weld's rows are the revolute soft rows with its own coefficients (DESIGN.md §3.15)
 	s2bSolveRevoluteVelocity<JSOLVE_SOFT, SHARED_MOTOR>(a, t, h, inv_h, useBias);
 }
 
@@ -1305,6 +1680,11 @@ __device__ __forceinline__ void s2bSolveJointBaumgarte(const SolveArgs& a, int t
 	if (S2B_JOINT_TYPE(flags) == S2B_JOINT_MOTOR)
 	{
 		s2bSolveMotorVelocity(a, t, h, inv_h);
+		return;
+	}
+	if (flags & S2B_JC_SOFT_WELD)
+	{
+		s2bSolveSoftWeldVelocity<SWELD_BAUMGARTE>(a, t, inv_h);
 		return;
 	}
 	s2bSolveRevoluteVelocity<JSOLVE_BAUMGARTE, false>(a, t, h, inv_h, useBias);
@@ -1424,6 +1804,11 @@ __device__ __forceinline__ void s2bSolveJointRigid(const SolveArgs& a, int t, fl
 		s2bSolveMotorVelocity(a, t, h, a.ctx.inv_h);
 		return;
 	}
+	if (a.jc.head[t].x & S2B_JC_SOFT_WELD)
+	{
+		s2bSolveSoftWeldVelocity<SWELD_RIGID>(a, t, 0.0f /* inv_h: unused by the rigid rows */);
+		return;
+	}
 	s2bSolveRevoluteRigid(a, t, h);
 }
 
@@ -1442,6 +1827,11 @@ __device__ __forceinline__ void s2bSolveJointPosition(const SolveArgs& a, int t)
 	if (S2B_JOINT_TYPE(head.x) == S2B_JOINT_PRISMATIC)
 	{
 		s2bSolvePrismaticPosition(a, t);
+		return;
+	}
+	if (head.x & S2B_JC_SOFT_WELD)
+	{
+		s2bSolveSoftWeldPosition(a, t);
 		return;
 	}
 	int ia = head.y, ib = head.z;
@@ -1536,6 +1926,11 @@ __device__ __forceinline__ void s2bSolveJointXpbd(const SolveArgs& a, int t)
 	if (S2B_JOINT_TYPE(head.x) == S2B_JOINT_MOTOR)
 	{
 		s2bSolveMotorXpbd(a, t);
+		return;
+	}
+	if (head.x & S2B_JC_SOFT_WELD)
+	{
+		s2bSolveSoftWeldXpbd(a, t);
 		return;
 	}
 	const float compliance = 0.0f;

@@ -77,10 +77,21 @@ s2JointId s2CreateRevoluteJoint(s2WorldId worldId, const s2RevoluteJointDef* def
 	return jointId;
 }
 
+static bool s2IsValidSpringValue(float value)
+{
+	return s2IsValid(value) && value >= 0.0f;
+}
+
 // The weld has no counterpart in the reference. Its row carries no limit or motor flags; like a revolute joint created
-// with collideConnected == false it removes the contacts that already exist between its bodies.
+// with collideConnected == false it removes the contacts that already exist between its bodies. A negative or non-finite
+// hertz or damping ratio creates nothing and returns s2_nullJointId.
 s2JointId s2CreateWeldJoint(s2WorldId worldId, const s2WeldJointDef* def)
 {
+	if (s2IsValidSpringValue(def->linearHertz) == false || s2IsValidSpringValue(def->linearDampingRatio) == false ||
+		s2IsValidSpringValue(def->angularHertz) == false || s2IsValidSpringValue(def->angularDampingRatio) == false)
+	{
+		return s2_nullJointId;
+	}
 	s2World* world = s2GetWorldFromId(worldId);
 	s2Body* bodyA = world->bodies + def->bodyIdA.index;
 	s2Body* bodyB = world->bodies + def->bodyIdB.index;
@@ -92,6 +103,10 @@ s2JointId s2CreateWeldJoint(s2WorldId worldId, const s2WeldJointDef* def)
 	joint->localOriginAnchorB = def->localAnchorB;
 	joint->referenceAngle = def->referenceAngle;
 	joint->collideConnected = def->collideConnected;
+	joint->linearHertz = def->linearHertz;
+	joint->linearDampingRatio = def->linearDampingRatio;
+	joint->angularHertz = def->angularHertz;
+	joint->angularDampingRatio = def->angularDampingRatio;
 
 	s2JointId jointId = {joint->object.index, world->index, joint->object.revision};
 	return jointId;
@@ -167,11 +182,6 @@ float s2RevoluteJoint_GetMotorTorque(s2JointId jointId, float inverseTimeStep)
 
 // ---- joint springs (DESIGN.md §3.14): revolute and prismatic joints; hertz and dampingRatio carry the spring ---------------
 
-static bool s2IsValidSpringValue(float value)
-{
-	return s2IsValid(value) && value >= 0.0f;
-}
-
 static void s2EnableJointSpring(s2JointId jointId, s2JointType type, bool enableSpring)
 {
 	s2World* world;
@@ -235,6 +245,95 @@ void s2PrismaticJoint_SetSpringHertz(s2JointId jointId, float hertz)
 void s2PrismaticJoint_SetSpringDampingRatio(s2JointId jointId, float dampingRatio)
 {
 	s2SetJointSpringValue(jointId, s2_prismaticJoint, dampingRatio, true);
+}
+
+// ---- soft weld (DESIGN.md §3.15): the weld's anchor and angle springs ------------------------------------------------------
+
+enum
+{
+	s2_weldLinearHertz,
+	s2_weldLinearDampingRatio,
+	s2_weldAngularHertz,
+	s2_weldAngularDampingRatio,
+};
+
+static float* s2WeldSpringField(s2Joint* joint, int field)
+{
+	switch (field)
+	{
+		case s2_weldLinearHertz:
+			return &joint->linearHertz;
+		case s2_weldLinearDampingRatio:
+			return &joint->linearDampingRatio;
+		case s2_weldAngularHertz:
+			return &joint->angularHertz;
+		default:
+			return &joint->angularDampingRatio;
+	}
+}
+
+static void s2SetWeldSpringValue(s2JointId jointId, int field, float value)
+{
+	if (s2IsValidSpringValue(value) == false)
+	{
+		return; // rejected: the joint keeps its value
+	}
+	s2World* world;
+	s2Joint* joint = s2GetJointForEdit(jointId, &world);
+	if (joint->type != s2_weldJoint)
+	{
+		return;
+	}
+	*s2WeldSpringField(joint, field) = value;
+	s2MarkJointDirty(world, joint);
+}
+
+static float s2GetWeldSpringValue(s2JointId jointId, int field)
+{
+	s2World* world = s2GetWorldFromIndex(jointId.world);
+	s2Joint* joint = world->joints + jointId.index;
+	S2_ASSERT(s2ObjectValid(&joint->object) && joint->object.revision == jointId.revision);
+	return joint->type == s2_weldJoint ? *s2WeldSpringField(joint, field) : 0.0f;
+}
+
+void s2WeldJoint_SetLinearHertz(s2JointId jointId, float hertz)
+{
+	s2SetWeldSpringValue(jointId, s2_weldLinearHertz, hertz);
+}
+
+void s2WeldJoint_SetLinearDampingRatio(s2JointId jointId, float dampingRatio)
+{
+	s2SetWeldSpringValue(jointId, s2_weldLinearDampingRatio, dampingRatio);
+}
+
+void s2WeldJoint_SetAngularHertz(s2JointId jointId, float hertz)
+{
+	s2SetWeldSpringValue(jointId, s2_weldAngularHertz, hertz);
+}
+
+void s2WeldJoint_SetAngularDampingRatio(s2JointId jointId, float dampingRatio)
+{
+	s2SetWeldSpringValue(jointId, s2_weldAngularDampingRatio, dampingRatio);
+}
+
+float s2WeldJoint_GetLinearHertz(s2JointId jointId)
+{
+	return s2GetWeldSpringValue(jointId, s2_weldLinearHertz);
+}
+
+float s2WeldJoint_GetLinearDampingRatio(s2JointId jointId)
+{
+	return s2GetWeldSpringValue(jointId, s2_weldLinearDampingRatio);
+}
+
+float s2WeldJoint_GetAngularHertz(s2JointId jointId)
+{
+	return s2GetWeldSpringValue(jointId, s2_weldAngularHertz);
+}
+
+float s2WeldJoint_GetAngularDampingRatio(s2JointId jointId)
+{
+	return s2GetWeldSpringValue(jointId, s2_weldAngularDampingRatio);
 }
 
 // The prismatic joint has no counterpart in the reference (DESIGN.md §3.9). Degenerate input creates nothing and returns

@@ -178,6 +178,9 @@ typedef struct s2Joint
 	// enableSpring as the device's last uploaded row has it: the reaction getters pair it with the synced impulses, which
 	// that row produced (a setter call between steps changes enableSpring but not yet the row)
 	bool springUploaded;
+	// weld: the soft parts (DESIGN.md §3.15), 0 hertz = rigid. s2FillJointRow moves them into the row lanes a weld row
+	// leaves free (hertz / dampingRatio, maxMotorTorque / motorSpeed).
+	float linearHertz, linearDampingRatio, angularHertz, angularDampingRatio;
 	s2Vec2 targetA;
 	// accumulated impulses (cache of the device columns)
 	s2Vec2 impulse;

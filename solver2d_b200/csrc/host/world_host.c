@@ -274,6 +274,14 @@ static void s2FillJointRow(s2bJointRow* r, const s2Joint* j)
 	r->localAxisA[1] = j->localAxisA.y;
 	r->breakForce = j->breakForce;
 	r->breakTorque = j->breakTorque;
+	if (j->type == s2_weldJoint)
+	{
+		// a weld row has no limit, motor or spring: its soft parts ride in those lanes (DESIGN.md §3.15)
+		r->hertz = j->linearHertz;
+		r->dampingRatio = j->linearDampingRatio;
+		r->maxMotorTorque = j->angularHertz;
+		r->motorSpeed = j->angularDampingRatio;
+	}
 }
 
 static int s2CompareU64(const void* a, const void* b)

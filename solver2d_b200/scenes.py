@@ -654,6 +654,128 @@ def welded_structures(lib: capi.Solver2D, solver="TGS_Soft", copies=1, platform=
     return sc
 
 
+SOFT_WELDS_PITCH = 30.0  # width of one copy of soft_welds (m)
+
+
+def soft_welds(lib: capi.Solver2D, solver="TGS_Soft", copies=1, kinematic=True) -> Scene:
+    """Soft weld coverage (DESIGN.md §3.15), `copies` side by side (34 bodies each). Per copy:
+
+    * a donut: a ring of eight capsules welded end to end with angular springs (and a stiff anchor spring on one weld),
+      dropped onto a small pile;
+    * two cantilevers of four boxes welded to a static wall: one soft (angular springs), one rigid; in the soft one the
+      boxes alternate between angle 0 and 3 rad, so its welds have reference angles of +3 and -3 rad (near +-pi);
+    * a box hanging from a static body on a linear-only soft weld;
+    * with `kinematic`: a box on a platform that moves sideways, held by a soft weld (both parts);
+    * a hanging chain of three revolute links, and (first copy only) a mouse joint pulling the donut.
+
+    On a library without s2CreateWeldJoint (the reference) every weld is created as a revolute joint with limits and
+    motor off, with the same bodies, anchors, reference angle and collideConnected, as ``welded_structures`` does.
+    ``sc.piles["welds"]`` lists the indices into ``sc.joints`` of every weld, soft or rigid; ``sc.piles["soft_welds"]``
+    lists one (joint index, linearHertz, linearDampingRatio, angularHertz, angularDampingRatio) per soft weld, so that a
+    test can turn the stand-in rows into soft weld rows."""
+    world = lib.create_world(solver)
+    sc = Scene(lib, world, name=f"soft_welds{copies}")
+    sc.piles["welds"] = []
+    sc.piles["soft_welds"] = []
+    has_weld = "s2CreateWeldJoint" not in lib.missing
+    gid = _ground(lib, world, 0.5 * SOFT_WELDS_PITCH * copies + 5.0)
+    sc.bodies.append(gid)
+    sd = default_shape_def()
+
+    def body(kind, x, y, angle=0.0, hx=0.5, hy=0.125, vx=0.0, capsule=None):
+        bd = default_body_def()
+        bd.type = kind
+        bd.position = Vec2(x, y)
+        bd.angle = angle
+        bd.linearVelocity = Vec2(vx, 0.0)
+        bid = lib.s2CreateBody(world, C.byref(bd))
+        if capsule is not None:
+            cap = Capsule(Vec2(-capsule[0], 0.0), Vec2(capsule[0], 0.0), capsule[1])
+            lib.s2CreateCapsuleShape(bid, C.byref(sd), C.byref(cap))
+        else:
+            box = lib.s2MakeBox(hx, hy)
+            lib.s2CreatePolygonShape(bid, C.byref(sd), C.byref(box))
+        sc.bodies.append(bid)
+        return bid
+
+    def weld(a, b, pivot, reference_angle, linear=(0.0, 0.0), angular=(0.0, 0.0)):
+        jd = capi.default_weld_def() if has_weld else default_revolute_def()
+        jd.bodyIdA = a
+        jd.bodyIdB = b
+        jd.localAnchorA = lib.s2Body_GetLocalPoint(a, pivot)
+        jd.localAnchorB = lib.s2Body_GetLocalPoint(b, pivot)
+        jd.referenceAngle = reference_angle
+        if has_weld:
+            jd.linearHertz, jd.linearDampingRatio = linear
+            jd.angularHertz, jd.angularDampingRatio = angular
+        create = lib.s2CreateWeldJoint if has_weld else lib.s2CreateRevoluteJoint
+        sc.piles["welds"].append(len(sc.joints))
+        if linear[0] > 0.0 or angular[0] > 0.0:
+            sc.piles["soft_welds"].append((len(sc.joints),) + tuple(linear) + tuple(angular))
+        sc.joints.append(create(world, C.byref(jd)))
+
+    D, S, K = capi.DYNAMIC_BODY, capi.STATIC_BODY, capi.KINEMATIC_BODY
+    for k in range(copies):
+        x0 = -0.5 * SOFT_WELDS_PITCH * (copies - 1) + SOFT_WELDS_PITCH * k - 10.0
+        # a small pile with a donut above it: eight capsules on a ring of radius 1.2, each welded to the next at their
+        # shared end point with an angular spring
+        for i in range(4):
+            for j in range(2):
+                body(D, x0 + 0.5 + 1.05 * i, 0.25 + 0.5 * j, hx=0.5, hy=0.25)
+        n, radius, cx, cy = 8, 1.2, x0 + 2.0, 4.0
+        half = radius * math.sin(math.pi / n)
+        ring = []
+        for i in range(n):
+            t = 2.0 * math.pi * (i + 0.5) / n
+            ring.append(body(D, cx + radius * math.cos(math.pi / n) * math.cos(t), cy + radius * math.cos(math.pi / n) * math.sin(t),
+                             angle=t + 0.5 * math.pi, capsule=(half, 0.15)))
+        for i in range(n):
+            t = 2.0 * math.pi * (i + 1) / n
+            pivot = Vec2(cx + radius * math.cos(t), cy + radius * math.sin(t))
+            weld(ring[i], ring[(i + 1) % n], pivot, 2.0 * math.pi / n if i < n - 1 else 2.0 * math.pi / n - 2.0 * math.pi,
+                 linear=(15.0, 1.0) if i == 0 else (0.0, 0.0), angular=(4.0, 0.3))
+        # cantilevers: the soft one at y = 9 with reference angles near +-pi, the rigid one at y = 7
+        for beam, y in enumerate((9.0, 7.0)):
+            wall = body(S, x0 + 6.0, y, hx=0.25, hy=1.0)
+            prev, prev_angle = wall, 0.0
+            for i in range(4):
+                angle = 3.0 if beam == 0 and i % 2 == 0 else 0.0
+                bid = body(D, x0 + 6.75 + 1.0 * i, y, angle=angle)
+                weld(prev, bid, Vec2(x0 + 6.25 + 1.0 * i, y), angle - prev_angle,
+                     angular=(3.0 + 0.5 * i, 0.2) if beam == 0 else (0.0, 0.0))
+                prev, prev_angle = bid, angle
+        # a box hanging on a linear-only soft weld
+        hook = body(S, x0 + 13.0, 8.0, hx=0.25, hy=0.25)
+        box = body(D, x0 + 13.0, 7.25, hx=0.25, hy=0.25)
+        weld(hook, box, Vec2(x0 + 13.0, 7.5), 0.0, linear=(2.0, 0.1))
+        if kinematic:
+            p = body(K, x0 + 16.0, 2.0, hx=1.0, hy=0.125, vx=0.5)
+            q = body(D, x0 + 16.0, 2.0 + 0.375, hx=0.25, hy=0.25)
+            weld(p, q, Vec2(x0 + 16.0, 2.0 + 0.125), 0.0, linear=(5.0, 0.5), angular=(2.0, 0.7))
+        # revolute chain
+        anchor = body(S, x0 + 19.0, 10.0, hx=0.25, hy=0.25)
+        prev = anchor
+        for i in range(3):
+            bid = body(D, x0 + 19.5 + 1.0 * i, 10.0)
+            jd = default_revolute_def()
+            pivot = Vec2(x0 + 19.0 + 1.0 * i, 10.0)
+            jd.bodyIdA = prev
+            jd.bodyIdB = bid
+            jd.localAnchorA = lib.s2Body_GetLocalPoint(prev, pivot)
+            jd.localAnchorB = lib.s2Body_GetLocalPoint(bid, pivot)
+            sc.joints.append(lib.s2CreateRevoluteJoint(world, C.byref(jd)))
+            prev = bid
+        if k == 0:
+            md = default_mouse_def()
+            md.bodyIdA = gid
+            md.bodyIdB = ring[0]
+            md.target = Vec2(cx + 1.5, cy + 1.0)
+            md.hertz = 2.0
+            md.dampingRatio = 0.7
+            sc.joints.append(lib.s2CreateMouseJoint(world, C.byref(md)))
+    return sc
+
+
 SLIDERS_PITCH = 32.0  # width of one copy of sliders (m)
 
 
