@@ -105,12 +105,14 @@ enum
 	S2B_JOINT_WELD = 2, // never carries S2B_JOINT_ENABLE_LIMIT or S2B_JOINT_ENABLE_MOTOR
 	S2B_JOINT_PRISMATIC = 3,
 	S2B_JOINT_MOTOR = 4, // never carries S2B_JOINT_ENABLE_LIMIT or S2B_JOINT_ENABLE_MOTOR
+	S2B_JOINT_DISTANCE = 5,
 };
 
 #define S2B_JOINT_ENABLE_LIMIT 0x10
 #define S2B_JOINT_ENABLE_MOTOR 0x20
 #define S2B_JOINT_COLLIDE_CONNECTED 0x40
-// revolute and prismatic rows only: a spring on the joint's axis (DESIGN.md §3.14), stiffness hertz, damping dampingRatio
+// revolute, prismatic and distance rows only: a spring on the joint's axis (DESIGN.md §3.14, §3.16), stiffness hertz,
+// damping dampingRatio
 #define S2B_JOINT_ENABLE_SPRING 0x80
 
 // One joint; mirrors s2Joint / s2RevoluteJoint / s2MouseJoint (reference src/joint.h:28-102).
@@ -139,6 +141,10 @@ typedef struct s2bJointRow
 	// A weld row (which never carries the limit, motor or spring flag) holds its soft parts (DESIGN.md §3.15): the anchor
 	// spring's stiffness (Hz) in hertz and its damping ratio in dampingRatio, the angle spring's stiffness (Hz) in
 	// maxMotorTorque and its damping ratio in motorSpeed. A hertz of 0 makes that part rigid.
+	// A distance row (DESIGN.md §3.16) holds its rest length in referenceAngle, its min / max length in lowerAngle /
+	// upperAngle, its maximum motor force (N) in maxMotorTorque and its spring (S2B_JOINT_ENABLE_SPRING) in hertz /
+	// dampingRatio; impulse[0] is the rigid length row's impulse, impulse[1] stays 0, and motorImpulse / lowerImpulse /
+	// upperImpulse / springImpulse are the axial impulses their names say.
 	float localAxisA[2];
 	// break thresholds (N, N-m) of the reaction pass (DESIGN.md §3.13); 0 = none. A row with either set is checked after every
 	// finalize; a row without them is never checked.

@@ -3,6 +3,7 @@
 #pragma once
 
 #include "s2b_device.h"
+#include "solver2d/constants.h"
 #include "solver2d/distance.h"
 #include "solver2d/geometry.h"
 #include "solver2d/id.h"
@@ -169,6 +170,67 @@ S2B_API s2Vec2 s2MotorJoint_GetConstraintForce(s2JointId jointId, float inverseT
 // The angular impulse of the last step times inverseTimeStep (N-m).
 S2B_API float s2MotorJoint_GetConstraintTorque(s2JointId jointId, float inverseTimeStep);
 
+// Distance joint (DESIGN.md §3.16; Box2D v3's semantics): holds anchor B at a distance from anchor A along the line between
+// them, which turns as the bodies move. Rows, all along that line: a spring toward `length` (enableSpring, acts when
+// minLength < maxLength and hertz > 0), a motor (enableMotor: drives the rate of change of the length to motorSpeed with at
+// most maxMotorForce), a lower and an upper limit (enableLimit, when minLength < maxLength) and a rigid row toward `length`
+// (whenever the spring is off or minLength == maxLength). A rope is enableSpring with hertz 0 and a limit: free inside
+// [minLength, maxLength], taut at maxLength. Anchors are relative to each body's origin. Under XPBD the motor is not applied.
+// Destroy it with s2DestroyJoint.
+typedef struct s2DistanceJointDef
+{
+	s2BodyId bodyIdA;
+	s2BodyId bodyIdB;
+	s2Vec2 localAnchorA;
+	s2Vec2 localAnchorB;
+	float length; // rest length (m)
+	bool enableSpring;
+	float hertz;		// the spring's stiffness as a frequency (Hz), >= 0; 0 exerts nothing
+	float dampingRatio; // the spring's damping ratio, >= 0 (1 = critical)
+	bool enableLimit;
+	float minLength; // m
+	float maxLength; // m
+	bool enableMotor;
+	float maxMotorForce; // N, >= 0
+	float motorSpeed;	 // m/s, positive lengthens
+	bool collideConnected; // keep the contacts the two bodies already have
+} s2DistanceJointDef;
+
+S2_INLINE struct s2DistanceJointDef s2DefaultDistanceJointDef(void)
+{
+	s2DistanceJointDef def = S2_ZERO_INIT;
+	def.bodyIdA = s2_nullBodyId;
+	def.bodyIdB = s2_nullBodyId;
+	def.length = 1.0f;
+	def.maxLength = s2_huge;
+	return def;
+}
+
+// Returns s2_nullJointId (and creates nothing) for any non-finite value, a negative length, minLength, hertz, dampingRatio or
+// maxMotorForce, or minLength > maxLength. Otherwise length, minLength and maxLength are each clamped into
+// [s2_linearSlop, s2_huge], as Box2D does: a rest length below the slop would leave the line between the anchors undefined.
+S2B_API s2JointId s2CreateDistanceJoint(s2WorldId worldId, const s2DistanceJointDef* def);
+// The setters ignore a non-finite or negative value (the joint keeps its value) and a joint that is not a distance joint;
+// lengths are clamped as at creation. A change takes effect at the next step. The getters return 0 for another type.
+S2B_API void s2DistanceJoint_SetLength(s2JointId jointId, float length);
+S2B_API float s2DistanceJoint_GetLength(s2JointId jointId);
+S2B_API void s2DistanceJoint_EnableLimit(s2JointId jointId, bool enableLimit);
+// Ignored when minLength > maxLength.
+S2B_API void s2DistanceJoint_SetLengthRange(s2JointId jointId, float minLength, float maxLength);
+S2B_API float s2DistanceJoint_GetMinLength(s2JointId jointId);
+S2B_API float s2DistanceJoint_GetMaxLength(s2JointId jointId);
+S2B_API void s2DistanceJoint_EnableSpring(s2JointId jointId, bool enableSpring);
+S2B_API void s2DistanceJoint_SetSpringHertz(s2JointId jointId, float hertz);
+S2B_API void s2DistanceJoint_SetSpringDampingRatio(s2JointId jointId, float dampingRatio);
+S2B_API void s2DistanceJoint_EnableMotor(s2JointId jointId, bool enableMotor);
+// Any finite speed.
+S2B_API void s2DistanceJoint_SetMotorSpeed(s2JointId jointId, float motorSpeed);
+S2B_API void s2DistanceJoint_SetMaxMotorForce(s2JointId jointId, float maxMotorForce);
+// The motor force of the last step (N): inverseTimeStep times the motor impulse.
+S2B_API float s2DistanceJoint_GetMotorForce(s2JointId jointId, float inverseTimeStep);
+// The current distance between the two anchors (m).
+S2B_API float s2DistanceJoint_GetCurrentLength(s2JointId jointId);
+
 // ---- joint reactions and breakable joints (DESIGN.md §3.13) --------------------------------------------------------
 
 // What a joint exerts on body B over the last step: force (N, world frame) and torque (N-m).
@@ -189,6 +251,9 @@ typedef struct s2JointReaction
 //   mouse, weld, motor                 force = rate impulse    torque = rate motorImpulse
 //   prismatic  force = rate (impulse.x perp + (motorImpulse + lowerImpulse - upperImpulse) axis), torque = rate impulse.y,
 //              axis = qA localAxisA, perp = leftPerp(axis)
+//   distance   force = rate (impulse.x + motorImpulse + lowerImpulse - upperImpulse) axis, torque = 0. Here localAxisA is the
+//              WORLD axis, the unit vector from anchor A to anchor B at the end of the step (zero when they coincide), and
+//              qA is not read; a distance joint with its spring enabled also passes motorImpulse + springImpulse.
 // Every operation is a separate float32 rounding, so the host and the device (built without contraction) agree bit for bit.
 S2_INLINE s2JointReaction s2MakeJointReaction(int32_t type, s2Vec2 impulse, float motorImpulse, float lowerImpulse,
 											  float upperImpulse, s2Rot qA, s2Vec2 localAxisA, float rate)
@@ -199,6 +264,13 @@ S2_INLINE s2JointReaction s2MakeJointReaction(int32_t type, s2Vec2 impulse, floa
 	if (type == S2B_JOINT_REVOLUTE)
 	{
 		t = motorImpulse + lowerImpulse - upperImpulse;
+	}
+	else if (type == S2B_JOINT_DISTANCE)
+	{
+		float axial = impulse.x + motorImpulse + lowerImpulse - upperImpulse;
+		f.x = axial * localAxisA.x;
+		f.y = axial * localAxisA.y;
+		t = 0.0f;
 	}
 	else if (type == S2B_JOINT_PRISMATIC)
 	{

@@ -179,6 +179,27 @@ class PrismaticJointDef(C.Structure):
     ]
 
 
+class DistanceJointDef(C.Structure):
+    """s2DistanceJointDef (include/solver2d_b200.h): an extension, absent from the reference."""
+    _fields_ = [
+        ("bodyIdA", BodyId),
+        ("bodyIdB", BodyId),
+        ("localAnchorA", Vec2),
+        ("localAnchorB", Vec2),
+        ("length", C.c_float),
+        ("enableSpring", C.c_bool),
+        ("hertz", C.c_float),
+        ("dampingRatio", C.c_float),
+        ("enableLimit", C.c_bool),
+        ("minLength", C.c_float),
+        ("maxLength", C.c_float),
+        ("enableMotor", C.c_bool),
+        ("maxMotorForce", C.c_float),
+        ("motorSpeed", C.c_float),
+        ("collideConnected", C.c_bool),
+    ]
+
+
 class MotorJointDef(C.Structure):
     """s2MotorJointDef (include/solver2d_b200.h): an extension, absent from the reference."""
     _fields_ = [
@@ -274,6 +295,16 @@ def default_prismatic_def() -> PrismaticJointDef:
     return d
 
 
+def default_distance_def() -> DistanceJointDef:
+    """s2DefaultDistanceJointDef (include/solver2d_b200.h)."""
+    d = DistanceJointDef()
+    d.bodyIdA = BodyId(-1, -1, 0)
+    d.bodyIdB = BodyId(-1, -1, 0)
+    d.length = 1.0
+    d.maxLength = 100000.0  # s2_huge
+    return d
+
+
 def default_motor_def() -> MotorJointDef:
     """s2DefaultMotorJointDef (include/solver2d_b200.h)."""
     d = MotorJointDef()
@@ -352,6 +383,22 @@ _API = {
     "s2PrismaticJoint_SetMotorSpeed": (None, [JointId, C.c_float]),
     "s2PrismaticJoint_GetMotorForce": (C.c_float, [JointId, C.c_float]),
     "s2PrismaticJoint_GetTranslation": (C.c_float, [JointId]),
+    # distance joint (DESIGN.md §3.16)
+    "s2CreateDistanceJoint": (JointId, [WorldId, C.POINTER(DistanceJointDef)]),
+    "s2DistanceJoint_SetLength": (None, [JointId, C.c_float]),
+    "s2DistanceJoint_GetLength": (C.c_float, [JointId]),
+    "s2DistanceJoint_EnableLimit": (None, [JointId, C.c_bool]),
+    "s2DistanceJoint_SetLengthRange": (None, [JointId, C.c_float, C.c_float]),
+    "s2DistanceJoint_GetMinLength": (C.c_float, [JointId]),
+    "s2DistanceJoint_GetMaxLength": (C.c_float, [JointId]),
+    "s2DistanceJoint_EnableSpring": (None, [JointId, C.c_bool]),
+    "s2DistanceJoint_SetSpringHertz": (None, [JointId, C.c_float]),
+    "s2DistanceJoint_SetSpringDampingRatio": (None, [JointId, C.c_float]),
+    "s2DistanceJoint_EnableMotor": (None, [JointId, C.c_bool]),
+    "s2DistanceJoint_SetMotorSpeed": (None, [JointId, C.c_float]),
+    "s2DistanceJoint_SetMaxMotorForce": (None, [JointId, C.c_float]),
+    "s2DistanceJoint_GetMotorForce": (C.c_float, [JointId, C.c_float]),
+    "s2DistanceJoint_GetCurrentLength": (C.c_float, [JointId]),
     # joint springs (DESIGN.md §3.14)
     "s2PrismaticJoint_EnableSpring": (None, [JointId, C.c_bool]),
     "s2PrismaticJoint_SetSpringHertz": (None, [JointId, C.c_float]),

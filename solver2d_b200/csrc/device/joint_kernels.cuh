@@ -5,6 +5,7 @@
 #pragma once
 
 #include "contact_kernels.cuh"
+#include "shared/s2_collide.h"
 
 #define S2B_JOINT_TYPE(flags) (((flags) >> 1) & 0x7)
 // row flags of the joint-constraint stream only (jc.head.x): an XPBD spring row's body A / B is static, so its sub-step start
@@ -16,6 +17,8 @@
 #define S2B_JC_SOFT_ANGULAR 0x400
 #define S2B_JC_SOFT_LINEAR 0x800
 #define S2B_JC_SOFT_WELD (S2B_JC_SOFT_ANGULAR | S2B_JC_SOFT_LINEAR)
+// on a distance row (DESIGN.md §3.16), S2B_JC_SOFT_LINEAR marks a length that is not rigid: enableSpring with
+// minLength < maxLength, whatever the hertz (a rope at hertz 0)
 
 struct JointBodies
 {
@@ -118,6 +121,41 @@ template <int KIND> __device__ __forceinline__ void s2bPrepareJointRows(const So
 	jc.lim[t] = lim;
 	jc.coef[t] = make_float4(a.softJoint.bias, a.softJoint.mass, a.softJoint.impulse, 0.0f);
 
+	if (S2B_JOINT_TYPE(flags) == S2B_JOINT_DISTANCE)
+	{
+		// DESIGN.md §3.16: lim = (rest length, min, max), motor = (maxMotorForce, motorSpeed); the frame and the axial mass
+		// are formed fresh in each solve. A row that does not act keeps no impulse: the limits need the flag and
+		// min < max, the rigid row needs the spring off or min == max.
+		bool range = lim.y < lim.z;
+		bool soft = (flags & S2B_JOINT_ENABLE_SPRING) != 0 && range;
+		flags = (range ? flags : flags & ~S2B_JOINT_ENABLE_LIMIT) | (soft ? S2B_JC_SOFT_LINEAR : 0);
+		jc.head[t] = make_int4(flags, ia, ib, slot);
+		jc.motor[t] = make_float4(motor.x, motor.y, 0.0f, 0.0f);
+		jc.d0ax[t] = make_float4(centerDiff0.x, centerDiff0.y, 0.0f, 0.0f);
+		jc.pivot[t] = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
+		if (KIND == JPREP_XPBD || warmStart == false)
+		{
+			imp = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
+			limp = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
+		}
+		if ((flags & S2B_JOINT_ENABLE_LIMIT) == 0)
+		{
+			limp.x = 0.0f;
+			limp.y = 0.0f;
+		}
+		if ((flags & S2B_JOINT_ENABLE_MOTOR) == 0)
+		{
+			imp.z = 0.0f;
+		}
+		if (soft)
+		{
+			imp.x = 0.0f;
+		}
+		imp.y = 0.0f;
+		jc.imp[t] = imp;
+		jc.limp[t] = limp;
+		return;
+	}
 	if (S2B_JOINT_TYPE(flags) == S2B_JOINT_PRISMATIC || S2B_JOINT_TYPE(flags) == S2B_JOINT_MOTOR)
 	{
 		// DESIGN.md §3.9: the local axis rides in the motor row's spare zw; every mass is formed fresh in each solve.
@@ -228,9 +266,9 @@ __device__ __forceinline__ void s2bStoreJointImpulses(const SolveArgs& a, int t)
 // jc.imp.w = accumulated spring impulse.
 // ---------------------------------------------------------------------------------------------------------------
 
-// the spring's part of prepare. A spring acts only on a revolute or prismatic row with a positive hertz and, on a revolute
-// row, a rotation to act on; every other row loses the flag in jc.head, so no solve or warm start evaluates a spring term
-// for it, and gets a zero spring impulse.
+// the spring's part of prepare. A spring acts only on a revolute, prismatic or distance row with a positive hertz and, on a
+// revolute row, a rotation to act on, on a distance row minLength < maxLength; every other row loses the flag in jc.head,
+// so no solve or warm start evaluates a spring term for it, and gets a zero spring impulse.
 template <int KIND> __device__ __forceinline__ void s2bPrepareSpring(const SolveArgs& a, int t, int slot, bool warmStart)
 {
 	const JointConstraintView& jc = a.jc;
@@ -245,8 +283,8 @@ template <int KIND> __device__ __forceinline__ void s2bPrepareSpring(const Solve
 	float4 motor = a.joints.motor[slot]; // hertz, damping ratio in zw
 	float iA = a.bodies.pos[head.y].z, iB = a.bodies.pos[head.z].z;
 	int type = S2B_JOINT_TYPE(flags);
-	if ((type != S2B_JOINT_REVOLUTE && type != S2B_JOINT_PRISMATIC) || (motor.z > 0.0f) == false ||
-		(type == S2B_JOINT_REVOLUTE && iA + iB == 0.0f))
+	if ((type != S2B_JOINT_REVOLUTE && type != S2B_JOINT_PRISMATIC && type != S2B_JOINT_DISTANCE) || (motor.z > 0.0f) == false ||
+		(type == S2B_JOINT_REVOLUTE && iA + iB == 0.0f) || (type == S2B_JOINT_DISTANCE && (flags & S2B_JC_SOFT_LINEAR) == 0))
 	{
 		jc.head[t] = make_int4(flags & ~S2B_JOINT_ENABLE_SPRING, head.y, head.z, head.w);
 		*lambda = 0.0f;
@@ -382,8 +420,26 @@ __device__ __forceinline__ PrismaticFrame s2bPrismaticFrame(float4 anchor, float
 	return f;
 }
 
+// the distance joint's frame at the given poses (DESIGN.md §3.16): centre-of-mass-relative anchors, the length of
+// d = (dcB - dcA) + (rB - rA) + centerDiff0 and the unit axis along d (zero for a degenerate d)
+struct DistanceFrame
+{
+	s2Vec2 rA, rB, axis;
+	float length;
+};
+
+__device__ __forceinline__ DistanceFrame s2bDistanceFrame(float4 anchor, float4 d0, s2Vec2 dcA, s2Rot qA, s2Vec2 dcB, s2Rot qB)
+{
+	DistanceFrame f;
+	f.rA = s2RotateVector(qA, V2(anchor.x, anchor.y));
+	f.rB = s2RotateVector(qB, V2(anchor.z, anchor.w));
+	s2Vec2 d = s2Add(s2Add(s2Sub(dcB, dcA), s2Sub(f.rB, f.rA)), V2(d0.x, d0.y));
+	f.axis = s2cGetLengthAndNormalize(&f.length, d);
+	return f;
+}
+
 // what warm starting adds to each body: v -/+= m * P, w -/+= i * L. Shared by the constraint-by-constraint warm start and
-// the per-body gather (warm_gather.cuh), so both add the same bits.
+// the per-body gather (warm_gather.cuh), so both add the same bits. Prismatic and distance rows.
 struct PrismaticWarm
 {
 	s2Vec2 P;
@@ -397,13 +453,24 @@ __device__ __forceinline__ PrismaticWarm s2bPrismaticWarmTerms(const SolveArgs& 
 	float4 imp = jc.imp[t];
 	float4 limp = jc.limp[t];
 	float4 poseA = a.bodies.pose[head.y], poseB = a.bodies.pose[head.z];
+	// axial = spring + motor + lower - upper (DESIGN.md §3.14); a row without a spring adds no spring term
+	float axialImpulse = ((head.x & S2B_JOINT_ENABLE_SPRING) != 0 ? imp.w + imp.z : imp.z) + limp.x - limp.y;
+	PrismaticWarm w;
+	if (S2B_JOINT_TYPE(head.x) == S2B_JOINT_DISTANCE)
+	{
+		// DESIGN.md §3.16: the rigid row's impulse joins the sum only where that row acts
+		DistanceFrame f = s2bDistanceFrame(jc.anchor[t], jc.d0ax[t], V2(poseA.x, poseA.y), R2(poseA.z, poseA.w),
+										   V2(poseB.x, poseB.y), R2(poseB.z, poseB.w));
+		axialImpulse = (head.x & S2B_JC_SOFT_LINEAR) == 0 ? imp.x + axialImpulse : axialImpulse;
+		w.P = s2MulSV(axialImpulse, f.axis);
+		w.LA = axialImpulse * s2Cross(f.rA, f.axis);
+		w.LB = axialImpulse * s2Cross(f.rB, f.axis);
+		return w;
+	}
 	PrismaticFrame f = s2bPrismaticFrame(jc.anchor[t], jc.d0ax[t], jc.motor[t], V2(poseA.x, poseA.y), R2(poseA.z, poseA.w),
 										 V2(poseB.x, poseB.y), R2(poseB.z, poseB.w));
 	s2Vec2 perp = s2LeftPerp(f.axis);
 	s2Vec2 dA = s2Add(f.d, f.rA);
-	// axial = spring + motor + lower - upper (DESIGN.md §3.14); a row without a spring adds no spring term
-	float axialImpulse = ((head.x & S2B_JOINT_ENABLE_SPRING) != 0 ? imp.w + imp.z : imp.z) + limp.x - limp.y;
-	PrismaticWarm w;
 	w.P = s2Add(s2MulSV(axialImpulse, f.axis), s2MulSV(imp.x, perp));
 	w.LA = axialImpulse * s2Cross(dA, f.axis) + imp.x * s2Cross(dA, perp) + imp.y;
 	w.LB = axialImpulse * s2Cross(f.rB, f.axis) + imp.x * s2Cross(f.rB, perp) + imp.y;
@@ -444,6 +511,64 @@ __device__ __forceinline__ float3 s2bPrismaticBias(float C, bool limit, float4 c
 	return make_float3(bias, massScale, impulseScale);
 }
 
+// the axial rows the prismatic and distance joints share (DESIGN.md §3.9, §3.16): the motor, then the lower and upper limit,
+// each along `axis` with lever arms a1 (body A) and a2 (body B) and the axial mass. x is the joint's coordinate along the
+// axis (the prismatic's translation, the distance joint's length), lim.yz its limits, motor.xy the maximum force and the
+// speed; imp.z is the motor impulse and limp.xy the limit impulses.
+template <int KIND>
+__device__ __forceinline__ void s2bSolveAxialRows(int flags, s2Vec2 axis, float a1, float a2, float axialMass, float x, float4 lim,
+												  float4 motor, float4 coef, float h, float inv_h, bool useBias, float mA, float iA,
+												  float mB, float iB, float4& imp, float4& limp, s2Vec2& vA, float& wA, s2Vec2& vB,
+												  float& wB)
+{
+	if (flags & S2B_JOINT_ENABLE_MOTOR)
+	{
+		float Cdot = s2Dot(axis, s2Sub(vB, vA)) + a2 * wB - a1 * wA;
+		float impulse = axialMass * (motor.y - Cdot);
+		float oldImpulse = imp.z;
+		float maxImpulse = h * motor.x;
+		imp.z = S2_CLAMP(oldImpulse + impulse, -maxImpulse, maxImpulse);
+		impulse = imp.z - oldImpulse;
+		s2Vec2 P = s2MulSV(impulse, axis);
+		vA = s2MulSub(vA, mA, P);
+		wA -= iA * (impulse * a1);
+		vB = s2MulAdd(vB, mB, P);
+		wB += iB * (impulse * a2);
+	}
+
+	if (flags & S2B_JOINT_ENABLE_LIMIT)
+	{
+		// lower limit
+		{
+			float3 s = s2bPrismaticBias<KIND>(x - lim.y, true, coef, h, inv_h, useBias);
+			float Cdot = s2Dot(axis, s2Sub(vB, vA)) + a2 * wB - a1 * wA;
+			float impulse = -axialMass * s.y * (Cdot + s.x) - s.z * limp.x;
+			float oldImpulse = limp.x;
+			limp.x = S2_MAX(oldImpulse + impulse, 0.0f);
+			impulse = limp.x - oldImpulse;
+			s2Vec2 P = s2MulSV(impulse, axis);
+			vA = s2MulSub(vA, mA, P);
+			wA -= iA * (impulse * a1);
+			vB = s2MulAdd(vB, mB, P);
+			wB += iB * (impulse * a2);
+		}
+		// upper limit (signs flipped so C stays positive when satisfied); it relaxes with its own impulse
+		{
+			float3 s = s2bPrismaticBias<KIND>(lim.z - x, true, coef, h, inv_h, useBias);
+			float Cdot = s2Dot(axis, s2Sub(vA, vB)) + a1 * wA - a2 * wB;
+			float impulse = -axialMass * s.y * (Cdot + s.x) - s.z * limp.y;
+			float oldImpulse = limp.y;
+			limp.y = S2_MAX(oldImpulse + impulse, 0.0f);
+			impulse = limp.y - oldImpulse;
+			s2Vec2 P = s2MulSV(impulse, axis);
+			vA = s2MulAdd(vA, mA, P);
+			wA += iA * (impulse * a1);
+			vB = s2MulSub(vB, mB, P);
+			wB -= iB * (impulse * a2);
+		}
+	}
+}
+
 template <int KIND>
 __device__ __forceinline__ void s2bSolvePrismaticVelocity(const SolveArgs& a, int t, float h, float inv_h, bool useBias)
 {
@@ -470,52 +595,8 @@ __device__ __forceinline__ void s2bSolvePrismaticVelocity(const SolveArgs& a, in
 	float k = mA + mB + iA * a1 * a1 + iB * a2 * a2;
 	float axialMass = k > 0.0f ? 1.0f / k : 0.0f;
 
-	if (head.x & S2B_JOINT_ENABLE_MOTOR)
-	{
-		float Cdot = s2Dot(axis, s2Sub(vB, vA)) + a2 * wB - a1 * wA;
-		float impulse = axialMass * (motor.y - Cdot);
-		float oldImpulse = imp.z;
-		float maxImpulse = h * motor.x;
-		imp.z = S2_CLAMP(oldImpulse + impulse, -maxImpulse, maxImpulse);
-		impulse = imp.z - oldImpulse;
-		s2Vec2 P = s2MulSV(impulse, axis);
-		vA = s2MulSub(vA, mA, P);
-		wA -= iA * (impulse * a1);
-		vB = s2MulAdd(vB, mB, P);
-		wB += iB * (impulse * a2);
-	}
-
-	if (head.x & S2B_JOINT_ENABLE_LIMIT)
-	{
-		// lower limit
-		{
-			float3 s = s2bPrismaticBias<KIND>(translation - lim.y, true, coef, h, inv_h, useBias);
-			float Cdot = s2Dot(axis, s2Sub(vB, vA)) + a2 * wB - a1 * wA;
-			float impulse = -axialMass * s.y * (Cdot + s.x) - s.z * limp.x;
-			float oldImpulse = limp.x;
-			limp.x = S2_MAX(oldImpulse + impulse, 0.0f);
-			impulse = limp.x - oldImpulse;
-			s2Vec2 P = s2MulSV(impulse, axis);
-			vA = s2MulSub(vA, mA, P);
-			wA -= iA * (impulse * a1);
-			vB = s2MulAdd(vB, mB, P);
-			wB += iB * (impulse * a2);
-		}
-		// upper limit (signs flipped so C stays positive when satisfied); it relaxes with its own impulse
-		{
-			float3 s = s2bPrismaticBias<KIND>(lim.z - translation, true, coef, h, inv_h, useBias);
-			float Cdot = s2Dot(axis, s2Sub(vA, vB)) + a1 * wA - a2 * wB;
-			float impulse = -axialMass * s.y * (Cdot + s.x) - s.z * limp.y;
-			float oldImpulse = limp.y;
-			limp.y = S2_MAX(oldImpulse + impulse, 0.0f);
-			impulse = limp.y - oldImpulse;
-			s2Vec2 P = s2MulSV(impulse, axis);
-			vA = s2MulAdd(vA, mA, P);
-			wA += iA * (impulse * a1);
-			vB = s2MulSub(vB, mB, P);
-			wB -= iB * (impulse * a2);
-		}
-	}
+	s2bSolveAxialRows<KIND>(head.x, axis, a1, a2, axialMass, translation, lim, motor, coef, h, inv_h, useBias, mA, iA, mB, iB, imp,
+							limp, vA, wA, vB, wB);
 
 	// the 2x2 block: perpendicular separation and relative angle
 	{
@@ -713,6 +794,168 @@ __device__ __forceinline__ void s2bSolvePrismaticXpbd(const SolveArgs& a, int t)
 }
 
 // ---------------------------------------------------------------------------------------------------------------
+// distance joint (extension, DESIGN.md §3.16; definition: tests/distance_oracle.c). Holds anchor B at a distance from
+// anchor A along the line between them: rows spring (s2bSolveSpringVelocity, ahead of these), motor, lower limit, upper
+// limit (the prismatic's axial rows, s2bSolveAxialRows) and the rigid length row, each along the axis of the current d.
+// Row columns: lim = (rest length, minLength, maxLength), motor = (maxMotorForce, motorSpeed), imp = (rigid, 0, motor,
+// spring), limp = (lower, upper). Prepare drops the limit flag where minLength == maxLength and marks a row whose length
+// is not rigid with S2B_JC_SOFT_LINEAR.
+// ---------------------------------------------------------------------------------------------------------------
+template <int KIND>
+__device__ __forceinline__ void s2bSolveDistanceVelocity(const SolveArgs& a, int t, float h, float inv_h, bool useBias)
+{
+	const JointConstraintView& jc = a.jc;
+	int4 head = jc.head[t];
+	int ia = head.y, ib = head.z;
+	float4 mass = jc.mass[t];
+	float4 lim = jc.lim[t];
+	float4 motor = jc.motor[t];
+	float4 coef = jc.coef[t];
+	float4 imp = jc.imp[t];
+	float4 limp = jc.limp[t];
+	float4 velA = a.bodies.vel[ia], velB = a.bodies.vel[ib];
+	float4 poseA = a.bodies.pose[ia], poseB = a.bodies.pose[ib];
+	s2Vec2 vA = V2(velA.x, velA.y), vB = V2(velB.x, velB.y);
+	float wA = velA.z, wB = velB.z;
+	float mA = mass.x, iA = mass.y, mB = mass.z, iB = mass.w;
+	DistanceFrame f = s2bDistanceFrame(jc.anchor[t], jc.d0ax[t], V2(poseA.x, poseA.y), R2(poseA.z, poseA.w), V2(poseB.x, poseB.y),
+									   R2(poseB.z, poseB.w));
+	s2Vec2 axis = f.axis;
+	float crA = s2Cross(f.rA, axis), crB = s2Cross(f.rB, axis);
+	float k = mA + mB + iA * crA * crA + iB * crB * crB;
+	float axialMass = k > 0.0f ? 1.0f / k : 0.0f;
+
+	s2bSolveAxialRows<KIND>(head.x, axis, crA, crB, axialMass, f.length, lim, motor, coef, h, inv_h, useBias, mA, iA, mB, iB, imp,
+							limp, vA, wA, vB, wB);
+
+	if ((head.x & S2B_JC_SOFT_LINEAR) == 0)
+	{
+		// the rigid row: the flavour's bilateral form of C = length - rest length
+		float3 s = s2bPrismaticBias<KIND>(f.length - lim.x, false, coef, h, inv_h, useBias);
+		float Cdot = s2Dot(axis, s2Sub(vB, vA)) + crB * wB - crA * wA;
+		float impulse = -axialMass * s.y * (Cdot + s.x) - s.z * imp.x;
+		imp.x += impulse;
+		s2Vec2 P = s2MulSV(impulse, axis);
+		vA = s2MulSub(vA, mA, P);
+		wA -= iA * (impulse * crA);
+		vB = s2MulAdd(vB, mB, P);
+		wB += iB * (impulse * crB);
+	}
+
+	jc.imp[t] = imp;
+	jc.limp[t] = limp;
+	s2bStoreJointVelocities(a, ia, ib, velA, velB, vA, wA, vB, wB, mA, iA, mB, iB);
+}
+
+// one axial position correction along the frame's axis: lambda = -C / k (0 when k is 0), applied to the poses
+__device__ __forceinline__ void s2bDistanceCorrect(const DistanceFrame& f, float C, float mA, float iA, float mB, float iB, s2Vec2& dcA,
+												   s2Rot& qA, s2Vec2& dcB, s2Rot& qB)
+{
+	float crA = s2Cross(f.rA, f.axis), crB = s2Cross(f.rB, f.axis);
+	float k = mA + mB + iA * crA * crA + iB * crB * crB;
+	float axialMass = k > 0.0f ? 1.0f / k : 0.0f;
+	float impulse = -axialMass * C;
+	s2Vec2 P = s2MulSV(impulse, f.axis);
+	dcA = s2MulSub(dcA, mA, P);
+	qA = s2IntegrateRot(qA, -iA * (impulse * crA));
+	dcB = s2MulAdd(dcB, mB, P);
+	qB = s2IntegrateRot(qB, iB * (impulse * crB));
+}
+
+// NGS position pass (Box2D 2.4's distance position solve): a rigid length corrects length - rest length; a length that is
+// not rigid corrects only a violated limit. Clamped to +/- s2_maxLinearCorrection. The spring and the motor do nothing.
+__device__ __forceinline__ void s2bSolveDistancePosition(const SolveArgs& a, int t)
+{
+	const JointConstraintView& jc = a.jc;
+	int4 head = jc.head[t];
+	int ia = head.y, ib = head.z;
+	float4 mass = jc.mass[t];
+	float4 lim = jc.lim[t];
+	float4 poseA = a.bodies.pose[ia], poseB = a.bodies.pose[ib];
+	s2Vec2 dcA = V2(poseA.x, poseA.y), dcB = V2(poseB.x, poseB.y);
+	s2Rot qA = R2(poseA.z, poseA.w), qB = R2(poseB.z, poseB.w);
+	float mA = mass.x, iA = mass.y, mB = mass.z, iB = mass.w;
+	DistanceFrame f = s2bDistanceFrame(jc.anchor[t], jc.d0ax[t], dcA, qA, dcB, qB);
+	float C;
+	if ((head.x & S2B_JC_SOFT_LINEAR) == 0)
+	{
+		C = f.length - lim.x;
+	}
+	else if ((head.x & S2B_JOINT_ENABLE_LIMIT) && f.length < lim.y)
+	{
+		C = f.length - lim.y;
+	}
+	else if ((head.x & S2B_JOINT_ENABLE_LIMIT) && f.length > lim.z)
+	{
+		C = f.length - lim.z;
+	}
+	else
+	{
+		return;
+	}
+	C = S2_CLAMP(C, -s2_maxLinearCorrection, s2_maxLinearCorrection);
+	s2bDistanceCorrect(f, C, mA, iA, mB, iB, dcA, qA, dcB, qB);
+	if ((mA != 0.0f) || (iA != 0.0f))
+	{
+		a.bodies.pose[ia] = make_float4(dcA.x, dcA.y, qA.s, qA.c);
+	}
+	if ((mB != 0.0f) || (iB != 0.0f))
+	{
+		a.bodies.pose[ib] = make_float4(dcB.x, dcB.y, qB.s, qB.c);
+	}
+}
+
+// XPBD, zero compliance: a violated limit as a position inequality, then the rigid length row on the corrected poses. The
+// spring (s2bSolveSpringXpbd) runs ahead; the motor is not applied, as the prismatic's XPBD form ignores its motor.
+__device__ __forceinline__ void s2bSolveDistanceXpbd(const SolveArgs& a, int t)
+{
+	const JointConstraintView& jc = a.jc;
+	int4 head = jc.head[t];
+	int ia = head.y, ib = head.z;
+	float4 anchor = jc.anchor[t];
+	float4 mass = jc.mass[t];
+	float4 d0 = jc.d0ax[t];
+	float4 lim = jc.lim[t];
+	float4 poseA = a.bodies.pose[ia], poseB = a.bodies.pose[ib];
+	s2Vec2 dcA = V2(poseA.x, poseA.y), dcB = V2(poseB.x, poseB.y);
+	s2Rot qA = R2(poseA.z, poseA.w), qB = R2(poseB.z, poseB.w);
+	float mA = mass.x, iA = mass.y, mB = mass.z, iB = mass.w;
+
+	if (head.x & S2B_JOINT_ENABLE_LIMIT)
+	{
+		DistanceFrame f = s2bDistanceFrame(anchor, d0, dcA, qA, dcB, qB);
+		float C = 0.0f;
+		if (f.length < lim.y)
+		{
+			C = f.length - lim.y;
+		}
+		else if (f.length > lim.z)
+		{
+			C = f.length - lim.z;
+		}
+		if (C != 0.0f)
+		{
+			s2bDistanceCorrect(f, C, mA, iA, mB, iB, dcA, qA, dcB, qB);
+		}
+	}
+
+	if ((head.x & S2B_JC_SOFT_LINEAR) == 0)
+	{
+		DistanceFrame f = s2bDistanceFrame(anchor, d0, dcA, qA, dcB, qB);
+		s2bDistanceCorrect(f, f.length - lim.x, mA, iA, mB, iB, dcA, qA, dcB, qB);
+	}
+
+	if ((mA != 0.0f) || (iA != 0.0f))
+	{
+		a.bodies.pose[ia] = make_float4(dcA.x, dcA.y, qA.s, qA.c);
+	}
+	if ((mB != 0.0f) || (iB != 0.0f))
+	{
+		a.bodies.pose[ib] = make_float4(dcB.x, dcB.y, qB.s, qB.c);
+	}
+}
+
+// ---------------------------------------------------------------------------------------------------------------
 // motor joint (extension, DESIGN.md §3.10; definition: tests/motor_oracle.c). Drives body B toward a pose relative to body
 // A with capped effort: an angular row toward angle(B) - angle(A) = angularOffset, its accumulated impulse clamped to
 // +/- h maxTorque, then a point row that takes B's origin to the linear offset in A's frame, its accumulated impulse scaled
@@ -875,16 +1118,32 @@ __device__ __forceinline__ void s2bSolveSpringVelocity(const SolveArgs& a, int t
 	}
 	else
 	{
-		// C = the translation, k = the axial mass §3.9 forms in every solve
-		PrismaticFrame f = s2bPrismaticFrame(jc.anchor[t], d0, jc.motor[t], V2(poseA.x, poseA.y), qA, V2(poseB.x, poseB.y), qB);
-		s2Vec2 dA = s2Add(f.d, f.rA);
-		float a1 = s2Cross(dA, f.axis), a2 = s2Cross(f.rB, f.axis);
+		// prismatic: C = the translation, k = the axial mass §3.9 forms in every solve; distance (§3.16): C = length - rest
+		// length along the current line
+		s2Vec2 axis;
+		float a1, a2, C;
+		if (S2B_JOINT_TYPE(head.x) == S2B_JOINT_DISTANCE)
+		{
+			DistanceFrame f = s2bDistanceFrame(jc.anchor[t], d0, V2(poseA.x, poseA.y), qA, V2(poseB.x, poseB.y), qB);
+			axis = f.axis;
+			a1 = s2Cross(f.rA, axis);
+			a2 = s2Cross(f.rB, axis);
+			C = f.length - lim.x;
+		}
+		else
+		{
+			PrismaticFrame f = s2bPrismaticFrame(jc.anchor[t], d0, jc.motor[t], V2(poseA.x, poseA.y), qA, V2(poseB.x, poseB.y), qB);
+			axis = f.axis;
+			a1 = s2Cross(s2Add(f.d, f.rA), axis);
+			a2 = s2Cross(f.rB, axis);
+			C = s2Dot(axis, f.d);
+		}
 		float k = mA + mB + iA * a1 * a1 + iB * a2 * a2;
 		float axialMass = k > 0.0f ? 1.0f / k : 0.0f;
-		float Cdot = s2Dot(f.axis, s2Sub(vB, vA)) + a2 * wB - a1 * wA;
-		float impulse = -axialMass * massScale * (Cdot + bias * s2Dot(f.axis, f.d)) - impulseScale * imp.w;
+		float Cdot = s2Dot(axis, s2Sub(vB, vA)) + a2 * wB - a1 * wA;
+		float impulse = -axialMass * massScale * (Cdot + bias * C) - impulseScale * imp.w;
 		imp.w += impulse;
-		s2Vec2 P = s2MulSV(impulse, f.axis);
+		s2Vec2 P = s2MulSV(impulse, axis);
 		vA = s2MulSub(vA, mA, P);
 		wA -= iA * (impulse * a1);
 		vB = s2MulAdd(vB, mB, P);
@@ -923,15 +1182,30 @@ __device__ __forceinline__ void s2bSolveSpringXpbd(const SolveArgs& a, int t)
 	}
 	else
 	{
-		float4 anchor = jc.anchor[t], d0 = jc.d0ax[t], motor = jc.motor[t];
-		PrismaticFrame f0 = s2bPrismaticFrame(anchor, d0, motor, V2(p0A.x, p0A.y), R2(p0A.z, p0A.w), V2(p0B.x, p0B.y), R2(p0B.z, p0B.w));
-		PrismaticFrame f = s2bPrismaticFrame(anchor, d0, motor, dcA, qA, dcB, qB);
-		axis = f.axis;
-		LA = s2Cross(s2Add(f.d, f.rA), f.axis);
-		LB = s2Cross(f.rB, f.axis);
+		float4 anchor = jc.anchor[t], d0 = jc.d0ax[t];
+		if (S2B_JOINT_TYPE(head.x) == S2B_JOINT_DISTANCE)
+		{
+			DistanceFrame f0 = s2bDistanceFrame(anchor, d0, V2(p0A.x, p0A.y), R2(p0A.z, p0A.w), V2(p0B.x, p0B.y), R2(p0B.z, p0B.w));
+			DistanceFrame f = s2bDistanceFrame(anchor, d0, dcA, qA, dcB, qB);
+			axis = f.axis;
+			LA = s2Cross(f.rA, f.axis);
+			LB = s2Cross(f.rB, f.axis);
+			C = f.length - lim.x;
+			C0 = f0.length - lim.x;
+		}
+		else
+		{
+			float4 motor = jc.motor[t];
+			PrismaticFrame f0 =
+				s2bPrismaticFrame(anchor, d0, motor, V2(p0A.x, p0A.y), R2(p0A.z, p0A.w), V2(p0B.x, p0B.y), R2(p0B.z, p0B.w));
+			PrismaticFrame f = s2bPrismaticFrame(anchor, d0, motor, dcA, qA, dcB, qB);
+			axis = f.axis;
+			LA = s2Cross(s2Add(f.d, f.rA), f.axis);
+			LB = s2Cross(f.rB, f.axis);
+			C = s2Dot(f.axis, f.d);
+			C0 = s2Dot(f0.axis, f0.d);
+		}
 		w = mA + mB + iA * LA * LA + iB * LB * LB;
-		C = s2Dot(f.axis, f.d);
-		C0 = s2Dot(f0.axis, f0.d);
 		if ((w > 0.0f) == false)
 		{
 			return;
@@ -940,7 +1214,7 @@ __device__ __forceinline__ void s2bSolveSpringXpbd(const SolveArgs& a, int t)
 	float alphaTilde = w / (omegaH * omegaH);
 	float gamma = 2.0f * zeta / omegaH;
 	float p = -(C + gamma * (C - C0)) / ((1.0f + gamma) * w + alphaTilde);
-	if (S2B_JOINT_TYPE(head.x) == S2B_JOINT_PRISMATIC)
+	if (S2B_JOINT_TYPE(head.x) != S2B_JOINT_REVOLUTE)
 	{
 		s2Vec2 P = s2MulSV(p, axis);
 		dcA = s2MulSub(dcA, mA, P);
@@ -1000,7 +1274,7 @@ __device__ __forceinline__ void s2bWarmStartJoint(const SolveArgs& a, int t)
 		return;
 	}
 
-	if (S2B_JOINT_TYPE(head.x) == S2B_JOINT_PRISMATIC)
+	if (S2B_JOINT_TYPE(head.x) == S2B_JOINT_PRISMATIC || S2B_JOINT_TYPE(head.x) == S2B_JOINT_DISTANCE)
 	{
 		float4 velA = a.bodies.vel[ia], velB = a.bodies.vel[ib];
 		float mA = mass.x, iA = mass.y, mB = mass.z, iB = mass.w;
@@ -1650,6 +1924,11 @@ __device__ __forceinline__ void s2bSolveJointSoft(const SolveArgs& a, int t, flo
 		s2bSolvePrismaticVelocity<PSOLVE_SOFT>(a, t, h, inv_h, useBias);
 		return;
 	}
+	if (S2B_JOINT_TYPE(flags) == S2B_JOINT_DISTANCE)
+	{
+		s2bSolveDistanceVelocity<PSOLVE_SOFT>(a, t, h, inv_h, useBias);
+		return;
+	}
 	if (SHARED_MOTOR == false && S2B_JOINT_TYPE(flags) == S2B_JOINT_MOTOR)
 	{
 		s2bSolveMotorVelocity(a, t, h, inv_h);
@@ -1675,6 +1954,11 @@ __device__ __forceinline__ void s2bSolveJointBaumgarte(const SolveArgs& a, int t
 	if (S2B_JOINT_TYPE(flags) == S2B_JOINT_PRISMATIC)
 	{
 		s2bSolvePrismaticVelocity<PSOLVE_BAUMGARTE>(a, t, h, inv_h, useBias);
+		return;
+	}
+	if (S2B_JOINT_TYPE(flags) == S2B_JOINT_DISTANCE)
+	{
+		s2bSolveDistanceVelocity<PSOLVE_BAUMGARTE>(a, t, h, inv_h, useBias);
 		return;
 	}
 	if (S2B_JOINT_TYPE(flags) == S2B_JOINT_MOTOR)
@@ -1799,6 +2083,11 @@ __device__ __forceinline__ void s2bSolveJointRigid(const SolveArgs& a, int t, fl
 		s2bSolvePrismaticVelocity<PSOLVE_RIGID>(a, t, h, 0.0f /* inv_h: unused by the rigid rows */, false);
 		return;
 	}
+	if (S2B_JOINT_TYPE(a.jc.head[t].x) == S2B_JOINT_DISTANCE)
+	{
+		s2bSolveDistanceVelocity<PSOLVE_RIGID>(a, t, h, 0.0f /* inv_h: unused by the rigid rows */, false);
+		return;
+	}
 	if (S2B_JOINT_TYPE(a.jc.head[t].x) == S2B_JOINT_MOTOR)
 	{
 		s2bSolveMotorVelocity(a, t, h, a.ctx.inv_h);
@@ -1827,6 +2116,11 @@ __device__ __forceinline__ void s2bSolveJointPosition(const SolveArgs& a, int t)
 	if (S2B_JOINT_TYPE(head.x) == S2B_JOINT_PRISMATIC)
 	{
 		s2bSolvePrismaticPosition(a, t);
+		return;
+	}
+	if (S2B_JOINT_TYPE(head.x) == S2B_JOINT_DISTANCE)
+	{
+		s2bSolveDistancePosition(a, t);
 		return;
 	}
 	if (head.x & S2B_JC_SOFT_WELD)
@@ -1921,6 +2215,11 @@ __device__ __forceinline__ void s2bSolveJointXpbd(const SolveArgs& a, int t)
 	if (S2B_JOINT_TYPE(head.x) == S2B_JOINT_PRISMATIC)
 	{
 		s2bSolvePrismaticXpbd(a, t);
+		return;
+	}
+	if (S2B_JOINT_TYPE(head.x) == S2B_JOINT_DISTANCE)
+	{
+		s2bSolveDistanceXpbd(a, t);
 		return;
 	}
 	if (S2B_JOINT_TYPE(head.x) == S2B_JOINT_MOTOR)

@@ -1,16 +1,19 @@
 // solver2d-b200 — joint reactions and break thresholds (DESIGN.md §3.13).
 //
 // One thread per joint slot evaluates s2MakeJointReaction (include/solver2d_b200.h) on the impulses the last solve stored,
-// body A's final rotation and the rate of that solve. After finalize (s2bFinalize) it compares the reaction with the
+// body A's final rotation (a distance joint: the line between its anchors at both bodies' final poses) and the rate of that
+// solve. After finalize (s2bFinalize) it compares the reaction with the
 // slot's thresholds and appends the slots over one to a list; on demand (s2b_download_joint_reactions) it writes the
 // reactions instead. The solver kernels are not touched: everything it reads is already in the joint and body columns.
 #include "s2b_internal.cuh"
+#include "shared/s2_distance_joint.h"
 #include "solver2d_b200.h"
 
 #include <algorithm>
 
-__global__ void s2bJointReactionKernel(JointView j, const float2* __restrict__ brk, const float4* __restrict__ pose, float rate,
-									   float* reactions, int* broken)
+__global__ void s2bJointReactionKernel(JointView j, const float2* __restrict__ brk, const float4* __restrict__ pose,
+									   const float4* __restrict__ pos, const float4* __restrict__ org, float rate, float* reactions,
+									   int* broken)
 {
 	int i = blockIdx.x * blockDim.x + threadIdx.x;
 	if (i >= j.capacity)
@@ -42,8 +45,19 @@ __global__ void s2bJointReactionKernel(JointView j, const float2* __restrict__ b
 	s2Rot qA = {qa.z, qa.w};
 	// a spring acts on the motor's axis: its impulse joins the motor argument (DESIGN.md §3.14)
 	float motorImpulse = (head.x & S2B_JOINT_ENABLE_SPRING) != 0 ? imp.z + imp.w : imp.z;
-	s2JointReaction r = s2MakeJointReaction((head.x >> 1) & 0x7, s2MakeVec2(imp.x, imp.y), motorImpulse, limp.x, limp.y, qA,
-											s2MakeVec2(target.z, target.w), rate);
+	int type = (head.x >> 1) & 0x7;
+	s2Vec2 axis = s2MakeVec2(target.z, target.w);
+	if (type == S2B_JOINT_DISTANCE)
+	{
+		// the world axis from anchor A to anchor B at the end of the step (DESIGN.md §3.16), as the host getters form it
+		float4 anchors = j.anchors[i];
+		float4 pa = pos[head.y], pb = pos[head.z], qb = pose[head.z], oa = org[head.y], ob = org[head.z];
+		float length;
+		axis = s2cDistanceJointAxis(&length, s2MakeVec2(pa.x, pa.y), qA, s2Sub(s2MakeVec2(anchors.x, anchors.y), s2MakeVec2(oa.z, oa.w)),
+									s2MakeVec2(pb.x, pb.y), s2Rot{qb.z, qb.w},
+									s2Sub(s2MakeVec2(anchors.z, anchors.w), s2MakeVec2(ob.z, ob.w)));
+	}
+	s2JointReaction r = s2MakeJointReaction(type, s2MakeVec2(imp.x, imp.y), motorImpulse, limp.x, limp.y, qA, axis, rate);
 	if (reactions != nullptr)
 	{
 		reactions[3 * i] = r.force.x;
@@ -85,8 +99,8 @@ void s2bJointBreakPass(s2bWorld* w, cudaStream_t cs)
 		w->dBroken.reserve((size_t)cap + 1, st, false, false);
 	}
 	S2B_CHECK(cudaMemsetAsync(w->dBroken.p, 0, sizeof(int), st));
-	S2B_LAUNCH(w, s2bJointReactionKernel, gridFor(cap, 128), 128, 0, jointView(w), w->jBreak.p, w->bPose.p, w->reactionRate,
-			   (float*)nullptr, w->dBroken.p);
+	S2B_LAUNCH(w, s2bJointReactionKernel, gridFor(cap, 128), 128, 0, jointView(w), w->jBreak.p, w->bPose.p, w->bPos.p, w->bOrg.p,
+			   w->reactionRate, (float*)nullptr, w->dBroken.p);
 	if (cs != st)
 	{
 		S2B_CHECK(cudaEventRecord(w->finalizedEvent, st));
@@ -113,8 +127,8 @@ extern "C" void s2b_download_joint_reactions(s2bWorld* w, float* out, int capaci
 	S2bEpochFreeze freeze; // transfer buffers are not part of any captured graph
 	float* d = nullptr;
 	S2B_CHECK(cudaMallocAsync((void**)&d, sizeof(float) * 3 * (size_t)w->jointCap, w->stream));
-	S2B_LAUNCH(w, s2bJointReactionKernel, gridFor(w->jointCap, 128), 128, 0, jointView(w), w->jBreak.p, w->bPose.p,
-			   w->reactionRate, d, (int*)nullptr);
+	S2B_LAUNCH(w, s2bJointReactionKernel, gridFor(w->jointCap, 128), 128, 0, jointView(w), w->jBreak.p, w->bPose.p, w->bPos.p,
+			   w->bOrg.p, w->reactionRate, d, (int*)nullptr);
 	S2B_CHECK(cudaMemcpyAsync(out, d, sizeof(float) * 3 * (size_t)n, cudaMemcpyDeviceToHost, w->stream));
 	S2B_CHECK(cudaFreeAsync(d, w->stream));
 	S2B_CHECK(cudaStreamSynchronize(w->stream));

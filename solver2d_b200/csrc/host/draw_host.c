@@ -3,6 +3,7 @@
 // body transforms (lazy sync), shape boxes (when AABBs are drawn) and the contact table (when contact points are
 // drawn). Nothing here is on the step path.
 #include "s2_host.h"
+#include "shared/s2_collide.h"
 
 #include <math.h>
 #include <stdio.h>
@@ -83,6 +84,24 @@ static void s2DrawJoint(s2DebugDraw* draw, s2World* world, const s2Joint* joint)
 	{
 		// the segment from the target point (A's linear offset) to B's origin: the pose error the motor is removing
 		draw->DrawSegment(pA, pB, s2Rgb(0.8f, 0.5f, 0.9f), draw->context);
+		return;
+	}
+
+	if (joint->type == s2_distanceJoint)
+	{
+		// the segment between the anchors and, with the limit on, a mark across the line at minLength and at maxLength from
+		// anchor A
+		draw->DrawSegment(pA, pB, s2Rgb(0.5f, 0.8f, 0.8f), draw->context);
+		if (joint->enableLimit)
+		{
+			float length;
+			s2Vec2 axis = s2cGetLengthAndNormalize(&length, s2Sub(pB, pA));
+			s2Vec2 perp = s2MulSV(0.5f * joint->drawSize, s2LeftPerp(axis));
+			s2Vec2 lower = s2MulAdd(pA, joint->lowerAngle, axis);
+			s2Vec2 upper = s2MulAdd(pA, joint->upperAngle, axis);
+			draw->DrawSegment(s2Sub(lower, perp), s2Add(lower, perp), s2Rgb(0.3f, 0.9f, 0.3f), draw->context);
+			draw->DrawSegment(s2Sub(upper, perp), s2Add(upper, perp), s2Rgb(0.9f, 0.3f, 0.3f), draw->context);
+		}
 		return;
 	}
 

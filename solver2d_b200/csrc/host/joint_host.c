@@ -1,6 +1,7 @@
 // solver2d-b200 — joints behind the public API (behaviour of reference src/joint.c:154-292, src/revolute_joint.c:825-888,
 // src/mouse_joint.c:18-29). Host bookkeeping only: the joint solvers run on the device.
 #include "s2_host.h"
+#include "shared/s2_distance_joint.h"
 #include "solver2d_b200.h"
 
 #include <float.h>
@@ -180,7 +181,7 @@ float s2RevoluteJoint_GetMotorTorque(s2JointId jointId, float inverseTimeStep)
 	return inverseTimeStep * world->joints[jointId.index].motorImpulse;
 }
 
-// ---- joint springs (DESIGN.md §3.14): revolute and prismatic joints; hertz and dampingRatio carry the spring ---------------
+// ---- joint springs (DESIGN.md §3.14): revolute, prismatic and distance joints; hertz and dampingRatio carry the spring ----
 
 static void s2EnableJointSpring(s2JointId jointId, s2JointType type, bool enableSpring)
 {
@@ -188,7 +189,7 @@ static void s2EnableJointSpring(s2JointId jointId, s2JointType type, bool enable
 	s2Joint* joint = s2GetJointForEdit(jointId, &world);
 	if (joint->type != type)
 	{
-		return; // only revolute and prismatic joints have a spring
+		return; // only revolute, prismatic and distance joints have a spring
 	}
 	joint->enableSpring = enableSpring;
 	s2MarkJointDirty(world, joint);
@@ -204,7 +205,7 @@ static void s2SetJointSpringValue(s2JointId jointId, s2JointType type, float val
 	s2Joint* joint = s2GetJointForEdit(jointId, &world);
 	if (joint->type != type)
 	{
-		return; // only revolute and prismatic joints have a spring
+		return; // only revolute, prismatic and distance joints have a spring
 	}
 	if (dampingRatio)
 	{
@@ -551,12 +552,224 @@ float s2PrismaticJoint_GetTranslation(s2JointId jointId)
 	return s2Dot(axis, s2Sub(pB, pA));
 }
 
+// ---- distance joint (DESIGN.md §3.16) ------------------------------------------------------------------------------------
+
+static float s2ClampDistanceLength(float length)
+{
+	return S2_CLAMP(length, s2_linearSlop, s2_huge);
+}
+
+static bool s2IsValidDistanceValue(float value)
+{
+	return s2IsValid(value) && value >= 0.0f;
+}
+
+// The distance joint has no counterpart in the reference. Invalid input creates nothing and returns s2_nullJointId; the lengths
+// are clamped into [s2_linearSlop, s2_huge] as Box2D clamps them.
+s2JointId s2CreateDistanceJoint(s2WorldId worldId, const s2DistanceJointDef* def)
+{
+	if (s2IsValidVec2(def->localAnchorA) == false || s2IsValidVec2(def->localAnchorB) == false ||
+		s2IsValidDistanceValue(def->length) == false || s2IsValidDistanceValue(def->minLength) == false ||
+		s2IsValidDistanceValue(def->maxLength) == false || (def->minLength <= def->maxLength) == false ||
+		s2IsValidDistanceValue(def->hertz) == false || s2IsValidDistanceValue(def->dampingRatio) == false ||
+		s2IsValidDistanceValue(def->maxMotorForce) == false || s2IsValid(def->motorSpeed) == false)
+	{
+		return s2_nullJointId;
+	}
+
+	s2World* world = s2GetWorldFromId(worldId);
+	s2Body* bodyA = world->bodies + def->bodyIdA.index;
+	s2Body* bodyB = world->bodies + def->bodyIdB.index;
+
+	s2Joint* joint = s2AllocJoint(world, bodyA, bodyB);
+	joint->type = s2_distanceJoint;
+	joint->drawSize = 1.0f;
+	joint->localOriginAnchorA = def->localAnchorA;
+	joint->localOriginAnchorB = def->localAnchorB;
+	joint->referenceAngle = s2ClampDistanceLength(def->length);
+	joint->lowerAngle = s2ClampDistanceLength(def->minLength);
+	joint->upperAngle = s2ClampDistanceLength(def->maxLength);
+	joint->enableSpring = def->enableSpring;
+	joint->hertz = def->hertz;
+	joint->dampingRatio = def->dampingRatio;
+	joint->enableLimit = def->enableLimit;
+	joint->enableMotor = def->enableMotor;
+	joint->maxMotorTorque = def->maxMotorForce;
+	joint->motorSpeed = def->motorSpeed;
+	joint->collideConnected = def->collideConnected;
+
+	s2JointId jointId = {joint->object.index, world->index, joint->object.revision};
+	return jointId;
+}
+
+// the joint to edit, or NULL for a joint of another type
+static s2Joint* s2GetDistanceJointForEdit(s2JointId jointId, s2World** worldOut)
+{
+	s2Joint* joint = s2GetJointForEdit(jointId, worldOut);
+	return joint->type == s2_distanceJoint ? joint : NULL;
+}
+
+static const s2Joint* s2GetDistanceJoint(s2JointId jointId)
+{
+	s2World* world = s2GetWorldFromIndex(jointId.world);
+	const s2Joint* joint = world->joints + jointId.index;
+	S2_ASSERT(s2ObjectValid(&joint->object) && joint->object.revision == jointId.revision);
+	return joint->type == s2_distanceJoint ? joint : NULL;
+}
+
+void s2DistanceJoint_SetLength(s2JointId jointId, float length)
+{
+	if (s2IsValidDistanceValue(length) == false)
+	{
+		return;
+	}
+	s2World* world;
+	s2Joint* joint = s2GetDistanceJointForEdit(jointId, &world);
+	if (joint != NULL)
+	{
+		joint->referenceAngle = s2ClampDistanceLength(length);
+		s2MarkJointDirty(world, joint);
+	}
+}
+
+float s2DistanceJoint_GetLength(s2JointId jointId)
+{
+	const s2Joint* joint = s2GetDistanceJoint(jointId);
+	return joint != NULL ? joint->referenceAngle : 0.0f;
+}
+
+void s2DistanceJoint_EnableLimit(s2JointId jointId, bool enableLimit)
+{
+	s2World* world;
+	s2Joint* joint = s2GetDistanceJointForEdit(jointId, &world);
+	if (joint != NULL)
+	{
+		joint->enableLimit = enableLimit;
+		s2MarkJointDirty(world, joint);
+	}
+}
+
+void s2DistanceJoint_SetLengthRange(s2JointId jointId, float minLength, float maxLength)
+{
+	if (s2IsValidDistanceValue(minLength) == false || s2IsValidDistanceValue(maxLength) == false || (minLength <= maxLength) == false)
+	{
+		return;
+	}
+	s2World* world;
+	s2Joint* joint = s2GetDistanceJointForEdit(jointId, &world);
+	if (joint != NULL)
+	{
+		joint->lowerAngle = s2ClampDistanceLength(minLength);
+		joint->upperAngle = s2ClampDistanceLength(maxLength);
+		s2MarkJointDirty(world, joint);
+	}
+}
+
+float s2DistanceJoint_GetMinLength(s2JointId jointId)
+{
+	const s2Joint* joint = s2GetDistanceJoint(jointId);
+	return joint != NULL ? joint->lowerAngle : 0.0f;
+}
+
+float s2DistanceJoint_GetMaxLength(s2JointId jointId)
+{
+	const s2Joint* joint = s2GetDistanceJoint(jointId);
+	return joint != NULL ? joint->upperAngle : 0.0f;
+}
+
+void s2DistanceJoint_EnableSpring(s2JointId jointId, bool enableSpring)
+{
+	s2EnableJointSpring(jointId, s2_distanceJoint, enableSpring);
+}
+
+void s2DistanceJoint_SetSpringHertz(s2JointId jointId, float hertz)
+{
+	s2SetJointSpringValue(jointId, s2_distanceJoint, hertz, false);
+}
+
+void s2DistanceJoint_SetSpringDampingRatio(s2JointId jointId, float dampingRatio)
+{
+	s2SetJointSpringValue(jointId, s2_distanceJoint, dampingRatio, true);
+}
+
+void s2DistanceJoint_EnableMotor(s2JointId jointId, bool enableMotor)
+{
+	s2World* world;
+	s2Joint* joint = s2GetDistanceJointForEdit(jointId, &world);
+	if (joint != NULL)
+	{
+		joint->enableMotor = enableMotor;
+		s2MarkJointDirty(world, joint);
+	}
+}
+
+void s2DistanceJoint_SetMotorSpeed(s2JointId jointId, float motorSpeed)
+{
+	if (s2IsValid(motorSpeed) == false)
+	{
+		return;
+	}
+	s2World* world;
+	s2Joint* joint = s2GetDistanceJointForEdit(jointId, &world);
+	if (joint != NULL)
+	{
+		joint->motorSpeed = motorSpeed;
+		s2MarkJointDirty(world, joint);
+	}
+}
+
+void s2DistanceJoint_SetMaxMotorForce(s2JointId jointId, float maxMotorForce)
+{
+	if (s2IsValidDistanceValue(maxMotorForce) == false)
+	{
+		return;
+	}
+	s2World* world;
+	s2Joint* joint = s2GetDistanceJointForEdit(jointId, &world);
+	if (joint != NULL)
+	{
+		joint->maxMotorTorque = maxMotorForce;
+		s2MarkJointDirty(world, joint);
+	}
+}
+
+float s2DistanceJoint_GetMotorForce(s2JointId jointId, float inverseTimeStep)
+{
+	s2World* world = s2GetWorldFromIndex(jointId.world);
+	s2SyncStateToHost(world);
+	const s2Joint* joint = s2GetDistanceJoint(jointId);
+	return joint != NULL ? inverseTimeStep * joint->motorImpulse : 0.0f;
+}
+
+// the line from anchor A to anchor B at the lazily synced poses
+static s2Vec2 s2DistanceJointAxis(s2World* world, const s2Joint* joint, float* length)
+{
+	const s2Body* bodyA = world->bodies + joint->bodyIndexA;
+	const s2Body* bodyB = world->bodies + joint->bodyIndexB;
+	return s2cDistanceJointAxis(length, bodyA->position, bodyA->rot, s2Sub(joint->localOriginAnchorA, bodyA->localCenter),
+								bodyB->position, bodyB->rot, s2Sub(joint->localOriginAnchorB, bodyB->localCenter));
+}
+
+float s2DistanceJoint_GetCurrentLength(s2JointId jointId)
+{
+	s2World* world = s2GetWorldFromIndex(jointId.world);
+	s2SyncStateToHost(world);
+	const s2Joint* joint = s2GetDistanceJoint(jointId);
+	if (joint == NULL)
+	{
+		return 0.0f;
+	}
+	float length;
+	s2DistanceJointAxis(world, joint, &length);
+	return length;
+}
+
 // ---- reactions and break thresholds (DESIGN.md §3.13) -----------------------------------------------------------------
 
 // s2JointType and the device's S2B_JOINT_* number the joint types alike
 _Static_assert((int)s2_revoluteJoint == S2B_JOINT_REVOLUTE && (int)s2_mouseJoint == S2B_JOINT_MOUSE &&
 				   (int)s2_weldJoint == S2B_JOINT_WELD && (int)s2_prismaticJoint == S2B_JOINT_PRISMATIC &&
-				   (int)s2_motorJoint == S2B_JOINT_MOTOR,
+				   (int)s2_motorJoint == S2B_JOINT_MOTOR && (int)s2_distanceJoint == S2B_JOINT_DISTANCE,
 			   "joint type numbering");
 
 s2JointReaction s2ComputeJointReaction(int32_t type, s2Vec2 impulse, float motorImpulse, float lowerImpulse, float upperImpulse,
@@ -576,8 +789,11 @@ static s2JointReaction s2GetJointReaction(s2JointId jointId)
 	// row the device last solved, so the getters read what the device's reaction and break pass read for that step even
 	// after s2*Joint_EnableSpring has changed the joint and before the next step uploads it.
 	float motorImpulse = joint->springUploaded ? joint->motorImpulse + joint->springImpulse : joint->motorImpulse;
+	// a distance joint passes its world axis at the end of the step (DESIGN.md §3.16)
+	float length;
+	s2Vec2 axis = joint->type == s2_distanceJoint ? s2DistanceJointAxis(world, joint, &length) : joint->localAxisA;
 	return s2MakeJointReaction((int32_t)joint->type, joint->impulse, motorImpulse, joint->lowerImpulse, joint->upperImpulse,
-							   world->bodies[joint->bodyIndexA].rot, joint->localAxisA, world->reactionRate);
+							   world->bodies[joint->bodyIndexA].rot, axis, world->reactionRate);
 }
 
 s2Vec2 s2Joint_GetReactionForce(s2JointId jointId)

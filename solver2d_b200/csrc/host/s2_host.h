@@ -88,6 +88,7 @@ typedef enum s2JointType
 	s2_weldJoint,
 	s2_prismaticJoint,
 	s2_motorJoint,
+	s2_distanceJoint,
 } s2JointType;
 
 typedef struct s2Body
@@ -163,7 +164,8 @@ typedef struct s2Joint
 	bool collideConnected;
 
 	// revolute; a prismatic joint keeps its translation limits in lowerAngle / upperAngle and its maximum motor force in
-	// maxMotorTorque, as its device row does
+	// maxMotorTorque, as its device row does. A distance joint keeps its rest length in referenceAngle, its min / max length
+	// in lowerAngle / upperAngle, its maximum motor force in maxMotorTorque and its spring in hertz / dampingRatio.
 	bool enableMotor, enableLimit;
 	float maxMotorTorque, motorSpeed;
 	float referenceAngle, lowerAngle, upperAngle;

@@ -78,7 +78,7 @@ JOINT_ENABLE_LIMIT, JOINT_ENABLE_MOTOR, JOINT_COLLIDE_CONNECTED, JOINT_ENABLE_SP
 # its translation limits in lowerAngle / upperAngle and its maximum motor force in maxMotorTorque; a motor row keeps its
 # linear offset in localOriginAnchorA, its angular offset in referenceAngle, its maximum torque in maxMotorTorque, its
 # maximum force in hertz and its correction factor in dampingRatio)
-JOINT_REVOLUTE, JOINT_MOUSE, JOINT_WELD, JOINT_PRISMATIC, JOINT_MOTOR = 0, 1, 2, 3, 4
+JOINT_REVOLUTE, JOINT_MOUSE, JOINT_WELD, JOINT_PRISMATIC, JOINT_MOTOR, JOINT_DISTANCE = 0, 1, 2, 3, 4, 5
 
 # symbols declared in include/s2b_device.h (checked by the CPU test-suite against the built library)
 ABI_SYMBOLS = [

@@ -15,6 +15,8 @@ Each recipe restates one of the reference's sample scenes or one of the syntheti
 * :func:`welded_structures` — cantilevers, welded assemblies, a welded platform rider and a chain (the weld joint).
 * :func:`sliders`         — pistons, an elevator, an inclined slider, a kinematic carriage, a slider-crank and a mouse
                             joint on a slider (the prismatic joint).
+* :func:`distance_joints` — ropes of boxes, rigid-rod pendulums, a spring ring of circles over a pile, winches, a tether
+                            to a kinematic platform, a revolute chain and a mouse joint (the distance joint).
 * :func:`motors`          — top-down friction, a driven platform with a pile, a weak motor under its load, a dynamic
                             pair, a rider on a kinematic carriage, a drive across the angle seam and a mouse joint
                             (the motor joint).
@@ -1054,6 +1056,147 @@ def springs(lib: capi.Solver2D, solver="TGS_Soft", copies=1, kinematic=True) -> 
             md.bodyIdA = gid
             md.bodyIdB = dragged
             md.target = Vec2(x0 + 37.5, 1.5)
+            md.hertz = 3.0
+            md.dampingRatio = 0.7
+            sc.joints.append(lib.s2CreateMouseJoint(world, C.byref(md)))
+    return sc
+
+
+DISTANCE_PITCH = 40.0  # width of one copy of distance_joints (m)
+
+
+def distance_joints(lib: capi.Solver2D, solver="TGS_Soft", copies=1, kinematic=True, stand_ins=None) -> Scene:
+    """Distance joint coverage (DESIGN.md §3.16), `copies` side by side (about 60 bodies each). Per copy:
+
+    * two hanging ropes of five boxes each (every link a rope: spring on at hertz 0, limit [slop, 0.6]) from a beam;
+    * a row of four rigid-rod pendulums (1.5 m) started at different angles, so the bobs hit one another;
+    * a soft ring of eight circles on springs (neighbours 6 Hz, opposite pairs 3 Hz) dropped on a pile of boxes;
+    * a winch (rope with a motor shortening at 0.5 m/s) lifting a box with 60 N, and one set below its load (3 N);
+    * with `kinematic`: a box on a sprung, limited tether below a kinematic platform that moves sideways;
+    * a revolute chain of four links hung from a post;
+    * a box pulled by a mouse joint (first copy only).
+
+    On a library without s2CreateDistanceJoint (the reference), or with `stand_ins` true, every distance joint is created as
+    a revolute joint at anchor B's start point with limits and motor off. ``sc.piles["distance"]`` lists the index into
+    ``sc.joints`` of every distance joint and ``sc.piles["distance_defs"]`` its definition (anchors relative to the body
+    origins, lengths clamped as s2CreateDistanceJoint clamps them), so that a test can turn the stand-in rows into distance
+    rows."""
+    world = lib.create_world(solver)
+    sc = Scene(lib, world, name=f"distance_joints{copies}")
+    sc.piles["distance"] = []
+    sc.piles["distance_defs"] = []
+    real = "s2CreateDistanceJoint" not in lib.missing and not stand_ins
+    gid = _ground(lib, world, 0.5 * DISTANCE_PITCH * copies + 5.0)
+    sc.bodies.append(gid)
+
+    def body(kind, x, y, hx=0.25, hy=0.25, vx=0.0, radius=None, group=0):
+        bd = default_body_def()
+        bd.type = kind
+        bd.position = Vec2(x, y)
+        bd.linearVelocity = Vec2(vx, 0.0)
+        bid = lib.s2CreateBody(world, C.byref(bd))
+        sd = default_shape_def()
+        sd.filter.groupIndex = group
+        if radius is not None:
+            lib.s2CreateCircleShape(bid, C.byref(sd), C.byref(Circle(Vec2(0.0, 0.0), radius)))
+        else:
+            lib.s2CreatePolygonShape(bid, C.byref(sd), C.byref(lib.s2MakeBox(hx, hy)))
+        sc.bodies.append(bid)
+        return bid
+
+    def clamp(length):
+        return float(np.clip(np.float32(length), np.float32(0.005), np.float32(100000.0)))
+
+    def distance(a, b, pa, pb, length, spring=None, limit=None, motor=None):
+        """pa, pb: the anchors' world points at creation."""
+        d = dict(localAnchorA=tuple(lib.s2Body_GetLocalPoint(a, pa)), localAnchorB=tuple(lib.s2Body_GetLocalPoint(b, pb)),
+                 length=clamp(length), enableSpring=spring is not None, hertz=spring[0] if spring else 0.0,
+                 dampingRatio=spring[1] if spring else 0.0, enableLimit=limit is not None,
+                 minLength=clamp(limit[0] if limit else 0.0), maxLength=clamp(limit[1] if limit else 100000.0),
+                 enableMotor=motor is not None, motorSpeed=motor[0] if motor else 0.0, maxMotorForce=motor[1] if motor else 0.0)
+        if real:
+            jd = capi.default_distance_def()
+            for name, value in d.items():
+                setattr(jd, name, Vec2(*value) if isinstance(value, tuple) else value)
+            create = lib.s2CreateDistanceJoint
+        else:
+            jd = default_revolute_def()
+            jd.localAnchorA = lib.s2Body_GetLocalPoint(a, pb)
+            jd.localAnchorB = lib.s2Body_GetLocalPoint(b, pb)
+            create = lib.s2CreateRevoluteJoint
+        jd.bodyIdA = a
+        jd.bodyIdB = b
+        sc.piles["distance"].append(len(sc.joints))
+        sc.piles["distance_defs"].append(d)
+        jid = create(world, C.byref(jd))
+        sc.joints.append(jid)
+        return jid
+
+    def revolute(a, b, pivot):
+        jd = default_revolute_def()
+        jd.bodyIdA = a
+        jd.bodyIdB = b
+        jd.localAnchorA = lib.s2Body_GetLocalPoint(a, pivot)
+        jd.localAnchorB = lib.s2Body_GetLocalPoint(b, pivot)
+        sc.joints.append(lib.s2CreateRevoluteJoint(world, C.byref(jd)))
+
+    D, S, K = capi.DYNAMIC_BODY, capi.STATIC_BODY, capi.KINEMATIC_BODY
+    rope = (0.0, 0.0)
+    for k in range(copies):
+        x0 = -0.5 * DISTANCE_PITCH * (copies - 1) + DISTANCE_PITCH * k - 18.0
+        # two hanging ropes of boxes from a beam, the second started swinging
+        beam = body(S, x0 + 1.5, 9.0, hx=1.5, hy=0.1)
+        for r, dx in enumerate((0.5, 2.5)):
+            prev, prev_at = beam, Vec2(x0 + dx, 8.9)
+            for i in range(5):
+                x = x0 + dx + 0.5 * (i + 1) * r
+                y = 8.9 - 0.55 * (i + 1)
+                box = body(D, x, y, hx=0.15, hy=0.15)
+                distance(prev, box, prev_at, Vec2(x, y + 0.15), 0.5, spring=rope, limit=(0.0, 0.6))
+                prev, prev_at = box, Vec2(x, y - 0.15)
+        # a row of rigid-rod pendulums that hit one another
+        for i in range(4):
+            pivot = Vec2(x0 + 5.0 + 0.6 * i, 6.0)
+            angle = 0.8 if i == 0 else 0.05 * i
+            bob = body(D, pivot.x - 1.5 * math.sin(angle), 6.0 - 1.5 * math.cos(angle), hx=0.25, hy=0.25)
+            distance(gid, bob, pivot, Vec2(pivot.x - 1.5 * math.sin(angle), 6.0 - 1.5 * math.cos(angle)), 1.5)
+        # a pile of boxes and a soft ring of circles falling onto it
+        for i in range(4):
+            for j in range(4 - i):
+                body(D, x0 + 11.0 + 0.55 * j + 0.275 * i, 0.25 + 0.5 * i, hx=0.25, hy=0.25)
+        ring = []
+        for i in range(8):
+            a = 2.0 * math.pi * i / 8
+            ring.append((body(D, x0 + 11.8 + math.cos(a), 5.0 + math.sin(a), radius=0.2), Vec2(x0 + 11.8 + math.cos(a), 5.0 + math.sin(a))))
+        for i in range(8):
+            (a, pa), (b, pb) = ring[i], ring[(i + 1) % 8]
+            distance(a, b, pa, pb, math.hypot(pb.x - pa.x, pb.y - pa.y), spring=(6.0, 0.5))
+        for i in range(4):
+            (a, pa), (b, pb) = ring[i], ring[i + 4]
+            distance(a, b, pa, pb, 2.0, spring=(3.0, 0.3), limit=(1.0, 2.5))
+        # a winch lifting its load, and one set below its load
+        for dx, force in ((17.0, 60.0), (19.0, 3.0)):
+            load = body(D, x0 + dx, 5.0, hx=0.3, hy=0.3)
+            distance(gid, load, Vec2(x0 + dx, 9.0), Vec2(x0 + dx, 5.3), 3.7, spring=rope, limit=(0.5, 4.0),
+                     motor=(-0.5, force))
+        # a sprung tether below a kinematic platform
+        if kinematic:
+            platform = body(K, x0 + 23.0, 7.0, hx=1.0, hy=0.125, vx=0.7)
+            rider = body(D, x0 + 23.0, 5.5, hx=0.25, hy=0.25)
+            distance(platform, rider, Vec2(x0 + 23.0, 6.875), Vec2(x0 + 23.0, 5.75), 1.2, spring=(2.0, 0.2), limit=(0.6, 1.6))
+        # a revolute chain
+        post = body(S, x0 + 27.0, 6.0, hx=0.1, hy=0.1)
+        prev = post
+        for i in range(4):
+            link = body(D, x0 + 27.5 + 1.0 * i, 6.0, hx=0.5, hy=0.1)
+            revolute(prev, link, Vec2(x0 + 27.0 + 1.0 * i, 6.0))
+            prev = link
+        if k == 0:
+            dragged = body(D, x0 + 33.0, 0.25)
+            md = default_mouse_def()
+            md.bodyIdA = gid
+            md.bodyIdB = dragged
+            md.target = Vec2(x0 + 33.5, 1.5)
             md.hertz = 3.0
             md.dampingRatio = 0.7
             sc.joints.append(lib.s2CreateMouseJoint(world, C.byref(md)))
