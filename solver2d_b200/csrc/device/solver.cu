@@ -3814,6 +3814,13 @@ void s2bSolve(s2bWorld* w, int solverType, const s2bStepContext* ctxIn)
 
 	bool capturing = graphable && sig == s->graphCandidate;
 	int launchesBefore = w->kernelLaunches;
+	if (capturing && s->scheduleSig != sig)
+	{
+		// the candidate's eager step was followed by a replay with other settings (which leaves graphCandidate alone): the
+		// schedule buffers and the narrow phase's contact rows are that replay's, so the captured gate has to rebuild them
+		int one = 1;
+		S2B_CHECK(cudaMemcpyAsync(w->schedDirty.p, &one, sizeof(int), cudaMemcpyHostToDevice, st));
+	}
 	s->graphCandidate = sig;
 	s->scheduleSig = sig;
 	if (capturing == false)
@@ -3931,7 +3938,8 @@ void s2bSolve(s2bWorld* w, int solverType, const s2bStepContext* ctxIn)
 	s->graphSig = sig;
 	s->graphLaunches = w->kernelLaunches - launchesBefore;
 	s->graphCaptures += 1;
-	// the schedule of the previous (eager) step is still valid unless the flag says otherwise: the gate decides
+	// the schedule of the previous solve is still valid unless the flag says otherwise (set above when that solve was a replay
+	// with other settings): the gate decides
 	S2B_CHECK(cudaGraphLaunch(s->graphExec, st));
 }
 

@@ -8,6 +8,8 @@ Each recipe restates one of the reference's sample scenes or one of the syntheti
 * :func:`bridge`          — ``Bridge`` (reference samples/collection/sample_joints.cpp:15-90).
 * :func:`joint_contact_stress` — config 4: stacked bridges + a grid of boxes dropped on them.
 * :func:`tumbler`         — config 3: motorised hollow container with a grid of small boxes.
+* :func:`damped_mix`      — a pile, thrown bodies and unconstrained bodies with body damping and gravity scales, and
+                            optionally a damped revolute chain.
 * :func:`mixed_shapes`    — circles/capsules/polygons/segments on a ground, exercising all nine manifold functions.
 * :func:`collision_zoo`   — every manifold kind, flipped pairs, dynamic segments, compound bodies, mixed frictions and
                             shape filters, thrown sideways.
@@ -289,6 +291,75 @@ def limited_chains(lib, solver="TGS_Soft", chains=3, links=6) -> Scene:
             bid = lib.s2CreateBody(world, C.byref(bd))
             lib.s2CreatePolygonShape(bid, C.byref(sd), C.byref(box))
             sc.bodies.append(bid)
+    return sc
+
+
+DAMPED_LINEAR = (0.0, 0.1, 0.5, 2.0)
+DAMPED_ANGULAR = (0.0, 0.3, 5.0)
+DAMPED_GRAVITY = (1.0, 0.5, 0.0, -0.25)
+
+
+def damped_mix(lib, solver="TGS_Soft", joints=False) -> Scene:
+    """Body damping and gravity scale coverage. Every dynamic body k gets linearDamping DAMPED_LINEAR[k % 4] and
+    angularDamping DAMPED_ANGULAR[k % 3] (all twelve pairs), and a gravityScale from DAMPED_GRAVITY:
+
+    * a pile of 24 boxes on the ground (gravity scale 1 or 0.5, so it stays a pile);
+    * eight circles, capsules and boxes thrown at the pile, spinning (every gravity scale);
+    * eight spinning bodies high above the ground and 3 m apart, drifting apart: they touch nothing during a test run, so
+      they are integrated as unconstrained bodies (every gravity scale, one rising);
+    * with `joints`: a chain of six capsules on revolute joints hanging from the ground, damped like the rest.
+
+    Without `joints` the world has no joints and no kinematic bodies."""
+    world = lib.create_world(solver)
+    sc = Scene(lib, world, name="damped_mix" + ("_joints" if joints else ""))
+    gid = _ground(lib, world, 30.0)
+    sc.bodies.append(gid)
+    sd = default_shape_def()
+    k = 0
+
+    def body(x, y, gravity, kind, vx=0.0, vy=0.0, w=0.0, angle=0.0):
+        nonlocal k
+        bd = default_body_def()
+        bd.type = capi.DYNAMIC_BODY
+        bd.position = Vec2(x, y)
+        bd.angle = angle
+        bd.linearVelocity = Vec2(vx, vy)
+        bd.angularVelocity = w
+        bd.linearDamping = DAMPED_LINEAR[k % 4]
+        bd.angularDamping = DAMPED_ANGULAR[k % 3]
+        bd.gravityScale = gravity
+        k += 1
+        bid = lib.s2CreateBody(world, C.byref(bd))
+        if kind == 0:
+            box = lib.s2MakeBox(0.4, 0.3)
+            lib.s2CreatePolygonShape(bid, C.byref(sd), C.byref(box))
+        elif kind == 1:
+            lib.s2CreateCircleShape(bid, C.byref(sd), C.byref(Circle(Vec2(0.05, 0.0), 0.35)))
+        else:
+            lib.s2CreateCapsuleShape(bid, C.byref(sd), C.byref(Capsule(Vec2(-0.35, 0.0), Vec2(0.35, 0.0), 0.2)))
+        sc.bodies.append(bid)
+        return bid
+
+    for i in range(4):
+        for j in range(6):
+            body(-10.0 + 0.85 * j + 0.2 * (i % 2), 0.3 + 0.6 * i, DAMPED_GRAVITY[(i + j) % 2], 0)
+    for n in range(8):
+        body(-1.0 + 0.9 * n, 1.0 + 0.5 * (n % 3), DAMPED_GRAVITY[n % 4], n % 3, vx=-6.0 - 0.5 * n, vy=1.5,
+             w=4.0 if n % 2 == 0 else -3.0, angle=0.3 * n)
+    for n in range(8):
+        body(10.0 + 3.0 * n, 40.0, DAMPED_GRAVITY[n % 4], n % 3, vx=0.5 * (n - 3.5), vy=0.8, w=2.0 + n, angle=0.2 * n)
+    if joints:
+        prev = gid
+        for i in range(6):
+            bid = body(2.5 + 1.0 * i, 10.0, DAMPED_GRAVITY[i % 2], 2)
+            jd = default_revolute_def()
+            pivot = Vec2(2.0 + 1.0 * i, 10.0)
+            jd.bodyIdA = prev
+            jd.bodyIdB = bid
+            jd.localAnchorA = lib.s2Body_GetLocalPoint(prev, pivot)
+            jd.localAnchorB = lib.s2Body_GetLocalPoint(bid, pivot)
+            sc.joints.append(lib.s2CreateRevoluteJoint(world, C.byref(jd)))
+            prev = bid
     return sc
 
 

@@ -109,8 +109,8 @@ def _distance_world(P, solver):
     return wid, joints, (ground, rod)
 
 
-def _step_and_compare(P, wid, dw, O, solver, steps, colour=False, edit=None):
-    ctx = device.make_context(solver, DT, 4, 2)
+def _step_and_compare(P, wid, dw, O, solver, steps, colour=False, edit=None, dt=DT, substeps=4, relax=2):
+    ctx = device.make_context(solver, dt, substeps, relax)
     moved = False
     for k in range(steps):
         if edit is not None:
@@ -119,7 +119,7 @@ def _step_and_compare(P, wid, dw, O, solver, steps, colour=False, edit=None):
         bodies = dw.download_all_bodies()
         joints = dw.download_joints()
         dp = dw.download_delta_positions()
-        P.s2World_Step(wid, DT, 4, 2, True)
+        P.s2World_Step(wid, dt, substeps, relax, True)
         assert dw.counters().constraintCount == 0
         order = None
         if colour:

@@ -43,10 +43,11 @@ def _same(g, w):
 
 
 def _run(R, P, dev, recipe, solver, steps, vel, pos, kw, min_replays=0, setup=None, observe=None, oracle=None,
-         as_joints=None, before_step=None, after_step=None, warm_start=True):
+         as_joints=None, before_step=None, after_step=None, warm_start=True, settings=None):
     """`oracle`: the oracle to replay (default oracle.port's); `as_joints(joints, sc)`: turns the reference's joint rows
     into the device's (stand-ins); `before_step(step, (lib, scene) pairs)`: public-API calls made on both worlds before a
-    step; `after_step(dw)`: called after every checked step."""
+    step; `after_step(dw)`: called after every checked step; `settings(step) -> (dt, sub-steps, relax iterations, warm
+    starting)`: the step's settings (default: DT, `vel`, `pos`, `warm_start` on every step)."""
     O = port.load() if oracle is None else oracle
     sr = recipe(R, solver, **kw)
     sp = recipe(P, solver, **kw)
@@ -57,7 +58,9 @@ def _run(R, P, dev, recipe, solver, steps, vel, pos, kw, min_replays=0, setup=No
     dw = device.DeviceWorld.attach(dev, sp.world)
     if setup is not None:
         setup(dw)
-    ctx = device.make_context(solver, DT, vel, pos, warm_start)
+    if settings is None:
+        def settings(step):
+            return DT, vel, pos, warm_start
     worst = {}
     sticky = solver == "TGS_Sticky"
     solved = {}  # TGS_Sticky: the oracle's rows of the previous step, by pair key
@@ -70,7 +73,9 @@ def _run(R, P, dev, recipe, solver, steps, vel, pos, kw, min_replays=0, setup=No
         load_bodies_into_ref(R, sr.world, pre)
         R.step_collide(sr.world)
 
-        sp.step(DT, vel, pos, warm_start)
+        dt, S, E, warm = settings(step)
+        ctx = device.make_context(solver, dt, S, E, warm)
+        sp.step(dt, S, E, warm)
 
         bodies = body_rows_from_ref(*R.bodies(sr.world))
         cf, ci = R.contacts(sr.world)

@@ -13,12 +13,13 @@ from solver2d_b200 import capi, device, scenes
 DT = 1.0 / 60.0
 
 
-def _pin(reference, recipe, solver, warm_steps, vel, pos, warm_start=True, **kw):
+def _pin(reference, recipe, solver, warm_steps, vel, pos, warm_start=True, dt=DT, **kw):
+    """`warm_steps` reference steps at (dt, vel, pos), then one stage solved by both at (dt, vel, pos, warm_start)."""
     R = reference
     O = port.load()
     sc = recipe(R, solver, **kw)
     for _ in range(warm_steps):
-        sc.step(DT, vel, pos, True)
+        sc.step(dt, vel, pos, True)
     R.step_collide(sc.world)
     bf, bi = R.bodies(sc.world)
     cf, ci = R.contacts(sc.world)
@@ -26,10 +27,10 @@ def _pin(reference, recipe, solver, warm_steps, vel, pos, warm_start=True, **kw)
     bodies = body_rows_from_ref(bf, bi)
     contacts, slots = contact_rows_from_ref(cf, ci)
     joints = joint_rows_from_ref(jf, ji)
-    ctx = device.make_context(solver, DT, vel, pos, warm_start)
+    ctx = device.make_context(solver, dt, vel, pos, warm_start)
     ob, oc, oj = O.solve(capi.SOLVER[solver], bodies, contacts, joints, ctx)
 
-    R.step_solve(sc.world, DT, vel, pos, warm_start)
+    R.step_solve(sc.world, dt, vel, pos, warm_start)
     bf2, bi2 = R.bodies(sc.world)
     cf2, ci2 = R.contacts(sc.world)
     valid = bi2[:, 0] == 1
