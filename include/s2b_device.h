@@ -106,13 +106,14 @@ enum
 	S2B_JOINT_PRISMATIC = 3,
 	S2B_JOINT_MOTOR = 4, // never carries S2B_JOINT_ENABLE_LIMIT or S2B_JOINT_ENABLE_MOTOR
 	S2B_JOINT_DISTANCE = 5,
+	S2B_JOINT_WHEEL = 6,
 };
 
 #define S2B_JOINT_ENABLE_LIMIT 0x10
 #define S2B_JOINT_ENABLE_MOTOR 0x20
 #define S2B_JOINT_COLLIDE_CONNECTED 0x40
-// revolute, prismatic and distance rows only: a spring on the joint's axis (DESIGN.md §3.14, §3.16), stiffness hertz,
-// damping dampingRatio
+// revolute, prismatic, distance and wheel rows only: a spring on the joint's axis (DESIGN.md §3.14, §3.16, §3.17),
+// stiffness hertz, damping dampingRatio
 #define S2B_JOINT_ENABLE_SPRING 0x80
 
 // One joint; mirrors s2Joint / s2RevoluteJoint / s2MouseJoint (reference src/joint.h:28-102).
@@ -145,6 +146,10 @@ typedef struct s2bJointRow
 	// upperAngle, its maximum motor force (N) in maxMotorTorque and its spring (S2B_JOINT_ENABLE_SPRING) in hertz /
 	// dampingRatio; impulse[0] is the rigid length row's impulse, impulse[1] stays 0, and motorImpulse / lowerImpulse /
 	// upperImpulse / springImpulse are the axial impulses their names say.
+	// A wheel row (DESIGN.md §3.17) holds its axis in localAxisA, its translation limits in lowerAngle / upperAngle, its
+	// maximum motor torque (N-m) in maxMotorTorque, its motor speed (rad/s) in motorSpeed and its spring in hertz /
+	// dampingRatio; impulse[0] is the perpendicular row's impulse, impulse[1] the angular motor's impulse, motorImpulse stays
+	// 0, lowerImpulse / upperImpulse / springImpulse are the axial impulses their names say and referenceAngle is unused.
 	float localAxisA[2];
 	// break thresholds (N, N-m) of the reaction pass (DESIGN.md §3.13); 0 = none. A row with either set is checked after every
 	// finalize; a row without them is never checked.

@@ -231,6 +231,66 @@ S2B_API float s2DistanceJoint_GetMotorForce(s2JointId jointId, float inverseTime
 // The current distance between the two anchors (m).
 S2B_API float s2DistanceJoint_GetCurrentLength(s2JointId jointId);
 
+// Wheel joint (DESIGN.md §3.17; Box2D v3's semantics): body B's anchor slides along an axis fixed in body A, and body B
+// turns freely about it. Rows: a spring along the axis toward translation 0 (enableSpring, acts when hertz > 0), a motor on
+// the relative rotation (enableMotor: drives angularVelocity(B) - angularVelocity(A) to motorSpeed with at most
+// maxMotorTorque; nothing when both rotations are fixed), a lower and an upper translation limit (enableLimit) and the
+// point-on-line row that keeps anchor B on the axis. Equal limits make a rigid axle. Anchors are relative to each body's
+// origin; the translation is measured along the axis from anchor A to anchor B. Under XPBD the motor is not applied.
+// Destroy it with s2DestroyJoint.
+typedef struct s2WheelJointDef
+{
+	s2BodyId bodyIdA;
+	s2BodyId bodyIdB;
+	s2Vec2 localAnchorA;
+	s2Vec2 localAnchorB;
+	s2Vec2 localAxisA; // the suspension axis in body A's frame; normalized at creation
+	bool enableSpring;
+	float hertz;		// the spring's stiffness as a frequency (Hz), >= 0; 0 exerts nothing
+	float dampingRatio; // the spring's damping ratio, >= 0 (1 = critical)
+	bool enableLimit;
+	float lowerTranslation; // m
+	float upperTranslation; // m
+	bool enableMotor;
+	float maxMotorTorque;  // N-m, >= 0
+	float motorSpeed;	   // rad/s
+	bool collideConnected; // keep the contacts the two bodies already have
+} s2WheelJointDef;
+
+S2_INLINE struct s2WheelJointDef s2DefaultWheelJointDef(void)
+{
+	s2WheelJointDef def = S2_ZERO_INIT;
+	def.bodyIdA = s2_nullBodyId;
+	def.bodyIdB = s2_nullBodyId;
+	def.localAxisA.y = 1.0f;
+	def.enableSpring = true;
+	def.hertz = 1.0f;
+	def.dampingRatio = 0.7f;
+	return def;
+}
+
+// Returns s2_nullJointId (and creates nothing) for an axis of zero length or with a non-finite component, a non-finite
+// anchor, lowerTranslation > upperTranslation, a negative or non-finite hertz, dampingRatio or maxMotorTorque, or a
+// non-finite motorSpeed.
+S2B_API s2JointId s2CreateWheelJoint(s2WorldId worldId, const s2WheelJointDef* def);
+// The setters ignore bad input (the joint keeps its value) and a joint that is not a wheel joint. A change takes effect at
+// the next step. The spring setters are the revolute and prismatic joints' (a negative or non-finite value is ignored).
+S2B_API void s2WheelJoint_EnableSpring(s2JointId jointId, bool enableSpring);
+S2B_API void s2WheelJoint_SetSpringHertz(s2JointId jointId, float hertz);
+S2B_API void s2WheelJoint_SetSpringDampingRatio(s2JointId jointId, float dampingRatio);
+S2B_API void s2WheelJoint_EnableLimit(s2JointId jointId, bool enableLimit);
+// Ignored when lower > upper or either is not finite.
+S2B_API void s2WheelJoint_SetLimits(s2JointId jointId, float lower, float upper);
+S2B_API void s2WheelJoint_EnableMotor(s2JointId jointId, bool enableMotor);
+// Any finite speed (rad/s).
+S2B_API void s2WheelJoint_SetMotorSpeed(s2JointId jointId, float motorSpeed);
+// Ignored when negative or not finite.
+S2B_API void s2WheelJoint_SetMaxMotorTorque(s2JointId jointId, float maxMotorTorque);
+// The motor torque of the last step (N-m): inverseTimeStep times the angular motor impulse. 0 for another joint type.
+S2B_API float s2WheelJoint_GetMotorTorque(s2JointId jointId, float inverseTimeStep);
+// The current translation (m) along the world axis, from anchor A to anchor B. 0 for another joint type.
+S2B_API float s2WheelJoint_GetTranslation(s2JointId jointId);
+
 // ---- joint reactions and breakable joints (DESIGN.md §3.13) --------------------------------------------------------
 
 // What a joint exerts on body B over the last step: force (N, world frame) and torque (N-m).
@@ -242,15 +302,18 @@ typedef struct s2JointReaction
 
 // The one definition of a joint's reaction, used by the device's reaction pass, the host getters and the tests. `type` is
 // an S2B_JOINT_* value; the impulses are the columns of s2bJointRow; qA is body A's rotation at the end of the step (only the
-// prismatic joint reads it, with localAxisA). `rate` is 1 / (the interval the solver variant accumulates the impulses over):
-// 1 / dt under TGS_Sticky, 1 / h under every other variant (h = dt for the variants that do not sub-step).
-// A revolute or prismatic joint with its spring enabled passes motorImpulse + springImpulse as `motorImpulse` (the spring
-// acts on the same axis: the revolute's torque, the prismatic's axial force), so its reaction and break test include the
-// spring's load; every other joint passes motorImpulse.
+// prismatic and wheel joints read it, with localAxisA). `rate` is 1 / (the interval the solver variant accumulates the
+// impulses over): 1 / dt under TGS_Sticky, 1 / h under every other variant (h = dt for the variants that do not sub-step).
+// A revolute, prismatic or wheel joint with its spring enabled passes motorImpulse + springImpulse as `motorImpulse` (the
+// spring acts on the same axis: the revolute's torque, the prismatic's and the wheel's axial force), so its reaction and
+// break test include the spring's load; every other joint passes motorImpulse.
 //   revolute   force = rate impulse    torque = rate (motorImpulse + lowerImpulse - upperImpulse)
 //   mouse, weld, motor                 force = rate impulse    torque = rate motorImpulse
 //   prismatic  force = rate (impulse.x perp + (motorImpulse + lowerImpulse - upperImpulse) axis), torque = rate impulse.y,
 //              axis = qA localAxisA, perp = leftPerp(axis)
+//   wheel      as prismatic: impulse.x is the perpendicular impulse, impulse.y the angular motor's and motorImpulse (0 in
+//              the row) carries the spring, so force = rate (impulse.x perp + (spring + lower - upper) axis) and
+//              torque = rate impulse.y
 //   distance   force = rate (impulse.x + motorImpulse + lowerImpulse - upperImpulse) axis, torque = 0. Here localAxisA is the
 //              WORLD axis, the unit vector from anchor A to anchor B at the end of the step (zero when they coincide), and
 //              qA is not read; a distance joint with its spring enabled also passes motorImpulse + springImpulse.
@@ -272,7 +335,7 @@ S2_INLINE s2JointReaction s2MakeJointReaction(int32_t type, s2Vec2 impulse, floa
 		f.y = axial * localAxisA.y;
 		t = 0.0f;
 	}
-	else if (type == S2B_JOINT_PRISMATIC)
+	else if (type == S2B_JOINT_PRISMATIC || type == S2B_JOINT_WHEEL)
 	{
 		s2Vec2 axis = s2RotateVector(qA, localAxisA);
 		s2Vec2 perp = s2LeftPerp(axis);

@@ -200,6 +200,27 @@ class DistanceJointDef(C.Structure):
     ]
 
 
+class WheelJointDef(C.Structure):
+    """s2WheelJointDef (include/solver2d_b200.h): an extension, absent from the reference."""
+    _fields_ = [
+        ("bodyIdA", BodyId),
+        ("bodyIdB", BodyId),
+        ("localAnchorA", Vec2),
+        ("localAnchorB", Vec2),
+        ("localAxisA", Vec2),
+        ("enableSpring", C.c_bool),
+        ("hertz", C.c_float),
+        ("dampingRatio", C.c_float),
+        ("enableLimit", C.c_bool),
+        ("lowerTranslation", C.c_float),
+        ("upperTranslation", C.c_float),
+        ("enableMotor", C.c_bool),
+        ("maxMotorTorque", C.c_float),
+        ("motorSpeed", C.c_float),
+        ("collideConnected", C.c_bool),
+    ]
+
+
 class MotorJointDef(C.Structure):
     """s2MotorJointDef (include/solver2d_b200.h): an extension, absent from the reference."""
     _fields_ = [
@@ -305,6 +326,18 @@ def default_distance_def() -> DistanceJointDef:
     return d
 
 
+def default_wheel_def() -> WheelJointDef:
+    """s2DefaultWheelJointDef (include/solver2d_b200.h): Box2D v3's defaults."""
+    d = WheelJointDef()
+    d.bodyIdA = BodyId(-1, -1, 0)
+    d.bodyIdB = BodyId(-1, -1, 0)
+    d.localAxisA = Vec2(0.0, 1.0)
+    d.enableSpring = True
+    d.hertz = 1.0
+    d.dampingRatio = 0.7
+    return d
+
+
 def default_motor_def() -> MotorJointDef:
     """s2DefaultMotorJointDef (include/solver2d_b200.h)."""
     d = MotorJointDef()
@@ -399,6 +432,18 @@ _API = {
     "s2DistanceJoint_SetMaxMotorForce": (None, [JointId, C.c_float]),
     "s2DistanceJoint_GetMotorForce": (C.c_float, [JointId, C.c_float]),
     "s2DistanceJoint_GetCurrentLength": (C.c_float, [JointId]),
+    # wheel joint (DESIGN.md §3.17)
+    "s2CreateWheelJoint": (JointId, [WorldId, C.POINTER(WheelJointDef)]),
+    "s2WheelJoint_EnableSpring": (None, [JointId, C.c_bool]),
+    "s2WheelJoint_SetSpringHertz": (None, [JointId, C.c_float]),
+    "s2WheelJoint_SetSpringDampingRatio": (None, [JointId, C.c_float]),
+    "s2WheelJoint_EnableLimit": (None, [JointId, C.c_bool]),
+    "s2WheelJoint_SetLimits": (None, [JointId, C.c_float, C.c_float]),
+    "s2WheelJoint_EnableMotor": (None, [JointId, C.c_bool]),
+    "s2WheelJoint_SetMotorSpeed": (None, [JointId, C.c_float]),
+    "s2WheelJoint_SetMaxMotorTorque": (None, [JointId, C.c_float]),
+    "s2WheelJoint_GetMotorTorque": (C.c_float, [JointId, C.c_float]),
+    "s2WheelJoint_GetTranslation": (C.c_float, [JointId]),
     # joint springs (DESIGN.md §3.14)
     "s2PrismaticJoint_EnableSpring": (None, [JointId, C.c_bool]),
     "s2PrismaticJoint_SetSpringHertz": (None, [JointId, C.c_float]),

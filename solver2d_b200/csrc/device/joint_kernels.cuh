@@ -156,17 +156,21 @@ template <int KIND> __device__ __forceinline__ void s2bPrepareJointRows(const So
 		jc.limp[t] = limp;
 		return;
 	}
-	if (S2B_JOINT_TYPE(flags) == S2B_JOINT_PRISMATIC || S2B_JOINT_TYPE(flags) == S2B_JOINT_MOTOR)
+	if (S2B_JOINT_TYPE(flags) == S2B_JOINT_PRISMATIC || S2B_JOINT_TYPE(flags) == S2B_JOINT_MOTOR ||
+		S2B_JOINT_TYPE(flags) == S2B_JOINT_WHEEL)
 	{
 		// DESIGN.md §3.9: the local axis rides in the motor row's spare zw; every mass is formed fresh in each solve.
 		// Limit and motor impulses are kept only with their flag and a warm start, the block impulse with the warm start.
 		// A motor joint (§3.10) carries its maximum force and correction factor in those zw instead, never has either
-		// flag, and keeps its angular impulse (imp.z) exactly when it keeps its linear one.
+		// flag, and keeps its angular impulse (imp.z) exactly when it keeps its linear one. A wheel joint (§3.17) keeps its
+		// perpendicular impulse in imp.x and its angular motor impulse in imp.y; imp.z stays 0.
 		bool motorJoint = S2B_JOINT_TYPE(flags) == S2B_JOINT_MOTOR;
+		bool wheel = S2B_JOINT_TYPE(flags) == S2B_JOINT_WHEEL;
 		float4 axis = a.joints.target[slot];
 		jc.motor[t] = motorJoint ? motor : make_float4(motor.x, motor.y, axis.z, axis.w);
-		// a motor joint's angular row uses the revolute's axial mass, 1 / (iA + iB) (0 when both rotations are fixed)
-		float motorAxialMass = motorJoint && iA + iB > 0.0f ? 1.0f / (iA + iB) : 0.0f;
+		// a motor joint's angular row and a wheel joint's motor use the revolute's axial mass, 1 / (iA + iB) (0 when both
+		// rotations are fixed)
+		float motorAxialMass = (motorJoint || wheel) && iA + iB > 0.0f ? 1.0f / (iA + iB) : 0.0f;
 		jc.d0ax[t] = make_float4(centerDiff0.x, centerDiff0.y, motorAxialMass, 0.0f);
 		jc.pivot[t] = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
 		if (KIND == JPREP_XPBD || warmStart == false)
@@ -181,6 +185,11 @@ template <int KIND> __device__ __forceinline__ void s2bPrepareJointRows(const So
 		}
 		if ((flags & S2B_JOINT_ENABLE_MOTOR) == 0 && motorJoint == false)
 		{
+			imp.z = 0.0f;
+		}
+		if (wheel)
+		{
+			imp.y = (flags & S2B_JOINT_ENABLE_MOTOR) != 0 && motorAxialMass > 0.0f ? imp.y : 0.0f;
 			imp.z = 0.0f;
 		}
 		jc.imp[t] = imp;
@@ -266,9 +275,9 @@ __device__ __forceinline__ void s2bStoreJointImpulses(const SolveArgs& a, int t)
 // jc.imp.w = accumulated spring impulse.
 // ---------------------------------------------------------------------------------------------------------------
 
-// the spring's part of prepare. A spring acts only on a revolute, prismatic or distance row with a positive hertz and, on a
-// revolute row, a rotation to act on, on a distance row minLength < maxLength; every other row loses the flag in jc.head,
-// so no solve or warm start evaluates a spring term for it, and gets a zero spring impulse.
+// the spring's part of prepare. A spring acts only on a revolute, prismatic, distance or wheel row with a positive hertz
+// and, on a revolute row, a rotation to act on, on a distance row minLength < maxLength; every other row loses the flag in
+// jc.head, so no solve or warm start evaluates a spring term for it, and gets a zero spring impulse.
 template <int KIND> __device__ __forceinline__ void s2bPrepareSpring(const SolveArgs& a, int t, int slot, bool warmStart)
 {
 	const JointConstraintView& jc = a.jc;
@@ -283,7 +292,8 @@ template <int KIND> __device__ __forceinline__ void s2bPrepareSpring(const Solve
 	float4 motor = a.joints.motor[slot]; // hertz, damping ratio in zw
 	float iA = a.bodies.pos[head.y].z, iB = a.bodies.pos[head.z].z;
 	int type = S2B_JOINT_TYPE(flags);
-	if ((type != S2B_JOINT_REVOLUTE && type != S2B_JOINT_PRISMATIC && type != S2B_JOINT_DISTANCE) || (motor.z > 0.0f) == false ||
+	if ((type != S2B_JOINT_REVOLUTE && type != S2B_JOINT_PRISMATIC && type != S2B_JOINT_DISTANCE && type != S2B_JOINT_WHEEL) ||
+		(motor.z > 0.0f) == false ||
 		(type == S2B_JOINT_REVOLUTE && iA + iB == 0.0f) || (type == S2B_JOINT_DISTANCE && (flags & S2B_JC_SOFT_LINEAR) == 0))
 	{
 		jc.head[t] = make_int4(flags & ~S2B_JOINT_ENABLE_SPRING, head.y, head.z, head.w);
@@ -439,7 +449,8 @@ __device__ __forceinline__ DistanceFrame s2bDistanceFrame(float4 anchor, float4 
 }
 
 // what warm starting adds to each body: v -/+= m * P, w -/+= i * L. Shared by the constraint-by-constraint warm start and
-// the per-body gather (warm_gather.cuh), so both add the same bits. Prismatic and distance rows.
+// the per-body gather (warm_gather.cuh), so both add the same bits. Prismatic, distance and wheel rows; a wheel row's imp.y
+// is its angular motor impulse, which enters L as the prismatic's angular impulse does (DESIGN.md §3.17).
 struct PrismaticWarm
 {
 	s2Vec2 P;
@@ -634,6 +645,85 @@ __device__ __forceinline__ void s2bSolvePrismaticVelocity(const SolveArgs& a, in
 	s2bStoreJointVelocities(a, ia, ib, velA, velB, vA, wA, vB, wB, mA, iA, mB, iB);
 }
 
+// the prismatic's NGS limit correction along its axis, on the given poses (slop s2_linearSlop; equal limits within
+// 2 s2_linearSlop are held both ways). The wheel joint's NGS pass runs it too (DESIGN.md §3.17).
+__device__ __forceinline__ void s2bAxialLimitPosition(float4 anchor, float4 d0, float4 motor, float4 lim, float mA, float iA, float mB,
+													  float iB, s2Vec2& dcA, s2Rot& qA, s2Vec2& dcB, s2Rot& qB)
+{
+	PrismaticFrame f = s2bPrismaticFrame(anchor, d0, motor, dcA, qA, dcB, qB);
+	s2Vec2 dA = s2Add(f.d, f.rA);
+	float a1 = s2Cross(dA, f.axis), a2 = s2Cross(f.rB, f.axis);
+	float translation = s2Dot(f.axis, f.d);
+	float C = 0.0f;
+	if (S2_ABS(lim.z - lim.y) < 2.0f * s2_linearSlop)
+	{
+		C = S2_CLAMP(translation - lim.y, -s2_maxLinearCorrection, s2_maxLinearCorrection);
+	}
+	else if (translation <= lim.y)
+	{
+		C = S2_CLAMP(translation - lim.y + s2_linearSlop, -s2_maxLinearCorrection, 0.0f);
+	}
+	else if (translation >= lim.z)
+	{
+		C = S2_CLAMP(translation - lim.z - s2_linearSlop, 0.0f, s2_maxLinearCorrection);
+	}
+	float k = mA + mB + iA * a1 * a1 + iB * a2 * a2;
+	float impulse = k > 0.0f ? -C / k : 0.0f;
+	s2Vec2 P = s2MulSV(impulse, f.axis);
+	dcA = s2MulSub(dcA, mA, P);
+	qA = s2IntegrateRot(qA, -iA * (impulse * a1));
+	dcB = s2MulAdd(dcB, mB, P);
+	qB = s2IntegrateRot(qB, iB * (impulse * a2));
+}
+
+// XPBD, zero compliance: the perpendicular row, C = perp . d, on the given poses. The prismatic's and the wheel's.
+__device__ __forceinline__ void s2bPerpendicularXpbd(float4 anchor, float4 d0, float4 motor, float mA, float iA, float mB, float iB,
+													 s2Vec2& dcA, s2Rot& qA, s2Vec2& dcB, s2Rot& qB)
+{
+	PrismaticFrame f = s2bPrismaticFrame(anchor, d0, motor, dcA, qA, dcB, qB);
+	s2Vec2 perp = s2LeftPerp(f.axis);
+	float sA = s2Cross(s2Add(f.d, f.rA), perp), sB = s2Cross(f.rB, perp);
+	float k = mA + mB + iA * sA * sA + iB * sB * sB;
+	if (k > 0.0f)
+	{
+		float lambda = -s2Dot(perp, f.d) / k;
+		s2Vec2 P = s2MulSV(lambda, perp);
+		dcA = s2MulSub(dcA, mA, P);
+		qA = s2IntegrateRot(qA, -iA * (lambda * sA));
+		dcB = s2MulAdd(dcB, mB, P);
+		qB = s2IntegrateRot(qB, iB * (lambda * sB));
+	}
+}
+
+// XPBD, zero compliance: a violated translation limit as a position inequality, on the given poses. The prismatic's and
+// the wheel's.
+__device__ __forceinline__ void s2bAxialLimitXpbd(float4 anchor, float4 d0, float4 motor, float4 lim, float mA, float iA, float mB,
+												  float iB, s2Vec2& dcA, s2Rot& qA, s2Vec2& dcB, s2Rot& qB)
+{
+	PrismaticFrame f = s2bPrismaticFrame(anchor, d0, motor, dcA, qA, dcB, qB);
+	float a1 = s2Cross(s2Add(f.d, f.rA), f.axis), a2 = s2Cross(f.rB, f.axis);
+	float translation = s2Dot(f.axis, f.d);
+	float C = 0.0f;
+	if (translation < lim.y)
+	{
+		C = translation - lim.y;
+	}
+	else if (translation > lim.z)
+	{
+		C = translation - lim.z;
+	}
+	float k = mA + mB + iA * a1 * a1 + iB * a2 * a2;
+	if (C != 0.0f && k > 0.0f)
+	{
+		float lambda = -C / k;
+		s2Vec2 P = s2MulSV(lambda, f.axis);
+		dcA = s2MulSub(dcA, mA, P);
+		qA = s2IntegrateRot(qA, -iA * (lambda * a1));
+		dcB = s2MulAdd(dcB, mB, P);
+		qB = s2IntegrateRot(qB, iB * (lambda * a2));
+	}
+}
+
 // NGS position pass: the block on the current poses (corrections clamped), then the limit row on the corrected poses
 __device__ __forceinline__ void s2bSolvePrismaticPosition(const SolveArgs& a, int t)
 {
@@ -680,30 +770,7 @@ __device__ __forceinline__ void s2bSolvePrismaticPosition(const SolveArgs& a, in
 
 	if (head.x & S2B_JOINT_ENABLE_LIMIT)
 	{
-		PrismaticFrame f = s2bPrismaticFrame(anchor, d0, motor, dcA, qA, dcB, qB);
-		s2Vec2 dA = s2Add(f.d, f.rA);
-		float a1 = s2Cross(dA, f.axis), a2 = s2Cross(f.rB, f.axis);
-		float translation = s2Dot(f.axis, f.d);
-		float C = 0.0f;
-		if (S2_ABS(lim.z - lim.y) < 2.0f * s2_linearSlop)
-		{
-			C = S2_CLAMP(translation - lim.y, -s2_maxLinearCorrection, s2_maxLinearCorrection);
-		}
-		else if (translation <= lim.y)
-		{
-			C = S2_CLAMP(translation - lim.y + s2_linearSlop, -s2_maxLinearCorrection, 0.0f);
-		}
-		else if (translation >= lim.z)
-		{
-			C = S2_CLAMP(translation - lim.z - s2_linearSlop, 0.0f, s2_maxLinearCorrection);
-		}
-		float k = mA + mB + iA * a1 * a1 + iB * a2 * a2;
-		float impulse = k > 0.0f ? -C / k : 0.0f;
-		s2Vec2 P = s2MulSV(impulse, f.axis);
-		dcA = s2MulSub(dcA, mA, P);
-		qA = s2IntegrateRot(qA, -iA * (impulse * a1));
-		dcB = s2MulAdd(dcB, mB, P);
-		qB = s2IntegrateRot(qB, iB * (impulse * a2));
+		s2bAxialLimitPosition(anchor, d0, motor, lim, mA, iA, mB, iB, dcA, qA, dcB, qB);
 	}
 
 	if ((mA != 0.0f) || (iA != 0.0f))
@@ -741,46 +808,11 @@ __device__ __forceinline__ void s2bSolvePrismaticXpbd(const SolveArgs& a, int t)
 		qB = s2IntegrateRot(qB, iB * p);
 	}
 
-	{
-		PrismaticFrame f = s2bPrismaticFrame(anchor, d0, motor, dcA, qA, dcB, qB);
-		s2Vec2 perp = s2LeftPerp(f.axis);
-		float sA = s2Cross(s2Add(f.d, f.rA), perp), sB = s2Cross(f.rB, perp);
-		float k = mA + mB + iA * sA * sA + iB * sB * sB;
-		if (k > 0.0f)
-		{
-			float lambda = -s2Dot(perp, f.d) / k;
-			s2Vec2 P = s2MulSV(lambda, perp);
-			dcA = s2MulSub(dcA, mA, P);
-			qA = s2IntegrateRot(qA, -iA * (lambda * sA));
-			dcB = s2MulAdd(dcB, mB, P);
-			qB = s2IntegrateRot(qB, iB * (lambda * sB));
-		}
-	}
+	s2bPerpendicularXpbd(anchor, d0, motor, mA, iA, mB, iB, dcA, qA, dcB, qB);
 
 	if (head.x & S2B_JOINT_ENABLE_LIMIT)
 	{
-		PrismaticFrame f = s2bPrismaticFrame(anchor, d0, motor, dcA, qA, dcB, qB);
-		float a1 = s2Cross(s2Add(f.d, f.rA), f.axis), a2 = s2Cross(f.rB, f.axis);
-		float translation = s2Dot(f.axis, f.d);
-		float C = 0.0f;
-		if (translation < lim.y)
-		{
-			C = translation - lim.y;
-		}
-		else if (translation > lim.z)
-		{
-			C = translation - lim.z;
-		}
-		float k = mA + mB + iA * a1 * a1 + iB * a2 * a2;
-		if (C != 0.0f && k > 0.0f)
-		{
-			float lambda = -C / k;
-			s2Vec2 P = s2MulSV(lambda, f.axis);
-			dcA = s2MulSub(dcA, mA, P);
-			qA = s2IntegrateRot(qA, -iA * (lambda * a1));
-			dcB = s2MulAdd(dcB, mB, P);
-			qB = s2IntegrateRot(qB, iB * (lambda * a2));
-		}
+		s2bAxialLimitXpbd(anchor, d0, motor, lim, mA, iA, mB, iB, dcA, qA, dcB, qB);
 	}
 
 	if ((mA != 0.0f) || (iA != 0.0f))
@@ -956,6 +988,159 @@ __device__ __forceinline__ void s2bSolveDistanceXpbd(const SolveArgs& a, int t)
 }
 
 // ---------------------------------------------------------------------------------------------------------------
+// wheel joint (extension, DESIGN.md §3.17; definition: tests/wheel_oracle.c). Body B's anchor slides along an axis fixed in
+// body A and B turns freely: rows spring (s2bSolveSpringVelocity, ahead of these), the motor on the relative rotation (the
+// revolute's form, axial mass 1 / (iA + iB) in jc.d0ax.z), lower and upper translation limit (s2bSolveAxialRows with the
+// motor flag masked off) and the perpendicular point-on-line row. The frame is the prismatic's. Row columns: lim =
+// (unused, lowerTranslation, upperTranslation), motor = (maxMotorTorque, motorSpeed, localAxisA.xy), imp = (perpendicular,
+// angular motor, 0, spring), limp = (lower, upper).
+// ---------------------------------------------------------------------------------------------------------------
+template <int KIND>
+__device__ __forceinline__ void s2bSolveWheelVelocity(const SolveArgs& a, int t, float h, float inv_h, bool useBias)
+{
+	const JointConstraintView& jc = a.jc;
+	int4 head = jc.head[t];
+	int ia = head.y, ib = head.z;
+	float4 mass = jc.mass[t];
+	float4 d0 = jc.d0ax[t];
+	float4 lim = jc.lim[t];
+	float4 motor = jc.motor[t];
+	float4 coef = jc.coef[t];
+	float4 imp = jc.imp[t];
+	float4 limp = jc.limp[t];
+	float4 velA = a.bodies.vel[ia], velB = a.bodies.vel[ib];
+	float4 poseA = a.bodies.pose[ia], poseB = a.bodies.pose[ib];
+	s2Vec2 vA = V2(velA.x, velA.y), vB = V2(velB.x, velB.y);
+	float wA = velA.z, wB = velB.z;
+	float mA = mass.x, iA = mass.y, mB = mass.z, iB = mass.w;
+	PrismaticFrame f = s2bPrismaticFrame(jc.anchor[t], d0, motor, V2(poseA.x, poseA.y), R2(poseA.z, poseA.w), V2(poseB.x, poseB.y),
+										 R2(poseB.z, poseB.w));
+	s2Vec2 axis = f.axis;
+	s2Vec2 dA = s2Add(f.d, f.rA);
+	float translation = s2Dot(axis, f.d);
+	float a1 = s2Cross(dA, axis), a2 = s2Cross(f.rB, axis);
+	float k = mA + mB + iA * a1 * a1 + iB * a2 * a2;
+	float axialMass = k > 0.0f ? 1.0f / k : 0.0f;
+
+	if ((head.x & S2B_JOINT_ENABLE_MOTOR) && d0.z > 0.0f)
+	{
+		float Cdot = wB - wA - motor.y;
+		float impulse = -d0.z * Cdot;
+		float oldImpulse = imp.y;
+		float maxImpulse = h * motor.x;
+		imp.y = S2_CLAMP(oldImpulse + impulse, -maxImpulse, maxImpulse);
+		impulse = imp.y - oldImpulse;
+		wA -= iA * impulse;
+		wB += iB * impulse;
+	}
+
+	s2bSolveAxialRows<KIND>(head.x & ~S2B_JOINT_ENABLE_MOTOR, axis, a1, a2, axialMass, translation, lim, motor, coef, h, inv_h,
+							useBias, mA, iA, mB, iB, imp, limp, vA, wA, vB, wB);
+
+	// the point-on-line row: C = perp . d
+	{
+		s2Vec2 perp = s2LeftPerp(axis);
+		float sA = s2Cross(dA, perp), sB = s2Cross(f.rB, perp);
+		float3 s = s2bPrismaticBias<KIND>(s2Dot(perp, f.d), false, coef, h, inv_h, useBias);
+		float Cdot = s2Dot(perp, s2Sub(vB, vA)) + sB * wB - sA * wA;
+		float kp = mA + mB + iA * sA * sA + iB * sB * sB;
+		float perpMass = kp > 0.0f ? 1.0f / kp : 0.0f;
+		float impulse = -perpMass * s.y * (Cdot + s.x) - s.z * imp.x;
+		imp.x += impulse;
+		s2Vec2 P = s2MulSV(impulse, perp);
+		vA = s2MulSub(vA, mA, P);
+		wA -= iA * (impulse * sA);
+		vB = s2MulAdd(vB, mB, P);
+		wB += iB * (impulse * sB);
+	}
+
+	jc.imp[t] = imp;
+	jc.limp[t] = limp;
+	s2bStoreJointVelocities(a, ia, ib, velA, velB, vA, wA, vB, wB, mA, iA, mB, iB);
+}
+
+// NGS position pass: the perpendicular row on the current poses (C clamped to +/- s2_maxLinearCorrection, impulse -C / k),
+// then the prismatic's limit correction on the corrected poses. The spring and the motor do nothing.
+__device__ __forceinline__ void s2bSolveWheelPosition(const SolveArgs& a, int t)
+{
+	const JointConstraintView& jc = a.jc;
+	int4 head = jc.head[t];
+	int ia = head.y, ib = head.z;
+	float4 anchor = jc.anchor[t];
+	float4 mass = jc.mass[t];
+	float4 d0 = jc.d0ax[t];
+	float4 lim = jc.lim[t];
+	float4 motor = jc.motor[t];
+	float4 poseA = a.bodies.pose[ia], poseB = a.bodies.pose[ib];
+	s2Vec2 dcA = V2(poseA.x, poseA.y), dcB = V2(poseB.x, poseB.y);
+	s2Rot qA = R2(poseA.z, poseA.w), qB = R2(poseB.z, poseB.w);
+	float mA = mass.x, iA = mass.y, mB = mass.z, iB = mass.w;
+
+	{
+		PrismaticFrame f = s2bPrismaticFrame(anchor, d0, motor, dcA, qA, dcB, qB);
+		s2Vec2 perp = s2LeftPerp(f.axis);
+		s2Vec2 dA = s2Add(f.d, f.rA);
+		float sA = s2Cross(dA, perp), sB = s2Cross(f.rB, perp);
+		float C = S2_CLAMP(s2Dot(perp, f.d), -s2_maxLinearCorrection, s2_maxLinearCorrection);
+		float k = mA + mB + iA * sA * sA + iB * sB * sB;
+		float impulse = k > 0.0f ? -C / k : 0.0f;
+		s2Vec2 P = s2MulSV(impulse, perp);
+		dcA = s2MulSub(dcA, mA, P);
+		qA = s2IntegrateRot(qA, -iA * (impulse * sA));
+		dcB = s2MulAdd(dcB, mB, P);
+		qB = s2IntegrateRot(qB, iB * (impulse * sB));
+	}
+
+	if (head.x & S2B_JOINT_ENABLE_LIMIT)
+	{
+		s2bAxialLimitPosition(anchor, d0, motor, lim, mA, iA, mB, iB, dcA, qA, dcB, qB);
+	}
+
+	if ((mA != 0.0f) || (iA != 0.0f))
+	{
+		a.bodies.pose[ia] = make_float4(dcA.x, dcA.y, qA.s, qA.c);
+	}
+	if ((mB != 0.0f) || (iB != 0.0f))
+	{
+		a.bodies.pose[ib] = make_float4(dcB.x, dcB.y, qB.s, qB.c);
+	}
+}
+
+// XPBD, zero compliance: the perpendicular row, then a violated limit. The spring (s2bSolveSpringXpbd) runs ahead; the
+// motor is not applied, as no joint's XPBD form applies its motor.
+__device__ __forceinline__ void s2bSolveWheelXpbd(const SolveArgs& a, int t)
+{
+	const JointConstraintView& jc = a.jc;
+	int4 head = jc.head[t];
+	int ia = head.y, ib = head.z;
+	float4 anchor = jc.anchor[t];
+	float4 mass = jc.mass[t];
+	float4 d0 = jc.d0ax[t];
+	float4 lim = jc.lim[t];
+	float4 motor = jc.motor[t];
+	float4 poseA = a.bodies.pose[ia], poseB = a.bodies.pose[ib];
+	s2Vec2 dcA = V2(poseA.x, poseA.y), dcB = V2(poseB.x, poseB.y);
+	s2Rot qA = R2(poseA.z, poseA.w), qB = R2(poseB.z, poseB.w);
+	float mA = mass.x, iA = mass.y, mB = mass.z, iB = mass.w;
+
+	s2bPerpendicularXpbd(anchor, d0, motor, mA, iA, mB, iB, dcA, qA, dcB, qB);
+
+	if (head.x & S2B_JOINT_ENABLE_LIMIT)
+	{
+		s2bAxialLimitXpbd(anchor, d0, motor, lim, mA, iA, mB, iB, dcA, qA, dcB, qB);
+	}
+
+	if ((mA != 0.0f) || (iA != 0.0f))
+	{
+		a.bodies.pose[ia] = make_float4(dcA.x, dcA.y, qA.s, qA.c);
+	}
+	if ((mB != 0.0f) || (iB != 0.0f))
+	{
+		a.bodies.pose[ib] = make_float4(dcB.x, dcB.y, qB.s, qB.c);
+	}
+}
+
+// ---------------------------------------------------------------------------------------------------------------
 // motor joint (extension, DESIGN.md §3.10; definition: tests/motor_oracle.c). Drives body B toward a pose relative to body
 // A with capped effort: an angular row toward angle(B) - angle(A) = angularOffset, its accumulated impulse clamped to
 // +/- h maxTorque, then a point row that takes B's origin to the linear offset in A's frame, its accumulated impulse scaled
@@ -1118,8 +1303,8 @@ __device__ __forceinline__ void s2bSolveSpringVelocity(const SolveArgs& a, int t
 	}
 	else
 	{
-		// prismatic: C = the translation, k = the axial mass §3.9 forms in every solve; distance (§3.16): C = length - rest
-		// length along the current line
+		// prismatic and wheel (§3.17): C = the translation, k = the axial mass §3.9 forms in every solve; distance (§3.16):
+		// C = length - rest length along the current line
 		s2Vec2 axis;
 		float a1, a2, C;
 		if (S2B_JOINT_TYPE(head.x) == S2B_JOINT_DISTANCE)
@@ -1274,7 +1459,8 @@ __device__ __forceinline__ void s2bWarmStartJoint(const SolveArgs& a, int t)
 		return;
 	}
 
-	if (S2B_JOINT_TYPE(head.x) == S2B_JOINT_PRISMATIC || S2B_JOINT_TYPE(head.x) == S2B_JOINT_DISTANCE)
+	if (S2B_JOINT_TYPE(head.x) == S2B_JOINT_PRISMATIC || S2B_JOINT_TYPE(head.x) == S2B_JOINT_DISTANCE ||
+		S2B_JOINT_TYPE(head.x) == S2B_JOINT_WHEEL)
 	{
 		float4 velA = a.bodies.vel[ia], velB = a.bodies.vel[ib];
 		float mA = mass.x, iA = mass.y, mB = mass.z, iB = mass.w;
@@ -1929,6 +2115,11 @@ __device__ __forceinline__ void s2bSolveJointSoft(const SolveArgs& a, int t, flo
 		s2bSolveDistanceVelocity<PSOLVE_SOFT>(a, t, h, inv_h, useBias);
 		return;
 	}
+	if (S2B_JOINT_TYPE(flags) == S2B_JOINT_WHEEL)
+	{
+		s2bSolveWheelVelocity<PSOLVE_SOFT>(a, t, h, inv_h, useBias);
+		return;
+	}
 	if (SHARED_MOTOR == false && S2B_JOINT_TYPE(flags) == S2B_JOINT_MOTOR)
 	{
 		s2bSolveMotorVelocity(a, t, h, inv_h);
@@ -1959,6 +2150,11 @@ __device__ __forceinline__ void s2bSolveJointBaumgarte(const SolveArgs& a, int t
 	if (S2B_JOINT_TYPE(flags) == S2B_JOINT_DISTANCE)
 	{
 		s2bSolveDistanceVelocity<PSOLVE_BAUMGARTE>(a, t, h, inv_h, useBias);
+		return;
+	}
+	if (S2B_JOINT_TYPE(flags) == S2B_JOINT_WHEEL)
+	{
+		s2bSolveWheelVelocity<PSOLVE_BAUMGARTE>(a, t, h, inv_h, useBias);
 		return;
 	}
 	if (S2B_JOINT_TYPE(flags) == S2B_JOINT_MOTOR)
@@ -2088,6 +2284,11 @@ __device__ __forceinline__ void s2bSolveJointRigid(const SolveArgs& a, int t, fl
 		s2bSolveDistanceVelocity<PSOLVE_RIGID>(a, t, h, 0.0f /* inv_h: unused by the rigid rows */, false);
 		return;
 	}
+	if (S2B_JOINT_TYPE(a.jc.head[t].x) == S2B_JOINT_WHEEL)
+	{
+		s2bSolveWheelVelocity<PSOLVE_RIGID>(a, t, h, 0.0f /* inv_h: unused by the rigid rows */, false);
+		return;
+	}
 	if (S2B_JOINT_TYPE(a.jc.head[t].x) == S2B_JOINT_MOTOR)
 	{
 		s2bSolveMotorVelocity(a, t, h, a.ctx.inv_h);
@@ -2121,6 +2322,11 @@ __device__ __forceinline__ void s2bSolveJointPosition(const SolveArgs& a, int t)
 	if (S2B_JOINT_TYPE(head.x) == S2B_JOINT_DISTANCE)
 	{
 		s2bSolveDistancePosition(a, t);
+		return;
+	}
+	if (S2B_JOINT_TYPE(head.x) == S2B_JOINT_WHEEL)
+	{
+		s2bSolveWheelPosition(a, t);
 		return;
 	}
 	if (head.x & S2B_JC_SOFT_WELD)
@@ -2220,6 +2426,11 @@ __device__ __forceinline__ void s2bSolveJointXpbd(const SolveArgs& a, int t)
 	if (S2B_JOINT_TYPE(head.x) == S2B_JOINT_DISTANCE)
 	{
 		s2bSolveDistanceXpbd(a, t);
+		return;
+	}
+	if (S2B_JOINT_TYPE(head.x) == S2B_JOINT_WHEEL)
+	{
+		s2bSolveWheelXpbd(a, t);
 		return;
 	}
 	if (S2B_JOINT_TYPE(head.x) == S2B_JOINT_MOTOR)

@@ -82,9 +82,10 @@ __device__ __forceinline__ GatherTerms s2bGatherTermsOf(const SolveArgs& a, int 
 			g.tv0 = s2MulSV(invMass, P);
 			g.tw0 = invI * (s2Cross(rB, P) + imp.z);
 		}
-		else if (S2B_JOINT_TYPE(head.x) == S2B_JOINT_PRISMATIC || S2B_JOINT_TYPE(head.x) == S2B_JOINT_DISTANCE)
+		else if (S2B_JOINT_TYPE(head.x) == S2B_JOINT_PRISMATIC || S2B_JOINT_TYPE(head.x) == S2B_JOINT_DISTANCE ||
+				 S2B_JOINT_TYPE(head.x) == S2B_JOINT_WHEEL)
 		{
-			// P and L depend on both poses (DESIGN.md §3.9, §3.16); poses are not written during the gather
+			// P and L depend on both poses (DESIGN.md §3.9, §3.16, §3.17); poses are not written during the gather
 			PrismaticWarm pw = s2bPrismaticWarmTerms(a, t);
 			s2Vec2 mp = s2MulSV(invMass, pw.P);
 			g.tv0 = sideB ? mp : V2(-mp.x, -mp.y);

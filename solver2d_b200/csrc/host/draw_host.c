@@ -105,10 +105,10 @@ static void s2DrawJoint(s2DebugDraw* draw, s2World* world, const s2Joint* joint)
 		return;
 	}
 
-	if (joint->type == s2_prismaticJoint)
+	if (joint->type == s2_prismaticJoint || joint->type == s2_wheelJoint)
 	{
 		// the axis through anchor A (drawSize each way), a mark across the axis at each translation limit, and the
-		// segment from anchor A to anchor B
+		// segment from anchor A to anchor B; the same for a wheel joint
 		const float L = joint->drawSize;
 		s2Vec2 axis = s2RotateVector(bodyA->rot, joint->localAxisA);
 		s2Vec2 perp = s2MulSV(0.5f * L, s2LeftPerp(axis));

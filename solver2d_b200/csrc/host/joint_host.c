@@ -181,7 +181,7 @@ float s2RevoluteJoint_GetMotorTorque(s2JointId jointId, float inverseTimeStep)
 	return inverseTimeStep * world->joints[jointId.index].motorImpulse;
 }
 
-// ---- joint springs (DESIGN.md §3.14): revolute, prismatic and distance joints; hertz and dampingRatio carry the spring ----
+// ---- joint springs (DESIGN.md §3.14): revolute, prismatic, distance and wheel joints; hertz and dampingRatio carry the spring
 
 static void s2EnableJointSpring(s2JointId jointId, s2JointType type, bool enableSpring)
 {
@@ -189,7 +189,7 @@ static void s2EnableJointSpring(s2JointId jointId, s2JointType type, bool enable
 	s2Joint* joint = s2GetJointForEdit(jointId, &world);
 	if (joint->type != type)
 	{
-		return; // only revolute, prismatic and distance joints have a spring
+		return; // only revolute, prismatic, distance and wheel joints have a spring
 	}
 	joint->enableSpring = enableSpring;
 	s2MarkJointDirty(world, joint);
@@ -205,7 +205,7 @@ static void s2SetJointSpringValue(s2JointId jointId, s2JointType type, float val
 	s2Joint* joint = s2GetJointForEdit(jointId, &world);
 	if (joint->type != type)
 	{
-		return; // only revolute, prismatic and distance joints have a spring
+		return; // only revolute, prismatic, distance and wheel joints have a spring
 	}
 	if (dampingRatio)
 	{
@@ -764,12 +764,162 @@ float s2DistanceJoint_GetCurrentLength(s2JointId jointId)
 	return length;
 }
 
+// ---- wheel joint (DESIGN.md §3.17) ---------------------------------------------------------------------------------------
+
+// The wheel joint has no counterpart in the reference. Invalid input creates nothing and returns s2_nullJointId.
+s2JointId s2CreateWheelJoint(s2WorldId worldId, const s2WheelJointDef* def)
+{
+	s2Vec2 axis = def->localAxisA;
+	float length = s2Length(axis);
+	if (s2IsValidVec2(def->localAnchorA) == false || s2IsValidVec2(def->localAnchorB) == false || s2IsValidVec2(axis) == false ||
+		s2IsValid(length) == false || length == 0.0f || s2IsValid(def->lowerTranslation) == false ||
+		s2IsValid(def->upperTranslation) == false || (def->lowerTranslation <= def->upperTranslation) == false ||
+		s2IsValidSpringValue(def->hertz) == false || s2IsValidSpringValue(def->dampingRatio) == false ||
+		s2IsValidSpringValue(def->maxMotorTorque) == false || s2IsValid(def->motorSpeed) == false)
+	{
+		return s2_nullJointId;
+	}
+
+	s2World* world = s2GetWorldFromId(worldId);
+	s2Body* bodyA = world->bodies + def->bodyIdA.index;
+	s2Body* bodyB = world->bodies + def->bodyIdB.index;
+
+	s2Joint* joint = s2AllocJoint(world, bodyA, bodyB);
+	joint->type = s2_wheelJoint;
+	joint->drawSize = 1.0f;
+	joint->localOriginAnchorA = def->localAnchorA;
+	joint->localOriginAnchorB = def->localAnchorB;
+	joint->localAxisA = s2MakeVec2(axis.x / length, axis.y / length);
+	joint->lowerAngle = def->lowerTranslation;
+	joint->upperAngle = def->upperTranslation;
+	joint->maxMotorTorque = def->maxMotorTorque;
+	joint->motorSpeed = def->motorSpeed;
+	joint->enableLimit = def->enableLimit;
+	joint->enableMotor = def->enableMotor;
+	joint->enableSpring = def->enableSpring;
+	joint->hertz = def->hertz;
+	joint->dampingRatio = def->dampingRatio;
+	joint->collideConnected = def->collideConnected;
+
+	s2JointId jointId = {joint->object.index, world->index, joint->object.revision};
+	return jointId;
+}
+
+// the joint to edit, or NULL for a joint of another type
+static s2Joint* s2GetWheelJointForEdit(s2JointId jointId, s2World** worldOut)
+{
+	s2Joint* joint = s2GetJointForEdit(jointId, worldOut);
+	return joint->type == s2_wheelJoint ? joint : NULL;
+}
+
+void s2WheelJoint_EnableSpring(s2JointId jointId, bool enableSpring)
+{
+	s2EnableJointSpring(jointId, s2_wheelJoint, enableSpring);
+}
+
+void s2WheelJoint_SetSpringHertz(s2JointId jointId, float hertz)
+{
+	s2SetJointSpringValue(jointId, s2_wheelJoint, hertz, false);
+}
+
+void s2WheelJoint_SetSpringDampingRatio(s2JointId jointId, float dampingRatio)
+{
+	s2SetJointSpringValue(jointId, s2_wheelJoint, dampingRatio, true);
+}
+
+void s2WheelJoint_EnableLimit(s2JointId jointId, bool enableLimit)
+{
+	s2World* world;
+	s2Joint* joint = s2GetWheelJointForEdit(jointId, &world);
+	if (joint != NULL)
+	{
+		joint->enableLimit = enableLimit;
+		s2MarkJointDirty(world, joint);
+	}
+}
+
+void s2WheelJoint_SetLimits(s2JointId jointId, float lower, float upper)
+{
+	if (s2IsValid(lower) == false || s2IsValid(upper) == false || (lower <= upper) == false)
+	{
+		return;
+	}
+	s2World* world;
+	s2Joint* joint = s2GetWheelJointForEdit(jointId, &world);
+	if (joint != NULL)
+	{
+		joint->lowerAngle = lower;
+		joint->upperAngle = upper;
+		s2MarkJointDirty(world, joint);
+	}
+}
+
+void s2WheelJoint_EnableMotor(s2JointId jointId, bool enableMotor)
+{
+	s2World* world;
+	s2Joint* joint = s2GetWheelJointForEdit(jointId, &world);
+	if (joint != NULL)
+	{
+		joint->enableMotor = enableMotor;
+		s2MarkJointDirty(world, joint);
+	}
+}
+
+void s2WheelJoint_SetMotorSpeed(s2JointId jointId, float motorSpeed)
+{
+	if (s2IsValid(motorSpeed) == false)
+	{
+		return;
+	}
+	s2World* world;
+	s2Joint* joint = s2GetWheelJointForEdit(jointId, &world);
+	if (joint != NULL)
+	{
+		joint->motorSpeed = motorSpeed;
+		s2MarkJointDirty(world, joint);
+	}
+}
+
+void s2WheelJoint_SetMaxMotorTorque(s2JointId jointId, float maxMotorTorque)
+{
+	if (s2IsValidSpringValue(maxMotorTorque) == false)
+	{
+		return;
+	}
+	s2World* world;
+	s2Joint* joint = s2GetWheelJointForEdit(jointId, &world);
+	if (joint != NULL)
+	{
+		joint->maxMotorTorque = maxMotorTorque;
+		s2MarkJointDirty(world, joint);
+	}
+}
+
+float s2WheelJoint_GetMotorTorque(s2JointId jointId, float inverseTimeStep)
+{
+	s2World* world = s2GetWorldFromIndex(jointId.world);
+	s2SyncStateToHost(world);
+	const s2Joint* joint = world->joints + jointId.index;
+	S2_ASSERT(s2ObjectValid(&joint->object) && joint->object.revision == jointId.revision);
+	// the angular motor's impulse rides in impulse.y (the row's impulse[1])
+	return joint->type == s2_wheelJoint ? inverseTimeStep * joint->impulse.y : 0.0f;
+}
+
+float s2WheelJoint_GetTranslation(s2JointId jointId)
+{
+	s2World* world = s2GetWorldFromIndex(jointId.world);
+	const s2Joint* joint = world->joints + jointId.index;
+	S2_ASSERT(s2ObjectValid(&joint->object) && joint->object.revision == jointId.revision);
+	return joint->type == s2_wheelJoint ? s2PrismaticJoint_GetTranslation(jointId) : 0.0f;
+}
+
 // ---- reactions and break thresholds (DESIGN.md §3.13) -----------------------------------------------------------------
 
 // s2JointType and the device's S2B_JOINT_* number the joint types alike
 _Static_assert((int)s2_revoluteJoint == S2B_JOINT_REVOLUTE && (int)s2_mouseJoint == S2B_JOINT_MOUSE &&
 				   (int)s2_weldJoint == S2B_JOINT_WELD && (int)s2_prismaticJoint == S2B_JOINT_PRISMATIC &&
-				   (int)s2_motorJoint == S2B_JOINT_MOTOR && (int)s2_distanceJoint == S2B_JOINT_DISTANCE,
+				   (int)s2_motorJoint == S2B_JOINT_MOTOR && (int)s2_distanceJoint == S2B_JOINT_DISTANCE &&
+				   (int)s2_wheelJoint == S2B_JOINT_WHEEL,
 			   "joint type numbering");
 
 s2JointReaction s2ComputeJointReaction(int32_t type, s2Vec2 impulse, float motorImpulse, float lowerImpulse, float upperImpulse,

@@ -89,6 +89,7 @@ typedef enum s2JointType
 	s2_prismaticJoint,
 	s2_motorJoint,
 	s2_distanceJoint,
+	s2_wheelJoint,
 } s2JointType;
 
 typedef struct s2Body
@@ -165,11 +166,13 @@ typedef struct s2Joint
 
 	// revolute; a prismatic joint keeps its translation limits in lowerAngle / upperAngle and its maximum motor force in
 	// maxMotorTorque, as its device row does. A distance joint keeps its rest length in referenceAngle, its min / max length
-	// in lowerAngle / upperAngle, its maximum motor force in maxMotorTorque and its spring in hertz / dampingRatio.
+	// in lowerAngle / upperAngle, its maximum motor force in maxMotorTorque and its spring in hertz / dampingRatio. A wheel
+	// joint keeps its translation limits in lowerAngle / upperAngle, its maximum motor torque in maxMotorTorque, its axis in
+	// localAxisA and its spring in hertz / dampingRatio; impulse.y is its angular motor impulse and motorImpulse stays 0.
 	bool enableMotor, enableLimit;
 	float maxMotorTorque, motorSpeed;
 	float referenceAngle, lowerAngle, upperAngle;
-	// prismatic
+	// prismatic, wheel
 	s2Vec2 localAxisA;
 	// mouse; a motor joint keeps its maximum force in hertz and its correction factor in dampingRatio, its linear offset
 	// in localOriginAnchorA (localOriginAnchorB is zero), its angular offset in referenceAngle and its maximum torque in

@@ -244,13 +244,16 @@ static void s2FillJointRow(s2bJointRow* r, const s2Joint* j)
 		case s2_distanceJoint:
 			type = S2B_JOINT_DISTANCE;
 			break;
+		case s2_wheelJoint:
+			type = S2B_JOINT_WHEEL;
+			break;
 	}
 	r->flags = S2B_ROW_VALID | (type << 1);
 	// welds and motor joints are created with enableLimit == enableMotor == false, so their rows never carry either flag
 	r->flags |= j->enableLimit ? S2B_JOINT_ENABLE_LIMIT : 0;
 	r->flags |= j->enableMotor ? S2B_JOINT_ENABLE_MOTOR : 0;
 	r->flags |= j->collideConnected ? S2B_JOINT_COLLIDE_CONNECTED : 0;
-	// only revolute, prismatic and distance joints have a spring setter, so no other row carries the flag
+	// only revolute, prismatic, distance and wheel joints have a spring setter, so no other row carries the flag
 	r->flags |= j->enableSpring ? S2B_JOINT_ENABLE_SPRING : 0;
 	r->bodyA = j->bodyIndexA;
 	r->bodyB = j->bodyIndexB;

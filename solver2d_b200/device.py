@@ -77,8 +77,9 @@ JOINT_ENABLE_LIMIT, JOINT_ENABLE_MOTOR, JOINT_COLLIDE_CONNECTED, JOINT_ENABLE_SP
 # joint types, stored in flags bits 1-3 (a weld keeps its angular impulse in the motorImpulse column; a prismatic row keeps
 # its translation limits in lowerAngle / upperAngle and its maximum motor force in maxMotorTorque; a motor row keeps its
 # linear offset in localOriginAnchorA, its angular offset in referenceAngle, its maximum torque in maxMotorTorque, its
-# maximum force in hertz and its correction factor in dampingRatio)
-JOINT_REVOLUTE, JOINT_MOUSE, JOINT_WELD, JOINT_PRISMATIC, JOINT_MOTOR, JOINT_DISTANCE = 0, 1, 2, 3, 4, 5
+# maximum force in hertz and its correction factor in dampingRatio; a wheel row keeps its translation limits in lowerAngle /
+# upperAngle, its maximum motor torque in maxMotorTorque and its angular motor impulse in impulse[1])
+JOINT_REVOLUTE, JOINT_MOUSE, JOINT_WELD, JOINT_PRISMATIC, JOINT_MOTOR, JOINT_DISTANCE, JOINT_WHEEL = 0, 1, 2, 3, 4, 5, 6
 
 # symbols declared in include/s2b_device.h (checked by the CPU test-suite against the built library)
 ABI_SYMBOLS = [

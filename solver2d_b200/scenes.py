@@ -19,6 +19,8 @@ Each recipe restates one of the reference's sample scenes or one of the syntheti
                             joint on a slider (the prismatic joint).
 * :func:`distance_joints` — ropes of boxes, rigid-rod pendulums, a spring ring of circles over a pile, winches, a tether
                             to a kinematic platform, a revolute chain and a mouse joint (the distance joint).
+* :func:`wheels`          — a motorised car over bumps, a car rolling down a slope, a barrow on a rigid axle, a trolley
+                            hanging from a kinematic rail and a mouse joint (the wheel joint).
 * :func:`motors`          — top-down friction, a driven platform with a pile, a weak motor under its load, a dynamic
                             pair, a rider on a kinematic carriage, a drive across the angle seam and a mouse joint
                             (the motor joint).
@@ -1268,6 +1270,119 @@ def distance_joints(lib: capi.Solver2D, solver="TGS_Soft", copies=1, kinematic=T
             md.bodyIdA = gid
             md.bodyIdB = dragged
             md.target = Vec2(x0 + 33.5, 1.5)
+            md.hertz = 3.0
+            md.dampingRatio = 0.7
+            sc.joints.append(lib.s2CreateMouseJoint(world, C.byref(md)))
+    return sc
+
+
+WHEELS_PITCH = 40.0  # width of one copy of wheels (m)
+
+
+def wheels(lib: capi.Solver2D, solver="TGS_Soft", copies=1, kinematic=True, stand_ins=None) -> Scene:
+    """Wheel joint coverage (DESIGN.md §3.17), `copies` side by side (about 20 bodies each). Per copy:
+
+    * a car driving over bumps: a chassis on two wheel joints (axis up, spring 4 Hz, damping ratio 0.7, limits +/- 0.25 m),
+      the rear one motorised (-8 rad/s, 12 N-m); the car's parts share a negative collision group, so only the wheels and
+      the chassis touch the world;
+    * a car without a motor rolling down a slope (spring 3 Hz, 0.5, limits +/- 0.2 m);
+    * a barrow: a plank on one wheel with equal limits (a rigid axle), its other end on the ground;
+    * with `kinematic`: a trolley hanging from a kinematic rail that moves sideways, on a wheel joint along the rail
+      (spring 1 Hz, 0.3, limits +/- 1.5 m), free to swing about its anchor;
+    * a box pulled by a mouse joint (first copy only).
+
+    On a library without s2CreateWheelJoint (the reference), or with `stand_ins` true, every wheel joint is created as a
+    revolute joint at the wheel's anchor that carries the same motor. ``sc.piles["wheel"]`` lists the index into
+    ``sc.joints`` of every wheel joint and ``sc.piles["wheel_defs"]`` its definition (anchors relative to the body origins),
+    so that a test can turn the stand-in rows into wheel rows."""
+    world = lib.create_world(solver)
+    sc = Scene(lib, world, name=f"wheels{copies}")
+    sc.piles["wheel"] = []
+    sc.piles["wheel_defs"] = []
+    real = "s2CreateWheelJoint" not in lib.missing and not stand_ins
+    gid = _ground(lib, world, 0.5 * WHEELS_PITCH * copies + 5.0)
+    sc.bodies.append(gid)
+
+    def body(kind, x, y, angle=0.0, hx=0.5, hy=0.125, vx=0.0, radius=None, group=0):
+        bd = default_body_def()
+        bd.type = kind
+        bd.position = Vec2(x, y)
+        bd.angle = angle
+        bd.linearVelocity = Vec2(vx, 0.0)
+        bid = lib.s2CreateBody(world, C.byref(bd))
+        sd = default_shape_def()
+        sd.filter.groupIndex = group
+        if radius is not None:
+            lib.s2CreateCircleShape(bid, C.byref(sd), C.byref(Circle(Vec2(0.0, 0.0), radius)))
+        else:
+            lib.s2CreatePolygonShape(bid, C.byref(sd), C.byref(lib.s2MakeBox(hx, hy)))
+        sc.bodies.append(bid)
+        return bid
+
+    def wheel(a, b, pivot, axis, spring=None, limit=None, motor=None):
+        """pivot: the anchors' world point at creation."""
+        d = dict(localAnchorA=tuple(lib.s2Body_GetLocalPoint(a, pivot)), localAnchorB=tuple(lib.s2Body_GetLocalPoint(b, pivot)),
+                 localAxisA=axis, enableSpring=spring is not None, hertz=spring[0] if spring else 0.0,
+                 dampingRatio=spring[1] if spring else 0.0, enableLimit=limit is not None,
+                 lowerTranslation=limit[0] if limit else 0.0, upperTranslation=limit[1] if limit else 0.0,
+                 enableMotor=motor is not None, motorSpeed=motor[0] if motor else 0.0, maxMotorTorque=motor[1] if motor else 0.0)
+        if real:
+            jd = capi.default_wheel_def()
+            for name, value in d.items():
+                setattr(jd, name, Vec2(*value) if isinstance(value, tuple) else value)
+            create = lib.s2CreateWheelJoint
+        else:
+            jd = default_revolute_def()
+            jd.localAnchorA = Vec2(*d["localAnchorA"])
+            jd.localAnchorB = Vec2(*d["localAnchorB"])
+            jd.enableMotor = d["enableMotor"]
+            jd.motorSpeed, jd.maxMotorTorque = d["motorSpeed"], d["maxMotorTorque"]
+            create = lib.s2CreateRevoluteJoint
+        jd.bodyIdA = a
+        jd.bodyIdB = b
+        sc.piles["wheel"].append(len(sc.joints))
+        sc.piles["wheel_defs"].append(d)
+        jid = create(world, C.byref(jd))
+        sc.joints.append(jid)
+        return jid
+
+    D, S, K = capi.DYNAMIC_BODY, capi.STATIC_BODY, capi.KINEMATIC_BODY
+    up = (0.0, 1.0)
+    for k in range(copies):
+        x0 = -0.5 * WHEELS_PITCH * (copies - 1) + WHEELS_PITCH * k - 18.0
+        group = -(k + 1)
+        # bumps on the ground, then a car with a rear motor driving over them
+        for i in range(4):
+            body(S, x0 + 4.0 + 2.5 * i, 0.05, hx=0.4, hy=0.05 + 0.05 * (i % 2))
+        chassis = body(D, x0, 1.3, hx=1.2, hy=0.2, group=group)
+        for dx, motor in ((-0.9, (-8.0, 12.0)), (0.9, None)):
+            tyre = body(D, x0 + dx, 0.7, radius=0.4, group=group)
+            wheel(chassis, tyre, Vec2(x0 + dx, 0.7), up, spring=(4.0, 0.7), limit=(-0.25, 0.25), motor=motor)
+        # a car without a motor rolling down a slope
+        body(S, x0 + 20.0, 2.0, angle=-0.25, hx=4.0, hy=0.2)
+        body2 = body(D, x0 + 18.0, 3.5, angle=-0.25, hx=0.9, hy=0.15, group=group)
+        for dx in (-0.6, 0.6):
+            c, s_ = math.cos(-0.25), math.sin(-0.25)
+            at = Vec2(x0 + 18.0 + c * dx + s_ * 0.45, 3.5 + s_ * dx - c * 0.45)
+            tyre = body(D, at.x, at.y, radius=0.3, group=group)
+            wheel(body2, tyre, at, up, spring=(3.0, 0.5), limit=(-0.2, 0.2))
+        # a barrow: a plank on one wheel with equal limits, its other end on the ground
+        plank = body(D, x0 + 27.0, 0.7, angle=0.3, hx=1.0, hy=0.1, group=group)
+        c, s_ = math.cos(0.3), math.sin(0.3)
+        at = Vec2(x0 + 27.0 + c * 0.9, 0.7 + s_ * 0.9 - 0.1)
+        tyre = body(D, at.x, at.y, radius=0.35, group=group)
+        wheel(plank, tyre, at, up, limit=(0.0, 0.0))
+        # a trolley hanging from a kinematic rail, along the rail
+        if kinematic:
+            rail = body(K, x0 + 32.0, 5.0, hx=2.0, hy=0.1, vx=0.5, group=group)
+            trolley = body(D, x0 + 32.3, 4.5, hx=0.25, hy=0.5, group=group)
+            wheel(rail, trolley, Vec2(x0 + 32.3, 5.0), (1.0, 0.0), spring=(1.0, 0.3), limit=(-1.5, 1.5))
+        if k == 0:
+            dragged = body(D, x0 + 36.0, 0.25, hx=0.25, hy=0.25)
+            md = default_mouse_def()
+            md.bodyIdA = gid
+            md.bodyIdB = dragged
+            md.target = Vec2(x0 + 36.5, 1.5)
             md.hertz = 3.0
             md.dampingRatio = 0.7
             sc.joints.append(lib.s2CreateMouseJoint(world, C.byref(md)))
