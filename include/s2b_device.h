@@ -107,6 +107,9 @@ enum
 	S2B_JOINT_MOTOR = 4, // never carries S2B_JOINT_ENABLE_LIMIT or S2B_JOINT_ENABLE_MOTOR
 	S2B_JOINT_DISTANCE = 5,
 	S2B_JOINT_WHEEL = 6,
+	// never carries S2B_JOINT_ENABLE_LIMIT, S2B_JOINT_ENABLE_MOTOR or S2B_JOINT_ENABLE_SPRING. 7 is the last value the 3-bit
+	// type field ((flags >> 1) & 0x7) holds: a further joint type needs a wider field.
+	S2B_JOINT_PULLEY = 7,
 };
 
 #define S2B_JOINT_ENABLE_LIMIT 0x10
@@ -150,6 +153,9 @@ typedef struct s2bJointRow
 	// maximum motor torque (N-m) in maxMotorTorque, its motor speed (rad/s) in motorSpeed and its spring in hertz /
 	// dampingRatio; impulse[0] is the perpendicular row's impulse, impulse[1] the angular motor's impulse, motorImpulse stays
 	// 0, lowerImpulse / upperImpulse / springImpulse are the axial impulses their names say and referenceAngle is unused.
+	// A pulley row (DESIGN.md §3.18) holds ground anchor A (world) in target, ground anchor B (world) in localAxisA, its ratio
+	// in referenceAngle and its rest lengths lengthA / lengthB in lowerAngle / upperAngle; impulse[0] is the rope impulse
+	// and every other impulse stays 0.
 	float localAxisA[2];
 	// break thresholds (N, N-m) of the reaction pass (DESIGN.md §3.13); 0 = none. A row with either set is checked after every
 	// finalize; a row without them is never checked.

@@ -291,6 +291,58 @@ S2B_API float s2WheelJoint_GetMotorTorque(s2JointId jointId, float inverseTimeSt
 // The current translation (m) along the world axis, from anchor A to anchor B. 0 for another joint type.
 S2B_API float s2WheelJoint_GetTranslation(s2JointId jointId);
 
+// Pulley joint (DESIGN.md §3.18; Box2D 2.4's b2PulleyJoint): anchor A hangs on a rope from the fixed world point
+// groundAnchorA, anchor B on a rope from groundAnchorB, and the joint holds lengthA + ratio lengthB at its value for the
+// rest lengths, lengthA + ratio lengthB, where each length is the distance from the ground anchor to the body anchor. Moving
+// anchor A by d along its rope moves anchor B by d / ratio along its own. It is an equality constraint, as in Box2D 2.4: the
+// ropes can push as well as pull (there is no slack, tension-only pulley). A rope whose anchor comes within
+// 10 s2_linearSlop of its ground anchor exerts nothing on its body. Anchors are relative to each body's origin. Destroy it
+// with s2DestroyJoint.
+typedef struct s2PulleyJointDef
+{
+	s2BodyId bodyIdA;
+	s2BodyId bodyIdB;
+	s2Vec2 groundAnchorA; // world
+	s2Vec2 groundAnchorB; // world
+	s2Vec2 localAnchorA;
+	s2Vec2 localAnchorB;
+	float lengthA; // the rest length of rope A (m), >= 0
+	float lengthB; // the rest length of rope B (m), >= 0
+	float ratio;   // > FLT_EPSILON
+	bool collideConnected;
+} s2PulleyJointDef;
+
+// Box2D 2.4's defaults, collideConnected = true included
+S2_INLINE struct s2PulleyJointDef s2DefaultPulleyJointDef(void)
+{
+	s2PulleyJointDef def = S2_ZERO_INIT;
+	def.bodyIdA = s2_nullBodyId;
+	def.bodyIdB = s2_nullBodyId;
+	def.groundAnchorA.x = -1.0f;
+	def.groundAnchorA.y = 1.0f;
+	def.groundAnchorB.x = 1.0f;
+	def.groundAnchorB.y = 1.0f;
+	def.localAnchorA.x = -1.0f;
+	def.localAnchorB.x = 1.0f;
+	def.ratio = 1.0f;
+	def.collideConnected = true;
+	return def;
+}
+
+// Returns s2_nullJointId (and creates nothing) for a non-finite anchor or length, a negative length, or a ratio that is not
+// finite or is <= FLT_EPSILON.
+S2B_API s2JointId s2CreatePulleyJoint(s2WorldId worldId, const s2PulleyJointDef* def);
+// The getters return 0 (or a zero vector) for a joint of another type.
+S2B_API s2Vec2 s2PulleyJoint_GetGroundAnchorA(s2JointId jointId);
+S2B_API s2Vec2 s2PulleyJoint_GetGroundAnchorB(s2JointId jointId);
+// the rest lengths (m)
+S2B_API float s2PulleyJoint_GetLengthA(s2JointId jointId);
+S2B_API float s2PulleyJoint_GetLengthB(s2JointId jointId);
+S2B_API float s2PulleyJoint_GetRatio(s2JointId jointId);
+// the current distance (m) from each ground anchor to its body anchor
+S2B_API float s2PulleyJoint_GetCurrentLengthA(s2JointId jointId);
+S2B_API float s2PulleyJoint_GetCurrentLengthB(s2JointId jointId);
+
 // ---- joint reactions and breakable joints (DESIGN.md §3.13) --------------------------------------------------------
 
 // What a joint exerts on body B over the last step: force (N, world frame) and torque (N-m).
@@ -317,6 +369,9 @@ typedef struct s2JointReaction
 //   distance   force = rate (impulse.x + motorImpulse + lowerImpulse - upperImpulse) axis, torque = 0. Here localAxisA is the
 //              WORLD axis, the unit vector from anchor A to anchor B at the end of the step (zero when they coincide), and
 //              qA is not read; a distance joint with its spring enabled also passes motorImpulse + springImpulse.
+//   pulley     the distance branch with localAxisA = -ratio uB, uB the unit vector from ground anchor B to anchor B at the end
+//              of the step (zero within 10 s2_linearSlop), and impulse.x the rope impulse: force = rate impulse.x (-ratio uB),
+//              torque = 0
 // Every operation is a separate float32 rounding, so the host and the device (built without contraction) agree bit for bit.
 S2_INLINE s2JointReaction s2MakeJointReaction(int32_t type, s2Vec2 impulse, float motorImpulse, float lowerImpulse,
 											  float upperImpulse, s2Rot qA, s2Vec2 localAxisA, float rate)
@@ -328,7 +383,7 @@ S2_INLINE s2JointReaction s2MakeJointReaction(int32_t type, s2Vec2 impulse, floa
 	{
 		t = motorImpulse + lowerImpulse - upperImpulse;
 	}
-	else if (type == S2B_JOINT_DISTANCE)
+	else if (type == S2B_JOINT_DISTANCE || type == S2B_JOINT_PULLEY)
 	{
 		float axial = impulse.x + motorImpulse + lowerImpulse - upperImpulse;
 		f.x = axial * localAxisA.x;

@@ -221,6 +221,22 @@ class WheelJointDef(C.Structure):
     ]
 
 
+class PulleyJointDef(C.Structure):
+    """s2PulleyJointDef (include/solver2d_b200.h): an extension, absent from the reference."""
+    _fields_ = [
+        ("bodyIdA", BodyId),
+        ("bodyIdB", BodyId),
+        ("groundAnchorA", Vec2),
+        ("groundAnchorB", Vec2),
+        ("localAnchorA", Vec2),
+        ("localAnchorB", Vec2),
+        ("lengthA", C.c_float),
+        ("lengthB", C.c_float),
+        ("ratio", C.c_float),
+        ("collideConnected", C.c_bool),
+    ]
+
+
 class MotorJointDef(C.Structure):
     """s2MotorJointDef (include/solver2d_b200.h): an extension, absent from the reference."""
     _fields_ = [
@@ -338,6 +354,20 @@ def default_wheel_def() -> WheelJointDef:
     return d
 
 
+def default_pulley_def() -> PulleyJointDef:
+    """s2DefaultPulleyJointDef (include/solver2d_b200.h): Box2D 2.4's defaults, collideConnected on."""
+    d = PulleyJointDef()
+    d.bodyIdA = BodyId(-1, -1, 0)
+    d.bodyIdB = BodyId(-1, -1, 0)
+    d.groundAnchorA = Vec2(-1.0, 1.0)
+    d.groundAnchorB = Vec2(1.0, 1.0)
+    d.localAnchorA = Vec2(-1.0, 0.0)
+    d.localAnchorB = Vec2(1.0, 0.0)
+    d.ratio = 1.0
+    d.collideConnected = True
+    return d
+
+
 def default_motor_def() -> MotorJointDef:
     """s2DefaultMotorJointDef (include/solver2d_b200.h)."""
     d = MotorJointDef()
@@ -444,6 +474,15 @@ _API = {
     "s2WheelJoint_SetMaxMotorTorque": (None, [JointId, C.c_float]),
     "s2WheelJoint_GetMotorTorque": (C.c_float, [JointId, C.c_float]),
     "s2WheelJoint_GetTranslation": (C.c_float, [JointId]),
+    # pulley joint (DESIGN.md §3.18)
+    "s2CreatePulleyJoint": (JointId, [WorldId, C.POINTER(PulleyJointDef)]),
+    "s2PulleyJoint_GetGroundAnchorA": (Vec2, [JointId]),
+    "s2PulleyJoint_GetGroundAnchorB": (Vec2, [JointId]),
+    "s2PulleyJoint_GetLengthA": (C.c_float, [JointId]),
+    "s2PulleyJoint_GetLengthB": (C.c_float, [JointId]),
+    "s2PulleyJoint_GetRatio": (C.c_float, [JointId]),
+    "s2PulleyJoint_GetCurrentLengthA": (C.c_float, [JointId]),
+    "s2PulleyJoint_GetCurrentLengthB": (C.c_float, [JointId]),
     # joint springs (DESIGN.md §3.14)
     "s2PrismaticJoint_EnableSpring": (None, [JointId, C.c_bool]),
     "s2PrismaticJoint_SetSpringHertz": (None, [JointId, C.c_float]),

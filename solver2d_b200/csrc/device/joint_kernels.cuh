@@ -6,6 +6,7 @@
 
 #include "contact_kernels.cuh"
 #include "shared/s2_collide.h"
+#include "shared/s2_distance_joint.h"
 
 #define S2B_JOINT_TYPE(flags) (((flags) >> 1) & 0x7)
 // row flags of the joint-constraint stream only (jc.head.x): an XPBD spring row's body A / B is static, so its sub-step start
@@ -121,6 +122,20 @@ template <int KIND> __device__ __forceinline__ void s2bPrepareJointRows(const So
 	jc.lim[t] = lim;
 	jc.coef[t] = make_float4(a.softJoint.bias, a.softJoint.mass, a.softJoint.impulse, 0.0f);
 
+	if (S2B_JOINT_TYPE(flags) == S2B_JOINT_PULLEY)
+	{
+		// DESIGN.md §3.18: the row's lim = (ratio, lengthA, lengthB) and target = (groundA, groundB) become lim = (constant,
+		// ratio) and d0ax = (cA - groundA, cB - groundB) at the start poses; the frame and the mass are formed fresh in each
+		// solve. The rope impulse is kept only with the variant's warm start, and never under XPBD.
+		float4 ground = a.joints.target[slot];
+		jc.lim[t] = make_float4(lim.y + lim.x * lim.z, lim.x, 0.0f, 0.0f);
+		jc.d0ax[t] = make_float4(posA.x - ground.x, posA.y - ground.y, posB.x - ground.z, posB.y - ground.w);
+		jc.motor[t] = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
+		jc.pivot[t] = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
+		jc.imp[t] = make_float4(KIND != JPREP_XPBD && warmStart ? imp.x : 0.0f, 0.0f, 0.0f, 0.0f);
+		jc.limp[t] = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
+		return;
+	}
 	if (S2B_JOINT_TYPE(flags) == S2B_JOINT_DISTANCE)
 	{
 		// DESIGN.md §3.16: lim = (rest length, min, max), motor = (maxMotorForce, motorSpeed); the frame and the axial mass
@@ -1141,6 +1156,146 @@ __device__ __forceinline__ void s2bSolveWheelXpbd(const SolveArgs& a, int t)
 }
 
 // ---------------------------------------------------------------------------------------------------------------
+// pulley joint (extension, DESIGN.md §3.18; definition: tests/pulley_oracle.c). Anchor A hangs on a rope from ground anchor
+// A, anchor B on one from ground anchor B, and one equality row holds C = constant - lengthA - ratio lengthB at zero with
+// J = (-uA, -ratio uB). Each rope is formed from its own body's pose alone, so the per-body gather can form its side's
+// warm-start term without the other body. Row columns: lim = (constant, ratio), d0ax = (cA - groundA, cB - groundB) at the
+// start poses, imp.x = the rope impulse.
+// ---------------------------------------------------------------------------------------------------------------
+
+// one rope at its body's pose: r = q anchor, and the length and unit direction u of (dc + r) + d0, the vector from the
+// ground anchor to the body anchor (u is zero within 10 s2_linearSlop)
+struct PulleyRope
+{
+	s2Vec2 r, u;
+	float length;
+};
+
+__device__ __forceinline__ PulleyRope s2bPulleyRope(float ax, float ay, float d0x, float d0y, s2Vec2 dc, s2Rot q)
+{
+	PulleyRope p;
+	p.r = s2RotateVector(q, V2(ax, ay));
+	p.u = s2cPulleyRope(&p.length, s2Add(s2Add(dc, p.r), V2(d0x, d0y)));
+	return p;
+}
+
+// the row's inverse effective mass, mA + iA ruA^2 + ratio^2 (mB + iB ruB^2)
+__device__ __forceinline__ float s2bPulleyInvMass(const PulleyRope& A, const PulleyRope& B, float ratio, float mA, float iA, float mB,
+												  float iB)
+{
+	float ruA = s2Cross(A.r, A.u), ruB = s2Cross(B.r, B.u);
+	return mA + iA * ruA * ruA + ratio * ratio * (mB + iB * ruB * ruB);
+}
+
+// what warm starting adds to one side (v += m P, w += i L): P = -lambda uA on side A, -(ratio lambda) uB on side B,
+// L = r x P. Shared by the constraint-by-constraint warm start and the per-body gather, so both add the same bits.
+struct PulleyWarm
+{
+	s2Vec2 P;
+	float L;
+};
+
+__device__ __forceinline__ PulleyWarm s2bPulleyWarmTerm(const SolveArgs& a, int t, bool sideB)
+{
+	const JointConstraintView& jc = a.jc;
+	int4 head = jc.head[t];
+	float4 anchor = jc.anchor[t], d0 = jc.d0ax[t];
+	float4 pose = a.bodies.pose[sideB ? head.z : head.y];
+	float lambda = jc.imp[t].x;
+	PulleyRope rope = sideB ? s2bPulleyRope(anchor.z, anchor.w, d0.z, d0.w, V2(pose.x, pose.y), R2(pose.z, pose.w))
+							: s2bPulleyRope(anchor.x, anchor.y, d0.x, d0.y, V2(pose.x, pose.y), R2(pose.z, pose.w));
+	PulleyWarm w;
+	w.P = s2MulSV(sideB ? -(jc.lim[t].y * lambda) : -lambda, rope.u);
+	w.L = s2Cross(rope.r, w.P);
+	return w;
+}
+
+// the velocity row in each flavour: the distance joint's rigid row (soft bias in the biased pass, Baumgarte in every pass,
+// none under the rigid flavour)
+template <int KIND>
+__device__ __forceinline__ void s2bSolvePulleyVelocity(const SolveArgs& a, int t, float h, float inv_h, bool useBias)
+{
+	const JointConstraintView& jc = a.jc;
+	int4 head = jc.head[t];
+	int ia = head.y, ib = head.z;
+	float4 anchor = jc.anchor[t];
+	float4 mass = jc.mass[t];
+	float4 d0 = jc.d0ax[t];
+	float4 lim = jc.lim[t];
+	float4 imp = jc.imp[t];
+	float4 velA = a.bodies.vel[ia], velB = a.bodies.vel[ib];
+	float4 poseA = a.bodies.pose[ia], poseB = a.bodies.pose[ib];
+	s2Vec2 vA = V2(velA.x, velA.y), vB = V2(velB.x, velB.y);
+	float wA = velA.z, wB = velB.z;
+	float mA = mass.x, iA = mass.y, mB = mass.z, iB = mass.w;
+	float ratio = lim.y;
+	PulleyRope A = s2bPulleyRope(anchor.x, anchor.y, d0.x, d0.y, V2(poseA.x, poseA.y), R2(poseA.z, poseA.w));
+	PulleyRope B = s2bPulleyRope(anchor.z, anchor.w, d0.z, d0.w, V2(poseB.x, poseB.y), R2(poseB.z, poseB.w));
+	float kInv = s2bPulleyInvMass(A, B, ratio, mA, iA, mB, iB);
+	float k = kInv > 0.0f ? 1.0f / kInv : 0.0f;
+
+	float3 s = s2bPrismaticBias<KIND>(lim.x - A.length - ratio * B.length, false, jc.coef[t], h, inv_h, useBias);
+	s2Vec2 vpA = s2Add(vA, s2CrossSV(wA, A.r));
+	s2Vec2 vpB = s2Add(vB, s2CrossSV(wB, B.r));
+	float Cdot = -s2Dot(A.u, vpA) - ratio * s2Dot(B.u, vpB);
+	float impulse = -k * s.y * (Cdot + s.x) - s.z * imp.x;
+	imp.x += impulse;
+	s2Vec2 PA = s2MulSV(-impulse, A.u);
+	s2Vec2 PB = s2MulSV(-(ratio * impulse), B.u);
+	vA = s2MulAdd(vA, mA, PA);
+	wA += iA * s2Cross(A.r, PA);
+	vB = s2MulAdd(vB, mB, PB);
+	wB += iB * s2Cross(B.r, PB);
+
+	jc.imp[t] = imp;
+	s2bStoreJointVelocities(a, ia, ib, velA, velB, vA, wA, vB, wB, mA, iA, mB, iB);
+}
+
+// one position correction of the row on the given poses: impulse = -k C with C clamped (NGS) or -C / (1 / k) (XPBD at zero
+// compliance, skipped when 1 / k is 0), applied as PA = -impulse uA, PB = -(ratio impulse) uB
+template <bool XPBD>
+__device__ __forceinline__ void s2bSolvePulleyPositionT(const SolveArgs& a, int t)
+{
+	const JointConstraintView& jc = a.jc;
+	int4 head = jc.head[t];
+	int ia = head.y, ib = head.z;
+	float4 anchor = jc.anchor[t];
+	float4 mass = jc.mass[t];
+	float4 d0 = jc.d0ax[t];
+	float4 lim = jc.lim[t];
+	float4 poseA = a.bodies.pose[ia], poseB = a.bodies.pose[ib];
+	s2Vec2 dcA = V2(poseA.x, poseA.y), dcB = V2(poseB.x, poseB.y);
+	s2Rot qA = R2(poseA.z, poseA.w), qB = R2(poseB.z, poseB.w);
+	float mA = mass.x, iA = mass.y, mB = mass.z, iB = mass.w;
+	float ratio = lim.y;
+	PulleyRope A = s2bPulleyRope(anchor.x, anchor.y, d0.x, d0.y, dcA, qA);
+	PulleyRope B = s2bPulleyRope(anchor.z, anchor.w, d0.z, d0.w, dcB, qB);
+	float kInv = s2bPulleyInvMass(A, B, ratio, mA, iA, mB, iB);
+	float C = lim.x - A.length - ratio * B.length;
+	if (XPBD && (kInv > 0.0f) == false)
+	{
+		return;
+	}
+	// NGS: C clamped as every NGS row here is (DESIGN.md §3.18; Box2D 2.4 does not clamp the pulley)
+	float impulse = XPBD ? -C / kInv
+						 : -(kInv > 0.0f ? 1.0f / kInv : 0.0f) * S2_CLAMP(C, -s2_maxLinearCorrection, s2_maxLinearCorrection);
+	s2Vec2 PA = s2MulSV(-impulse, A.u);
+	s2Vec2 PB = s2MulSV(-(ratio * impulse), B.u);
+	dcA = s2MulAdd(dcA, mA, PA);
+	qA = s2IntegrateRot(qA, iA * s2Cross(A.r, PA));
+	dcB = s2MulAdd(dcB, mB, PB);
+	qB = s2IntegrateRot(qB, iB * s2Cross(B.r, PB));
+	if ((mA != 0.0f) || (iA != 0.0f))
+	{
+		a.bodies.pose[ia] = make_float4(dcA.x, dcA.y, qA.s, qA.c);
+	}
+	if ((mB != 0.0f) || (iB != 0.0f))
+	{
+		a.bodies.pose[ib] = make_float4(dcB.x, dcB.y, qB.s, qB.c);
+	}
+}
+
+// ---------------------------------------------------------------------------------------------------------------
 // motor joint (extension, DESIGN.md §3.10; definition: tests/motor_oracle.c). Drives body B toward a pose relative to body
 // A with capped effort: an angular row toward angle(B) - angle(A) = angularOffset, its accumulated impulse clamped to
 // +/- h maxTorque, then a point row that takes B's origin to the linear offset in A's frame, its accumulated impulse scaled
@@ -1469,6 +1624,20 @@ __device__ __forceinline__ void s2bWarmStartJoint(const SolveArgs& a, int t)
 		float wA = velA.z - iA * pw.LA;
 		s2Vec2 vB = s2MulAdd(V2(velB.x, velB.y), mB, pw.P);
 		float wB = velB.z + iB * pw.LB;
+		s2bStoreJointVelocities(a, ia, ib, velA, velB, vA, wA, vB, wB, mA, iA, mB, iB);
+		return;
+	}
+
+	if (S2B_JOINT_TYPE(head.x) == S2B_JOINT_PULLEY)
+	{
+		float4 velA = a.bodies.vel[ia], velB = a.bodies.vel[ib];
+		float mA = mass.x, iA = mass.y, mB = mass.z, iB = mass.w;
+		PulleyWarm wa = s2bPulleyWarmTerm(a, t, false);
+		PulleyWarm wb = s2bPulleyWarmTerm(a, t, true);
+		s2Vec2 vA = s2MulAdd(V2(velA.x, velA.y), mA, wa.P);
+		float wA = velA.z + iA * wa.L;
+		s2Vec2 vB = s2MulAdd(V2(velB.x, velB.y), mB, wb.P);
+		float wB = velB.z + iB * wb.L;
 		s2bStoreJointVelocities(a, ia, ib, velA, velB, vA, wA, vB, wB, mA, iA, mB, iB);
 		return;
 	}
@@ -2120,6 +2289,11 @@ __device__ __forceinline__ void s2bSolveJointSoft(const SolveArgs& a, int t, flo
 		s2bSolveWheelVelocity<PSOLVE_SOFT>(a, t, h, inv_h, useBias);
 		return;
 	}
+	if (S2B_JOINT_TYPE(flags) == S2B_JOINT_PULLEY)
+	{
+		s2bSolvePulleyVelocity<PSOLVE_SOFT>(a, t, h, inv_h, useBias);
+		return;
+	}
 	if (SHARED_MOTOR == false && S2B_JOINT_TYPE(flags) == S2B_JOINT_MOTOR)
 	{
 		s2bSolveMotorVelocity(a, t, h, inv_h);
@@ -2155,6 +2329,11 @@ __device__ __forceinline__ void s2bSolveJointBaumgarte(const SolveArgs& a, int t
 	if (S2B_JOINT_TYPE(flags) == S2B_JOINT_WHEEL)
 	{
 		s2bSolveWheelVelocity<PSOLVE_BAUMGARTE>(a, t, h, inv_h, useBias);
+		return;
+	}
+	if (S2B_JOINT_TYPE(flags) == S2B_JOINT_PULLEY)
+	{
+		s2bSolvePulleyVelocity<PSOLVE_BAUMGARTE>(a, t, h, inv_h, useBias);
 		return;
 	}
 	if (S2B_JOINT_TYPE(flags) == S2B_JOINT_MOTOR)
@@ -2289,6 +2468,11 @@ __device__ __forceinline__ void s2bSolveJointRigid(const SolveArgs& a, int t, fl
 		s2bSolveWheelVelocity<PSOLVE_RIGID>(a, t, h, 0.0f /* inv_h: unused by the rigid rows */, false);
 		return;
 	}
+	if (S2B_JOINT_TYPE(a.jc.head[t].x) == S2B_JOINT_PULLEY)
+	{
+		s2bSolvePulleyVelocity<PSOLVE_RIGID>(a, t, h, 0.0f /* inv_h: unused by the rigid row */, false);
+		return;
+	}
 	if (S2B_JOINT_TYPE(a.jc.head[t].x) == S2B_JOINT_MOTOR)
 	{
 		s2bSolveMotorVelocity(a, t, h, a.ctx.inv_h);
@@ -2327,6 +2511,11 @@ __device__ __forceinline__ void s2bSolveJointPosition(const SolveArgs& a, int t)
 	if (S2B_JOINT_TYPE(head.x) == S2B_JOINT_WHEEL)
 	{
 		s2bSolveWheelPosition(a, t);
+		return;
+	}
+	if (S2B_JOINT_TYPE(head.x) == S2B_JOINT_PULLEY)
+	{
+		s2bSolvePulleyPositionT<false>(a, t);
 		return;
 	}
 	if (head.x & S2B_JC_SOFT_WELD)
@@ -2431,6 +2620,11 @@ __device__ __forceinline__ void s2bSolveJointXpbd(const SolveArgs& a, int t)
 	if (S2B_JOINT_TYPE(head.x) == S2B_JOINT_WHEEL)
 	{
 		s2bSolveWheelXpbd(a, t);
+		return;
+	}
+	if (S2B_JOINT_TYPE(head.x) == S2B_JOINT_PULLEY)
+	{
+		s2bSolvePulleyPositionT<true>(a, t);
 		return;
 	}
 	if (S2B_JOINT_TYPE(head.x) == S2B_JOINT_MOTOR)

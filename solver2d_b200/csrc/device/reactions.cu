@@ -1,7 +1,8 @@
 // solver2d-b200 — joint reactions and break thresholds (DESIGN.md §3.13).
 //
 // One thread per joint slot evaluates s2MakeJointReaction (include/solver2d_b200.h) on the impulses the last solve stored,
-// body A's final rotation (a distance joint: the line between its anchors at both bodies' final poses) and the rate of that
+// body A's final rotation (a distance joint: the line between its anchors at both bodies' final poses; a pulley: -ratio times
+// rope B's direction at body B's final pose) and the rate of that
 // solve. After finalize (s2bFinalize) it compares the reaction with the
 // slot's thresholds and appends the slots over one to a list; on demand (s2b_download_joint_reactions) it writes the
 // reactions instead. The solver kernels are not touched: everything it reads is already in the joint and body columns.
@@ -56,6 +57,15 @@ __global__ void s2bJointReactionKernel(JointView j, const float2* __restrict__ b
 		axis = s2cDistanceJointAxis(&length, s2MakeVec2(pa.x, pa.y), qA, s2Sub(s2MakeVec2(anchors.x, anchors.y), s2MakeVec2(oa.z, oa.w)),
 									s2MakeVec2(pb.x, pb.y), s2Rot{qb.z, qb.w},
 									s2Sub(s2MakeVec2(anchors.z, anchors.w), s2MakeVec2(ob.z, ob.w)));
+	}
+	else if (type == S2B_JOINT_PULLEY)
+	{
+		// -ratio uB at the end of the step (DESIGN.md §3.18): ground anchor B rides in target.zw, the ratio in lim.x
+		float4 anchors = j.anchors[i];
+		float4 pb = pos[head.z], qb = pose[head.z], ob = org[head.z];
+		float length;
+		axis = s2cPulleyJointAxis(&length, axis, s2MakeVec2(pb.x, pb.y), s2Rot{qb.z, qb.w},
+								  s2Sub(s2MakeVec2(anchors.z, anchors.w), s2MakeVec2(ob.z, ob.w)), j.lim[i].x);
 	}
 	s2JointReaction r = s2MakeJointReaction(type, s2MakeVec2(imp.x, imp.y), motorImpulse, limp.x, limp.y, qA, axis, rate);
 	if (reactions != nullptr)

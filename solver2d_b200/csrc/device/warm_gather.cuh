@@ -91,6 +91,13 @@ __device__ __forceinline__ GatherTerms s2bGatherTermsOf(const SolveArgs& a, int 
 			g.tv0 = sideB ? mp : V2(-mp.x, -mp.y);
 			g.tw0 = sideB ? invI * pw.LB : -(invI * pw.LA);
 		}
+		else if (S2B_JOINT_TYPE(head.x) == S2B_JOINT_PULLEY)
+		{
+			// each side's term depends on its own body's pose only (DESIGN.md §3.18)
+			PulleyWarm pw = s2bPulleyWarmTerm(a, t, sideB);
+			g.tv0 = s2MulSV(invMass, pw.P);
+			g.tw0 = invI * pw.L;
+		}
 		else
 		{
 			float4 limp = a.jc.limp[t];

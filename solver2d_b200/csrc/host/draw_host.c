@@ -87,6 +87,17 @@ static void s2DrawJoint(s2DebugDraw* draw, s2World* world, const s2Joint* joint)
 		return;
 	}
 
+	if (joint->type == s2_pulleyJoint)
+	{
+		// Box2D 2.4's three segments: each rope from its ground anchor to its body anchor, and the line between the ground
+		// anchors
+		s2Color color = s2Rgb(0.5f, 0.8f, 0.8f);
+		draw->DrawSegment(joint->targetA, pA, color, draw->context);
+		draw->DrawSegment(joint->localAxisA, pB, color, draw->context);
+		draw->DrawSegment(joint->targetA, joint->localAxisA, color, draw->context);
+		return;
+	}
+
 	if (joint->type == s2_distanceJoint)
 	{
 		// the segment between the anchors and, with the limit on, a mark across the line at minLength and at maxLength from

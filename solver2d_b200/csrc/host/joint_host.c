@@ -913,13 +913,118 @@ float s2WheelJoint_GetTranslation(s2JointId jointId)
 	return joint->type == s2_wheelJoint ? s2PrismaticJoint_GetTranslation(jointId) : 0.0f;
 }
 
+// ---- pulley joint (DESIGN.md §3.18) --------------------------------------------------------------------------------------
+
+// The pulley joint has no counterpart in the reference. Invalid input creates nothing and returns s2_nullJointId.
+s2JointId s2CreatePulleyJoint(s2WorldId worldId, const s2PulleyJointDef* def)
+{
+	if (s2IsValidVec2(def->groundAnchorA) == false || s2IsValidVec2(def->groundAnchorB) == false ||
+		s2IsValidVec2(def->localAnchorA) == false || s2IsValidVec2(def->localAnchorB) == false ||
+		s2IsValidDistanceValue(def->lengthA) == false || s2IsValidDistanceValue(def->lengthB) == false ||
+		s2IsValid(def->ratio) == false || (def->ratio > FLT_EPSILON) == false)
+	{
+		return s2_nullJointId;
+	}
+
+	s2World* world = s2GetWorldFromId(worldId);
+	s2Body* bodyA = world->bodies + def->bodyIdA.index;
+	s2Body* bodyB = world->bodies + def->bodyIdB.index;
+
+	s2Joint* joint = s2AllocJoint(world, bodyA, bodyB);
+	joint->type = s2_pulleyJoint;
+	joint->drawSize = 1.0f;
+	joint->localOriginAnchorA = def->localAnchorA;
+	joint->localOriginAnchorB = def->localAnchorB;
+	joint->targetA = def->groundAnchorA;
+	joint->localAxisA = def->groundAnchorB;
+	joint->referenceAngle = def->ratio;
+	joint->lowerAngle = def->lengthA;
+	joint->upperAngle = def->lengthB;
+	joint->collideConnected = def->collideConnected;
+
+	s2JointId jointId = {joint->object.index, world->index, joint->object.revision};
+	return jointId;
+}
+
+// the joint, or NULL for a joint of another type
+static const s2Joint* s2GetPulleyJoint(s2JointId jointId)
+{
+	s2World* world = s2GetWorldFromIndex(jointId.world);
+	const s2Joint* joint = world->joints + jointId.index;
+	S2_ASSERT(s2ObjectValid(&joint->object) && joint->object.revision == jointId.revision);
+	return joint->type == s2_pulleyJoint ? joint : NULL;
+}
+
+s2Vec2 s2PulleyJoint_GetGroundAnchorA(s2JointId jointId)
+{
+	const s2Joint* joint = s2GetPulleyJoint(jointId);
+	return joint != NULL ? joint->targetA : s2Vec2_zero;
+}
+
+s2Vec2 s2PulleyJoint_GetGroundAnchorB(s2JointId jointId)
+{
+	const s2Joint* joint = s2GetPulleyJoint(jointId);
+	return joint != NULL ? joint->localAxisA : s2Vec2_zero;
+}
+
+float s2PulleyJoint_GetLengthA(s2JointId jointId)
+{
+	const s2Joint* joint = s2GetPulleyJoint(jointId);
+	return joint != NULL ? joint->lowerAngle : 0.0f;
+}
+
+float s2PulleyJoint_GetLengthB(s2JointId jointId)
+{
+	const s2Joint* joint = s2GetPulleyJoint(jointId);
+	return joint != NULL ? joint->upperAngle : 0.0f;
+}
+
+float s2PulleyJoint_GetRatio(s2JointId jointId)
+{
+	const s2Joint* joint = s2GetPulleyJoint(jointId);
+	return joint != NULL ? joint->referenceAngle : 0.0f;
+}
+
+// -ratio uB (sideB) or -uA, and the rope's length, at the lazily synced poses
+static s2Vec2 s2PulleyJointAxis(s2World* world, const s2Joint* joint, bool sideB, float* length)
+{
+	const s2Body* body = world->bodies + (sideB ? joint->bodyIndexB : joint->bodyIndexA);
+	s2Vec2 local = s2Sub(sideB ? joint->localOriginAnchorB : joint->localOriginAnchorA, body->localCenter);
+	return s2cPulleyJointAxis(length, sideB ? joint->localAxisA : joint->targetA, body->position, body->rot, local,
+							  sideB ? joint->referenceAngle : 1.0f);
+}
+
+static float s2PulleyJointCurrentLength(s2JointId jointId, bool sideB)
+{
+	s2World* world = s2GetWorldFromIndex(jointId.world);
+	s2SyncStateToHost(world);
+	const s2Joint* joint = s2GetPulleyJoint(jointId);
+	if (joint == NULL)
+	{
+		return 0.0f;
+	}
+	float length;
+	s2PulleyJointAxis(world, joint, sideB, &length);
+	return length;
+}
+
+float s2PulleyJoint_GetCurrentLengthA(s2JointId jointId)
+{
+	return s2PulleyJointCurrentLength(jointId, false);
+}
+
+float s2PulleyJoint_GetCurrentLengthB(s2JointId jointId)
+{
+	return s2PulleyJointCurrentLength(jointId, true);
+}
+
 // ---- reactions and break thresholds (DESIGN.md §3.13) -----------------------------------------------------------------
 
 // s2JointType and the device's S2B_JOINT_* number the joint types alike
 _Static_assert((int)s2_revoluteJoint == S2B_JOINT_REVOLUTE && (int)s2_mouseJoint == S2B_JOINT_MOUSE &&
 				   (int)s2_weldJoint == S2B_JOINT_WELD && (int)s2_prismaticJoint == S2B_JOINT_PRISMATIC &&
 				   (int)s2_motorJoint == S2B_JOINT_MOTOR && (int)s2_distanceJoint == S2B_JOINT_DISTANCE &&
-				   (int)s2_wheelJoint == S2B_JOINT_WHEEL,
+				   (int)s2_wheelJoint == S2B_JOINT_WHEEL && (int)s2_pulleyJoint == S2B_JOINT_PULLEY,
 			   "joint type numbering");
 
 s2JointReaction s2ComputeJointReaction(int32_t type, s2Vec2 impulse, float motorImpulse, float lowerImpulse, float upperImpulse,
@@ -939,9 +1044,17 @@ static s2JointReaction s2GetJointReaction(s2JointId jointId)
 	// row the device last solved, so the getters read what the device's reaction and break pass read for that step even
 	// after s2*Joint_EnableSpring has changed the joint and before the next step uploads it.
 	float motorImpulse = joint->springUploaded ? joint->motorImpulse + joint->springImpulse : joint->motorImpulse;
-	// a distance joint passes its world axis at the end of the step (DESIGN.md §3.16)
+	// a distance joint passes its world axis at the end of the step (DESIGN.md §3.16), a pulley -ratio uB (§3.18)
 	float length;
-	s2Vec2 axis = joint->type == s2_distanceJoint ? s2DistanceJointAxis(world, joint, &length) : joint->localAxisA;
+	s2Vec2 axis = joint->localAxisA;
+	if (joint->type == s2_distanceJoint)
+	{
+		axis = s2DistanceJointAxis(world, joint, &length);
+	}
+	else if (joint->type == s2_pulleyJoint)
+	{
+		axis = s2PulleyJointAxis(world, joint, true, &length);
+	}
 	return s2MakeJointReaction((int32_t)joint->type, joint->impulse, motorImpulse, joint->lowerImpulse, joint->upperImpulse,
 							   world->bodies[joint->bodyIndexA].rot, axis, world->reactionRate);
 }

@@ -90,6 +90,7 @@ typedef enum s2JointType
 	s2_motorJoint,
 	s2_distanceJoint,
 	s2_wheelJoint,
+	s2_pulleyJoint,
 } s2JointType;
 
 typedef struct s2Body
@@ -168,7 +169,9 @@ typedef struct s2Joint
 	// maxMotorTorque, as its device row does. A distance joint keeps its rest length in referenceAngle, its min / max length
 	// in lowerAngle / upperAngle, its maximum motor force in maxMotorTorque and its spring in hertz / dampingRatio. A wheel
 	// joint keeps its translation limits in lowerAngle / upperAngle, its maximum motor torque in maxMotorTorque, its axis in
-	// localAxisA and its spring in hertz / dampingRatio; impulse.y is its angular motor impulse and motorImpulse stays 0.
+	// localAxisA and its spring in hertz / dampingRatio; impulse.y is its angular motor impulse and motorImpulse stays 0. A
+	// pulley joint keeps its ratio in referenceAngle, its rest lengths in lowerAngle / upperAngle, ground anchor A in targetA
+	// and ground anchor B in localAxisA; impulse.x is its rope impulse.
 	bool enableMotor, enableLimit;
 	float maxMotorTorque, motorSpeed;
 	float referenceAngle, lowerAngle, upperAngle;

@@ -247,9 +247,13 @@ static void s2FillJointRow(s2bJointRow* r, const s2Joint* j)
 		case s2_wheelJoint:
 			type = S2B_JOINT_WHEEL;
 			break;
+		case s2_pulleyJoint:
+			type = S2B_JOINT_PULLEY;
+			break;
 	}
 	r->flags = S2B_ROW_VALID | (type << 1);
-	// welds and motor joints are created with enableLimit == enableMotor == false, so their rows never carry either flag
+	// welds, motor joints and pulleys are created with enableLimit == enableMotor == false, so their rows never carry either
+	// flag
 	r->flags |= j->enableLimit ? S2B_JOINT_ENABLE_LIMIT : 0;
 	r->flags |= j->enableMotor ? S2B_JOINT_ENABLE_MOTOR : 0;
 	r->flags |= j->collideConnected ? S2B_JOINT_COLLIDE_CONNECTED : 0;

@@ -78,8 +78,11 @@ JOINT_ENABLE_LIMIT, JOINT_ENABLE_MOTOR, JOINT_COLLIDE_CONNECTED, JOINT_ENABLE_SP
 # its translation limits in lowerAngle / upperAngle and its maximum motor force in maxMotorTorque; a motor row keeps its
 # linear offset in localOriginAnchorA, its angular offset in referenceAngle, its maximum torque in maxMotorTorque, its
 # maximum force in hertz and its correction factor in dampingRatio; a wheel row keeps its translation limits in lowerAngle /
-# upperAngle, its maximum motor torque in maxMotorTorque and its angular motor impulse in impulse[1])
-JOINT_REVOLUTE, JOINT_MOUSE, JOINT_WELD, JOINT_PRISMATIC, JOINT_MOTOR, JOINT_DISTANCE, JOINT_WHEEL = 0, 1, 2, 3, 4, 5, 6
+# upperAngle, its maximum motor torque in maxMotorTorque and its angular motor impulse in impulse[1]; a pulley row keeps
+# ground anchor A in target, ground anchor B in localAxisA, its ratio in referenceAngle and its rest lengths in lowerAngle /
+# upperAngle, and fills the 3-bit type field)
+JOINT_REVOLUTE, JOINT_MOUSE, JOINT_WELD, JOINT_PRISMATIC, JOINT_MOTOR, JOINT_DISTANCE, JOINT_WHEEL, JOINT_PULLEY = \
+    0, 1, 2, 3, 4, 5, 6, 7
 
 # symbols declared in include/s2b_device.h (checked by the CPU test-suite against the built library)
 ABI_SYMBOLS = [

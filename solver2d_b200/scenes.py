@@ -1389,6 +1389,145 @@ def wheels(lib: capi.Solver2D, solver="TGS_Soft", copies=1, kinematic=True, stan
     return sc
 
 
+PULLEYS_PITCH = 40.0  # width of one copy of pulleys (m)
+
+
+def pulleys(lib: capi.Solver2D, solver="TGS_Soft", copies=1, kinematic=True, stand_ins=None) -> Scene:
+    """Pulley joint coverage (DESIGN.md §3.18), `copies` side by side (18 bodies each). Per copy:
+
+    * Box2D 2.4's testbed pulley: two equal boxes hung from ground anchors 6 m apart, ratio 1.5, so box A sinks;
+    * a counterweighted lift: a platform on a vertical prismatic joint (limits -1.5 m and 3 m) hung over a pulley against a
+      counterweight, with a pile of boxes dropped onto it, so contacts share the pulley's bodies;
+    * a block-and-tackle at ratio 2: a load on side A that balances one twice its mass on side B, and the same with a side B
+      1.1 times as heavy again, which lifts its load;
+    * with `kinematic`: a kinematic body on side A moving down at 0.4 m/s, raising the load on side B (ratio 1.5);
+    * a revolute chain of three links hung from a post, and a box pulled by a mouse joint (first copy only).
+
+    Every pulley keeps s2DefaultPulleyJointDef's collideConnected = true. On a library without s2CreatePulleyJoint (the
+    reference), or with `stand_ins` true, every pulley is created as a revolute joint between the same two bodies at anchor
+    B's start point, with the same collideConnected; on a library without s2CreatePrismaticJoint the lift's prismatic joint
+    is such a stand-in too. ``sc.piles["pulley"]`` lists the index into ``sc.joints`` of every pulley and
+    ``sc.piles["pulley_defs"]`` its definition (anchors relative to the body origins, rest lengths as the float32 values the
+    row carries); ``sc.piles["prismatic"]`` and ``["prismatic_defs"]`` describe the prismatic joint as ``sliders`` does, so
+    that a test can turn the stand-in rows into pulley and prismatic rows."""
+    world = lib.create_world(solver)
+    sc = Scene(lib, world, name=f"pulleys{copies}")
+    sc.piles["pulley"] = []
+    sc.piles["pulley_defs"] = []
+    sc.piles["prismatic"] = []
+    sc.piles["prismatic_defs"] = []
+    real = "s2CreatePulleyJoint" not in lib.missing and not stand_ins
+    has_prismatic = "s2CreatePrismaticJoint" not in lib.missing
+    gid = _ground(lib, world, 0.5 * PULLEYS_PITCH * copies + 5.0)
+    sc.bodies.append(gid)
+
+    def body(kind, x, y, hx=0.25, hy=0.25, vy=0.0):
+        bd = default_body_def()
+        bd.type = kind
+        bd.position = Vec2(x, y)
+        bd.linearVelocity = Vec2(0.0, vy)
+        bid = lib.s2CreateBody(world, C.byref(bd))
+        lib.s2CreatePolygonShape(bid, C.byref(default_shape_def()), C.byref(lib.s2MakeBox(hx, hy)))
+        sc.bodies.append(bid)
+        return bid
+
+    def pulley(a, b, ga, gb, pa, pb, ratio):
+        """ga, gb: the ground anchors; pa, pb: the anchors' world points at creation."""
+        f32 = np.float32
+        d = dict(groundAnchorA=ga, groundAnchorB=gb, localAnchorA=tuple(lib.s2Body_GetLocalPoint(a, Vec2(*pa))),
+                 localAnchorB=tuple(lib.s2Body_GetLocalPoint(b, Vec2(*pb))),
+                 lengthA=float(f32(math.hypot(pa[0] - ga[0], pa[1] - ga[1]))),
+                 lengthB=float(f32(math.hypot(pb[0] - gb[0], pb[1] - gb[1]))), ratio=float(f32(ratio)), collideConnected=True)
+        if real:
+            jd = capi.default_pulley_def()
+            for name, value in d.items():
+                setattr(jd, name, Vec2(*value) if isinstance(value, tuple) else value)
+            create = lib.s2CreatePulleyJoint
+        else:
+            jd = default_revolute_def()
+            jd.localAnchorA = lib.s2Body_GetLocalPoint(a, Vec2(*pb))
+            jd.localAnchorB = Vec2(*d["localAnchorB"])
+            jd.collideConnected = True
+            create = lib.s2CreateRevoluteJoint
+        jd.bodyIdA = a
+        jd.bodyIdB = b
+        sc.piles["pulley"].append(len(sc.joints))
+        sc.piles["pulley_defs"].append(d)
+        jid = create(world, C.byref(jd))
+        sc.joints.append(jid)
+        return jid
+
+    def prismatic(a, b, pivot, limit):
+        d = dict(localAnchorA=tuple(lib.s2Body_GetLocalPoint(a, pivot)), localAnchorB=tuple(lib.s2Body_GetLocalPoint(b, pivot)),
+                 localAxisA=(0.0, 1.0), referenceAngle=0.0, enableLimit=True, lowerTranslation=limit[0],
+                 upperTranslation=limit[1], enableMotor=False, motorSpeed=0.0, maxMotorForce=0.0, collideConnected=False)
+        if has_prismatic:
+            jd = capi.default_prismatic_def()
+            for name, value in d.items():
+                setattr(jd, name, Vec2(*value) if isinstance(value, tuple) else value)
+            create = lib.s2CreatePrismaticJoint
+        else:
+            jd = default_revolute_def()
+            jd.localAnchorA = Vec2(*d["localAnchorA"])
+            jd.localAnchorB = Vec2(*d["localAnchorB"])
+            create = lib.s2CreateRevoluteJoint
+        jd.bodyIdA = a
+        jd.bodyIdB = b
+        sc.piles["prismatic"].append(len(sc.joints))
+        sc.piles["prismatic_defs"].append(d)
+        sc.joints.append(create(world, C.byref(jd)))
+
+    def revolute(a, b, pivot):
+        jd = default_revolute_def()
+        jd.bodyIdA = a
+        jd.bodyIdB = b
+        jd.localAnchorA = lib.s2Body_GetLocalPoint(a, pivot)
+        jd.localAnchorB = lib.s2Body_GetLocalPoint(b, pivot)
+        sc.joints.append(lib.s2CreateRevoluteJoint(world, C.byref(jd)))
+
+    D, S, K = capi.DYNAMIC_BODY, capi.STATIC_BODY, capi.KINEMATIC_BODY
+    for k in range(copies):
+        x0 = -0.5 * PULLEYS_PITCH * (copies - 1) + PULLEYS_PITCH * k - 18.0
+        # Box2D 2.4's testbed pulley (scaled): anchors at the boxes' tops, ratio 1.5
+        a = body(D, x0 - 3.0, 5.0, hx=0.5, hy=1.0)
+        b = body(D, x0 + 3.0, 5.0, hx=0.5, hy=1.0)
+        pulley(a, b, (x0 - 3.0, 10.0), (x0 + 3.0, 10.0), (x0 - 3.0, 6.0), (x0 + 3.0, 6.0), 1.5)
+        # a counterweighted lift carrying a pile dropped onto it
+        platform = body(D, x0 + 9.0, 2.0, hx=1.2, hy=0.1)
+        prismatic(gid, platform, Vec2(x0 + 9.0, 2.0), (-1.5, 3.0))
+        weight = body(D, x0 + 12.0, 5.0, hx=0.4, hy=0.5)
+        pulley(platform, weight, (x0 + 9.0, 9.0), (x0 + 12.0, 9.0), (x0 + 9.0, 2.1), (x0 + 12.0, 5.5), 1.0)
+        for i in range(4):
+            body(D, x0 + 8.3 + 0.45 * i, 3.5 + 0.6 * i)
+        # block-and-tackle at ratio 2: balanced, then a side B 1.1 times heavier again
+        for dx, hxB in ((15.0, 0.6), (20.0, 0.66)):
+            load = body(D, x0 + dx, 5.0, hx=0.3, hy=0.3)
+            heavy = body(D, x0 + dx + 2.0, 5.0, hx=hxB, hy=0.3)
+            pulley(load, heavy, (x0 + dx, 9.0), (x0 + dx + 2.0, 9.0), (x0 + dx, 5.0), (x0 + dx + 2.0, 5.0), 2.0)
+        # a kinematic driver on side A raising the load on side B
+        if kinematic:
+            driver = body(K, x0 + 26.0, 6.0, hx=0.3, hy=0.3, vy=-0.4)
+            lifted = body(D, x0 + 28.0, 4.0, hx=0.3, hy=0.3)
+            pulley(driver, lifted, (x0 + 26.0, 10.0), (x0 + 28.0, 10.0), (x0 + 26.0, 6.3), (x0 + 28.0, 4.3), 1.5)
+        # a revolute chain
+        post = body(S, x0 + 31.0, 6.0, hx=0.1, hy=0.1)
+        prev = post
+        for i in range(3):
+            link = body(D, x0 + 31.5 + 1.0 * i, 6.0, hx=0.5, hy=0.1)
+            revolute(prev, link, Vec2(x0 + 31.0 + 1.0 * i, 6.0))
+            prev = link
+        if k == 0:
+            dragged = body(D, x0 + 36.0, 0.25)
+            md = default_mouse_def()
+            md.bodyIdA = gid
+            md.bodyIdB = dragged
+            md.target = Vec2(x0 + 36.5, 1.5)
+            md.hertz = 3.0
+            md.dampingRatio = 0.7
+            sc.joints.append(lib.s2CreateMouseJoint(world, C.byref(md)))
+    return sc
+
+
 MOTORS_PITCH = 30.0  # width of one copy of motors (m)
 
 
