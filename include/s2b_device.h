@@ -27,6 +27,13 @@ typedef struct s2bWorld s2bWorld;
 	#define S2B_API
 #endif
 
+// as solver2d/types.h defines it (an identical redefinition is allowed), for the inline helpers below
+#if defined(__CUDACC__)
+	#define S2_INLINE static inline __host__ __device__
+#else
+	#define S2_INLINE static inline
+#endif
+
 // ---- rows -----------------------------------------------------------------------------------------------------
 
 // flags shared by all rows
@@ -107,9 +114,11 @@ enum
 	S2B_JOINT_MOTOR = 4, // never carries S2B_JOINT_ENABLE_LIMIT or S2B_JOINT_ENABLE_MOTOR
 	S2B_JOINT_DISTANCE = 5,
 	S2B_JOINT_WHEEL = 6,
-	// never carries S2B_JOINT_ENABLE_LIMIT, S2B_JOINT_ENABLE_MOTOR or S2B_JOINT_ENABLE_SPRING. 7 is the last value the 3-bit
-	// type field ((flags >> 1) & 0x7) holds: a further joint type needs a wider field.
+	// never carries S2B_JOINT_ENABLE_LIMIT, S2B_JOINT_ENABLE_MOTOR or S2B_JOINT_ENABLE_SPRING
 	S2B_JOINT_PULLEY = 7,
+	// never carries S2B_JOINT_ENABLE_LIMIT, S2B_JOINT_ENABLE_MOTOR or S2B_JOINT_ENABLE_SPRING. The first type past the 3-bit
+	// field: its fourth bit is S2B_JOINT_TYPE_HIGH, so decode the type with s2bJointType
+	S2B_JOINT_GEAR = 8,
 };
 
 #define S2B_JOINT_ENABLE_LIMIT 0x10
@@ -118,6 +127,24 @@ enum
 // revolute, prismatic, distance and wheel rows only: a spring on the joint's axis (DESIGN.md §3.14, §3.16, §3.17),
 // stiffness hertz, damping dampingRatio
 #define S2B_JOINT_ENABLE_SPRING 0x80
+// (0x100 - 0x800 are the joint-constraint stream's own flags; a row never carries them)
+// the fourth bit of the joint type: (flags >> 1) & 0x7 holds the low three, so a row of types 0 - 7 reads as it always has
+#define S2B_JOINT_TYPE_HIGH 0x1000
+// gear rows only (DESIGN.md §3.19): the linked joint of side 1 / side 2 is prismatic (without the flag: revolute)
+#define S2B_JOINT_GEAR_PRISMATIC1 0x2000
+#define S2B_JOINT_GEAR_PRISMATIC2 0x4000
+
+// The joint type (S2B_JOINT_*) of a row's flags: the 3-bit field and S2B_JOINT_TYPE_HIGH
+S2_INLINE int32_t s2bJointType(int32_t flags)
+{
+	return ((flags >> 1) & 0x7) | ((flags & S2B_JOINT_TYPE_HIGH) != 0 ? 0x8 : 0);
+}
+
+// The flags that encode joint type `type` (the inverse of s2bJointType)
+S2_INLINE int32_t s2bJointTypeFlags(int32_t type)
+{
+	return ((type & 0x7) << 1) | ((type & 0x8) != 0 ? S2B_JOINT_TYPE_HIGH : 0);
+}
 
 // One joint; mirrors s2Joint / s2RevoluteJoint / s2MouseJoint (reference src/joint.h:28-102).
 typedef struct s2bJointRow
@@ -156,6 +183,11 @@ typedef struct s2bJointRow
 	// A pulley row (DESIGN.md §3.18) holds ground anchor A (world) in target, ground anchor B (world) in localAxisA, its ratio
 	// in referenceAngle and its rest lengths lengthA / lengthB in lowerAngle / upperAngle; impulse[0] is the rope impulse
 	// and every other impulse stays 0.
+	// A gear row (DESIGN.md §3.19) holds side 1's frame in target / localAxisA and side 2's in maxMotorTorque / motorSpeed /
+	// hertz / dampingRatio: a revolute side's frame rotation (s, c) and reference angle, a prismatic side's world anchor and
+	// world axis. Its local anchors are the linked joints' anchors on the geared bodies, its ratio rides in referenceAngle
+	// and its constant in lowerAngle. impulse[0] is the gear impulse and lowerImpulse / upperImpulse are the unwound
+	// coordinates of a revolute side 1 / side 2 (simulation state; 0 for a prismatic side).
 	float localAxisA[2];
 	// break thresholds (N, N-m) of the reaction pass (DESIGN.md §3.13); 0 = none. A row with either set is checked after every
 	// finalize; a row without them is never checked.

@@ -343,6 +343,40 @@ S2B_API float s2PulleyJoint_GetRatio(s2JointId jointId);
 S2B_API float s2PulleyJoint_GetCurrentLengthA(s2JointId jointId);
 S2B_API float s2PulleyJoint_GetCurrentLengthB(s2JointId jointId);
 
+// Gear joint (DESIGN.md §3.19; Box2D 2.4's b2GearJoint): couples two revolute or prismatic joints whose body A (the frame)
+// is static. The gear's body A is joint 1's body B and its body B is joint 2's body B, and it holds
+// coordinate1 + ratio coordinate2 at the value it has when created, where a revolute joint's coordinate is its angle
+// (angle(B) - angle(A) - referenceAngle, unwound: it does not wrap at +/- pi, so a gear train may turn any number of times)
+// and a prismatic joint's its translation along its axis. Turning joint 1 by d turns joint 2 by -d / ratio. The linked
+// joints keep acting on their own. s2DestroyJoint on a linked joint (a break included) destroys the gears that link it
+// first, so their ids go stale (s2DestroyJoint on a stale id does nothing); s2Body_SetTransform on a frame body moves the gear's frames with it and keeps its constant. Destroy it with
+// s2DestroyJoint.
+typedef struct s2GearJointDef
+{
+	s2JointId jointId1;
+	s2JointId jointId2;
+	float ratio; // finite; the sign sets the direction of the coupling
+	bool collideConnected;
+} s2GearJointDef;
+
+// Box2D 2.4's defaults: ratio 1, collideConnected false
+S2_INLINE struct s2GearJointDef s2DefaultGearJointDef(void)
+{
+	s2GearJointDef def = S2_ZERO_INIT;
+	def.jointId1 = s2_nullJointId;
+	def.jointId2 = s2_nullJointId;
+	def.ratio = 1.0f;
+	return def;
+}
+
+// Returns s2_nullJointId (and creates nothing) for a stale, null or foreign joint id, a joint that is not revolute or
+// prismatic, a joint whose body A is not static, two joints with the same body B, or a non-finite ratio.
+S2B_API s2JointId s2CreateGearJoint(s2WorldId worldId, const s2GearJointDef* def);
+// The getters return s2_nullJointId or 0 for a joint of another type.
+S2B_API s2JointId s2GearJoint_GetJoint1(s2JointId jointId);
+S2B_API s2JointId s2GearJoint_GetJoint2(s2JointId jointId);
+S2B_API float s2GearJoint_GetRatio(s2JointId jointId);
+
 // ---- joint reactions and breakable joints (DESIGN.md §3.13) --------------------------------------------------------
 
 // What a joint exerts on body B over the last step: force (N, world frame) and torque (N-m).
@@ -372,6 +406,8 @@ typedef struct s2JointReaction
 //   pulley     the distance branch with localAxisA = -ratio uB, uB the unit vector from ground anchor B to anchor B at the end
 //              of the step (zero within 10 s2_linearSlop), and impulse.x the rope impulse: force = rate impulse.x (-ratio uB),
 //              torque = 0
+//   gear       the generic branch: impulse = (lambda Jv2) and motorImpulse = lambda Jw2, side 2's Jacobian at the end of
+//              the step scaled by the ratio (s2cGearReaction), so force = rate lambda Jv2, torque = rate lambda Jw2
 // Every operation is a separate float32 rounding, so the host and the device (built without contraction) agree bit for bit.
 S2_INLINE s2JointReaction s2MakeJointReaction(int32_t type, s2Vec2 impulse, float motorImpulse, float lowerImpulse,
 											  float upperImpulse, s2Rot qA, s2Vec2 localAxisA, float rate)

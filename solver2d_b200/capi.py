@@ -237,6 +237,16 @@ class PulleyJointDef(C.Structure):
     ]
 
 
+class GearJointDef(C.Structure):
+    """s2GearJointDef (include/solver2d_b200.h): an extension, absent from the reference."""
+    _fields_ = [
+        ("jointId1", JointId),
+        ("jointId2", JointId),
+        ("ratio", C.c_float),
+        ("collideConnected", C.c_bool),
+    ]
+
+
 class MotorJointDef(C.Structure):
     """s2MotorJointDef (include/solver2d_b200.h): an extension, absent from the reference."""
     _fields_ = [
@@ -368,6 +378,15 @@ def default_pulley_def() -> PulleyJointDef:
     return d
 
 
+def default_gear_def() -> GearJointDef:
+    """s2DefaultGearJointDef (include/solver2d_b200.h): Box2D 2.4's defaults, ratio 1, collideConnected off."""
+    d = GearJointDef()
+    d.jointId1 = JointId(-1, -1, 0)
+    d.jointId2 = JointId(-1, -1, 0)
+    d.ratio = 1.0
+    return d
+
+
 def default_motor_def() -> MotorJointDef:
     """s2DefaultMotorJointDef (include/solver2d_b200.h)."""
     d = MotorJointDef()
@@ -483,6 +502,11 @@ _API = {
     "s2PulleyJoint_GetRatio": (C.c_float, [JointId]),
     "s2PulleyJoint_GetCurrentLengthA": (C.c_float, [JointId]),
     "s2PulleyJoint_GetCurrentLengthB": (C.c_float, [JointId]),
+    # gear joint (DESIGN.md §3.19)
+    "s2CreateGearJoint": (JointId, [WorldId, C.POINTER(GearJointDef)]),
+    "s2GearJoint_GetJoint1": (JointId, [JointId]),
+    "s2GearJoint_GetJoint2": (JointId, [JointId]),
+    "s2GearJoint_GetRatio": (C.c_float, [JointId]),
     # joint springs (DESIGN.md §3.14)
     "s2PrismaticJoint_EnableSpring": (None, [JointId, C.c_bool]),
     "s2PrismaticJoint_SetSpringHertz": (None, [JointId, C.c_float]),

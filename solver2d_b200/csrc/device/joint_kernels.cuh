@@ -7,8 +7,9 @@
 #include "contact_kernels.cuh"
 #include "shared/s2_collide.h"
 #include "shared/s2_distance_joint.h"
+#include "shared/s2_gear_joint.h"
 
-#define S2B_JOINT_TYPE(flags) (((flags) >> 1) & 0x7)
+#define S2B_JOINT_TYPE(flags) s2bJointType(flags)
 // row flags of the joint-constraint stream only (jc.head.x): an XPBD spring row's body A / B is static, so its sub-step start
 // pose is its pose (a static body's aux0 row is never written)
 #define S2B_JC_STATIC_A 0x100
@@ -122,6 +123,38 @@ template <int KIND> __device__ __forceinline__ void s2bPrepareJointRows(const So
 	jc.lim[t] = lim;
 	jc.coef[t] = make_float4(a.softJoint.bias, a.softJoint.mass, a.softJoint.impulse, 0.0f);
 
+	if (S2B_JOINT_TYPE(flags) == S2B_JOINT_GEAR)
+	{
+		// DESIGN.md §3.19: side 1's frame (the row's target) goes to d0ax and side 2's (the row's motor) to pivot, a prismatic
+		// side's world anchor pC becoming the body's start offset c - pC; lim = (constant, ratio). Each revolute side's
+		// unwound coordinate moves to the start pose in limp.xy under every variant (it is state, not an impulse). The gear
+		// impulse is kept only with the variant's warm start, and never under XPBD.
+		float4 f1 = a.joints.target[slot], f2 = a.joints.motor[slot];
+		float theta1 = 0.0f, theta2 = 0.0f;
+		if ((flags & S2B_JOINT_GEAR_PRISMATIC1) != 0)
+		{
+			f1 = make_float4(posA.x - f1.x, posA.y - f1.y, f1.z, f1.w);
+		}
+		else
+		{
+			theta1 = s2cGearRevolute(f1.x, f1.y, f1.z, limp.x, R2(poseA.z, poseA.w)).coordinate;
+		}
+		if ((flags & S2B_JOINT_GEAR_PRISMATIC2) != 0)
+		{
+			f2 = make_float4(posB.x - f2.x, posB.y - f2.y, f2.z, f2.w);
+		}
+		else
+		{
+			theta2 = s2cGearRevolute(f2.x, f2.y, f2.z, limp.y, R2(poseB.z, poseB.w)).coordinate;
+		}
+		jc.lim[t] = make_float4(lim.y, lim.x, 0.0f, 0.0f);
+		jc.d0ax[t] = f1;
+		jc.pivot[t] = f2;
+		jc.motor[t] = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
+		jc.imp[t] = make_float4(KIND != JPREP_XPBD && warmStart ? imp.x : 0.0f, 0.0f, 0.0f, 0.0f);
+		jc.limp[t] = make_float4(theta1, theta2, 0.0f, 0.0f);
+		return;
+	}
 	if (S2B_JOINT_TYPE(flags) == S2B_JOINT_PULLEY)
 	{
 		// DESIGN.md §3.18: the row's lim = (ratio, lengthA, lengthB) and target = (groundA, groundB) become lim = (constant,
@@ -1296,6 +1329,146 @@ __device__ __forceinline__ void s2bSolvePulleyPositionT(const SolveArgs& a, int 
 }
 
 // ---------------------------------------------------------------------------------------------------------------
+// gear joint (extension, DESIGN.md §3.19; definition: tests/gear_oracle.c). Couples two revolute or prismatic joints whose
+// frame bodies are static: one equality row holds C = coordinate1 + ratio coordinate2 - constant at zero, each side's
+// coordinate and Jacobian formed by s2cGearRevolute / s2cGearPrismatic from its own body's pose alone, so the per-body
+// gather can form its side's warm-start term without the other body. Row columns: lim = (constant, ratio), d0ax = side
+// 1's frame, pivot = side 2's frame (revolute: qC.s, qC.c, referenceAngle; prismatic: c - pC at the start poses, u),
+// limp.xy = the revolute sides' unwound coordinates at the start poses, imp.x = the gear impulse.
+// ---------------------------------------------------------------------------------------------------------------
+
+// one side at the body's current pose: frame and theta as the row keeps them, (lx, ly) the side's local anchor
+__device__ __forceinline__ s2cGearSide s2bGearSide(bool prismatic, float4 frame, float theta, float4 pose, float lx, float ly)
+{
+	s2Rot q = R2(pose.z, pose.w);
+	return prismatic ? s2cGearPrismatic(V2(frame.x, frame.y), V2(frame.z, frame.w), V2(pose.x, pose.y), q, V2(lx, ly))
+					 : s2cGearRevolute(frame.x, frame.y, frame.z, theta, q);
+}
+
+__device__ __forceinline__ s2cGearSide s2bGearSideOf(const SolveArgs& a, int t, bool sideB, float4 pose)
+{
+	const JointConstraintView& jc = a.jc;
+	int flags = jc.head[t].x;
+	float4 anchor = jc.anchor[t];
+	float4 limp = jc.limp[t];
+	return sideB ? s2bGearSide((flags & S2B_JOINT_GEAR_PRISMATIC2) != 0, jc.pivot[t], limp.y, pose, anchor.z, anchor.w)
+				 : s2bGearSide((flags & S2B_JOINT_GEAR_PRISMATIC1) != 0, jc.d0ax[t], limp.x, pose, anchor.x, anchor.y);
+}
+
+// what warm starting adds to one side (v += m P, w += i L): P = s Jv, L = s Jw with s = lambda on side 1 and ratio lambda
+// on side 2. Shared by the constraint-by-constraint warm start and the per-body gather, so both add the same bits.
+struct GearWarm
+{
+	s2Vec2 P;
+	float L;
+};
+
+__device__ __forceinline__ GearWarm s2bGearWarmTerm(const SolveArgs& a, int t, bool sideB)
+{
+	const JointConstraintView& jc = a.jc;
+	int4 head = jc.head[t];
+	float4 pose = a.bodies.pose[sideB ? head.z : head.y];
+	s2cGearSide side = s2bGearSideOf(a, t, sideB, pose);
+	float lambda = jc.imp[t].x;
+	float s = sideB ? jc.lim[t].y * lambda : lambda;
+	GearWarm w;
+	w.P = s2MulSV(s, side.Jv);
+	w.L = s * side.Jw;
+	return w;
+}
+
+// the constraint-by-constraint warm start: each side's term from s2bGearWarmTerm
+__device__ __forceinline__ void s2bWarmStartGear(const SolveArgs& a, int t)
+{
+	int4 head = a.jc.head[t];
+	int ia = head.y, ib = head.z;
+	float4 mass = a.jc.mass[t];
+	float4 velA = a.bodies.vel[ia], velB = a.bodies.vel[ib];
+	float mA = mass.x, iA = mass.y, mB = mass.z, iB = mass.w;
+	GearWarm wa = s2bGearWarmTerm(a, t, false);
+	GearWarm wb = s2bGearWarmTerm(a, t, true);
+	s2Vec2 vA = s2MulAdd(V2(velA.x, velA.y), mA, wa.P);
+	float wA = velA.z + iA * wa.L;
+	s2Vec2 vB = s2MulAdd(V2(velB.x, velB.y), mB, wb.P);
+	float wB = velB.z + iB * wb.L;
+	s2bStoreJointVelocities(a, ia, ib, velA, velB, vA, wA, vB, wB, mA, iA, mB, iB);
+}
+
+// the velocity row in each flavour: soft bias in the biased pass, Baumgarte in every pass, none under the rigid flavour
+template <int KIND>
+__device__ __forceinline__ void s2bSolveGearVelocity(const SolveArgs& a, int t, float h, float inv_h, bool useBias)
+{
+	const JointConstraintView& jc = a.jc;
+	int4 head = jc.head[t];
+	int ia = head.y, ib = head.z;
+	float4 mass = jc.mass[t];
+	float4 lim = jc.lim[t];
+	float4 imp = jc.imp[t];
+	float4 velA = a.bodies.vel[ia], velB = a.bodies.vel[ib];
+	s2cGearSide A = s2bGearSideOf(a, t, false, a.bodies.pose[ia]);
+	s2cGearSide B = s2bGearSideOf(a, t, true, a.bodies.pose[ib]);
+	s2Vec2 vA = V2(velA.x, velA.y), vB = V2(velB.x, velB.y);
+	float wA = velA.z, wB = velB.z;
+	float mA = mass.x, iA = mass.y, mB = mass.z, iB = mass.w;
+	float ratio = lim.y;
+	float kInv = s2cGearSideMass(A, mA, iA) + ratio * ratio * s2cGearSideMass(B, mB, iB);
+	float k = kInv > 0.0f ? 1.0f / kInv : 0.0f;
+
+	float3 s = s2bPrismaticBias<KIND>(A.coordinate + ratio * B.coordinate - lim.x, false, jc.coef[t], h, inv_h, useBias);
+	float Cdot = (s2Dot(A.Jv, vA) + A.Jw * wA) + ratio * (s2Dot(B.Jv, vB) + B.Jw * wB);
+	float impulse = -k * s.y * (Cdot + s.x) - s.z * imp.x;
+	imp.x += impulse;
+	float impulseB = ratio * impulse;
+	vA = s2MulAdd(vA, mA, s2MulSV(impulse, A.Jv));
+	wA += iA * (impulse * A.Jw);
+	vB = s2MulAdd(vB, mB, s2MulSV(impulseB, B.Jv));
+	wB += iB * (impulseB * B.Jw);
+
+	jc.imp[t] = imp;
+	s2bStoreJointVelocities(a, ia, ib, velA, velB, vA, wA, vB, wB, mA, iA, mB, iB);
+}
+
+// one position correction of the row on the given poses: impulse = -k C with C clamped in side 1's units (NGS: Box2D 2.4's
+// gear correction) or -C / (1 / k) (XPBD at zero compliance, skipped when 1 / k is 0)
+template <bool XPBD>
+__device__ __forceinline__ void s2bSolveGearPositionT(const SolveArgs& a, int t)
+{
+	const JointConstraintView& jc = a.jc;
+	int4 head = jc.head[t];
+	int ia = head.y, ib = head.z;
+	float4 mass = jc.mass[t];
+	float4 lim = jc.lim[t];
+	float4 poseA = a.bodies.pose[ia], poseB = a.bodies.pose[ib];
+	s2cGearSide A = s2bGearSideOf(a, t, false, poseA);
+	s2cGearSide B = s2bGearSideOf(a, t, true, poseB);
+	s2Vec2 dcA = V2(poseA.x, poseA.y), dcB = V2(poseB.x, poseB.y);
+	s2Rot qA = R2(poseA.z, poseA.w), qB = R2(poseB.z, poseB.w);
+	float mA = mass.x, iA = mass.y, mB = mass.z, iB = mass.w;
+	float ratio = lim.y;
+	float kInv = s2cGearSideMass(A, mA, iA) + ratio * ratio * s2cGearSideMass(B, mB, iB);
+	float C = A.coordinate + ratio * B.coordinate - lim.x;
+	if (XPBD && (kInv > 0.0f) == false)
+	{
+		return;
+	}
+	float maxC = (head.x & S2B_JOINT_GEAR_PRISMATIC1) != 0 ? s2_maxLinearCorrection : s2_maxAngularCorrection;
+	float impulse = XPBD ? -C / kInv : -(kInv > 0.0f ? 1.0f / kInv : 0.0f) * S2_CLAMP(C, -maxC, maxC);
+	float impulseB = ratio * impulse;
+	dcA = s2MulAdd(dcA, mA, s2MulSV(impulse, A.Jv));
+	qA = s2IntegrateRot(qA, iA * (impulse * A.Jw));
+	dcB = s2MulAdd(dcB, mB, s2MulSV(impulseB, B.Jv));
+	qB = s2IntegrateRot(qB, iB * (impulseB * B.Jw));
+	if ((mA != 0.0f) || (iA != 0.0f))
+	{
+		a.bodies.pose[ia] = make_float4(dcA.x, dcA.y, qA.s, qA.c);
+	}
+	if ((mB != 0.0f) || (iB != 0.0f))
+	{
+		a.bodies.pose[ib] = make_float4(dcB.x, dcB.y, qB.s, qB.c);
+	}
+}
+
+// ---------------------------------------------------------------------------------------------------------------
 // motor joint (extension, DESIGN.md §3.10; definition: tests/motor_oracle.c). Drives body B toward a pose relative to body
 // A with capped effort: an angular row toward angle(B) - angle(A) = angularOffset, its accumulated impulse clamped to
 // +/- h maxTorque, then a point row that takes B's origin to the linear offset in A's frame, its accumulated impulse scaled
@@ -1628,6 +1801,11 @@ __device__ __forceinline__ void s2bWarmStartJoint(const SolveArgs& a, int t)
 		return;
 	}
 
+	if (S2B_JOINT_TYPE(head.x) == S2B_JOINT_GEAR)
+	{
+		s2bWarmStartGear(a, t);
+		return;
+	}
 	if (S2B_JOINT_TYPE(head.x) == S2B_JOINT_PULLEY)
 	{
 		float4 velA = a.bodies.vel[ia], velB = a.bodies.vel[ib];
@@ -2289,6 +2467,11 @@ __device__ __forceinline__ void s2bSolveJointSoft(const SolveArgs& a, int t, flo
 		s2bSolveWheelVelocity<PSOLVE_SOFT>(a, t, h, inv_h, useBias);
 		return;
 	}
+	if (S2B_JOINT_TYPE(flags) == S2B_JOINT_GEAR)
+	{
+		s2bSolveGearVelocity<PSOLVE_SOFT>(a, t, h, inv_h, useBias);
+		return;
+	}
 	if (S2B_JOINT_TYPE(flags) == S2B_JOINT_PULLEY)
 	{
 		s2bSolvePulleyVelocity<PSOLVE_SOFT>(a, t, h, inv_h, useBias);
@@ -2329,6 +2512,11 @@ __device__ __forceinline__ void s2bSolveJointBaumgarte(const SolveArgs& a, int t
 	if (S2B_JOINT_TYPE(flags) == S2B_JOINT_WHEEL)
 	{
 		s2bSolveWheelVelocity<PSOLVE_BAUMGARTE>(a, t, h, inv_h, useBias);
+		return;
+	}
+	if (S2B_JOINT_TYPE(flags) == S2B_JOINT_GEAR)
+	{
+		s2bSolveGearVelocity<PSOLVE_BAUMGARTE>(a, t, h, inv_h, useBias);
 		return;
 	}
 	if (S2B_JOINT_TYPE(flags) == S2B_JOINT_PULLEY)
@@ -2468,6 +2656,11 @@ __device__ __forceinline__ void s2bSolveJointRigid(const SolveArgs& a, int t, fl
 		s2bSolveWheelVelocity<PSOLVE_RIGID>(a, t, h, 0.0f /* inv_h: unused by the rigid rows */, false);
 		return;
 	}
+	if (S2B_JOINT_TYPE(a.jc.head[t].x) == S2B_JOINT_GEAR)
+	{
+		s2bSolveGearVelocity<PSOLVE_RIGID>(a, t, h, 0.0f /* inv_h: unused by the rigid row */, false);
+		return;
+	}
 	if (S2B_JOINT_TYPE(a.jc.head[t].x) == S2B_JOINT_PULLEY)
 	{
 		s2bSolvePulleyVelocity<PSOLVE_RIGID>(a, t, h, 0.0f /* inv_h: unused by the rigid row */, false);
@@ -2511,6 +2704,11 @@ __device__ __forceinline__ void s2bSolveJointPosition(const SolveArgs& a, int t)
 	if (S2B_JOINT_TYPE(head.x) == S2B_JOINT_WHEEL)
 	{
 		s2bSolveWheelPosition(a, t);
+		return;
+	}
+	if (S2B_JOINT_TYPE(head.x) == S2B_JOINT_GEAR)
+	{
+		s2bSolveGearPositionT<false>(a, t);
 		return;
 	}
 	if (S2B_JOINT_TYPE(head.x) == S2B_JOINT_PULLEY)
@@ -2620,6 +2818,11 @@ __device__ __forceinline__ void s2bSolveJointXpbd(const SolveArgs& a, int t)
 	if (S2B_JOINT_TYPE(head.x) == S2B_JOINT_WHEEL)
 	{
 		s2bSolveWheelXpbd(a, t);
+		return;
+	}
+	if (S2B_JOINT_TYPE(head.x) == S2B_JOINT_GEAR)
+	{
+		s2bSolveGearPositionT<true>(a, t);
 		return;
 	}
 	if (S2B_JOINT_TYPE(head.x) == S2B_JOINT_PULLEY)

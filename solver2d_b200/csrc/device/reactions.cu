@@ -2,12 +2,14 @@
 //
 // One thread per joint slot evaluates s2MakeJointReaction (include/solver2d_b200.h) on the impulses the last solve stored,
 // body A's final rotation (a distance joint: the line between its anchors at both bodies' final poses; a pulley: -ratio times
-// rope B's direction at body B's final pose) and the rate of that
+// rope B's direction at body B's final pose; a gear: its impulse times side 2's Jacobian at body B's final pose) and the rate
+// of that
 // solve. After finalize (s2bFinalize) it compares the reaction with the
 // slot's thresholds and appends the slots over one to a list; on demand (s2b_download_joint_reactions) it writes the
 // reactions instead. The solver kernels are not touched: everything it reads is already in the joint and body columns.
 #include "s2b_internal.cuh"
 #include "shared/s2_distance_joint.h"
+#include "shared/s2_gear_joint.h"
 #include "solver2d_b200.h"
 
 #include <algorithm>
@@ -46,7 +48,7 @@ __global__ void s2bJointReactionKernel(JointView j, const float2* __restrict__ b
 	s2Rot qA = {qa.z, qa.w};
 	// a spring acts on the motor's axis: its impulse joins the motor argument (DESIGN.md §3.14)
 	float motorImpulse = (head.x & S2B_JOINT_ENABLE_SPRING) != 0 ? imp.z + imp.w : imp.z;
-	int type = (head.x >> 1) & 0x7;
+	int type = s2bJointType(head.x);
 	s2Vec2 axis = s2MakeVec2(target.z, target.w);
 	if (type == S2B_JOINT_DISTANCE)
 	{
@@ -66,6 +68,23 @@ __global__ void s2bJointReactionKernel(JointView j, const float2* __restrict__ b
 		float length;
 		axis = s2cPulleyJointAxis(&length, axis, s2MakeVec2(pb.x, pb.y), s2Rot{qb.z, qb.w},
 								  s2Sub(s2MakeVec2(anchors.z, anchors.w), s2MakeVec2(ob.z, ob.w)), j.lim[i].x);
+	}
+	else if (type == S2B_JOINT_GEAR)
+	{
+		// (lambda Jv2, lambda Jw2) at the end of the step through the generic branch (DESIGN.md §3.19): side 2's frame rides
+		// in motor, the ratio in lim.x. Only the Jacobian is read, so the revolute side's coordinate is formed at theta 0.
+		float4 anchors = j.anchors[i], frame = j.motor[i];
+		float4 pb = pos[head.z], qb = pose[head.z], ob = org[head.z];
+		s2Rot qB = {qb.z, qb.w};
+		s2cGearSide side2 = (head.x & S2B_JOINT_GEAR_PRISMATIC2) != 0
+								? s2cGearPrismatic(s2Sub(s2MakeVec2(pb.x, pb.y), s2MakeVec2(frame.x, frame.y)), s2MakeVec2(frame.z, frame.w),
+												   s2MakeVec2(0.0f, 0.0f), qB, s2Sub(s2MakeVec2(anchors.z, anchors.w), s2MakeVec2(ob.z, ob.w)))
+								: s2cGearRevolute(frame.x, frame.y, frame.z, 0.0f, qB);
+		float angular;
+		s2Vec2 linear = s2cGearReaction(&angular, imp.x, j.lim[i].x, side2);
+		imp = make_float4(linear.x, linear.y, 0.0f, 0.0f);
+		motorImpulse = angular;
+		limp = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
 	}
 	s2JointReaction r = s2MakeJointReaction(type, s2MakeVec2(imp.x, imp.y), motorImpulse, limp.x, limp.y, qA, axis, rate);
 	if (reactions != nullptr)

@@ -215,7 +215,7 @@ __global__ void s2bItemEndpoints(int* counts, const int* jointSlots, const int* 
 		int4 head = joints.head[jointSlots[i]];
 		a = head.y;
 		b = head.z;
-		if (((head.x >> 1) & 0x7) == S2B_JOINT_MOUSE)
+		if (s2bJointType(head.x) == S2B_JOINT_MOUSE)
 		{
 			a = -1; // the mouse joint only acts on body B
 		}

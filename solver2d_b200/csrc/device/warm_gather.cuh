@@ -91,6 +91,13 @@ __device__ __forceinline__ GatherTerms s2bGatherTermsOf(const SolveArgs& a, int 
 			g.tv0 = sideB ? mp : V2(-mp.x, -mp.y);
 			g.tw0 = sideB ? invI * pw.LB : -(invI * pw.LA);
 		}
+		else if (S2B_JOINT_TYPE(head.x) == S2B_JOINT_GEAR)
+		{
+			// each side's term depends on its own body's pose only (DESIGN.md §3.19)
+			GearWarm gw = s2bGearWarmTerm(a, t, sideB);
+			g.tv0 = s2MulSV(invMass, gw.P);
+			g.tw0 = invI * gw.L;
+		}
 		else if (S2B_JOINT_TYPE(head.x) == S2B_JOINT_PULLEY)
 		{
 			// each side's term depends on its own body's pose only (DESIGN.md §3.18)

@@ -930,7 +930,7 @@ __global__ void s2bSetMotorOffsetsKernel(const int* __restrict__ indices, const 
 		return;
 	}
 	int flags = j.head[i].x;
-	if ((flags & S2B_ROW_VALID) == 0 || ((flags >> 1) & 0x7) != S2B_JOINT_MOTOR)
+	if ((flags & S2B_ROW_VALID) == 0 || s2bJointType(flags) != S2B_JOINT_MOTOR)
 	{
 		return;
 	}

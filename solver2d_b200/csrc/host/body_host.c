@@ -384,6 +384,7 @@ void s2Body_SetTransform(s2BodyId bodyId, s2Vec2 position, float angle)
 	// the body is placed exactly where asked: the delta position XPBD carries for a kinematic body goes (DESIGN.md §3.8)
 	body->teleported = true;
 	s2MarkBodyDirty(world, body);
+	s2MoveGearFrames(world, bodyId.index);
 	s2Transform xf = {body->origin, body->rot};
 	for (int32_t si = body->shapeList; si != S2_NULL_INDEX;)
 	{

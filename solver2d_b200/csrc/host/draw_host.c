@@ -98,6 +98,16 @@ static void s2DrawJoint(s2DebugDraw* draw, s2World* world, const s2Joint* joint)
 		return;
 	}
 
+	if (joint->type == s2_gearJoint)
+	{
+		// Box2D 2.4's default joint lines: each body's origin to its anchor, and anchor A to anchor B
+		s2Color color = s2Rgb(0.5f, 0.8f, 0.8f);
+		draw->DrawSegment(xfA.p, pA, color, draw->context);
+		draw->DrawSegment(pA, pB, color, draw->context);
+		draw->DrawSegment(xfB.p, pB, color, draw->context);
+		return;
+	}
+
 	if (joint->type == s2_distanceJoint)
 	{
 		// the segment between the anchors and, with the limit on, a mark across the line at minLength and at maxLength from

@@ -2,6 +2,7 @@
 // src/mouse_joint.c:18-29). Host bookkeeping only: the joint solvers run on the device.
 #include "s2_host.h"
 #include "shared/s2_distance_joint.h"
+#include "shared/s2_gear_joint.h"
 #include "solver2d_b200.h"
 
 #include <float.h>
@@ -119,9 +120,34 @@ void s2DestroyJoint(s2JointId jointId)
 	s2World* world = s2GetWorldFromIndex(jointId.world);
 	s2FetchBrokenJoints(world); // (the slot may be one the last step broke)
 	s2Joint* joint = world->joints + jointId.index;
+	if (jointId.index < 0 || jointId.index >= world->jointPool.capacity || s2ObjectValid(&joint->object) == false ||
+		joint->object.revision != jointId.revision)
+	{
+		// a stale id, such as a gear that the destruction of a joint it links already took (DESIGN.md §3.19): nothing to do
+		return;
+	}
 	if (joint->breakForce > 0.0f || joint->breakTorque > 0.0f)
 	{
 		world->breakableCount -= 1;
+	}
+	if (world->gearCount > 0 && joint->type != s2_gearJoint)
+	{
+		// the gears that link this joint go first (DESIGN.md §3.19)
+		for (int32_t i = 0; i < world->jointPool.capacity; ++i)
+		{
+			const s2Joint* gear = world->joints + i;
+			if (s2ObjectValid(&gear->object) && gear->type == s2_gearJoint &&
+				((gear->gearJoint1.index == jointId.index && gear->gearJoint1.revision == jointId.revision) ||
+				 (gear->gearJoint2.index == jointId.index && gear->gearJoint2.revision == jointId.revision)))
+			{
+				s2JointId gearId = {i, world->index, gear->object.revision};
+				s2DestroyJoint(gearId);
+			}
+		}
+	}
+	if (joint->type == s2_gearJoint)
+	{
+		world->gearCount -= 1;
 	}
 	world->bodies[joint->bodyIndexA].jointCount -= 1;
 	world->bodies[joint->bodyIndexB].jointCount -= 1;
@@ -1018,13 +1044,176 @@ float s2PulleyJoint_GetCurrentLengthB(s2JointId jointId)
 	return s2PulleyJointCurrentLength(jointId, true);
 }
 
+// ---- gear joint (DESIGN.md §3.19) ----------------------------------------------------------------------------------------
+
+// the live joint `jointId` names in `world`, or NULL for a stale, null or foreign id
+static s2Joint* s2FindJoint(s2World* world, s2JointId jointId)
+{
+	if (jointId.world != world->index || jointId.index < 0 || jointId.index >= world->jointPool.capacity)
+	{
+		return NULL;
+	}
+	s2Joint* joint = world->joints + jointId.index;
+	return s2ObjectValid(&joint->object) && joint->object.revision == jointId.revision ? joint : NULL;
+}
+
+// a linked joint's frame in the four row lanes of its side: a revolute joint's frame rotation (s, c) and reference angle, a
+// prismatic joint's world anchor and world axis
+static void s2GearFrame(const s2World* world, const s2Joint* link, float frame[4])
+{
+	const s2Body* body = world->bodies + link->bodyIndexA;
+	if (link->type == s2_prismaticJoint)
+	{
+		s2Vec2 p = s2Add(body->origin, s2RotateVector(body->rot, link->localOriginAnchorA));
+		s2Vec2 u = s2RotateVector(body->rot, link->localAxisA);
+		frame[0] = p.x;
+		frame[1] = p.y;
+		frame[2] = u.x;
+		frame[3] = u.y;
+	}
+	else
+	{
+		frame[0] = body->rot.s;
+		frame[1] = body->rot.c;
+		frame[2] = link->referenceAngle;
+		frame[3] = 0.0f;
+	}
+}
+
+static void s2SetGearFrames(s2World* world, s2Joint* gear)
+{
+	float f1[4], f2[4];
+	s2GearFrame(world, world->joints + gear->gearJoint1.index, f1);
+	s2GearFrame(world, world->joints + gear->gearJoint2.index, f2);
+	gear->targetA = s2MakeVec2(f1[0], f1[1]);
+	gear->localAxisA = s2MakeVec2(f1[2], f1[3]);
+	gear->maxMotorTorque = f2[0];
+	gear->motorSpeed = f2[1];
+	gear->hertz = f2[2];
+	gear->dampingRatio = f2[3];
+}
+
+// one side at the host's body state; a revolute side is unwound from its stored coordinate
+static s2cGearSide s2GearSideAt(const s2World* world, const s2Joint* gear, bool side2)
+{
+	const s2Body* body = world->bodies + (side2 ? gear->bodyIndexB : gear->bodyIndexA);
+	s2Vec2 local = s2Sub(side2 ? gear->localOriginAnchorB : gear->localOriginAnchorA, body->localCenter);
+	float f[4] = {gear->targetA.x, gear->targetA.y, gear->localAxisA.x, gear->localAxisA.y};
+	if (side2)
+	{
+		f[0] = gear->maxMotorTorque;
+		f[1] = gear->motorSpeed;
+		f[2] = gear->hertz;
+		f[3] = gear->dampingRatio;
+	}
+	if (side2 ? gear->gearPrismatic2 : gear->gearPrismatic1)
+	{
+		return s2cGearPrismatic(s2Sub(body->position, s2MakeVec2(f[0], f[1])), s2MakeVec2(f[2], f[3]), s2Vec2_zero, body->rot,
+								local);
+	}
+	return s2cGearRevolute(f[0], f[1], f[2], side2 ? gear->upperImpulse : gear->lowerImpulse, body->rot);
+}
+
+static bool s2IsGearInput(const s2World* world, const s2Joint* joint)
+{
+	return joint != NULL && (joint->type == s2_revoluteJoint || joint->type == s2_prismaticJoint) &&
+		   world->bodies[joint->bodyIndexA].type == s2_staticBody;
+}
+
+// The gear joint has no counterpart in the reference. Invalid input creates nothing and returns s2_nullJointId.
+s2JointId s2CreateGearJoint(s2WorldId worldId, const s2GearJointDef* def)
+{
+	s2World* world = s2GetWorldFromId(worldId);
+	s2Joint* joint1 = s2FindJoint(world, def->jointId1);
+	s2Joint* joint2 = s2FindJoint(world, def->jointId2);
+	if (s2IsGearInput(world, joint1) == false || s2IsGearInput(world, joint2) == false ||
+		joint1->bodyIndexB == joint2->bodyIndexB || s2IsValid(def->ratio) == false)
+	{
+		return s2_nullJointId;
+	}
+
+	// the constant is taken at the current poses
+	s2SyncStateToHost(world);
+	s2Joint* joint = s2AllocJoint(world, world->bodies + joint1->bodyIndexB, world->bodies + joint2->bodyIndexB);
+	// (the allocation may have moved the joint array)
+	joint1 = world->joints + def->jointId1.index;
+	joint2 = world->joints + def->jointId2.index;
+	joint->type = s2_gearJoint;
+	joint->drawSize = 1.0f;
+	joint->localOriginAnchorA = joint1->localOriginAnchorB;
+	joint->localOriginAnchorB = joint2->localOriginAnchorB;
+	joint->gearJoint1 = def->jointId1;
+	joint->gearJoint2 = def->jointId2;
+	joint->gearPrismatic1 = joint1->type == s2_prismaticJoint;
+	joint->gearPrismatic2 = joint2->type == s2_prismaticJoint;
+	joint->referenceAngle = def->ratio;
+	joint->collideConnected = def->collideConnected;
+	s2SetGearFrames(world, joint);
+	s2cGearSide side1 = s2GearSideAt(world, joint, false);
+	s2cGearSide side2 = s2GearSideAt(world, joint, true);
+	joint->lowerImpulse = joint->gearPrismatic1 ? 0.0f : side1.coordinate;
+	joint->upperImpulse = joint->gearPrismatic2 ? 0.0f : side2.coordinate;
+	joint->lowerAngle = side1.coordinate + def->ratio * side2.coordinate;
+	world->gearCount += 1;
+
+	s2JointId jointId = {joint->object.index, world->index, joint->object.revision};
+	return jointId;
+}
+
+void s2MoveGearFrames(s2World* world, int32_t bodyIndex)
+{
+	if (world->gearCount == 0 || world->bodies[bodyIndex].type != s2_staticBody)
+	{
+		return;
+	}
+	for (int32_t i = 0; i < world->jointPool.capacity; ++i)
+	{
+		s2Joint* gear = world->joints + i;
+		if (s2ObjectValid(&gear->object) && gear->type == s2_gearJoint &&
+			(world->joints[gear->gearJoint1.index].bodyIndexA == bodyIndex ||
+			 world->joints[gear->gearJoint2.index].bodyIndexA == bodyIndex))
+		{
+			s2SetGearFrames(world, gear);
+			s2MarkJointDirty(world, gear);
+		}
+	}
+}
+
+// the joint, or NULL for a joint of another type
+static const s2Joint* s2GetGearJoint(s2JointId jointId)
+{
+	s2World* world = s2GetWorldFromIndex(jointId.world);
+	const s2Joint* joint = world->joints + jointId.index;
+	S2_ASSERT(s2ObjectValid(&joint->object) && joint->object.revision == jointId.revision);
+	return joint->type == s2_gearJoint ? joint : NULL;
+}
+
+s2JointId s2GearJoint_GetJoint1(s2JointId jointId)
+{
+	const s2Joint* joint = s2GetGearJoint(jointId);
+	return joint != NULL ? joint->gearJoint1 : s2_nullJointId;
+}
+
+s2JointId s2GearJoint_GetJoint2(s2JointId jointId)
+{
+	const s2Joint* joint = s2GetGearJoint(jointId);
+	return joint != NULL ? joint->gearJoint2 : s2_nullJointId;
+}
+
+float s2GearJoint_GetRatio(s2JointId jointId)
+{
+	const s2Joint* joint = s2GetGearJoint(jointId);
+	return joint != NULL ? joint->referenceAngle : 0.0f;
+}
+
 // ---- reactions and break thresholds (DESIGN.md §3.13) -----------------------------------------------------------------
 
 // s2JointType and the device's S2B_JOINT_* number the joint types alike
 _Static_assert((int)s2_revoluteJoint == S2B_JOINT_REVOLUTE && (int)s2_mouseJoint == S2B_JOINT_MOUSE &&
 				   (int)s2_weldJoint == S2B_JOINT_WELD && (int)s2_prismaticJoint == S2B_JOINT_PRISMATIC &&
 				   (int)s2_motorJoint == S2B_JOINT_MOTOR && (int)s2_distanceJoint == S2B_JOINT_DISTANCE &&
-				   (int)s2_wheelJoint == S2B_JOINT_WHEEL && (int)s2_pulleyJoint == S2B_JOINT_PULLEY,
+				   (int)s2_wheelJoint == S2B_JOINT_WHEEL && (int)s2_pulleyJoint == S2B_JOINT_PULLEY &&
+				   (int)s2_gearJoint == S2B_JOINT_GEAR,
 			   "joint type numbering");
 
 s2JointReaction s2ComputeJointReaction(int32_t type, s2Vec2 impulse, float motorImpulse, float lowerImpulse, float upperImpulse,
@@ -1043,6 +1232,14 @@ static s2JointReaction s2GetJointReaction(s2JointId jointId)
 	// a spring acts on the motor's axis: its impulse joins the motor argument (DESIGN.md §3.14). The flag is the one of the
 	// row the device last solved, so the getters read what the device's reaction and break pass read for that step even
 	// after s2*Joint_EnableSpring has changed the joint and before the next step uploads it.
+	if (joint->type == s2_gearJoint)
+	{
+		// (lambda Jv2, lambda Jw2) through the generic branch, as the device's pass forms them (DESIGN.md §3.19)
+		float angular;
+		s2Vec2 linear = s2cGearReaction(&angular, joint->impulse.x, joint->referenceAngle, s2GearSideAt(world, joint, true));
+		return s2MakeJointReaction(S2B_JOINT_GEAR, linear, angular, 0.0f, 0.0f, world->bodies[joint->bodyIndexA].rot,
+								   s2Vec2_zero, world->reactionRate);
+	}
 	float motorImpulse = joint->springUploaded ? joint->motorImpulse + joint->springImpulse : joint->motorImpulse;
 	// a distance joint passes its world axis at the end of the step (DESIGN.md §3.16), a pulley -ratio uB (§3.18)
 	float length;

@@ -91,6 +91,7 @@ typedef enum s2JointType
 	s2_distanceJoint,
 	s2_wheelJoint,
 	s2_pulleyJoint,
+	s2_gearJoint,
 } s2JointType;
 
 typedef struct s2Body
@@ -195,6 +196,11 @@ typedef struct s2Joint
 	float motorImpulse, lowerImpulse, upperImpulse, springImpulse;
 	// break thresholds (s2Joint_SetBreakForce / _SetBreakTorque), 0 = none
 	float breakForce, breakTorque;
+	// gear (DESIGN.md §3.19): the linked joints and which of them is prismatic. Side 1's frame is in targetA / localAxisA,
+	// side 2's in maxMotorTorque / motorSpeed / hertz / dampingRatio, the ratio in referenceAngle, the constant in lowerAngle
+	// and the revolute sides' unwound coordinates in lowerImpulse / upperImpulse, as the device row has them.
+	s2JointId gearJoint1, gearJoint2;
+	bool gearPrismatic1, gearPrismatic2;
 
 	bool rowDirty;
 } s2Joint;
@@ -243,6 +249,8 @@ typedef struct s2World
 	// a threshold, and the joints the last step's reaction pass found over one, fetched once per step (s2FetchBrokenJoints)
 	float reactionRate;
 	int32_t breakableCount;
+	// live gear joints: destroying a joint or moving a static body looks for the gears it affects only when there are any
+	int32_t gearCount;
 	bool brokenPending; // the last step ran the reaction pass and its list has not been fetched yet
 	s2JointId* broken;
 	int32_t* brokenSlots; // the device's list, read into this buffer (brokenCapacity entries, as broken)
@@ -289,6 +297,8 @@ void s2MarkJointDirty(s2World* world, s2Joint* joint);
 // the ids of the joints the last step broke, read from the device while they still name those joints: before any slot is
 // freed or reused, and before the next step destroys them
 void s2FetchBrokenJoints(s2World* world);
+// s2Body_SetTransform on a static body: the gears whose linked joints hang off it take their frames from its new pose
+void s2MoveGearFrames(s2World* world, int32_t bodyIndex);
 void s2IndexListPush(s2IndexList* list, int32_t value);
 
 int32_t s2AllocProxyId(s2ProxyIds* ids);

@@ -250,10 +250,15 @@ static void s2FillJointRow(s2bJointRow* r, const s2Joint* j)
 		case s2_pulleyJoint:
 			type = S2B_JOINT_PULLEY;
 			break;
+		case s2_gearJoint:
+			type = S2B_JOINT_GEAR;
+			break;
 	}
-	r->flags = S2B_ROW_VALID | (type << 1);
-	// welds, motor joints and pulleys are created with enableLimit == enableMotor == false, so their rows never carry either
-	// flag
+	r->flags = S2B_ROW_VALID | s2bJointTypeFlags(type);
+	r->flags |= j->type == s2_gearJoint && j->gearPrismatic1 ? S2B_JOINT_GEAR_PRISMATIC1 : 0;
+	r->flags |= j->type == s2_gearJoint && j->gearPrismatic2 ? S2B_JOINT_GEAR_PRISMATIC2 : 0;
+	// welds, motor joints, pulleys and gears are created with enableLimit == enableMotor == false, so their rows never carry
+	// either flag
 	r->flags |= j->enableLimit ? S2B_JOINT_ENABLE_LIMIT : 0;
 	r->flags |= j->enableMotor ? S2B_JOINT_ENABLE_MOTOR : 0;
 	r->flags |= j->collideConnected ? S2B_JOINT_COLLIDE_CONNECTED : 0;

@@ -83,6 +83,20 @@ JOINT_ENABLE_LIMIT, JOINT_ENABLE_MOTOR, JOINT_COLLIDE_CONNECTED, JOINT_ENABLE_SP
 # upperAngle, and fills the 3-bit type field)
 JOINT_REVOLUTE, JOINT_MOUSE, JOINT_WELD, JOINT_PRISMATIC, JOINT_MOTOR, JOINT_DISTANCE, JOINT_WHEEL, JOINT_PULLEY = \
     0, 1, 2, 3, 4, 5, 6, 7
+# a gear row (DESIGN.md §3.19) is the first type past the 3-bit field: its fourth bit is JOINT_TYPE_HIGH, so read a row's
+# type with joint_type. JOINT_GEAR_PRISMATIC1 / 2 mark a prismatic side 1 / 2.
+JOINT_GEAR = 8
+JOINT_TYPE_HIGH, JOINT_GEAR_PRISMATIC1, JOINT_GEAR_PRISMATIC2 = 0x1000, 0x2000, 0x4000
+
+
+def joint_type(flags):
+    """s2bJointType (include/s2b_device.h): the joint type of row flags (an int or a numpy array)."""
+    return ((flags >> 1) & 0x7) | ((flags & JOINT_TYPE_HIGH) != 0) * 0x8
+
+
+def joint_type_flags(kind: int) -> int:
+    """s2bJointTypeFlags (include/s2b_device.h): the flags that encode joint type `kind`."""
+    return ((kind & 0x7) << 1) | (JOINT_TYPE_HIGH if kind & 0x8 else 0)
 
 # symbols declared in include/s2b_device.h (checked by the CPU test-suite against the built library)
 ABI_SYMBOLS = [

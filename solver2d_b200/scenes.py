@@ -1528,6 +1528,143 @@ def pulleys(lib: capi.Solver2D, solver="TGS_Soft", copies=1, kinematic=True, sta
     return sc
 
 
+GEARS_PITCH = 60.0  # width of one copy of gears (m)
+GEARS_HUB_PLANETS = 52  # planets on the first copy's sun: more than S2B_HUB_DEGREE (48)
+
+
+def gears(lib: capi.Solver2D, solver="TGS_Soft", copies=1, stand_ins=None, hub=True) -> Scene:
+    """Gear joint coverage (DESIGN.md §3.19), `copies` side by side. Per copy:
+
+    * Box2D 2.4's testbed Gears: two wheels (radius 1 and 2) on revolute joints geared at r2 / r1 = 2, and a rack on a
+      vertical prismatic joint geared to the second wheel at -1 / r2;
+    * a gear train of four wheels (three stages, ratios 1.5, -0.75, 1.5) driven by a motor on the first wheel's joint;
+    * a rack and pinion lifting a pile: a motorised pinion geared to a platform on a vertical prismatic joint, with boxes
+      dropped onto the platform, so contacts share a geared body;
+    * a wheel spun at 150 rad/s geared at ratio 1 to another, so both turn through more than ten turns in 90 steps;
+    * with `hub` (first copy only): a sun geared to GEARS_HUB_PLANETS planets at ratio 10, more than S2B_HUB_DEGREE.
+
+    Every linked joint hangs off the static ground; every gear keeps s2DefaultGearJointDef's collideConnected = false. On
+    a library without s2CreateGearJoint (the reference), or with `stand_ins` true, every gear is created as a revolute joint
+    between its two bodies at body B's origin, with collideConnected false; on a library without s2CreatePrismaticJoint
+    the racks' prismatic joints are such stand-ins too. ``sc.piles["gear"]`` lists the index into ``sc.joints`` of every gear
+    and ``sc.piles["prismatic"]`` / ``["prismatic_defs"]`` describe the prismatic joints as ``sliders`` does, so that a test
+    can turn the stand-in rows into gear and prismatic rows."""
+    world = lib.create_world(solver)
+    sc = Scene(lib, world, name=f"gears{copies}")
+    sc.piles["gear"] = []
+    sc.piles["prismatic"] = []
+    sc.piles["prismatic_defs"] = []
+    real = "s2CreateGearJoint" not in lib.missing and not stand_ins
+    has_prismatic = "s2CreatePrismaticJoint" not in lib.missing
+    gid = _ground(lib, world, 0.5 * GEARS_PITCH * copies + 5.0)
+    sc.bodies.append(gid)
+
+    def body(x, y, radius=None, hx=0.25, hy=0.25, w=0.0):
+        bd = default_body_def()
+        bd.type = capi.DYNAMIC_BODY
+        bd.position = Vec2(x, y)
+        bd.angularVelocity = w
+        bid = lib.s2CreateBody(world, C.byref(bd))
+        if radius is not None:
+            lib.s2CreateCircleShape(bid, C.byref(default_shape_def()), C.byref(capi.Circle(Vec2(0.0, 0.0), radius)))
+        else:
+            lib.s2CreatePolygonShape(bid, C.byref(default_shape_def()), C.byref(lib.s2MakeBox(hx, hy)))
+        sc.bodies.append(bid)
+        return bid
+
+    def revolute(b, pivot, motor=None):
+        jd = default_revolute_def()
+        jd.bodyIdA = gid
+        jd.bodyIdB = b
+        jd.localAnchorA = lib.s2Body_GetLocalPoint(gid, Vec2(*pivot))
+        jd.localAnchorB = lib.s2Body_GetLocalPoint(b, Vec2(*pivot))
+        if motor is not None:
+            jd.enableMotor, jd.motorSpeed, jd.maxMotorTorque = True, motor[0], motor[1]
+        jid = lib.s2CreateRevoluteJoint(world, C.byref(jd))
+        sc.joints.append(jid)
+        return jid
+
+    def prismatic(b, pivot, limit):
+        d = dict(localAnchorA=tuple(lib.s2Body_GetLocalPoint(gid, Vec2(*pivot))),
+                 localAnchorB=tuple(lib.s2Body_GetLocalPoint(b, Vec2(*pivot))), localAxisA=(0.0, 1.0), referenceAngle=0.0,
+                 enableLimit=True, lowerTranslation=limit[0], upperTranslation=limit[1], enableMotor=False, motorSpeed=0.0,
+                 maxMotorForce=0.0, collideConnected=False)
+        if has_prismatic:
+            jd = capi.default_prismatic_def()
+            for name, value in d.items():
+                setattr(jd, name, Vec2(*value) if isinstance(value, tuple) else value)
+            create = lib.s2CreatePrismaticJoint
+        else:
+            jd = default_revolute_def()
+            jd.localAnchorA = Vec2(*d["localAnchorA"])
+            jd.localAnchorB = Vec2(*d["localAnchorB"])
+            create = lib.s2CreateRevoluteJoint
+        jd.bodyIdA = gid
+        jd.bodyIdB = b
+        sc.piles["prismatic"].append(len(sc.joints))
+        sc.piles["prismatic_defs"].append(d)
+        jid = create(world, C.byref(jd))
+        sc.joints.append(jid)
+        return jid
+
+    def gear(j1, b1, j2, b2, ratio):
+        """j1 / j2 link the ground to b1 / b2."""
+        if real:
+            gd = capi.default_gear_def()
+            gd.jointId1, gd.jointId2, gd.ratio = j1, j2, ratio
+            jid = lib.s2CreateGearJoint(world, C.byref(gd))
+        else:
+            jd = default_revolute_def()
+            jd.bodyIdA = b1
+            jd.bodyIdB = b2
+            jd.localAnchorA = lib.s2Body_GetLocalPoint(b1, lib.s2Body_GetPosition(b2))
+            jid = lib.s2CreateRevoluteJoint(world, C.byref(jd))
+        sc.piles["gear"].append(len(sc.joints))
+        sc.joints.append(jid)
+        return jid
+
+    for k in range(copies):
+        x0 = -0.5 * GEARS_PITCH * (copies - 1) + GEARS_PITCH * k - 25.0
+        # Box2D 2.4's testbed Gears
+        w1 = body(x0, 8.0, radius=1.0)
+        w2 = body(x0 + 4.0, 8.0, radius=2.0)
+        rack = body(x0 + 7.0, 8.0, hx=0.5, hy=2.0)
+        j1 = revolute(w1, (x0, 8.0))
+        j2 = revolute(w2, (x0 + 4.0, 8.0))
+        j3 = prismatic(rack, (x0 + 7.0, 8.0), (-3.0, 3.0))
+        gear(j1, w1, j2, w2, 2.0)
+        gear(j2, w2, j3, rack, -0.5)
+        # a gear train of three stages driven by the first wheel's motor
+        wheels = [body(x0 + 11.0 + 2.5 * i, 8.0, radius=1.0) for i in range(4)]
+        joints = [revolute(wheels[0], (x0 + 11.0, 8.0), motor=(1.5, 50.0))]
+        joints += [revolute(wheels[i], (x0 + 11.0 + 2.5 * i, 8.0)) for i in range(1, 4)]
+        for i, ratio in enumerate((1.5, -0.75, 1.5)):
+            gear(joints[i], wheels[i], joints[i + 1], wheels[i + 1], ratio)
+        # a rack and pinion lifting a pile
+        pinion = body(x0 + 23.0, 6.0, radius=0.5)
+        platform = body(x0 + 26.0, 2.0, hx=1.2, hy=0.1)
+        jp = revolute(pinion, (x0 + 23.0, 6.0), motor=(-1.0, 200.0))
+        jl = prismatic(platform, (x0 + 26.0, 2.0), (-1.5, 4.0))
+        gear(jp, pinion, jl, platform, 2.0)
+        for i in range(4):
+            body(x0 + 25.3 + 0.45 * i, 3.0 + 0.6 * i)
+        # a wheel geared through many turns
+        fast = body(x0 + 31.0, 8.0, radius=0.5, w=150.0)
+        slow = body(x0 + 33.0, 8.0, radius=0.5)
+        gear(revolute(fast, (x0 + 31.0, 8.0)), fast, revolute(slow, (x0 + 33.0, 8.0)), slow, 1.0)
+        # a sun meshing more planets than S2B_HUB_DEGREE
+        if hub and k == 0:
+            cx, cy = x0 + 45.0, 14.0
+            sun = body(cx, cy, radius=2.0, w=1.0)
+            js = revolute(sun, (cx, cy))
+            for i in range(GEARS_HUB_PLANETS):
+                angle = 2.0 * math.pi * i / GEARS_HUB_PLANETS
+                px, py = cx + 9.0 * math.cos(angle), cy + 9.0 * math.sin(angle)
+                planet = body(px, py, radius=0.3)
+                gear(js, sun, revolute(planet, (px, py)), planet, 10.0)
+    return sc
+
+
 MOTORS_PITCH = 30.0  # width of one copy of motors (m)
 
 
