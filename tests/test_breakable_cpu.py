@@ -1,7 +1,7 @@
 """CPU: joint reactions (s2MakeJointReaction, include/solver2d_b200.h, DESIGN.md §3.13) on oracle rows and hand-built rows.
 
-* Static load: a 2 kg box hangs at rest from a static body on each of the five joint types, solved by the oracle (the weld,
-  prismatic and motor oracles for those types) under every variant. The reaction at the rate of the variant must read the
+* Static load: a 2 kg box hangs at rest from a static body on each of the five joint types, solved by the oracle (the joint
+  oracle for the weld, prismatic and motor joints) under every variant. The reaction at the rate of the variant must read the
   weight, (0, m g), and no torque. Under XPBD the revolute, weld, prismatic and motor joints are position rows that keep no
   impulses and read exactly zero.
 * The mouse joint does not hold a hanging load under TGS_Sticky and XPBD, in the oracle as in the reference: after 3 s the
@@ -27,9 +27,7 @@ import pytest
 
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 
-import motor_oracle  # noqa: E402
-import prismatic_oracle  # noqa: E402
-import weld_oracle  # noqa: E402
+import joint_oracle  # noqa: E402
 from oracle import port  # noqa: E402
 from solver2d_b200 import capi, device  # noqa: E402
 
@@ -54,7 +52,7 @@ def _lib():
 
 
 def _oracle(kind):
-    return {"weld": weld_oracle, "prismatic": prismatic_oracle, "motor": motor_oracle}.get(kind, port).load()
+    return port.load() if kind in ("revolute", "mouse") else joint_oracle.load()
 
 
 def _bodies(a_kind=capi.STATIC_BODY, b_kind=capi.DYNAMIC_BODY, a_y=0.0, b_y=-1.0):

@@ -5,7 +5,7 @@
   under every variant and schedule (colour, wavefront, regions, launch by launch). Its broken list is exactly the joints
   whose reaction exceeds a threshold, in slot order.
 * scenes.breakables every step under every variant against the reference: the reference's collide and finalize on the
-  stand-in world, the oracle's solve (the weld, prismatic or motor oracle, one extension type per scene) in the device's
+  stand-in world, the joint oracle's solve (one extension type per scene: weld, prismatic or motor) in the device's
   order. The reference destroys with its own s2DestroyJoint, at the start of the next step, exactly the joints whose oracle
   reactions exceed their thresholds. Every step the device's broken list equals the oracle's, the contact set (after each
   break included) equals the reference's, and bodies, contact and joint impulses match bit for bit.
@@ -27,9 +27,7 @@ import math
 import numpy as np
 import pytest
 
-import motor_oracle
-import prismatic_oracle
-import weld_oracle
+import joint_oracle
 from helpers import (bit_equal, body_rows_from_ref, carry_sticky_friction, contact_rows_from_ref, joint_rows_from_ref,
                      load_bodies_into_ref, ref_delta_positions, store_oracle_bodies)
 from oracle import ref as refmod
@@ -144,7 +142,7 @@ def reference():
     return refmod.load()
 
 
-ORACLES = {"weld": weld_oracle, "prismatic": prismatic_oracle, "motor": motor_oracle}
+EXTENSIONS = ["motor", "prismatic", "weld"]  # the joint types the reference lacks, built on its revolute stand-ins
 
 
 def _own_rows(rows, sc):
@@ -176,7 +174,7 @@ def _own_rows(rows, sc):
     return rows
 
 
-@pytest.mark.parametrize("ext", sorted(ORACLES))
+@pytest.mark.parametrize("ext", EXTENSIONS)
 @pytest.mark.parametrize("solver", VARIANTS)
 def test_breakables_against_reference(reference, product, dev, solver, ext):
     """Reference collide on the stand-in world, the oracle in the device's order, reference finalize, and the reference's
@@ -184,7 +182,7 @@ def test_breakables_against_reference(reference, product, dev, solver, ext):
     s2World_Step. Every step: the broken lists, the contact sets and, bit for bit, bodies (XPBD's delta positions included),
     contact and joint impulses."""
     R, P = reference, product
-    O = ORACLES[ext].load()
+    O = joint_oracle.load()
     sr = scenes.breakables(R, solver, parts=(ext,))
     sp = scenes.breakables(P, solver, parts=(ext,))
     assert "s2Joint_SetBreakForce" in R.missing and sr.piles["types"] == sp.piles["types"]

@@ -1,4 +1,4 @@
-"""GPU: the distance joint (DESIGN.md §3.16). The device against the distance oracle (tests/distance_oracle.c) bit for bit:
+"""GPU: the distance joint (DESIGN.md §3.16). The device against the joint oracle (tests/joint_oracle.c) bit for bit:
 every step of scenes.distance_joints (ropes, pendulums, a spring ring over a pile, winches, a kinematic tether, contacts
 throughout) through the public API against reference collide and finalize around the oracle, in the wavefront and the
 colour schedule; every step of a contact-free world for all ten variants, in both schedules, persistent and launch by
@@ -16,7 +16,7 @@ import math
 import numpy as np
 import pytest
 
-import distance_oracle
+import joint_oracle
 from helpers import (bit_equal, body_rows_from_ref, carry_sticky_friction, contact_rows_from_ref, joint_rows_from_ref,
                      load_bodies_into_ref, ref_delta_positions, store_oracle_bodies)
 from oracle import ref as refmod
@@ -176,7 +176,7 @@ def test_distance_scene_every_step(reference, product, dev, solver, mode):
     finalize; the device runs the same steps through s2World_Step with real distance joints. Every step bit for bit: bodies,
     delta positions, contact impulses and joint impulses, the spring impulse included."""
     R, P = reference, product
-    O = distance_oracle.load()
+    O = joint_oracle.load()
     sr = scenes.distance_joints(R, solver)
     sp = scenes.distance_joints(P, solver)
     assert "s2CreateDistanceJoint" in R.missing and "s2CreateDistanceJoint" not in P.missing
@@ -276,7 +276,7 @@ def test_public_world_every_step(product, dev, solver, mode, persistent, gather)
     dw.set_schedule(device.SCHEDULE_WAVEFRONT if mode == "wavefront" else device.SCHEDULE_COLOR)
     dw.set_persistent(persistent)
     dw.set_warm_gather(gather)
-    _step_and_compare(P, wid, dw, distance_oracle.load(), solver, 60, colour=mode == "color")
+    _step_and_compare(P, wid, dw, joint_oracle.load(), solver, 60, colour=mode == "color")
     P.s2DestroyWorld(wid)
 
 
@@ -305,7 +305,7 @@ def test_setter_edits_between_replayed_steps(product, dev, solver):
             P.s2DistanceJoint_EnableSpring(joints[1], True)
 
     replays = dw.counters().graphReplays
-    _step_and_compare(P, wid, dw, distance_oracle.load(), solver, 45, colour=True, edit=edit)
+    _step_and_compare(P, wid, dw, joint_oracle.load(), solver, 45, colour=True, edit=edit)
     assert dw.counters().graphReplays > replays
     assert P.s2DistanceJoint_GetLength(joints[0]) == np.float32(1.5)
     assert (P.s2DistanceJoint_GetMinLength(joints[2]), P.s2DistanceJoint_GetMaxLength(joints[2])) == (0.5, np.float32(1.2))
@@ -321,7 +321,7 @@ def test_slot_reuse_across_types(product, dev):
     P.s2World_Step(wid, DT, 4, 2, True)
     dw = device.DeviceWorld.attach(dev, wid)
     dw.set_schedule(device.SCHEDULE_WAVEFRONT)
-    O = distance_oracle.load()
+    O = joint_oracle.load()
     _step_and_compare(P, wid, dw, O, solver, 10)
     P.s2DestroyJoint(joints[0])  # the rod
     rd = capi.default_revolute_def()

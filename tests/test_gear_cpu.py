@@ -1,4 +1,4 @@
-"""CPU: the gear joint's oracle (tests/gear_oracle.c, DESIGN.md §3.19) on hand-built rows, for all ten variants.
+"""CPU: the gear joint in the joint oracle (tests/joint_oracle.c, DESIGN.md §3.19) on hand-built rows, for all ten variants.
 
 No contacts and every local centre at zero, so finalize is the identity (origin == position) and solver stages chain
 directly. A gear row needs no row for the joints it links: its frames are in the row. The bounds below were measured on
@@ -8,7 +8,7 @@ Mutations each test catches: a ratio left out of side 2's impulse or of the mass
 speed; a bias with its sign flipped lets the coordinate drift; a revolute side read from the wrapped angle, or an unwound
 coordinate not carried from step to step (XPBD's included), jumps by 2 pi within the ten turns; a reaction without the
 ratio or on the wrong side misreads the rack's weight; a gear branch that takes another type's rows, or a type decoded
-from the 3-bit field alone, changes the pulley oracle's bits."""
+from the 3-bit field alone, changes the bits tests/test_joint_oracle_cpu.py pins."""
 import ctypes as C
 import math
 import os
@@ -19,8 +19,7 @@ import pytest
 
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 
-import gear_oracle  # noqa: E402
-import pulley_oracle  # noqa: E402
+import joint_oracle  # noqa: E402
 from solver2d_b200 import capi, device  # noqa: E402
 
 VARIANTS = ["Jacobi", "PGS", "PGS_NGS", "PGS_NGS_Block", "PGS_Soft", "SoftStep", "TGS_Sticky", "TGS_Soft", "TGS_NGS", "XPBD"]
@@ -77,8 +76,8 @@ def _gear(a, b, side1, side2, ratio, constant, slot=0):
     return r
 
 
-def _run(solver, bodies, joints, steps, gravity=(0.0, -G), oracle=None):
-    O = oracle or gear_oracle.load()
+def _run(solver, bodies, joints, steps, gravity=(0.0, -G)):
+    O = joint_oracle.load()
     ctx = device.make_context(solver, DT, 4, 2)
     contacts = np.zeros(0, dtype=device.CONTACT_ROW)
     history = []
@@ -191,44 +190,6 @@ def test_motor_driven_train(solver, max_torque, lifts):
 
 
 # ---- other joint types and layout -----------------------------------------------------------------------------------------
-
-@pytest.mark.parametrize("solver", VARIANTS)
-def test_other_types_keep_the_pulley_oracles_bits(solver):
-    """A world of pulley, wheel, prismatic (with spring), revolute (with limit and motor) and weld rows: the gear oracle and
-    the pulley oracle give the same bytes."""
-    bodies = _bodies([(capi.STATIC_BODY, 0, 0, 0), (capi.DYNAMIC_BODY, 0.0, -1.0, 2.0), (capi.DYNAMIC_BODY, 1.0, 0.0, 2.0),
-                      (capi.DYNAMIC_BODY, 2.0, -0.5, 2.0), (capi.DYNAMIC_BODY, 3.0, 0.0, 2.0), (capi.DYNAMIC_BODY, 4.0, -0.3, 2.0),
-                      (capi.DYNAMIC_BODY, 6.0, -2.0, 1.0)])
-    bodies["linearVelocity"][1] = (0.5, 0.0)
-    bodies["angularVelocity"][3] = 1.0
-
-    def row(kind, a, b, slot, anchor_a=(0.0, 0.0), axis=(0.0, 1.0)):
-        r = np.zeros(1, dtype=device.JOINT_ROW)[0]
-        r["index"], r["flags"], r["bodyA"], r["bodyB"] = slot, device.ROW_VALID | (kind << 1), a, b
-        r["localOriginAnchorA"], r["localAxisA"] = anchor_a, axis
-        return r
-
-    rows = np.zeros(5, dtype=device.JOINT_ROW)
-    rows[0] = row(device.JOINT_PULLEY, 1, 6, 0)
-    rows[0]["target"], rows[0]["localAxisA"] = (0.0, 3.0), (6.0, 3.0)
-    rows[0]["referenceAngle"], rows[0]["lowerAngle"], rows[0]["upperAngle"] = 1.5, 4.0, 5.0
-    rows[1] = row(device.JOINT_PRISMATIC, 0, 2, 1, anchor_a=(1.0, 0.0), axis=(1.0, 0.0))
-    rows[1]["flags"] |= device.JOINT_ENABLE_SPRING | device.JOINT_ENABLE_LIMIT | device.JOINT_ENABLE_MOTOR
-    rows[1]["hertz"], rows[1]["dampingRatio"], rows[1]["lowerAngle"], rows[1]["upperAngle"] = 1.5, 0.2, -0.5, 0.5
-    rows[1]["motorSpeed"], rows[1]["maxMotorTorque"] = 0.3, 4.0
-    rows[2] = row(device.JOINT_REVOLUTE, 2, 3, 2, anchor_a=(1.0, -0.5))
-    rows[2]["flags"] |= device.JOINT_ENABLE_LIMIT | device.JOINT_ENABLE_MOTOR
-    rows[2]["lowerAngle"], rows[2]["upperAngle"], rows[2]["motorSpeed"], rows[2]["maxMotorTorque"] = -0.4, 0.4, 1.0, 3.0
-    rows[3] = row(device.JOINT_WELD, 3, 4, 3, anchor_a=(1.0, 0.5))
-    rows[4] = row(device.JOINT_WHEEL, 4, 5, 4, anchor_a=(1.0, -0.3))
-    rows[4]["flags"] |= device.JOINT_ENABLE_SPRING | device.JOINT_ENABLE_LIMIT | device.JOINT_ENABLE_MOTOR
-    rows[4]["hertz"], rows[4]["dampingRatio"], rows[4]["lowerAngle"], rows[4]["upperAngle"] = 2.0, 0.5, -0.3, 0.3
-    rows[4]["motorSpeed"], rows[4]["maxMotorTorque"] = 2.0, 1.0
-    a = _run(solver, bodies.copy(), rows.copy(), 30)
-    b = _run(solver, bodies.copy(), rows.copy(), 30, oracle=pulley_oracle.load())
-    for (ba, ja), (bb, jb) in zip(a, b):
-        assert ba.tobytes() == bb.tobytes() and ja.tobytes() == jb.tobytes()
-
 
 def test_type_field():
     """The gear's fourth type bit leaves every other type's flags as they were: the 3-bit field reads 0 - 7 unchanged, and

@@ -1,4 +1,4 @@
-"""GPU: the gear joint (DESIGN.md §3.19). The device against the gear oracle (tests/gear_oracle.c) bit for bit on every step of
+"""GPU: the gear joint (DESIGN.md §3.19). The device against the joint oracle (tests/joint_oracle.c) bit for bit on every step of
 a contact-free world (revolute-revolute gears, a motor-driven train of three stages, a rack and pinion lifting a load, two
 racks, a frame turned away from zero, a wheel geared through more than ten turns, and a sun meshing more planets than
 S2B_HUB_DEGREE) for all ten variants, in both schedules, persistent and launch by launch, with the warm-start gather on and
@@ -16,7 +16,7 @@ import ctypes as C
 import numpy as np
 import pytest
 
-import gear_oracle
+import joint_oracle
 from helpers import (bit_equal, body_rows_from_ref, carry_sticky_friction, contact_rows_from_ref, joint_rows_from_ref,
                      load_bodies_into_ref, ref_delta_positions, store_oracle_bodies)
 from oracle import ref as refmod
@@ -142,7 +142,7 @@ def test_gear_scene_every_step(reference, product, dev, solver, mode):
     Mutations it catches beyond the contact-free world's: a gear row that the colouring, the hub path or the schedules
     treat otherwise than a two-body row while contacts share its bodies."""
     R, P = reference, product
-    O = gear_oracle.load()
+    O = joint_oracle.load()
     sr = scenes.gears(R, solver)
     sp = scenes.gears(P, solver)
     assert "s2CreateGearJoint" in R.missing and "s2CreateGearJoint" not in P.missing
@@ -252,7 +252,7 @@ def test_public_world_every_step(product, dev, solver, mode, persistent, gather)
     dw.set_schedule(device.SCHEDULE_WAVEFRONT if mode == "wavefront" else device.SCHEDULE_COLOR)
     dw.set_persistent(persistent)
     dw.set_warm_gather(gather)
-    _step_and_compare(P, wid, dw, gear_oracle.load(), solver, 60, colour=mode == "color")
+    _step_and_compare(P, wid, dw, joint_oracle.load(), solver, 60, colour=mode == "color")
     rows = dw.download_joints()
     assert all(device.joint_type(int(rows["flags"][g.index])) == device.JOINT_GEAR for g in gears)
     # the fast pair turned through more than ten turns in 1 s without a jump in its unwound coordinates; XPBD's position
@@ -272,7 +272,7 @@ def test_slot_reuse_across_types(product, dev):
     P.s2World_Step(wid, DT, 4, 2, True)
     dw = device.DeviceWorld.attach(dev, wid)
     dw.set_schedule(device.SCHEDULE_WAVEFRONT)
-    O = gear_oracle.load()
+    O = joint_oracle.load()
     _step_and_compare(P, wid, dw, O, solver, 10)
     slot = gears[0].index
     P.s2DestroyJoint(gears[0])
@@ -307,7 +307,7 @@ def test_teleported_static_frame(product, dev):
         if k == 5:
             P.s2Body_SetTransform(plate, capi.Vec2(40.5, 0.2), 1.1)
 
-    _step_and_compare(P, wid, dw, gear_oracle.load(), solver, 20, edit=edit)
+    _step_and_compare(P, wid, dw, joint_oracle.load(), solver, 20, edit=edit)
     after = dw.download_joints()
     for slot in train:
         # both sides' frames turned with the plate: side 1's rotation in target, side 2's in maxMotorTorque / motorSpeed
@@ -329,7 +329,7 @@ def test_unwound_coordinate_survives_a_reupload(product, dev):
     P.s2World_Step(wid, DT, 4, 2, True)
     dw = device.DeviceWorld.attach(dev, wid)
     dw.set_schedule(device.SCHEDULE_WAVEFRONT)
-    O = gear_oracle.load()
+    O = joint_oracle.load()
     _step_and_compare(P, wid, dw, O, solver, 40)
     fast = gears[6]
     before = dw.download_joints()[fast.index]

@@ -29,9 +29,7 @@ import pytest
 import torch
 
 import hub_cases
-import motor_oracle
-import prismatic_oracle
-import weld_oracle
+import joint_oracle
 from helpers import bit_equal
 from hub_cases import SCENES, build_rows, check_sizes, degrees, item_ends
 from oracle import port
@@ -82,8 +80,6 @@ def _convert(joints, slots, kind):
     return joints
 
 
-ORACLES = {None: port.load, "revolute": port.load, "weld": weld_oracle.load, "prismatic": prismatic_oracle.load,
-           "motor": motor_oracle.load}
 
 
 def _run(reference, dev, monkeypatch, name, solver, persistent=True, regions=0, kind=None, gather=True, dataflow=False,
@@ -139,7 +135,8 @@ def _run(reference, dev, monkeypatch, name, solver, persistent=True, regions=0, 
     _, cnt = np.unique(both[:, 0].astype(np.int64) * (len(bodies) + 1) + both[:, 1], return_counts=True)
     assert (cnt == 1).all(), "a movable body appears twice in a parallel group"
 
-    ob, oc, oj = ORACLES[kind]().solve(capi.SOLVER[solver], bodies, contacts, joints, ctx, order=order)
+    O = port.load() if kind in (None, "revolute") else joint_oracle.load()
+    ob, oc, oj = O.solve(capi.SOLVER[solver], bodies, contacts, joints, ctx, order=order)
     valid = (bodies["flags"] & 1) == 1
     for field in ("position", "rot", "linearVelocity", "angularVelocity"):
         g = np.ascontiguousarray(got[field][valid]).reshape(int(valid.sum()), -1)

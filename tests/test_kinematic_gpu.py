@@ -15,7 +15,7 @@ import ctypes as C
 import numpy as np
 import pytest
 
-import prismatic_oracle
+import joint_oracle
 from helpers import bit_equal
 from oracle import ref as refmod
 from solver2d_b200 import capi, device, scenes
@@ -66,7 +66,7 @@ def test_every_step(reference, product, dev, solver, mode):
     setup, ran = MODES[mode]
     seen = _Seen()
     _run(reference, product, dev, scenes.kinematic_rigs, solver, _steps(solver, 30), 4, 2, KW, setup=setup,
-         oracle=prismatic_oracle.load(), as_joints=_as_joints, after_step=seen)
+         oracle=joint_oracle.load(), as_joints=_as_joints, after_step=seen)
     assert seen.max["constraintCount"] > 512, seen.max
     assert ran(seen.max), f"{mode}: the schedule did not run as asked: {seen.max}"
 
@@ -93,7 +93,7 @@ def _drive(turn):
 def test_public_api_drive_every_step(reference, product, dev, solver):
     """Velocity setters on the kinematic bodies every few steps and a shape added to one: each re-uploads the body's row.
     Every step against the reference pipeline replayed in the device's order."""
-    _run(reference, product, dev, scenes.kinematic_rigs, solver, _steps(solver, 30), 4, 2, KW, oracle=prismatic_oracle.load(),
+    _run(reference, product, dev, scenes.kinematic_rigs, solver, _steps(solver, 30), 4, 2, KW, oracle=joint_oracle.load(),
          as_joints=_as_joints, before_step=_drive(True))
 
 
@@ -145,5 +145,5 @@ def test_tgs_soft_gather_pass_kept_every_step(reference, product, dev):
         sc.destroy()
     seen = _Seen()
     _run(reference, product, dev, scenes.kinematic_rigs, "TGS_Soft", 40, SUBSTEPS, 2, KW, setup=lambda dw: dw.set_regions(0),
-         oracle=prismatic_oracle.load(), as_joints=_as_joints, after_step=seen)
+         oracle=joint_oracle.load(), as_joints=_as_joints, after_step=seen)
     assert seen.max["regionCount"] == 0 and seen.max["neighbourSync"] > 1, seen.max

@@ -1,4 +1,4 @@
-"""CPU: the motor joint's oracle (tests/motor_oracle.c, DESIGN.md §3.10) on hand-built rows, for all ten variants.
+"""CPU: the motor joint in the joint oracle (tests/joint_oracle.c, DESIGN.md §3.10) on hand-built rows, for all ten variants.
 
 No contacts and every local centre at zero, so finalize is the identity (origin == position) and solver stages chain
 directly. The bounds below were measured on these deterministic runs (the largest value over the ten variants, printed by
@@ -17,7 +17,7 @@ import pytest
 
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 
-import motor_oracle  # noqa: E402
+import joint_oracle  # noqa: E402
 from solver2d_b200 import capi, device  # noqa: E402
 
 VARIANTS = ["Jacobi", "PGS", "PGS_NGS", "PGS_NGS_Block", "PGS_Soft", "SoftStep", "TGS_Sticky", "TGS_Soft", "TGS_NGS", "XPBD"]
@@ -79,7 +79,7 @@ def _motor(a, b, offset=(0.0, 0.0), angle=0.0, max_force=1000.0, max_torque=1000
 
 
 def _run(solver, bodies, joints, steps, gravity=(0.0, 0.0), torque=None):
-    O = motor_oracle.load()
+    O = joint_oracle.load()
     ctx = device.make_context(solver, DT, ITERS, 2)
     contacts = np.zeros(0, dtype=device.CONTACT_ROW)
     history = []

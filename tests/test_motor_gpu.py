@@ -1,4 +1,4 @@
-"""GPU: the motor joint (DESIGN.md §3.10). The device's motor rows against the motor oracle (tests/motor_oracle.c) bit for
+"""GPU: the motor joint (DESIGN.md §3.10). The device's motor rows against the joint oracle (tests/joint_oracle.c) bit for
 bit, in every schedule, for all ten variants and with the warm-start gather on and off; every step of scenes.motors through
 the public API; setter edits between replayed steps; the bulk offset path (s2World_SetMotorJointOffsets) against the
 per-joint setters, its precedence rule, its input check and its launch cost; contacts between jointed bodies; the joint's
@@ -18,7 +18,7 @@ import math
 import numpy as np
 import pytest
 
-import motor_oracle
+import joint_oracle
 from helpers import (bit_equal, body_rows_from_ref, carry_sticky_friction, contact_rows_from_ref, joint_rows_from_ref,
                      load_bodies_into_ref, ref_delta_positions, store_oracle_bodies)
 from oracle import port
@@ -101,7 +101,7 @@ def test_stage_matches_oracle(reference, dev, solver, mode, persistent, gather):
     if not gather and solver not in SUBSTEPPING:
         pytest.skip("the warm-start gather serves the sub-stepping variants only")
     R = reference
-    O = motor_oracle.load()
+    O = joint_oracle.load()
     sc = scenes.motors(R, solver, copies=2)
     for _ in range(30):
         sc.step(DT, 4, 2, True)
@@ -150,7 +150,7 @@ def test_motors_every_step(reference, product, dev, solver):
     s2World_SetMotorJointOffsets. Every step bit for bit: bodies (the kinematic carriage and XPBD's delta positions
     included), contact and joint impulses."""
     R, P = reference, product
-    O = motor_oracle.load()
+    O = joint_oracle.load()
     sr = scenes.motors(R, solver)
     sp = scenes.motors(P, solver)
     assert "s2CreateMotorJoint" in R.missing and "s2CreateMotorJoint" not in P.missing
@@ -264,7 +264,7 @@ def test_edits_between_steps(product, dev, solver):
     """Every setter between steps of a captured, replayed step graph: each takes effect at the next step, every step matches
     the oracle run on the rows the host now holds, and the getters return what was set."""
     P = product
-    O = motor_oracle.load()
+    O = joint_oracle.load()
     wid, box, jid = _single(P, solver)
     _flush(dev, wid)
     dw = device.DeviceWorld.attach(dev, wid)
@@ -307,7 +307,7 @@ def test_zero_force_cap_matches_oracle(product, dev, solver):
     length 0, so its components are zeros whose signs depend on how the total impulse is formed. Every step matches the
     oracle bit for bit, the impulse columns included, through the persistent kernels (the soft variants' shared branches)."""
     P = product
-    O = motor_oracle.load()
+    O = joint_oracle.load()
     wid, _, _ = _single(P, solver, velocity=(3.0, 0.0))
     _flush(dev, wid)
     dw = device.DeviceWorld.attach(dev, wid)

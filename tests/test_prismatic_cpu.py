@@ -1,4 +1,4 @@
-"""CPU: the prismatic joint's oracle (tests/prismatic_oracle.c, DESIGN.md §3.9) on hand-built rows, for all ten variants.
+"""CPU: the prismatic joint in the joint oracle (tests/joint_oracle.c, DESIGN.md §3.9) on hand-built rows, for all ten variants.
 
 No contacts and every local centre at zero, so finalize is the identity (origin == position) and solver stages chain
 directly. The bounds below were measured on these deterministic runs (the largest value over the ten variants, printed
@@ -17,7 +17,7 @@ import pytest
 
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 
-import prismatic_oracle  # noqa: E402
+import joint_oracle  # noqa: E402
 from solver2d_b200 import capi, device  # noqa: E402
 
 VARIANTS = ["Jacobi", "PGS", "PGS_NGS", "PGS_NGS_Block", "PGS_Soft", "SoftStep", "TGS_Sticky", "TGS_Soft", "TGS_NGS", "XPBD"]
@@ -95,7 +95,7 @@ def _prismatic(bodies, a, b, pivot, axis, ref=0.0, limit=None, motor=None):
 
 
 def _run(solver, bodies, joints, steps, gravity=(0.0, 0.0)):
-    O = prismatic_oracle.load()
+    O = joint_oracle.load()
     ctx = device.make_context(solver, DT, 4, 2)
     contacts = np.zeros(0, dtype=device.CONTACT_ROW)
     history = []

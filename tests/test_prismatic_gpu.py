@@ -1,5 +1,5 @@
-"""GPU: the prismatic joint (DESIGN.md §3.9). The device's prismatic rows against the prismatic oracle
-(tests/prismatic_oracle.c) bit for bit, in every schedule, for all ten variants and with the warm-start gather on and off;
+"""GPU: the prismatic joint (DESIGN.md §3.9). The device's prismatic rows against the joint oracle
+(tests/joint_oracle.c) bit for bit, in every schedule, for all ten variants and with the warm-start gather on and off;
 every step of scenes.sliders through the public API; parameter edits between replayed steps; contacts between jointed
 bodies; the joint's lifecycle, input checks, translation getter and debug drawing.
 
@@ -16,7 +16,7 @@ import math
 import numpy as np
 import pytest
 
-import prismatic_oracle
+import joint_oracle
 from helpers import (bit_equal, body_rows_from_ref, carry_sticky_friction, contact_rows_from_ref, joint_rows_from_ref,
                      load_bodies_into_ref, ref_delta_positions, store_oracle_bodies)
 from oracle import port
@@ -88,7 +88,7 @@ def test_stage_matches_oracle(reference, dev, solver, mode, persistent, gather):
     if not gather and solver not in SUBSTEPPING:
         pytest.skip("the warm-start gather serves the sub-stepping variants only")
     R = reference
-    O = prismatic_oracle.load()
+    O = joint_oracle.load()
     sc = scenes.sliders(R, solver, copies=2)
     for _ in range(30):
         sc.step(DT, 4, 2, True)
@@ -144,7 +144,7 @@ def test_sliders_every_step(reference, product, dev, solver):
     runs the same steps through s2World_Step with real prismatic joints. Every step bit for bit: bodies, contact and joint
     impulses."""
     R, P = reference, product
-    O = prismatic_oracle.load()
+    O = joint_oracle.load()
     sr = scenes.sliders(R, solver)
     sp = scenes.sliders(P, solver)
     assert "s2CreatePrismaticJoint" in R.missing and "s2CreatePrismaticJoint" not in P.missing
@@ -254,7 +254,7 @@ def test_edits_between_steps(product, dev, solver):
     """SetMotorSpeed, EnableLimit and SetLimits between steps of a captured, replayed step graph: each takes effect at the
     next step and every step matches the oracle run on the rows the host now holds."""
     P = product
-    O = prismatic_oracle.load()
+    O = joint_oracle.load()
     wid, load, jid = _piston(P, solver)
     _flush(dev, wid)
     dw = device.DeviceWorld.attach(dev, wid)

@@ -1,4 +1,4 @@
-"""GPU: the pulley joint (DESIGN.md §3.18). The device against the pulley oracle (tests/pulley_oracle.c) bit for bit: every
+"""GPU: the pulley joint (DESIGN.md §3.18). The device against the joint oracle (tests/joint_oracle.c) bit for bit: every
 step of scenes.pulleys (Box2D 2.4's testbed pulley, a counterweighted lift on a prismatic joint carrying a pile, a
 block-and-tackle at ratio 2, a kinematic driver, contacts throughout) through the public API against reference collide and
 finalize around the oracle, in the wavefront and the colour schedule; every step of a contact-free world for all ten
@@ -14,7 +14,7 @@ import ctypes as C
 import numpy as np
 import pytest
 
-import pulley_oracle
+import joint_oracle
 from helpers import (bit_equal, body_rows_from_ref, carry_sticky_friction, contact_rows_from_ref, joint_rows_from_ref,
                      load_bodies_into_ref, ref_delta_positions, store_oracle_bodies)
 from oracle import ref as refmod
@@ -117,7 +117,7 @@ def test_pulley_scene_every_step(reference, product, dev, solver, mode):
     the device runs the same steps through s2World_Step with real pulleys and a real prismatic joint. Every step bit for
     bit: bodies, delta positions, contact impulses and joint impulses."""
     R, P = reference, product
-    O = pulley_oracle.load()
+    O = joint_oracle.load()
     sr = scenes.pulleys(R, solver)
     sp = scenes.pulleys(P, solver)
     assert "s2CreatePulleyJoint" in R.missing and "s2CreatePulleyJoint" not in P.missing
@@ -221,7 +221,7 @@ def test_public_world_every_step(product, dev, solver, mode, persistent, gather)
     dw.set_schedule(device.SCHEDULE_WAVEFRONT if mode == "wavefront" else device.SCHEDULE_COLOR)
     dw.set_persistent(persistent)
     dw.set_warm_gather(gather)
-    _step_and_compare(P, wid, dw, pulley_oracle.load(), solver, 60, colour=mode == "color")
+    _step_and_compare(P, wid, dw, joint_oracle.load(), solver, 60, colour=mode == "color")
     P.s2DestroyWorld(wid)
 
 
@@ -234,7 +234,7 @@ def test_slot_reuse_across_types(product, dev):
     P.s2World_Step(wid, DT, 4, 2, True)
     dw = device.DeviceWorld.attach(dev, wid)
     dw.set_schedule(device.SCHEDULE_WAVEFRONT)
-    O = pulley_oracle.load()
+    O = joint_oracle.load()
     _step_and_compare(P, wid, dw, O, solver, 10)
     P.s2DestroyJoint(joints[0])
     wheel = _wheel(P, wid, a, b, (0.0, 0.0), (-4.0, 0.0), axis=(1.0, 0.0), spring=(2.0, 0.5), limit=(-0.4, 0.4), motor=(1.0, 2.0))

@@ -1,4 +1,4 @@
-"""CPU: the soft weld's oracle (tests/soft_weld_oracle.c, DESIGN.md §3.15) on hand-built rows, for all ten variants.
+"""CPU: the soft weld in the joint oracle (tests/joint_oracle.c, DESIGN.md §3.15) on hand-built rows, for all ten variants.
 
 No contacts and every local centre at zero, so finalize is the identity (origin == position) and solver stages chain
 directly. Gravity is off unless a test says otherwise. The bounds below were measured on these deterministic runs (the
@@ -8,7 +8,7 @@ each.
 Mutations each test catches: a coefficient formed with the wrong h or the wrong expression shifts the frequency or the sag;
 a soft part that is not soft (the error fed back at 1 / h) overshoots with zeta = 1; an impulse applied to one body only
 breaks momentum; a missing s2UnwindAngle turns the seam case the long way round; a soft term evaluated on a weld with both
-hertz at 0, or on another joint, changes the weld oracle's bits; an angular spring on a body without rotation moves it."""
+hertz at 0, or on another joint, changes the bits tests/test_joint_oracle_cpu.py pins; an angular spring on a body without rotation moves it."""
 import ctypes as C
 import math
 import os
@@ -19,8 +19,7 @@ import pytest
 
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 
-import soft_weld_oracle  # noqa: E402
-import weld_oracle  # noqa: E402
+import joint_oracle  # noqa: E402
 from solver2d_b200 import capi, device  # noqa: E402
 
 VARIANTS = ["Jacobi", "PGS", "PGS_NGS", "PGS_NGS_Block", "PGS_Soft", "SoftStep", "TGS_Sticky", "TGS_Soft", "TGS_NGS", "XPBD"]
@@ -154,7 +153,7 @@ def _frequency(e):
 
 
 def _measure_frequency(solver, part):
-    e = _errors(part, _run(soft_weld_oracle.load(), solver, *_oscillator(part, (1.0, 0.0)), 240))
+    e = _errors(part, _run(joint_oracle.load(), solver, *_oscillator(part, (1.0, 0.0)), 240))
     return abs(_frequency(e) - 1.0)
 
 
@@ -166,7 +165,7 @@ def test_oscillates_at_hertz(solver, part):
 
 
 def _measure_overshoot(solver, part):
-    e = _errors(part, _run(soft_weld_oracle.load(), solver, *_oscillator(part, (2.0, 1.0)), 180))
+    e = _errors(part, _run(joint_oracle.load(), solver, *_oscillator(part, (2.0, 1.0)), 180))
     return float(max(0.0, -e.min())), abs(float(e[-1]))
 
 
@@ -179,7 +178,7 @@ def test_critical_damping_does_not_overshoot(solver, part):
 
 
 def _measure_keep(solver, part):
-    e = _errors(part, _run(soft_weld_oracle.load(), solver, *_oscillator(part, (1.0, 0.0)), 300))
+    e = _errors(part, _run(joint_oracle.load(), solver, *_oscillator(part, (1.0, 0.0)), 300))
     return float(np.abs(e[240:]).max() / np.abs(e[:60]).max())
 
 
@@ -195,7 +194,7 @@ def _measure_rest(solver):
     omega = 2.0 * math.pi * hertz
     bodies = _bodies([(capi.STATIC_BODY, 0, 0, 0, 0, 0, 0), (capi.DYNAMIC_BODY, 0, 0, 0, 0, 0, 0)])
     joints = np.array([weld_row(bodies, 0, 1, (0.0, 0.0), linear=(hertz, 0.7))])
-    h = _run(soft_weld_oracle.load(), solver, bodies, joints, 300, gravity=(0.0, -G))
+    h = _run(joint_oracle.load(), solver, bodies, joints, 300, gravity=(0.0, -G))
     rest = -G / (omega * omega)
     b, j = h[-1]
     return abs(float(_separation(b, j[0])[1]) - rest) / abs(rest)
@@ -244,7 +243,7 @@ def test_free_pair_conserves_momentum(solver):
     soft weld drifts in angular momentum no more than the rigid weld does (the position passes of the NGS variants and
     XPBD move it either way). A soft anchor lets the anchors part, and its impulse is not along the line between them, so
     it turns the pair: angular momentum is not a property of a linear soft part (as for Box2D's soft weld)."""
-    O = soft_weld_oracle.load()
+    O = joint_oracle.load()
     rigid_L = _measure_momentum(solver, O, linear=(0.0, 0.0), angular=(0.0, 0.0))[1]
     assert _measure_momentum(solver, O)[0] <= LINEAR_MOMENTUM_BOUND
     assert _measure_momentum(solver, O, linear=(0.0, 0.0))[1] <= 2.0 * rigid_L + MOMENTUM_SLACK
@@ -257,7 +256,7 @@ def _measure_seam(solver):
     joints = np.array([weld_row(bodies, 0, 1, (0.0, 0.0), ref=ref, angular=(2.0, 1.0))])
     travelled = 0.0
     prev = _angle(bodies, 1)
-    hist = _run(soft_weld_oracle.load(), solver, bodies, joints, 180)
+    hist = _run(joint_oracle.load(), solver, bodies, joints, 180)
     for b, _ in hist:
         a = _angle(b, 1)
         travelled += (a - prev + math.pi) % (2.0 * math.pi) - math.pi
@@ -299,17 +298,6 @@ def _mixed_bodies():
 
 
 @pytest.mark.parametrize("solver", VARIANTS)
-def test_rigid_welds_keep_the_weld_oracle_bits(solver):
-    """Both hertz at 0: the soft weld oracle gives the weld oracle's bits, beside revolute and mouse rows."""
-    bodies = _mixed_bodies()
-    joints = _mixed_rows(bodies)
-    a = _run(soft_weld_oracle.load(), solver, bodies, joints, 40, gravity=(0.0, -G))
-    b = _run(weld_oracle.load(), solver, bodies, joints, 40, gravity=(0.0, -G))
-    for (b1, j1), (b2, j2) in zip(a, b):
-        assert b1.tobytes() == b2.tobytes() and j1.tobytes() == j2.tobytes()
-
-
-@pytest.mark.parametrize("solver", VARIANTS)
 def test_soft_welds_act_beside_rigid_rows(solver):
     """The same rows with the welds made soft: the welds move differently and the other rows still solve (no NaN)."""
     bodies = _mixed_bodies()
@@ -317,7 +305,7 @@ def test_soft_welds_act_beside_rigid_rows(solver):
     soft = joints.copy()
     soft[0]["hertz"], soft[0]["dampingRatio"] = 3.0, 0.5
     soft[2]["maxMotorTorque"], soft[2]["motorSpeed"] = 2.0, 0.1
-    O = soft_weld_oracle.load()
+    O = joint_oracle.load()
     a = _run(O, solver, bodies, soft, 40, gravity=(0.0, -G))
     b = _run(O, solver, bodies, joints, 40, gravity=(0.0, -G))
     assert np.isfinite(a[-1][0]["position"]).all()
@@ -332,7 +320,7 @@ def test_angular_spring_without_rotation_does_nothing(solver):
     joints = np.array([weld_row(bodies, 0, 1, (0.0, 0.0), angular=(1.0, 0.5))])
     rigid = joints.copy()
     rigid[0]["maxMotorTorque"], rigid[0]["motorSpeed"] = 0.0, 0.0
-    O = soft_weld_oracle.load()
+    O = joint_oracle.load()
     for (b1, j1), (b2, j2) in zip(_run(O, solver, bodies, joints, 10), _run(O, solver, bodies, rigid, 10)):
         assert b1.tobytes() == b2.tobytes()
         assert float(j1[0]["motorImpulse"]) == float(j2[0]["motorImpulse"])
@@ -370,7 +358,7 @@ if __name__ == "__main__":
         print(part, "frequency rel error", {s: round(_measure_frequency(s, part), 4) for s in VARIANTS})
         print(part, "zeta=1 (overshoot, last)", {s: tuple(f"{v:.1e}" for v in _measure_overshoot(s, part)) for s in VARIANTS})
         print(part, "zeta=0 amplitude kept", {s: round(_measure_keep(s, part), 3) for s in VARIANTS})
-    O = soft_weld_oracle.load()
+    O = joint_oracle.load()
     print("momentum drift (linear both soft, angular angular-only soft, angular rigid)",
           {s: (f"{_measure_momentum(s, O)[0]:.1e}", f"{_measure_momentum(s, O, linear=(0, 0))[1]:.1e}",
                f"{_measure_momentum(s, O, linear=(0, 0), angular=(0, 0))[1]:.1e}") for s in VARIANTS})

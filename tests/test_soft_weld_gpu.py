@@ -1,4 +1,4 @@
-"""GPU: soft welds (DESIGN.md §3.15). The device's soft weld rows against the soft weld oracle (tests/soft_weld_oracle.c) bit
+"""GPU: soft welds (DESIGN.md §3.15). The device's soft weld rows against the joint oracle (tests/joint_oracle.c) bit
 for bit, in every schedule, for all ten variants, persistent and launch by launch, with the warm-start gather on and off;
 every step of scenes.soft_welds (a donut of capsules on angular springs dropped on a pile, soft and rigid cantilevers, a
 box hanging on a linear spring, a box on a kinematic platform, contacts throughout) through the public API against
@@ -16,8 +16,7 @@ import math
 import numpy as np
 import pytest
 
-import soft_weld_oracle
-import weld_oracle
+import joint_oracle
 from helpers import (bit_equal, body_rows_from_ref, carry_sticky_friction, contact_rows_from_ref, joint_rows_from_ref,
                      load_bodies_into_ref, ref_delta_positions, store_oracle_bodies)
 from oracle import ref as refmod
@@ -102,14 +101,18 @@ def test_stage_matches_oracle(reference, dev, solver, mode, persistent, gather):
     order, _ = dw.solve_order(len(contacts) + len(joints))
     dw.destroy()
     order = None if mode == "wavefront" else order
-    ob, oc, oj = soft_weld_oracle.load().solve(capi.SOLVER[solver], bodies, contacts, joints, ctx, order=order)
+    ob, oc, oj = joint_oracle.load().solve(capi.SOLVER[solver], bodies, contacts, joints, ctx, order=order)
     valid = (bodies["flags"] & 1) == 1
     _compare_bodies(got, ob, valid)
     _compare_joints(got_joints, oj)
     live = contacts["pointCount"] > 0
     assert bit_equal(got_contacts["points"]["normalImpulse"][live], oc["points"]["normalImpulse"][live])
-    # the soft parts did work: the weld oracle, which reads no hertz, ends elsewhere
-    wb, _, _ = weld_oracle.load().solve(capi.SOLVER[solver], bodies, contacts, joints, ctx, order=order)
+    # the soft parts did work: the same rows with both weld hertz at 0 end elsewhere
+    rigid = joints.copy()
+    welds = device.joint_type(rigid["flags"]) == device.JOINT_WELD
+    rigid["hertz"][welds] = 0.0
+    rigid["maxMotorTorque"][welds] = 0.0
+    wb, _, _ = joint_oracle.load().solve(capi.SOLVER[solver], bodies, contacts, rigid, ctx, order=order)
     assert not bit_equal(wb["position"][valid], ob["position"][valid])
 
 
@@ -125,7 +128,7 @@ def test_soft_welds_scene_every_step(reference, product, dev, solver):
     finalize; the device runs the same steps through s2World_Step with real soft welds. Every step bit for bit: bodies,
     delta positions, contact impulses and joint impulses."""
     R, P = reference, product
-    O = soft_weld_oracle.load()
+    O = joint_oracle.load()
     sr = scenes.soft_welds(R, solver)
     sp = scenes.soft_welds(P, solver)
     assert "s2CreateWeldJoint" in R.missing and "s2CreateWeldJoint" not in P.missing
@@ -277,7 +280,7 @@ def test_public_world_every_step(product, dev, solver):
     P.s2World_Step(wid, DT, 4, 2, True)  # uploads the world
     dw = device.DeviceWorld.attach(dev, wid)
     dw.set_schedule(device.SCHEDULE_WAVEFRONT)
-    O = soft_weld_oracle.load()
+    O = joint_oracle.load()
     ctx = device.make_context(solver, DT, 4, 2)
     for _ in range(90):
         bodies = dw.download_all_bodies()
@@ -302,7 +305,7 @@ def test_setter_edits_between_replayed_steps(product, dev, solver):
     P.s2World_Step(wid, DT, 4, 2, True)
     dw = device.DeviceWorld.attach(dev, wid)
     dw.set_schedule(device.SCHEDULE_WAVEFRONT)
-    O = soft_weld_oracle.load()
+    O = joint_oracle.load()
     ctx = device.make_context(solver, DT, 4, 2)
     chain, hanging, rigid = joints[1], joints[4], joints[7]
     edits = {5: lambda: P.s2WeldJoint_SetLinearHertz(chain, 9.0),
@@ -335,15 +338,14 @@ def test_setter_edits_between_replayed_steps(product, dev, solver):
 def test_slot_reuse_across_types(product, dev):
     """A slot freed by a soft weld and taken by a revolute joint between the same bodies at the same anchor gives the
     revolute's own bits: its row carries none of the weld's soft lanes and each step equals the oracle's. The slot freed
-    again and taken by a prismatic joint carries none either (the soft weld oracle has no prismatic rows, so that step is
-    checked by its row only)."""
+    again and taken by a prismatic joint carries none either (that step is checked by its row only)."""
     P = product
     wid, joints, (a, b) = _soft_weld_world(P, "TGS_Soft")
     for _ in range(5):
         P.s2World_Step(wid, DT, 4, 2, True)
     dw = device.DeviceWorld.attach(dev, wid)
     dw.set_schedule(device.SCHEDULE_WAVEFRONT)
-    O = soft_weld_oracle.load()
+    O = joint_oracle.load()
     ctx = device.make_context("TGS_Soft", DT, 4, 2)
     slot = joints[4].index
     P.s2DestroyJoint(joints[4])

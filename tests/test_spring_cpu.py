@@ -1,4 +1,4 @@
-"""CPU: the joint spring's oracle (tests/spring_oracle.c, DESIGN.md §3.14) on hand-built rows, for all ten variants.
+"""CPU: the joint spring in the joint oracle (tests/joint_oracle.c, DESIGN.md §3.14) on hand-built rows, for all ten variants.
 
 No contacts and every local centre at zero, so finalize is the identity (origin == position) and solver stages chain
 directly. Gravity is off unless a test says otherwise. The bounds below were measured on these deterministic runs (the
@@ -8,7 +8,8 @@ each.
 Mutations each test catches: a spring coefficient formed with the wrong h or the wrong expression shifts the frequency or
 the rest translation; a spring that is not soft (the position error fed back at 1 / h) overshoots with zeta = 1; a spring
 impulse applied to one body only breaks momentum; a missing s2UnwindAngle turns the seam case the long way round; a
-spring term evaluated on a row without the flag (or with hertz == 0) changes the parent's bits."""
+spring term evaluated on a row without the flag (or with hertz == 0) changes the bits tests/test_joint_oracle_cpu.py
+pins."""
 import ctypes as C
 import math
 import os
@@ -19,8 +20,7 @@ import pytest
 
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 
-import prismatic_oracle  # noqa: E402
-import spring_oracle  # noqa: E402
+import joint_oracle  # noqa: E402
 from solver2d_b200 import capi, device  # noqa: E402
 
 VARIANTS = ["Jacobi", "PGS", "PGS_NGS", "PGS_NGS_Block", "PGS_Soft", "SoftStep", "TGS_Sticky", "TGS_Soft", "TGS_NGS", "XPBD"]
@@ -159,7 +159,7 @@ KIND_IDS = ["revolute", "prismatic"]
 
 
 def _measure_frequency(solver, kind):
-    e = _errors(kind, _run(spring_oracle.load(), solver, *_oscillator(kind, (1.0, 0.0)), 240))
+    e = _errors(kind, _run(joint_oracle.load(), solver, *_oscillator(kind, (1.0, 0.0)), 240))
     return abs(_frequency(e) - 1.0)
 
 
@@ -171,20 +171,20 @@ def test_oscillates_at_hertz(solver, kind):
 
 
 def _measure_overshoot(solver, kind):
-    e = _errors(kind, _run(spring_oracle.load(), solver, *_oscillator(kind, (2.0, 1.0)), 180))
+    e = _errors(kind, _run(joint_oracle.load(), solver, *_oscillator(kind, (2.0, 1.0)), 180))
     return float(max(0.0, -e.min()))
 
 
 @pytest.mark.parametrize("kind", KINDS, ids=KIND_IDS)
 @pytest.mark.parametrize("solver", VARIANTS)
 def test_critical_damping_does_not_overshoot(solver, kind):
-    e = _errors(kind, _run(spring_oracle.load(), solver, *_oscillator(kind, (2.0, 1.0)), 180))
+    e = _errors(kind, _run(joint_oracle.load(), solver, *_oscillator(kind, (2.0, 1.0)), 180))
     assert e.min() >= -(OVERSHOOT_STICKY if solver == "TGS_Sticky" else OVERSHOOT_BOUND)
     assert abs(e[-1]) < 0.1 * 0.2  # and it returns
 
 
 def _measure_keep(solver, kind):
-    e = _errors(kind, _run(spring_oracle.load(), solver, *_oscillator(kind, (1.0, 0.0)), 300))
+    e = _errors(kind, _run(joint_oracle.load(), solver, *_oscillator(kind, (1.0, 0.0)), 300))
     first = np.abs(e[:60]).max()
     last = np.abs(e[240:]).max()
     return float(last / first)
@@ -201,7 +201,7 @@ def _measure_rest(solver):
     omega = 2.0 * math.pi * hertz
     bodies = _bodies([(capi.STATIC_BODY, 0, 0, 0, 0, 0, 0), (capi.DYNAMIC_BODY, 0, 0, 0, 0, 0, 0)])
     joints = np.array([_joint(bodies, device.JOINT_PRISMATIC, 0, 1, (0.0, 0.0), axis=(0.0, 1.0), spring=(hertz, 0.7))])
-    h = _run(spring_oracle.load(), solver, bodies, joints, 300, gravity=(0.0, -G))
+    h = _run(joint_oracle.load(), solver, bodies, joints, 300, gravity=(0.0, -G))
     rest = -G / (omega * omega)
     b, j = h[-1]
     return abs(_error(device.JOINT_PRISMATIC, b, j[0]) - rest) / abs(rest)
@@ -238,7 +238,7 @@ def _measure_momentum(solver, kind, hertz=None):
         joints[0]["hertz"] = hertz
     p0, L0 = _momentum(bodies)
     worst = 0.0
-    for b, _ in _run(spring_oracle.load(), solver, bodies, joints, 60):
+    for b, _ in _run(joint_oracle.load(), solver, bodies, joints, 60):
         p, L = _momentum(b)
         worst = max(worst, float(np.abs(p - p0).max()), abs(L - L0))
     return worst
@@ -263,7 +263,7 @@ def test_zero_hertz_exerts_nothing(solver, kind):
     off = joints.copy()
     off[0]["flags"] &= ~device.JOINT_ENABLE_SPRING
     joints[0]["hertz"] = 0.0
-    O = spring_oracle.load()
+    O = joint_oracle.load()
     for (b1, j1), (b2, j2) in zip(_run(O, solver, bodies, joints, 30, gravity=(0.0, -G)),
                                   _run(O, solver, bodies, off, 30, gravity=(0.0, -G))):
         assert b1.tobytes() == b2.tobytes()
@@ -281,7 +281,7 @@ def _measure_seam(solver):
     joints = np.array([_joint(bodies, device.JOINT_REVOLUTE, 0, 1, (0.0, 0.0), ref=ref, spring=(2.0, 1.0))])
     travelled = 0.0
     prev = _angle(bodies, 1)
-    hist = _run(spring_oracle.load(), solver, bodies, joints, 180)
+    hist = _run(joint_oracle.load(), solver, bodies, joints, 180)
     for b, _ in hist:
         a = _angle(b, 1)
         travelled += (a - prev + math.pi) % (2.0 * math.pi) - math.pi
@@ -295,37 +295,11 @@ def test_rest_angle_across_the_seam(solver):
     assert travel_error <= SEAM_BOUND and rest_error <= SEAM_BOUND
 
 
-def _mixed_rows(bodies):
-    """A revolute with limit and motor, a prismatic with limit and motor, and a mouse row: none carries the spring flag."""
-    rev = _joint(bodies, device.JOINT_REVOLUTE, 0, 1, (0.0, 0.0), limit=(-0.3, 0.4), motor=(1.0, 5.0), slot=0)
-    pri = _joint(bodies, device.JOINT_PRISMATIC, 1, 2, (1.0, 0.0), axis=(1.0, 0.3), limit=(-0.2, 0.3), motor=(-0.5, 8.0),
-                 slot=1)
-    mouse = np.zeros(1, dtype=device.JOINT_ROW)[0]
-    mouse["index"] = 2
-    mouse["flags"] = device.ROW_VALID | (device.JOINT_MOUSE << 1)
-    mouse["bodyA"], mouse["bodyB"] = 0, 2
-    mouse["localOriginAnchorB"] = (0.1, 0.0)
-    mouse["target"] = (2.5, 0.5)
-    mouse["hertz"], mouse["dampingRatio"] = 5.0, 0.7
-    return np.array([rev, pri, mouse])
-
-
-@pytest.mark.parametrize("solver", VARIANTS)
-def test_rows_without_the_flag_keep_the_parent_bits(solver):
-    bodies = _bodies([(capi.STATIC_BODY, 0, 0, 0, 0, 0, 0), (capi.DYNAMIC_BODY, 0.0, 0.0, 0.1, 0.2, 0.0, 1.0),
-                      (capi.DYNAMIC_BODY, 1.2, 0.1, 0.0, 0.0, 0.3, -0.5)])
-    joints = _mixed_rows(bodies)
-    a = _run(spring_oracle.load(), solver, bodies, joints, 40, gravity=(0.0, -G))
-    b = _run(prismatic_oracle.load(), solver, bodies, joints, 40, gravity=(0.0, -G))
-    for (b1, j1), (b2, j2) in zip(a, b):
-        assert b1.tobytes() == b2.tobytes() and j1.tobytes() == j2.tobytes()
-
-
 @pytest.mark.parametrize("solver", ["TGS_Soft", "PGS", "TGS_Sticky"])
 def test_spring_impulse_is_kept_only_with_the_flag_and_warm_start(solver):
     """The stored spring impulse: nonzero on a loaded spring, 0 once the flag is cleared (the row is re-prepared cold)."""
     bodies, joints = _oscillator(device.JOINT_REVOLUTE, (1.0, 0.2))
-    O = spring_oracle.load()
+    O = joint_oracle.load()
     ctx = device.make_context(solver, DT, 4, 2)
     contacts = np.zeros(0, dtype=device.CONTACT_ROW)
     bodies, _, joints = O.solve(capi.SOLVER[solver], bodies, contacts, joints, ctx, gravity=(0.0, 0.0))
@@ -347,7 +321,7 @@ def test_revolute_spring_without_rotation_does_nothing(solver):
     bodies, joints = _fixed_rotation_rows()
     off = joints.copy()
     off[0]["flags"] &= ~device.JOINT_ENABLE_SPRING
-    O = spring_oracle.load()
+    O = joint_oracle.load()
     for (b1, j1), (b2, _) in zip(_run(O, solver, bodies, joints, 10), _run(O, solver, bodies, off, 10)):
         assert b1.tobytes() == b2.tobytes() and float(j1[0]["springImpulse"]) == 0.0
 

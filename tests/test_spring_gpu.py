@@ -1,5 +1,5 @@
-"""GPU: joint springs on revolute and prismatic joints (DESIGN.md §3.14). The device's spring rows against the spring oracle
-(tests/spring_oracle.c) bit for bit, in every schedule, for all ten variants, persistent and launch by launch, with the
+"""GPU: joint springs on revolute and prismatic joints (DESIGN.md §3.14). The device's spring rows against the joint oracle
+(tests/joint_oracle.c) bit for bit, in every schedule, for all ten variants, persistent and launch by launch, with the
 warm-start gather on and off; every step of scenes.springs (cars on suspension springs over bumps, a soft chain falling on a
 pile, contacts throughout) through the public API against reference collide and finalize around the spring oracle, with
 the kinematic carriage and XPBD's delta positions carried; a contact-free world stepped against the oracle alone; setter
@@ -16,8 +16,7 @@ import math
 import numpy as np
 import pytest
 
-import prismatic_oracle
-import spring_oracle
+import joint_oracle
 from helpers import (bit_equal, body_rows_from_ref, carry_sticky_friction, contact_rows_from_ref, joint_rows_from_ref,
                      load_bodies_into_ref, ref_delta_positions, store_oracle_bodies)
 from oracle import ref as refmod
@@ -93,12 +92,14 @@ def test_stage_matches_oracle(reference, dev, solver, mode, persistent, gather):
     order, _ = dw.solve_order(len(contacts) + len(joints))
     dw.destroy()
     order = None if mode == "wavefront" else order
-    ob, _, oj = spring_oracle.load().solve(capi.SOLVER[solver], bodies, contacts, joints, ctx, order=order)
+    ob, _, oj = joint_oracle.load().solve(capi.SOLVER[solver], bodies, contacts, joints, ctx, order=order)
     valid = (bodies["flags"] & 1) == 1
     _compare_bodies(got, ob, valid)
     _compare_joints(got_joints, oj)
-    # the springs did work: the prismatic oracle, which has no spring, ends elsewhere
-    pb, _, _ = prismatic_oracle.load().solve(capi.SOLVER[solver], bodies, contacts, joints, ctx, order=order)
+    # the springs did work: the same rows with the spring flag cleared end elsewhere
+    unsprung = joints.copy()
+    unsprung["flags"] &= ~device.JOINT_ENABLE_SPRING
+    pb, _, _ = joint_oracle.load().solve(capi.SOLVER[solver], bodies, contacts, unsprung, ctx, order=order)
     assert not bit_equal(pb["position"][valid], ob["position"][valid])
     if solver != "XPBD":
         assert np.any(oj["springImpulse"][sprung] != 0.0)
@@ -126,7 +127,7 @@ def test_springs_scene_every_step(reference, product, dev, solver):
     finalize; the device runs the same steps through s2World_Step with real springs. Every step bit for bit: bodies, delta
     positions, contact impulses and joint impulses, the spring impulse included."""
     R, P = reference, product
-    O = spring_oracle.load()
+    O = joint_oracle.load()
     sr = scenes.springs(R, solver)
     sp = scenes.springs(P, solver)
     assert "s2CreatePrismaticJoint" in R.missing and "s2CreatePrismaticJoint" not in P.missing
@@ -295,7 +296,7 @@ def test_public_world_every_step(product, dev, solver):
     dw = device.DeviceWorld.attach(dev, wid)
     assert dw.body_cap >= 12 and dw.joint_cap >= 8
     dw.set_schedule(device.SCHEDULE_WAVEFRONT)
-    O = spring_oracle.load()
+    O = joint_oracle.load()
     ctx = device.make_context(solver, DT, 4, 2)
     for _ in range(90):
         bodies = dw.download_all_bodies()
@@ -321,7 +322,7 @@ def test_setter_edits_between_replayed_steps(product, dev, solver):
     dw = device.DeviceWorld.attach(dev, wid)
     assert dw.body_cap >= 12 and dw.joint_cap >= 8
     dw.set_schedule(device.SCHEDULE_WAVEFRONT)
-    O = spring_oracle.load()
+    O = joint_oracle.load()
     ctx = device.make_context(solver, DT, 4, 2)
     rev, pri = joints[0], joints[4]
     edits = {5: lambda: P.s2RevoluteJoint_SetSpringHertz(rev, 5.0),

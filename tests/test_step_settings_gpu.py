@@ -28,8 +28,7 @@ sub-step's warm start reads them."""
 import numpy as np
 import pytest
 
-import distance_oracle
-import soft_weld_oracle
+import joint_oracle
 from solver2d_b200 import capi, device, scenes
 from test_distance_gpu import _distance_world, _step_and_compare
 from test_e2e_gpu import _angles, _positions, _ref_pair_table
@@ -213,8 +212,7 @@ def test_settings_change_mid_run(reference, product, dev, solver, sequence):
 
 # ---- (d) contact-free joint worlds ----------------------------------------------------------------------------------------
 
-JOINT_WORLDS = {"springs": (_spring_world, distance_oracle), "distance": (_distance_world, distance_oracle),
-                "soft_welds": (_soft_weld_world, soft_weld_oracle)}
+JOINT_WORLDS = {"springs": _spring_world, "distance": _distance_world, "soft_welds": _soft_weld_world}
 
 
 @pytest.mark.parametrize("substeps", [1, 8])
@@ -222,12 +220,12 @@ JOINT_WORLDS = {"springs": (_spring_world, distance_oracle), "distance": (_dista
 @pytest.mark.parametrize("solver", VARIANTS)
 def test_joint_worlds_at_substeps(product, dev, solver, world, substeps):
     P = product
-    build, oracle = JOINT_WORLDS[world]
+    build = JOINT_WORLDS[world]
     wid, _, _ = build(P, solver)
     P.s2World_Step(wid, 1.0 / 30.0, substeps, 0, True)  # uploads the world
     dw = device.DeviceWorld.attach(dev, wid)
     dw.set_schedule(device.SCHEDULE_COLOR)
-    _step_and_compare(P, wid, dw, oracle.load(), solver, 30, colour=True, dt=1.0 / 30.0, substeps=substeps, relax=0)
+    _step_and_compare(P, wid, dw, joint_oracle.load(), solver, 30, colour=True, dt=1.0 / 30.0, substeps=substeps, relax=0)
     P.s2DestroyWorld(wid)
 
 

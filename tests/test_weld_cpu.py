@@ -1,4 +1,4 @@
-"""CPU: the weld joint's oracle (tests/weld_oracle.c, DESIGN.md §3.8) on hand-built rows, for all ten variants.
+"""CPU: the weld joint in the joint oracle (tests/joint_oracle.c, DESIGN.md §3.8) on hand-built rows, for all ten variants.
 
 No contacts and every local centre at zero, so finalize is the identity (origin == position) and solver stages chain
 directly. The bounds below were measured on these deterministic runs (the largest value over the ten variants, printed
@@ -16,7 +16,7 @@ import pytest
 
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 
-import weld_oracle  # noqa: E402
+import joint_oracle  # noqa: E402
 from solver2d_b200 import capi, device  # noqa: E402
 
 VARIANTS = ["Jacobi", "PGS", "PGS_NGS", "PGS_NGS_Block", "PGS_Soft", "SoftStep", "TGS_Sticky", "TGS_Soft", "TGS_NGS", "XPBD"]
@@ -74,7 +74,7 @@ def _welds(bodies, links):
 
 
 def _run(solver, bodies, joints, steps, gravity=(0.0, 0.0)):
-    O = weld_oracle.load()
+    O = joint_oracle.load()
     ctx = device.make_context(solver, DT, 4, 2)
     contacts = np.zeros(0, dtype=device.CONTACT_ROW)
     history = []

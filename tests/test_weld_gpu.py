@@ -1,4 +1,4 @@
-"""GPU: the weld joint (DESIGN.md §3.8). The device's weld rows against the weld oracle (tests/weld_oracle.c) bit for bit, in
+"""GPU: the weld joint (DESIGN.md §3.8). The device's weld rows against the joint oracle (tests/joint_oracle.c) bit for bit, in
 every schedule and for all ten variants; every step of scenes.welded_structures through the public API; contacts between
 welded bodies; and the weld's lifecycle.
 
@@ -14,7 +14,7 @@ import ctypes as C
 import numpy as np
 import pytest
 
-import weld_oracle
+import joint_oracle
 from helpers import (bit_equal, body_rows_from_ref, carry_sticky_friction, contact_rows_from_ref, joint_rows_from_ref,
                      load_bodies_into_ref, ref_delta_positions, store_oracle_bodies)
 from oracle import ref as refmod
@@ -63,7 +63,7 @@ def test_stage_matches_oracle(reference, dev, solver, mode, persistent):
     """One stage of welded_structures rows (welds, revolutes with limit and motor, a mouse joint, contacts), the welds
     warm-started with an angular impulse."""
     R = reference
-    O = weld_oracle.load()
+    O = joint_oracle.load()
     sc = scenes.welded_structures(R, solver, copies=2)
     for _ in range(30):
         sc.step(DT, 4, 2, True)
@@ -105,7 +105,7 @@ def test_welded_structures_every_step(reference, product, dev, solver):
     """Reference collide on the stand-in world, the weld oracle in the device's order, reference finalize; the device runs
     the same steps through s2World_Step with real welds. Every step bit for bit: bodies, contact and joint impulses."""
     R, P = reference, product
-    O = weld_oracle.load()
+    O = joint_oracle.load()
     sr = scenes.welded_structures(R, solver)
     sp = scenes.welded_structures(P, solver)
     assert "s2CreateWeldJoint" in R.missing and "s2CreateWeldJoint" not in P.missing

@@ -1,4 +1,4 @@
-"""CPU: the wheel joint's oracle (tests/wheel_oracle.c, DESIGN.md §3.17) on hand-built rows, for all ten variants.
+"""CPU: the wheel joint in the joint oracle (tests/joint_oracle.c, DESIGN.md §3.17) on hand-built rows, for all ten variants.
 
 No contacts and every local centre at zero, so finalize is the identity (origin == position) and solver stages chain
 directly. The bounds below were measured on these deterministic runs (the largest value over the variants a test covers,
@@ -8,8 +8,8 @@ Mutations each test catches: a motor that acts on the axis instead of the rotati
 that is not clamped lifts a load it should not; a spring coefficient formed with another h shifts the frequency or the
 sag; a perpendicular row without its bias lets the anchor drift off the axis; a limit with its sign flipped lets the
 translation leave its range; a motor mass formed without the fixed-rotation test makes NaNs; a reaction that leaves the
-perpendicular or spring impulse out misreads the hanging load; a wheel branch that takes another type's rows changes the
-distance oracle's bits."""
+perpendicular or spring impulse out misreads the hanging load; a wheel branch that takes another type's rows changes the bits
+tests/test_joint_oracle_cpu.py pins."""
 import ctypes as C
 import math
 import os
@@ -20,8 +20,7 @@ import pytest
 
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 
-import distance_oracle  # noqa: E402
-import wheel_oracle  # noqa: E402
+import joint_oracle  # noqa: E402
 from solver2d_b200 import capi, device  # noqa: E402
 
 VARIANTS = ["Jacobi", "PGS", "PGS_NGS", "PGS_NGS_Block", "PGS_Soft", "SoftStep", "TGS_Sticky", "TGS_Soft", "TGS_NGS", "XPBD"]
@@ -96,8 +95,8 @@ def _wheel(a, b, anchor_a=(0.0, 0.0), anchor_b=(0.0, 0.0), axis=(0.0, 1.0), spri
     return r
 
 
-def _run(solver, bodies, joints, steps, gravity=(0.0, -G), oracle=None):
-    O = oracle or wheel_oracle.load()
+def _run(solver, bodies, joints, steps, gravity=(0.0, -G)):
+    O = joint_oracle.load()
     ctx = device.make_context(solver, DT, 4, 2)
     contacts = np.zeros(0, dtype=device.CONTACT_ROW)
     history = []
@@ -297,34 +296,6 @@ def test_hanging_sprung_wheel_reads_mg(solver):
 
 
 # ---- other joint types and layout -----------------------------------------------------------------------------------------
-
-@pytest.mark.parametrize("solver", VARIANTS)
-def test_other_types_keep_the_distance_oracles_bits(solver):
-    """A world of distance, prismatic (with spring), revolute (with limit and motor) and weld rows: the wheel oracle and the
-    distance oracle give the same bytes."""
-    bodies = _bodies([(capi.STATIC_BODY, 0, 0, 0, 0, 0, 1), (capi.DYNAMIC_BODY, 0.0, -1.0, 0.5, 0, 0.3, 1),
-                      (capi.DYNAMIC_BODY, 1.0, 0.0, 0, 0, 0, 1), (capi.DYNAMIC_BODY, 2.0, -0.5, 0, 0, 1.0, 1),
-                      (capi.DYNAMIC_BODY, 3.0, 0.0, 0, 0, 0, 1)])
-    rows = np.zeros(4, dtype=device.JOINT_ROW)
-    rows[0] = distance_row = _wheel(0, 1, slot=0)
-    distance_row["flags"] = device.ROW_VALID | (device.JOINT_DISTANCE << 1) | device.JOINT_ENABLE_SPRING
-    distance_row["referenceAngle"], distance_row["hertz"], distance_row["dampingRatio"] = 1.0, 2.0, 0.3
-    distance_row["lowerAngle"], distance_row["upperAngle"] = 0.005, 100000.0
-    rows[0] = distance_row
-    prismatic = _wheel(0, 2, anchor_a=(1.0, 0.0), axis=(1.0, 0.0), spring=(1.5, 0.2), limit=(-0.5, 0.5), motor=(0.3, 4.0), slot=1)
-    prismatic["flags"] = (int(prismatic["flags"]) & ~0xE) | (device.JOINT_PRISMATIC << 1)
-    rows[1] = prismatic
-    revolute = _wheel(2, 3, anchor_a=(1.0, -0.5), anchor_b=(0.0, 0.0), limit=(-0.4, 0.4), motor=(1.0, 3.0), slot=2)
-    revolute["flags"] = (int(revolute["flags"]) & ~0xE) | (device.JOINT_REVOLUTE << 1)
-    rows[2] = revolute
-    weld = _wheel(3, 4, anchor_a=(1.0, 0.5), anchor_b=(0.0, 0.0), slot=3)
-    weld["flags"] = device.ROW_VALID | (device.JOINT_WELD << 1)
-    rows[3] = weld
-    a = _run(solver, bodies.copy(), rows.copy(), 30)
-    b = _run(solver, bodies.copy(), rows.copy(), 30, oracle=distance_oracle.load())
-    for (ba, ja), (bb, jb) in zip(a, b):
-        assert ba.tobytes() == bb.tobytes() and ja.tobytes() == jb.tobytes()
-
 
 def test_struct_sizes_unchanged():
     """The wheel row reuses columns: s2bJointRow stays 108 bytes and every other ABI size is the parent's."""

@@ -1,4 +1,4 @@
-"""GPU: the wheel joint (DESIGN.md §3.17). The device against the wheel oracle (tests/wheel_oracle.c) bit for bit: every
+"""GPU: the wheel joint (DESIGN.md §3.17). The device against the joint oracle (tests/joint_oracle.c) bit for bit: every
 step of scenes.wheels (a motorised car over bumps, a car down a slope, a barrow on a rigid axle, a trolley on a kinematic
 rail, contacts throughout) through the public API against reference collide and finalize around the oracle, in the
 wavefront and the colour schedule; every step of a contact-free world for all ten variants, in both schedules, persistent
@@ -15,7 +15,7 @@ import ctypes as C
 import numpy as np
 import pytest
 
-import wheel_oracle
+import joint_oracle
 from helpers import (bit_equal, body_rows_from_ref, carry_sticky_friction, contact_rows_from_ref, joint_rows_from_ref,
                      load_bodies_into_ref, ref_delta_positions, store_oracle_bodies)
 from oracle import ref as refmod
@@ -172,7 +172,7 @@ def test_wheel_scene_every_step(reference, product, dev, solver, mode):
     the device runs the same steps through s2World_Step with real wheel joints. Every step bit for bit: bodies, delta
     positions, contact impulses and joint impulses, the spring impulse included."""
     R, P = reference, product
-    O = wheel_oracle.load()
+    O = joint_oracle.load()
     sr = scenes.wheels(R, solver)
     sp = scenes.wheels(P, solver)
     assert "s2CreateWheelJoint" in R.missing and "s2CreateWheelJoint" not in P.missing
@@ -275,7 +275,7 @@ def test_public_world_every_step(product, dev, solver, mode, persistent, gather)
     dw.set_schedule(device.SCHEDULE_WAVEFRONT if mode == "wavefront" else device.SCHEDULE_COLOR)
     dw.set_persistent(persistent)
     dw.set_warm_gather(gather)
-    _step_and_compare(P, wid, dw, wheel_oracle.load(), solver, 60, colour=mode == "color")
+    _step_and_compare(P, wid, dw, joint_oracle.load(), solver, 60, colour=mode == "color")
     P.s2DestroyWorld(wid)
 
 
@@ -305,7 +305,7 @@ def test_setter_edits_between_replayed_steps(product, dev, solver):
             P.s2WheelJoint_EnableSpring(joints[3], True)
 
     replays = dw.counters().graphReplays
-    _step_and_compare(P, wid, dw, wheel_oracle.load(), solver, 45, colour=True, edit=edit)
+    _step_and_compare(P, wid, dw, joint_oracle.load(), solver, 45, colour=True, edit=edit)
     assert dw.counters().graphReplays > replays
     P.s2DestroyWorld(wid)
 
@@ -319,7 +319,7 @@ def test_slot_reuse_across_types(product, dev):
     P.s2World_Step(wid, DT, 4, 2, True)
     dw = device.DeviceWorld.attach(dev, wid)
     dw.set_schedule(device.SCHEDULE_WAVEFRONT)
-    O = wheel_oracle.load()
+    O = joint_oracle.load()
     _step_and_compare(P, wid, dw, O, solver, 10)
     P.s2DestroyJoint(joints[0])
     pd = capi.default_prismatic_def()
